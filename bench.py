@@ -49,7 +49,7 @@ def gen_ascii(nbytes, seed):
 
 
 class ClockSampler:
-    """nvidia-smi sampling DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampling of clocks, throttle reasons and the power limit DURING the timed region."""
 
     def __init__(self, index):
         self.index = index
@@ -58,7 +58,7 @@ class ClockSampler:
 
     def start(self):
         q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
-             "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit")
         try:
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(self.index), "--query-gpu=" + q, "--format=csv,noheader,nounits", "-lms", "50"],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
@@ -96,29 +96,13 @@ class ClockSampler:
                 for nm, v in zip(names, r[5:9]):
                     if v.lower().startswith("active"):
                         reasons.add(nm)
+        plim = [float(r[9]) for r in self.rows if len(r) > 9 and r[9].replace(".", "").isdigit()]
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": sorted(reasons),
-                "samples": len(self.rows), "window": self.window}
+                "power_limit_w": max(plim) if plim else None, "samples": len(self.rows), "window": self.window}
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        try:
-            return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-        except Exception:
-            pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def traffic_from_profiles():
-    """DRAM bytes per record of the BWT kernels from the committed `ncu --set full` captures."""
-    p = os.path.join(ROOT, "profiles", "bwt_kernel_traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p))
-        except Exception:
-            return None
-    return None
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 def host_cores():
@@ -172,6 +156,27 @@ def run_reference(args):
 
 
 # ---------------------------------------------------------------------------------------------------
+DUMP_SAMPLE = 2 << 20   # bytes of the stream written by --dump-outputs: 8 MiB of float32 + 16 MiB of float64 indices
+
+
+def dump_outputs(dirname, stream):
+    """--dump-outputs: what b2_bzip2_compress_dev handed back in the last timed step -- the .bz2 stream (`stream`, a
+    uint8 tensor on the GPU) and its length.  A stream longer than DUMP_SAMPLE bytes is written as a sample at
+    positions drawn from a fixed seed and the stream length, so that equal streams give equal files."""
+    import torch
+    os.makedirs(dirname, exist_ok=True)
+    n = int(stream.numel())
+    if n > DUMP_SAMPLE:
+        g = np.random.Generator(np.random.PCG64(SEED))
+        idx = np.unique(g.integers(0, n, size=DUMP_SAMPLE, dtype=np.int64))
+    else:
+        idx = np.arange(n, dtype=np.int64)
+    vals = stream[torch.from_numpy(idx).to(stream.device)].cpu().numpy()
+    np.save(os.path.join(dirname, "compressed_size.npy"), np.array([n], dtype=np.float64))
+    np.save(os.path.join(dirname, "compressed_stream_sample_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(dirname, "compressed_stream_sample.npy"), vals.astype(np.float32))
+
+
 def _check(rc, what, _native):
     if rc:
         raise SystemExit("%s failed: %s" % (what, _native.last_error()))
@@ -337,6 +342,8 @@ def main():
     ap.add_argument("--mb", type=int, default=int(os.environ.get("B2_BENCH_MB", "1024")), help="MiB of input per GPU and step")
     ap.add_argument("--no-cpu", action="store_true", help="skip every leg that runs the CPU oracle (cpu_baseline, parity)")
     ap.add_argument("--no-extra", action="store_true", help="skip the config3 and bwtc legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write the last step's .bz2 stream (a seeded sample "
+                    "of its bytes) and its length as DIR/*.npy")
     ap.add_argument("--bwtc-mb", type=int, default=int(os.environ.get("B2_BENCH_BWTC_MB", "64")), help="MiB of the config-2 buffer for the BWTC leg (config 4 = 1024)")
     args = ap.parse_args()
     if args.impl == "reference":
@@ -352,6 +359,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench.py: no CUDA device (the product path has no CPU fallback)")
     torch.cuda.set_device(local)
+    props = torch.cuda.get_device_properties(local)
     if world > 1:
         import datetime
         # a mismatched collective must fail fast, not sit out the default 10 minute watchdog on N GPUs
@@ -454,6 +462,8 @@ def main():
     clocks = sampler.stop(t0, t0 + wall) if rank == 0 else None
     comp_bytes = state["comp"]
     trace = _native.last_trace() if world == 1 else []
+    if args.dump_outputs and world == 1:
+        dump_outputs(args.dump_outputs, d_out[:comp_bytes])
 
     # device time: max over ranks (events on the library's launching stream)
     t = torch.tensor([dev_ms, wall * 1e3], dtype=torch.float64, device="cuda")
@@ -476,6 +486,8 @@ def main():
         tg = torch.tensor([g0.elapsed_time(g1) / gsteps], dtype=torch.float64, device="cuda")
         dist.all_reduce(tg, op=dist.ReduceOp.MAX)
         gathered_ms = float(tg.item())
+        if args.dump_outputs and rank == 0:   # the fragments of the timed steps, assembled: the same stream
+            dump_outputs(args.dump_outputs, state["out"])
 
     # ---- multi-rank parity: the stream assembled from the ranks' fragments == the one-GPU stream of the same input ----
     sharded_parity = None
@@ -545,26 +557,22 @@ def main():
         value = total_raw * args.steps / (dev_ms_max / 1e3) / 1e6
         peak, peak_src = peaks()
         bwt_gbs = (agg["bwt_bytes"] / 1e9) / (agg["ms_bwt"] / 1e3) if agg.get("ms_bwt") else 0.0
-        tr = traffic_from_profiles() or {}
         msd = agg.get("msd_launches", 0) > 0
         if msd:
             nl = agg["msd_launches"]
             kb, ks = agg["msd_bucket_bytes"] / nl, agg["msd_scatter_bytes"] / nl
             mb_ms, ms_ms = agg["ms_msd_bucket"] / nl, agg["ms_msd_scatter"] / nl
             bucket_gbs, scatter_gbs = kb / 1e9 / (mb_ms / 1e3), ks / 1e9 / (ms_ms / 1e3)
-            recs = kb / 9.0
             roof = {"bound": "hbm", "kernel": "k_msd_bucket (shared-memory bucket sort of the forward BWT: records in, BWT column out)",
                     "achieved": bucket_gbs, "peak": peak, "unit": "GB/s", "frac": bucket_gbs / peak,
-                    "traffic": (tr.get("k_msd_bucket_dram_bytes_per_record") or 0) * recs or None, "traffic_source": tr.get("source"),
                     "peak_source": peak_src, "launches": int(nl), "algorithmic_bytes_per_launch": kb, "avg_launch_ms": mb_ms,
                     "algorithmic_bytes_per_unit": "9 per text byte (8-byte record read, 1 byte of the column written)",
                     "k_msd_scatter": {"achieved": scatter_gbs, "frac": scatter_gbs / peak, "algorithmic_bytes_per_launch": ks, "avg_launch_ms": ms_ms,
-                                      "traffic": (tr.get("k_msd_scatter_dram_bytes_per_record") or 0) * recs or None,
                                       "algorithmic_bytes_per_unit": "9 per text byte (1 read, 8-byte record written)"}}
         else:
             radix_gbs = (agg["radix_bytes"] / 1e9) / (agg["ms_radix"] / 1e3) if agg.get("ms_radix") else 0.0
             roof = {"bound": "hbm", "kernel": "k_radix_pass (BWT onesweep pass)", "achieved": radix_gbs, "peak": peak, "unit": "GB/s",
-                    "frac": radix_gbs / peak if peak else None, "traffic": None, "peak_source": peak_src, "launches": int(agg["radix_launches"]),
+                    "frac": radix_gbs / peak if peak else None, "peak_source": peak_src, "launches": int(agg["radix_launches"]),
                     "algorithmic_bytes_per_launch": agg["radix_bytes"] / max(agg["radix_launches"], 1),
                     "avg_launch_ms": agg["ms_radix"] / max(agg["radix_launches"], 1)}
         # the survey's formula for an LSD prefix-doubling sort, B = N (91 + 224 R), as an equivalent rate next to the executed bytes
@@ -578,11 +586,12 @@ def main():
                                      "91 N + 224 N R formula of a 4-pass LSD sort to the same time"}
         line = {
             "metric": METRIC, "value": value, "unit": "MB/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
-            "ms_per_step": dev_ms_max / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8",
+            "gpu": props.name, "ms_per_step": dev_ms_max / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8",
             "data": "synthetic",
             "config": {"workload": "%d MiB synthetic ASCII per GPU (PCG64 seed %d+rank), bzip2 -9 (900k blocks) encode" % (args.mb, SEED),
                        "level": LEVEL, "bytes_per_gpu": shard, "total_bytes": nbytes, "blocks_per_gpu": int(agg["blocks"] // max(args.steps, 1)),
-                       "l2": "inputs (%d MiB) larger than L2 (126 MB); no flush needed" % args.mb, "bwt_batch_blocks": int(os.environ.get("B2_BWT_BATCH", "296")),
+                       "l2": "inputs (%d MiB) larger than L2 (50 MB); no flush needed" % args.mb,
+                       "bwt_batch_blocks": int(os.environ.get("B2_BWT_BATCH") or 2 * props.multi_processor_count),
                        "compressed_bytes": comp_bytes, "wall_ms_per_step": wall_ms_max / args.steps},
             "e2e": {"value": total_raw * e2e_steps / e2e_wall / 1e6, "unit": "MB/s", "h2d_bytes_per_step": nbytes if world == 1 else nbytes + (world - 1) * HALO, "d2h_bytes_per_step": e2e_comp,
                     "steps": e2e_steps, "api": "b2_bzip2_compress (host pinned in, library-pinned out; upload in 64 MiB chunks and download per batch overlapped with the encode)" if world == 1 else

@@ -1,8 +1,8 @@
-"""compressjs_b200 -- B200-native drop-in for the bzip2 block pipeline of cscott/compressjs.
+"""compressjs_b200 -- GPU-native (H100) drop-in for the bzip2 block pipeline of cscott/compressjs.
 
 Mirrors the reference's package surface for that path (main.js:1-29): ``Bzip2``, ``BWT`` and (experimental)
 ``BWTC`` with the reference's member names and argument meaning.  All compute runs
-in libb2bz.so (hand-written CUDA for sm_100a) through the C ABI in include/b2bz.h; there is no
+in libb2bz.so (hand-written CUDA for sm_90a) through the C ABI in include/b2bz.h; there is no
 CPU fallback.
 """
 from . import _native

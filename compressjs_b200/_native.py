@@ -46,7 +46,7 @@ def lib():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             "compressjs_b200: %s is missing -- build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). There is no CPU fallback." % LIB_PATH)
+            "(nvcc, sm_90a). There is no CPU fallback." % LIB_PATH)
     L = C.CDLL(LIB_PATH)
     u8pp, szp = C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(C.c_size_t)
     L.b2_init.argtypes = [C.c_int]

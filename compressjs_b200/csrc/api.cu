@@ -138,6 +138,9 @@ static Ctx& ctx_locked() {
     CUDA_CHECK(cudaDeviceGetDefaultMemPool(&pool, dev));
     uint64_t thr = UINT64_MAX;
     CUDA_CHECK(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr));
+    int sms = 0;
+    CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    c->bwt_batch = 2u * (u32)sms;
     const char* b = getenv("B2_BWT_BATCH");
     if (b && atoi(b) > 0) c->bwt_batch = (u32)atoi(b);
     const char* msd = getenv("B2_BWT_MSD");

@@ -1,9 +1,8 @@
 // bwtc.cu -- compressjs' BWTC container (lib/BWTC.js:12-231) on the GPU.
 //
 // STATUS: new in round 1.  The serial model / range-coder code (bwtc_core.cuh) is verified on its host build against
-// the oracle (tests/test_host_api.py::test_bwtc_core_matches_oracle); the kernels and the orchestration below ran on a
-// B200 once with the last seconds of the round's GPU budget (tools/bwtc_try.py -> profiles/r1e_bwtc_try.txt: 12 cases,
-// levels 1 and 9, one to three blocks, encode bit exact and decode correct).  Not yet measured at BASELINE config 4.
+// the oracle (tests/test_host_api.py::test_bwtc_core_matches_oracle); the kernels and the orchestration below are
+// checked against the oracle by tests/test_gpu_zz_bwtc.py.  Not yet measured at BASELINE config 4.
 //
 // Per block the container needs: sentinel BWT (lib/BWT.js:328-350), MTF over the used bytes, zero runs as
 // RUNA/RUNB digits, an adaptive model (Fenwick tree, or the deferred-sum model below level 6) that turns every

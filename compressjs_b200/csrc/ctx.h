@@ -21,7 +21,7 @@ struct Ctx {
   size_t ev_used = 0;
   std::vector<std::pair<int, size_t>> ev_tags;  // (stage id, pool index) recorded in the current call
   std::vector<b2_block_trace> trace;
-  u32 bwt_batch = 296;  // bzip2 blocks processed together in one batch (2 CTAs x 148 SMs for the per-block kernels)
+  u32 bwt_batch = 264;  // bzip2 blocks processed together in one batch: 2 CTAs per SM for the per-block kernels (set from the SM count)
   bool timing = true;
   bool bwt_msd = true;  // MSD + shared-memory bucket sort for sparse-tie batches (bwt_msd.cu); B2_BWT_MSD=0 disables it
   bool bwt_wide = false, bwt_wide_forced = false, bwt_mode_known = false;  // 8-byte initial sort for text-like batches (see bwt.cu)

@@ -123,8 +123,8 @@ struct BitReader {
 
 // ---- header + Huffman decode: one CTA per candidate ------------------------------------------
 // One CTA per block.  The per-group phases are spread over the CTA's warps, and a block's ~18 000 groups are strictly
-// serial, so a launch lasts as long as one block takes: with all SM slots taken (9 x 128 threads: ~1300 blocks, a 1 GiB
-// file) four warps per block give the best throughput; with fewer blocks the same thread budget goes to fewer, wider CTAs
+// serial, so a launch lasts as long as one block takes: with all SM slots taken (10 x 128 threads on 132 SMs: 1320 blocks,
+// a 1 GiB file) four warps per block give the best throughput; with fewer blocks the same thread budget goes to fewer, wider CTAs
 // (256 or 512 threads: fewer window offsets per thread, a shorter group).
 #define HD_THREADS 128
 #define HD_LUT_BITS 9   // 6 tables x 512 entries: keeps a warp's state under 19 KB so that 12 blocks fit per SM
@@ -166,9 +166,11 @@ __device__ __noinline__ u32 hdec_slow(const HdecWarp& s, u32 g, u32 bits20, int 
   return 0;
 }
 
-// 128 threads: 9 CTAs per SM (56 registers, 19 KB of shared memory each): a 1 GiB file's ~1200 blocks are resident at once
+// 128 threads: 10 CTAs per SM (45 registers, 19 KB of shared memory each), so that the ~1200 blocks of a 1 GiB file are
+// resident at once on the 132 SMs of an H100.  At 9 per SM (1188 slots) the last blocks ran as a second wave: 66 ms
+// instead of 44 ms per GiB (H100 SXM, 400 W power limit).
 template <int HD_T>
-__global__ void __launch_bounds__(HD_T, 1152 / HD_T)
+__global__ void __launch_bounds__(HD_T, HD_T == 128 ? 10 : 1152 / HD_T)
 k_hdec(const u8* __restrict__ in, u64 nbytes, const Cand* __restrict__ cands, u32 first, u32 count, u32 dbuf_size, u8* __restrict__ sel_buf,
        u16* __restrict__ sym_out, CandRes* __restrict__ res) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -1213,7 +1215,7 @@ static void dec_open(Ctx& c, DecSession& S, const u8* d_in_user, size_t n, bool 
 
   // ---- 2. decode the own share of the candidate blocks, in batches ----
   // the per-block Huffman stage is one CTA per block and latency bound: give it every block at once
-  // (about 19 MB of scratch per block; 180 GB of HBM take thousands)
+  // (about 19 MB of scratch per block: a batch of 2048 takes about half of an 80 GB H100)
   const u32 DB = dec_batch_blocks(c);
   dec_attr_once();
   if (nb) {

@@ -365,7 +365,8 @@ struct EncSession {
     const u32 B = (u32)((count + nbatches - 1) / nbatches);
     reserve((u32)std::min<size_t>(B, count));
     // all stage temporaries of one batch come to ~40 bytes per slot; size the pool for the batch class once
-    if (B > 74) c.prewarm((size_t)(B > 148 ? std::max<u32>(B, c.bwt_batch) : 148u) * 40 << SEG_SHIFT);
+    const u32 half = c.bwt_batch / 2, quarter = c.bwt_batch / 4;
+    if (B > quarter) c.prewarm((size_t)(B > half ? std::max<u32>(B, c.bwt_batch) : half) * 40 << SEG_SHIFT);
     const size_t done0 = all_crc.size();
     all_crc.resize(done0 + count);
     tr.resize(done0 + count);

@@ -1,5 +1,5 @@
 // tma.cuh -- bulk asynchronous copies (the 1-D form of the Tensor Memory Accelerator path) and the
-// mbarrier they complete on, as inline PTX for sm_100a.  SASS: UBLKCP (cp.async.bulk), SYNCS (mbarrier).
+// mbarrier they complete on, as inline PTX for sm_90a.  SASS: UBLKCP (cp.async.bulk), SYNCS (mbarrier).
 // Used to stage contiguous runs of sort records / text tiles into shared memory while the CTA works on
 // something else (bwt_msd.cu, mtf.cu).
 #pragma once

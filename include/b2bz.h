@@ -1,9 +1,9 @@
 /*
- * b2bz.h -- C ABI of libb2bz.so, the B200-native bzip2 / BWT block pipeline.
+ * b2bz.h -- C ABI of libb2bz.so, the GPU-native (H100) bzip2 / BWT block pipeline.
  *
  * This is the drop-in boundary for compressjs' bzip2 hot path.  Every entry point
- * below replaces one JavaScript function of the reference (file:line under
- * /root/reference); a Node N-API addon (compressjs_b200/napi/addon.cc), or any other
+ * below replaces one JavaScript function of the reference (file:line in
+ * cscott/compressjs); a Node N-API addon (compressjs_b200/napi/addon.cc), or any other
  * FFI, binds exactly these symbols.  Plain pointers and sizes only.
  *
  * Conventions

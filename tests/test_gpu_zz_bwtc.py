@@ -1,6 +1,6 @@
 """GPU parity of the BWTC container path (compressjs_b200/csrc/bwtc.cu; lib/BWTC.js:12-231) against the oracle.
-The file sorts last on purpose: the path is the newest one (first B200 run: profiles/r1e_bwtc_try.txt, 12 cases bit
-exact); the serial code it executes is also checked on the host by tests/test_host_api.py::test_bwtc_core_matches_oracle."""
+The file sorts last on purpose: the path is the newest one; the serial code it executes is also checked on the host
+by tests/test_host_api.py::test_bwtc_core_matches_oracle."""
 import pytest
 
 from oracle import oracle as O

@@ -85,12 +85,11 @@ def test_stream_coercion():
         S.deliver_output(bytearray(6), data)
 
 
-def test_device_allocator_port_matches_kats():
+def test_device_allocator_port_matches_kats(tmp_path):
     """compressjs_b200/csrc/huffalloc.cuh compiled for the host == test/huffman.js known answers."""
     import ctypes as C
     import subprocess
-    import tempfile
-    so = os.path.join(tempfile.gettempdir(), "libha_test.so")
+    so = str(tmp_path / "libha_test.so")
     subprocess.check_call(["gcc", "-O2", "-shared", "-fPIC", "-x", "c", os.path.join(ROOT, "tests", "host", "huffalloc_host.c"), "-o", so])
     L = C.CDLL(so)
     fib = [0, 1]
@@ -113,14 +112,13 @@ def test_device_allocator_port_matches_kats():
         assert f(fr, 20) == O.huffman_code_lengths(fr.tolist(), 20)
 
 
-def test_bwtc_core_matches_oracle():
+def test_bwtc_core_matches_oracle(tmp_path):
     """compressjs_b200/csrc/bwtc_core.cuh (the serial model + range coder that bwtc.cu runs on the GPU) built for the
     host: container bytes and decoded L columns must equal the oracle's for every level family."""
     import ctypes as C
     import subprocess
-    import tempfile
     from oracle import oracle as O
-    so = os.path.join(tempfile.gettempdir(), "libbwtc_host_test.so")
+    so = str(tmp_path / "libbwtc_host_test.so")
     subprocess.check_call(["gcc", "-O2", "-shared", "-fPIC", "-x", "c", os.path.join(ROOT, "tests", "host", "bwtc_host.c"), "-o", so])
     L = C.CDLL(so)
     L.host_bwtc_encode.restype = C.c_size_t

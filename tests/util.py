@@ -3,21 +3,14 @@ import ctypes as C
 import os
 
 import numpy as np
-import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_FIX_DIRS = [os.path.join(ROOT, "oracle", "_ref", "fixtures"), "/root/reference/test"]
 
 
 def fixture(name):
-    """Reference test fixture (test/sample*.ref, *.bz2, *.bzt ...).  They are not copied into git:
-    __graft_entry__.build() mirrors them into oracle/_ref/fixtures (git-ignored, travels to the GPU box)."""
-    for d in _FIX_DIRS:
-        p = os.path.join(d, name)
-        if os.path.exists(p):
-            with open(p, "rb") as f:
-                return f.read()
-    pytest.skip("reference fixture %s not available" % name)
+    """compressjs test fixture (test/sample*.ref, *.bz2, *.bzt ...), rebuilt from tests/golden/fixtures.xz."""
+    from oracle import fixtures
+    return fixtures.load(name)
 
 
 def rng(seed):
