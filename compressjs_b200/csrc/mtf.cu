@@ -4,15 +4,15 @@
 // lib/Bzip2.js:53-60 (mtf()).  The reference walks the block byte by byte with a linear
 // search in M.  Parallel form:
 //   k_used        : 256-bit "byte occurs in block" map per block
-//   k_mtf_lastpos : per 4 KiB chunk, last position of every byte value inside the chunk
+//   k_mtf_lastpos : per 4 KiB chunk (one warp each), last position of every byte value inside the chunk
 //   k_mtf_prefix  : per block, running max over the chunks -> last occurrence BEFORE each chunk;
 //                   the MTF list at a chunk start is "bytes by most recent occurrence, then the
 //                   not-yet-seen used bytes in ascending order" (the initial list M)
 //   k_mtf_ranks   : one warp per chunk, 32 bytes per step: every byte value carries a recency key
-//                   (255 - rank at the chunk start, or 256 + position of its last occurrence inside
-//                   the chunk); the rank of a byte is the number of live keys above its own, counted
-//                   through a bucketed live-key bitmap with suffix sums, and the bytes of one step
-//                   that precede each other are settled with SWAR pair compares
+//                   (255 - rank at the chunk start, found by a register bitonic sort, or 256 + position
+//                   of its last occurrence inside the chunk); the rank of a byte is the number of live
+//                   keys above its own, counted through a bucketed live-key bitmap with suffix sums, and
+//                   the bytes of one step that precede each other are settled with a ballot radix compare
 //                   The same pass summarises the chunk for the zero-run coder: leading / trailing zeros and the number
 //                   of symbols its non-zero ranks and interior runs will emit.
 //   k_rle2_scan   : one warp per block walks the chunk summaries: output offset and carried-in run length of every chunk
@@ -49,52 +49,76 @@ __global__ void __launch_bounds__(256) k_used_from_hist(const u32* __restrict__ 
   if ((threadIdx.x & 31) == 0) used[blockIdx.x * 8 + (threadIdx.x >> 5)] = bal;
 }
 
-// lastpos[(seg*cps + chunk)*256 + c] = (last position of byte c inside the chunk) + 1, 0 if none
-__global__ void __launch_bounds__(256) k_mtf_lastpos(const u8* __restrict__ U, const u32* __restrict__ seg_n, u32 cps, u32* __restrict__ lastpos) {
-  __shared__ u32 last[256];
-  last[threadIdx.x] = 0;
-  __syncthreads();
-  const u32 seg = blockIdx.x / cps, ch = blockIdx.x % cps;
+// lastpos[(seg*cps + chunk)*256 + c] = (last position of byte c inside the chunk) + 1, 0 if none.
+// One warp per chunk; every lane reads 16 bytes at a time and folds them into the warp's table with shared atomicMax.
+#define LP_WARPS 8
+__global__ void __launch_bounds__(LP_WARPS * 32)
+k_mtf_lastpos(const u8* __restrict__ U, const u32* __restrict__ seg_n, u32 cps, u32 nchunks, u32* __restrict__ lastpos) {
+  __shared__ __align__(16) u32 last[LP_WARPS][256];
+  const u32 w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const u32 gchunk = blockIdx.x * LP_WARPS + w;
+  if (gchunk >= nchunks) return;
+  u32* L = last[w];
+  uint4* L4 = reinterpret_cast<uint4*>(L);
+  L4[2 * lane] = make_uint4(0, 0, 0, 0);
+  L4[2 * lane + 1] = make_uint4(0, 0, 0, 0);
+  __syncwarp();
+  const u32 seg = gchunk / cps, ch = gchunk % cps;
   const u32 n = seg_n[seg];
   const u32 start = ch * MTF_CHUNK;
   if (start < n) {
     const u8* p = U + ((size_t)seg << SEG_SHIFT);
     const u32 end = min(n, start + MTF_CHUNK);
-    for (u32 i = start + threadIdx.x; i < end; i += 256) atomicMax(&last[p[i]], i + 1);
+    for (u32 i0 = start + lane * 16; i0 < end; i0 += 512) {
+      const uint4 x = *reinterpret_cast<const uint4*>(p + i0);  // inside the 1 MiB slot; bytes past n are skipped
+      const u32 xw[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+      for (int j = 0; j < 16; j++)
+        if (i0 + j < end) atomicMax(&L[(xw[j >> 2] >> (8 * (j & 3))) & 255u], i0 + j + 1);
+    }
   }
-  __syncthreads();
-  lastpos[(size_t)blockIdx.x * 256 + threadIdx.x] = last[threadIdx.x];
+  __syncwarp();
+  uint4* out = reinterpret_cast<uint4*>(lastpos + (size_t)gchunk * 256);
+  out[2 * lane] = L4[2 * lane];
+  out[2 * lane + 1] = L4[2 * lane + 1];
 }
 
-// in place: lastpos[chunk] := max over earlier chunks (exclusive)
+// in place: lastpos[chunk] := max over earlier chunks (exclusive).  The loads of 16 chunks are issued together, so the
+// walk over a block's ~220 chunks waits for memory 14 times instead of 220.
+#define MP_BATCH 16
 __global__ void __launch_bounds__(256) k_mtf_prefix(const u32* __restrict__ seg_n, u32 cps, u32* __restrict__ lastpos) {
   const u32 seg = blockIdx.x;
   const u32 n = seg_n[seg];
   const u32 nch = (n + MTF_CHUNK - 1) / MTF_CHUNK;
+  u32* p = lastpos + (size_t)seg * cps * 256 + threadIdx.x;
   u32 run = 0;
-  for (u32 ch = 0; ch < nch; ch++) {
-    u32* p = lastpos + ((size_t)seg * cps + ch) * 256 + threadIdx.x;
-    u32 t = *p;
-    *p = run;
-    run = max(run, t);
+  for (u32 ch0 = 0; ch0 < nch; ch0 += MP_BATCH) {
+    u32 t[MP_BATCH];
+#pragma unroll
+    for (int j = 0; j < MP_BATCH; j++) t[j] = ch0 + j < nch ? p[(size_t)(ch0 + j) * 256] : 0u;
+#pragma unroll
+    for (int j = 0; j < MP_BATCH; j++) {
+      if (ch0 + j < nch) p[(size_t)(ch0 + j) * 256] = run;
+      run = max(run, t[j]);
+    }
   }
 }
 
 #define MR_WARPS 8
-#define MB_BUCKETS 36   // recency keys live in [0, 256 + 4096): 34 buckets of 128 values (+ slack)
+#define MB_BUCKETS 36   // recency keys live in [0, 256 + 4096): 34 buckets of 128 values (+ slack), two per lane
 struct MtfWarp {
-  u32 skey[256];              // scratch for the start-of-chunk ranking
-  u16 K[256];                 // recency key of every byte value (larger = used more recently)
-  u32 bm[MB_BUCKETS][4];      // bitmap of the key values that are currently somebody's key
-  u32 S[MB_BUCKETS];          // S[b] = number of live keys in buckets above b
-  u32 Pw[16];                 // the window's previous-use times, two 16-bit values per word
+  u16 K[256];                       // recency key of every byte value (larger = used more recently)
+  __align__(16) u32 bm[MB_BUCKETS][4];  // bitmap of the key values that are currently somebody's key
 };
 // MTF rank of a byte = number of byte values used more recently than it.  Every byte value carries
-// a 15-bit recency key: 255 - (list position at the chunk start) until it is used inside the chunk,
-// 256 + (position inside the chunk) afterwards.  A warp ranks 32 bytes per step:
-//   * P_i = time of the previous use of lane i's byte (an earlier lane of the window, or its key)
-//   * rank_i = #{keys alive before the window that are > P_i}        (bucket suffix sums + bitmap)
-//            + #{k in (prev_i, i) : P_k < P_i}                       (first use after P_i inside the window)
+// a 13-bit recency key: (list position at the chunk start, 0 = back of the list) until it is used inside
+// the chunk, 256 + (position inside the chunk) afterwards.  A warp ranks 32 bytes per step:
+//   * first use of a byte in the window: r0_i = #{keys alive before the window that are > its key}
+//     (bucket suffix sums + bitmap) -- its rank at the window start
+//   * T_i = time of the previous use of lane i's byte on a 9-bit scale that keeps the order of those times:
+//     255 - r0_i for a first use, 256 + prev_i for a byte an earlier lane prev_i of the window holds
+//   * rank_i = (r0_i for a first use) + #{k in (prev_i, i) : T_k < T_i}   (bytes first used after T_i inside the
+//     window), with the T_k < T_i lane mask built by a 9-round ballot radix compare
 //   * only the last use of a byte inside the window rewrites its key.
 __global__ void __launch_bounds__(MR_WARPS * 32)
 k_mtf_ranks(const u8* __restrict__ U, const u32* __restrict__ seg_n, u32 cps, const u32* __restrict__ lastpos,
@@ -110,60 +134,76 @@ k_mtf_ranks(const u8* __restrict__ U, const u32* __restrict__ seg_n, u32 cps, co
   if (start >= n) return;
   const u32 count = min((u32)MTF_CHUNK, n - start);
   MtfWarp& s = sm[w];
-  // ---- list position of every byte value at the chunk start (rank by counting) ----
-  const u32* lp = lastpos + (size_t)gchunk * 256;
-  u32 mykey[8];
+  const uint4* bm4 = reinterpret_cast<const uint4*>(&s.bm[0][0]);
+  // ---- list position of every byte value at the chunk start ----
+  // The list is: bytes seen before the chunk, most recent first; then the used bytes not seen yet, ascending; then the
+  // bytes the block never holds.  Sort keys carry the byte value in their low 8 bits and are all distinct:
+  //   seen 2^30 | lastpos << 8 | c,   not seen yet 2^29 | (255 - c) << 8 | c,   never held (255 - c) << 8 | c.
+  // A bitonic sort of the 256 keys, 8 per lane in lane-major order, puts them in ascending order; the sorted index of
+  // a byte is then its list position counted from the back.
+  u32 v[8];
+  {
+    const uint4* lp4 = reinterpret_cast<const uint4*>(lastpos + (size_t)gchunk * 256 + lane * 8);
+    const uint4 l0 = lp4[0], l1 = lp4[1];
+    const u32 l[8] = {l0.x, l0.y, l0.z, l0.w, l1.x, l1.y, l1.z, l1.w};
+    const u32 uw = used[seg * 8 + (lane >> 2)] >> ((lane & 3) * 8);
 #pragma unroll
-  for (int i = 0; i < 8; i++) {
-    const u32 c = lane * 8 + i;
-    const u32 l = lp[c];
-    const bool isused = (used[seg * 8 + (c >> 5)] >> (c & 31)) & 1;
-    u32 key;
-    if (l) key = 0x40000000u | l;          // seen: most recent first
-    else if (isused) key = 0x200u + (255u - c);  // not seen yet: ascending byte value
-    else key = 255u - c;                    // never occurs: behind everything
-    mykey[i] = key;
-    s.skey[c] = key;
-  }
-  __syncwarp();
-  u32 rk[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  for (u32 c2 = 0; c2 < 256; c2++) {
-    const u32 k2 = s.skey[c2];
-#pragma unroll
-    for (int i = 0; i < 8; i++) rk[i] += (k2 > mykey[i]) ? 1u : 0u;
+    for (int i = 0; i < 8; i++) {
+      const u32 c = lane * 8 + i;
+      if (l[i]) v[i] = 0x40000000u | (l[i] << 8) | c;
+      else v[i] = (((uw >> i) & 1u) << 29) | ((255u - c) << 8) | c;
+    }
   }
 #pragma unroll
-  for (int i = 0; i < 8; i++) s.K[lane * 8 + i] = (u16)(255u - rk[i]);
+  for (u32 k = 2; k <= 256; k <<= 1) {
+#pragma unroll
+    for (u32 j = k >> 1; j > 0; j >>= 1) {
+      if (j >= 8) {  // partner in lane ^ (j / 8), same register
+        const bool lower = !(lane & (j >> 3));
+        const bool asc = !((lane * 8) & k);
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+          const u32 o = __shfl_xor_sync(FULL_MASK, v[i], j >> 3);
+          v[i] = (lower == asc) ? min(v[i], o) : max(v[i], o);
+        }
+      } else {       // partner in the same lane, register i ^ j
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+          if (i & j) continue;
+          const bool asc = !((lane * 8 + i) & k);
+          const u32 a = v[i], b = v[i | j];
+          v[i] = asc ? min(a, b) : max(a, b);
+          v[i | j] = asc ? max(a, b) : min(a, b);
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 8; i++) s.K[v[i] & 255u] = (u16)(lane * 8 + i);
   // all 256 start keys 0..255 are alive: buckets 0 and 1 full, the rest empty
   for (u32 i = lane; i < MB_BUCKETS * 4; i += 32) (&s.bm[0][0])[i] = (i < 8) ? 0xffffffffu : 0u;
   __syncwarp();
   const u8* src = U + ((size_t)seg << SEG_SHIFT) + start;
   u8* dst = R + ((size_t)seg << SEG_SHIFT) + start;
-  const u32 H = 0x80008000u, ONE = 0x00010001u;
   // zero-run summary of the chunk (warp-uniform state + a per-lane count of emitted symbols)
   u32 z_open = 0, z_lead = 0, z_acc = 0;
   bool z_seen = false;
   for (u32 base = 0; base < count; base += 32) {
     const bool valid = base + lane < count;
     const u32 c = valid ? (u32)src[base + lane] : (256u + lane);
-    // ---- bucket suffix sums of the keys alive before this window ----
-    if (lane < MB_BUCKETS) {
-      // handled below with a full-warp reverse scan (MB_BUCKETS > 32 -> two steps)
-    }
+    // ---- bucket suffix sums of the keys alive before this window: lane l holds buckets 2l and 2l+1 ----
+    u32 spair;  // (S[2l] << 16) | S[2l+1], S[b] = number of live keys in buckets above b
     {
-      u32 c0 = __popc(s.bm[lane][0]) + __popc(s.bm[lane][1]) + __popc(s.bm[lane][2]) + __popc(s.bm[lane][3]);
-      u32 c1 = 0;
-      if (lane < MB_BUCKETS - 32) c1 = __popc(s.bm[32 + lane][0]) + __popc(s.bm[32 + lane][1]) + __popc(s.bm[32 + lane][2]) + __popc(s.bm[32 + lane][3]);
-      // inclusive suffix sums over lanes (high lanes first)
-      u32 hi = c1;
+      u32 ca = 0, cb = 0;
+      if (lane < MB_BUCKETS / 2) {
+        const uint4 a = bm4[2 * lane], b = bm4[2 * lane + 1];
+        ca = __popc(a.x) + __popc(a.y) + __popc(a.z) + __popc(a.w);
+        cb = __popc(b.x) + __popc(b.y) + __popc(b.z) + __popc(b.w);
+      }
+      u32 x = ca + cb;  // inclusive suffix sum over lanes (high lanes first)
 #pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const u32 t = __shfl_down_sync(FULL_MASK, hi, o); if (lane + o < 32) hi += t; }
-      const u32 tot_hi = __shfl_sync(FULL_MASK, hi, 0);
-      u32 lo = c0;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const u32 t = __shfl_down_sync(FULL_MASK, lo, o); if (lane + o < 32) lo += t; }
-      s.S[lane] = lo - c0 + tot_hi;
-      if (lane < MB_BUCKETS - 32) s.S[32 + lane] = hi - c1;
+      for (int o = 1; o < MB_BUCKETS / 2; o <<= 1) { const u32 t = __shfl_down_sync(FULL_MASK, x, o); if (lane + o < 32) x += t; }
+      spair = ((x - ca) << 16) | (x - ca - cb);
     }
     // ---- who used my byte last? ----
     const u32 m = __match_any_sync(FULL_MASK, c);
@@ -172,41 +212,34 @@ k_mtf_ranks(const u8* __restrict__ U, const u32* __restrict__ seg_n, u32 cps, co
     const bool is_last = (m >> lane) <= 1u;  // no higher lane holds the same byte
     const u32 tb = 256u + base;
     const u32 q = valid ? (u32)s.K[c] : 0u;
-    const u32 Pi = prev >= 0 ? (tb + (u32)prev) : q;
-    // publish P (two lanes per word)
-    {
-      const u32 other = __shfl_down_sync(FULL_MASK, Pi, 1);
-      if (!(lane & 1)) s.Pw[lane >> 1] = Pi | (other << 16);
-    }
-    __syncwarp();
-    // ---- keys alive before the window and more recent than P_i (only when P_i is such a key) ----
-    u32 rank = 0;
-    if (prev < 0 && valid) {
-      const u32 b = q >> 7, off = q & 127u, wi = off >> 5;
-      rank = s.S[b];
-      const u32 w0 = s.bm[b][0], w1 = s.bm[b][1], w2 = s.bm[b][2], w3 = s.bm[b][3];
-      const u32 cur = wi == 0 ? w0 : (wi == 1 ? w1 : (wi == 2 ? w2 : w3));
-      rank += __popc(cur & ((0xfffffffeu) << (off & 31u)));
-      if (wi < 1) rank += __popc(w1);
-      if (wi < 2) rank += __popc(w2);
-      if (wi < 3) rank += __popc(w3);
-    }
-    // ---- first uses after P_i inside the window: k in (prev_i, i) with P_k < P_i ----
-    {
-      const u32 PiPi = ((Pi * ONE) | H) - ONE;          // (P_i | 0x8000) - 1 in both halves
-      const u32 lanes2 = ((lane * ONE) | H) - ONE;        // for k < i
-      const u32 pe = (u32)(prev + 1) * ONE;               // for k >= prev + 1
-      u32 acc = 0;
-#pragma unroll
-      for (u32 j = 0; j < 16; j++) {
-        const u32 Pk = s.Pw[j];
-        const u32 kk = (2 * j) | ((2 * j + 1) << 16);
-        const u32 z1 = PiPi - Pk;                         // bit15/31: P_k < P_i
-        const u32 z2 = lanes2 - kk;                       // k < i
-        const u32 z3 = ((kk + ONE) | H) - ONE - pe;       // k + 1 > prev + 1 - 1 ... k >= prev + 1
-        acc |= ((z1 & z2 & z3) & H) >> j;
+    const u32 b = q >> 7;
+    const u32 sb = __shfl_sync(FULL_MASK, spair, b >> 1);
+    // ---- r0: keys alive before the window and more recent than q (only for the first use of a byte) ----
+    u32 rank = 0, T = 256u + (u32)prev;
+    if (prev < 0) {
+      if (valid) {
+        const u32 off = q & 127u, wi = off >> 5;
+        const uint4 bw = bm4[b];
+        rank = (b & 1) ? (sb & 0xffffu) : (sb >> 16);
+        const u32 cur = wi == 0 ? bw.x : (wi == 1 ? bw.y : (wi == 2 ? bw.z : bw.w));
+        rank += __popc(cur & ((0xfffffffeu) << (off & 31u)));
+        if (wi < 1) rank += __popc(bw.y);
+        if (wi < 2) rank += __popc(bw.z);
+        if (wi < 3) rank += __popc(bw.w);
       }
-      rank += __popc(acc);
+      T = 255u - rank;
+    }
+    // ---- bytes first used after T_i inside the window: k in (prev_i, i) with T_k < T_i ----
+    {
+      u32 lt = 0, eq = FULL_MASK;
+#pragma unroll
+      for (int bit = 8; bit >= 0; bit--) {
+        const bool one = (T >> bit) & 1u;
+        const u32 B = __ballot_sync(FULL_MASK, one);
+        if (one) { lt |= eq & ~B; eq &= B; }
+        else eq &= ~B;
+      }
+      rank += __popc(lt & lanemask_lt() & (FULL_MASK << (u32)(prev + 1)));
     }
     if (valid) dst[base + lane] = (u8)rank;
     {
@@ -234,8 +267,8 @@ k_mtf_ranks(const u8* __restrict__ U, const u32* __restrict__ seg_n, u32 cps, co
       s.K[c] = (u16)(tb + lane);
     }
     const u32 newbits = __ballot_sync(FULL_MASK, valid && is_last);
-    __syncwarp();
-    if (lane == 0) s.bm[tb >> 7][(tb & 127u) >> 5] = newbits;  // windows are 32-aligned: this word is ours alone
+    // windows are 32-aligned and every old key is below tb: this word is ours alone
+    if (lane == 0) s.bm[tb >> 7][(tb & 127u) >> 5] = newbits;
     __syncwarp();
   }
   {
@@ -413,7 +446,7 @@ void mtf_rle2_batch(Ctx& c, const u8* d_T, const u8* d_U, const u32* d_n, const 
   DBuf<u8> R(c, (size_t)nblk << SEG_SHIFT);
   DBuf<uint4> rsum(c, (size_t)nblk * cps);
   DBuf<uint2> plan(c, (size_t)nblk * cps);
-  k_mtf_lastpos<<<cps * nblk, 256, 0, c.stream>>>(d_U, d_n, cps, lastpos);
+  k_mtf_lastpos<<<(cps * nblk + LP_WARPS - 1) / LP_WARPS, LP_WARPS * 32, 0, c.stream>>>(d_U, d_n, cps, cps * nblk, lastpos);
   KLAUNCH(c); KCHECK();
   k_mtf_prefix<<<nblk, 256, 0, c.stream>>>(d_n, cps, lastpos);
   KLAUNCH(c); KCHECK();
