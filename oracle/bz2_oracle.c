@@ -714,7 +714,9 @@ static int get_next_block(bunzip_t* bz) {
   if (groupCount < MIN_GROUPS || groupCount > MAX_GROUPS) THROW(ORC_DATA_ERROR, "Data error");
   int nSelectors = (int)br_bits(reader, 15);
   if (nSelectors == 0) THROW(ORC_DATA_ERROR, "Data error");
+  /* Util.makeU8Buffer(256) is zero-filled: a selector MTF index j == groupCount is legal and reads slot groupCount as 0 */
   uint8_t mtfSymbol[256];
+  memset(mtfSymbol, 0, sizeof mtfSymbol);
   for (int i = 0; i < groupCount; i++) mtfSymbol[i] = (uint8_t)i;
   uint8_t* selectors = (uint8_t*)malloc((size_t)nSelectors);
   for (int i = 0; i < nSelectors; i++) {
