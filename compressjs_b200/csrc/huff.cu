@@ -6,10 +6,19 @@
 // lib/HuffmanAllocator.js (huffalloc.cuh).
 //
 // One CTA owns one bzip2 block for the whole search (the refinement rounds are sequential
-// inside a block); hundreds of blocks are in flight.  Inside the CTA:
-//   * a 50-symbol group is costed under all tables at once: the <=6 code lengths of a symbol
-//     are packed 10 bits apart into one 64-bit word, so one shared-memory add per symbol
-//     accumulates every table's cost (staged through shared memory, conflict-free stride 25)
+// inside a block); hundreds of blocks are in flight, two CTAs per SM, so the serial phases of one
+// block (table builds, scans) hide behind the symbol passes of others.  Inside the CTA:
+//   * the search makes 9 passes over the block's symbols (4 rounds of assign + recount, one final
+//     assign), and a batch's symbols are far larger than L2, so every pass streams from HBM.  A
+//     prologue narrows the u16 symbols once to a byte per symbol plus a 50-bit mask per group of the
+//     symbols >= 256, in a scratch buffer; the passes stream that copy (1 byte per symbol, + 8 bytes
+//     per group in the rare blocks that have a symbol >= 256), staged through shared memory a tile
+//     of 256 groups at a time.  Counting the symbols during the assign pass and re-reading only the
+//     groups the split moved measured slower (scattered per-thread loads), so recount stays a pass
+//   * a 50-symbol group is costed under all tables at once: the <=6 code lengths of a symbol are
+//     packed 5 bits apart into one 32-bit word, stored 16 times ([sym][lane & 15]: at most a 2-way
+//     bank conflict per lookup); even and odd fields go to two accumulators whose fields are 10 bits
+//     apart (a group costs at most 50 x 20 < 1024 bits)
 //   * the stable median split needs no sort: histogram of costs -> threshold cost, then an
 //     ordered prefix count among the groups that sit exactly on the threshold
 //   * tables are rebuilt with a rank-by-counting sort of (freq<<9|sym) and one thread per table
@@ -19,13 +28,18 @@
 
 #define HF_THREADS 256
 #define HF_TILE_GROUPS 256
-#define HF_TILE_WORDS (HF_TILE_GROUPS * 25)
+#define HF_TILE_BYTES (HF_TILE_GROUPS * HUFF_GROUP)
+#define HF_TILE_VEC (HF_TILE_BYTES / 16)               // 16-byte pieces of a tile
+#define HF_TILE_REGS ((HF_TILE_VEC + HF_THREADS - 1) / HF_THREADS)
+#define HF_COPIES 16                                   // copies of the lookup table (32 would not leave room for 2 CTAs per SM)
+#define HF_EVEN 0x01F07C1Fu                            // the 5-bit fields of tables 0, 2, 4 (bits 0, 10, 20)
+#define HF_NAR_STRIDE ((size_t)SEL_STRIDE * HUFF_GROUP)  // bytes of a block's narrowed symbols
 
 struct HuffSmem {
-  u32 tile[HF_TILE_WORDS];             // staged symbols: 256 groups x 25 words
+  u8 tile[HF_TILE_BYTES + 16];         // staged low bytes of 256 groups (+ slack for the 14th word of the last group)
   u16 cost[SEL_STRIDE];                // best cost per group
   u8 sel[SEL_STRIDE];                  // selector per group
-  unsigned long long pk[HUFF_MAXSYM + 2];  // packed code lengths (10 bits per table)
+  u32 tbl[HUFF_MAXSYM][HF_COPIES];     // packed code lengths (5 bits per table), one copy per lane & 15
   u32 freq[HUFF_MAXGROUPS][HUFF_MAXSYM + 2];
   int work[HUFF_MAXGROUPS][HUFF_MAXSYM + 2];   // allocator arrays (sorted frequencies -> lengths)
   u32 skey[HUFF_MAXGROUPS][HUFF_MAXSYM + 2];   // sort keys (freq << 9 | sym)
@@ -62,62 +76,93 @@ __device__ void build_tables(HuffSmem& s, u32 ntab, u32 A) {
     s.len[t][s.order[t][r]] = (u8)s.work[t][r];
   }
   __syncthreads();
-  for (u32 sym = tid; sym < A; sym += HF_THREADS) {
-    unsigned long long p = 0;
-    for (u32 t = 0; t < ntab; t++) p |= (unsigned long long)s.len[t][sym] << (10 * t);
-    s.pk[sym] = p;
+  for (u32 i = tid; i < A * HF_COPIES; i += HF_THREADS) {
+    const u32 sym = i / HF_COPIES;
+    u32 p = 0;
+    for (u32 t = 0; t < ntab; t++) p |= (u32)s.len[t][sym] << (5 * t);
+    s.tbl[sym][i % HF_COPIES] = p;
   }
   __syncthreads();
 }
 
-// lib/Bzip2.js:671-684: every group goes to the table that codes it in the fewest bits
-// (ties -> lowest table index).  Fills s.sel / s.cost.
-// Tiles of 256 groups (6400 words) are staged through shared memory; the next tile's global loads are
-// issued into registers before the current tile is consumed, so the L2/HBM latency overlaps the math.
-struct TileRegs { u32 r[HF_TILE_WORDS / HF_THREADS]; };
-__device__ __forceinline__ void tile_fetch(TileRegs& t, const u32* __restrict__ symw, u32 w0, u32 nwords) {
+// The narrowed symbols are written by this kernel, so they are read through L2 (ld.global.cg), never
+// through the read-only path.  Tiles of 256 groups are staged through shared memory; the next tile's
+// loads (and each thread's own group mask) are issued into registers before the current tile is
+// consumed, so the L2/HBM latency overlaps the math.
+struct TileRegs {
+  uint4 r[HF_TILE_REGS];
+  unsigned long long hm;  // bit j: symbol j of the thread's group is >= 256
+};
+__device__ __forceinline__ void tile_fetch(TileRegs& t, const u8* nar, const unsigned long long* hmask, u32 g0, u32 nsel, bool any_hi) {
+  const uint4* src = reinterpret_cast<const uint4*>(nar + (size_t)g0 * HUFF_GROUP);
 #pragma unroll
-  for (int k = 0; k < HF_TILE_WORDS / HF_THREADS; k++) {
-    const u32 i = w0 + k * HF_THREADS + threadIdx.x;
-    t.r[k] = i < nwords ? symw[i] : 0u;
+  for (int k = 0; k < HF_TILE_REGS; k++) {
+    const u32 i = k * HF_THREADS + threadIdx.x;
+    if (i < HF_TILE_VEC) t.r[k] = __ldcg(src + i);
+  }
+  t.hm = any_hi && g0 + threadIdx.x < nsel ? __ldcg(hmask + g0 + threadIdx.x) : 0ull;
+}
+__device__ __forceinline__ void tile_store(const TileRegs& t, u8* tile) {
+#pragma unroll
+  for (int k = 0; k < HF_TILE_REGS; k++) {
+    const u32 i = k * HF_THREADS + threadIdx.x;
+    if (i < HF_TILE_VEC) reinterpret_cast<uint4*>(tile)[i] = t.r[k];
   }
 }
-__device__ __forceinline__ void tile_store(const TileRegs& t, u32* tile) {
+
+// Calls f(sym) for the cnt symbols of the thread's group in the tile (bytes 50*tid ..).  Full groups
+// without a symbol >= 256 (all but a few) read 13 words; odd-numbered groups start 2 bytes into a
+// word and are realigned by a funnel shift.
+template <class F>
+__device__ __forceinline__ void for_group(const u8* tile, u32 cnt, unsigned long long hm, F f) {
+  const u32 base = threadIdx.x * HUFF_GROUP;
+  if (cnt == HUFF_GROUP && hm == 0) {
+    const u32* wp = reinterpret_cast<const u32*>(tile + (base & ~3u));
+    const u32 sh = (base & 2u) * 8u;
+    u32 nxt = wp[0];
 #pragma unroll
-  for (int k = 0; k < HF_TILE_WORDS / HF_THREADS; k++) tile[k * HF_THREADS + threadIdx.x] = t.r[k];
+    for (u32 k = 0; k < 13; k++) {
+      const u32 cur = nxt;
+      nxt = wp[k + 1];
+      const u32 w = __funnelshift_r(cur, nxt, sh);
+      f(w & 0xffu);
+      f((w >> 8) & 0xffu);
+      if (k < 12) {
+        f((w >> 16) & 0xffu);
+        f(w >> 24);
+      }
+    }
+  } else {
+    for (u32 j = 0; j < cnt; j++) f((u32)tile[base + j] | (u32)((hm >> j) & 1u) << 8);
+  }
 }
 
-__device__ void assign_selectors(HuffSmem& s, const u32* __restrict__ symw, u32 m, u32 nsel, u32 ntab) {
-  const u32 tid = threadIdx.x;
-  const u32 nwords = (m + 1) >> 1;
+// lib/Bzip2.js:671-684: every group goes to the table that codes it in the fewest bits
+// (ties -> lowest table index).  Fills s.sel / s.cost.
+__device__ __forceinline__ void assign_selectors(HuffSmem& s, const u8* nar, const unsigned long long* hmask, u32 m, u32 nsel, u32 ntab,
+                                                 bool any_hi) {
+  const u32 tid = threadIdx.x, lane = tid % HF_COPIES;
   TileRegs tr;
-  tile_fetch(tr, symw, 0, nwords);
+  tile_fetch(tr, nar, hmask, 0, nsel, any_hi);
   for (u32 g0 = 0; g0 < nsel; g0 += HF_TILE_GROUPS) {
     tile_store(tr, s.tile);
+    const unsigned long long hm = tr.hm;
     __syncthreads();
-    if (g0 + HF_TILE_GROUPS < nsel) tile_fetch(tr, symw, (g0 + HF_TILE_GROUPS) * 25, nwords);
+    if (g0 + HF_TILE_GROUPS < nsel) tile_fetch(tr, nar, hmask, g0 + HF_TILE_GROUPS, nsel, any_hi);
     const u32 g = g0 + tid;
     if (g < nsel) {
       const u32 cnt = min(50u, m - 50u * g);
-      unsigned long long acc = 0;
-      if (cnt == 50) {
-#pragma unroll 5
-        for (u32 k = 0; k < 25; k++) {
-          const u32 w = s.tile[tid * 25 + k];
-          acc += s.pk[w & 0xffffu] + s.pk[w >> 16];
-        }
-      } else {
-        for (u32 k = 0; k < 25; k++) {
-          const u32 w = s.tile[tid * 25 + k];
-          if (2 * k < cnt) acc += s.pk[w & 0xffffu];
-          if (2 * k + 1 < cnt) acc += s.pk[w >> 16];
-        }
-      }
-      u32 best = 0, bc = (u32)(acc & 1023u);
-      for (u32 t = 1; t < ntab; t++) {
-        const u32 cst = (u32)((acc >> (10 * t)) & 1023u);
-        if (cst < bc) { best = t; bc = cst; }
-      }
+      u32 ae = 0, ao = 0;
+      for_group(s.tile, cnt, hm, [&](u32 sy) {
+        const u32 v = s.tbl[sy][lane];
+        ae += v & HF_EVEN;
+        ao += (v >> 5) & HF_EVEN;
+      });
+      const u32 c[HUFF_MAXGROUPS] = {ae & 1023u, ao & 1023u, (ae >> 10) & 1023u, (ao >> 10) & 1023u, ae >> 20, ao >> 20};
+      u32 best = 0, bc = c[0];
+#pragma unroll
+      for (u32 t = 1; t < HUFF_MAXGROUPS; t++)
+        if (t < ntab && c[t] < bc) { best = t; bc = c[t]; }
       s.sel[g] = (u8)best;
       s.cost[g] = (u16)bc;
     }
@@ -125,30 +170,63 @@ __device__ void assign_selectors(HuffSmem& s, const u32* __restrict__ symw, u32 
   }
 }
 
-__device__ void recount(HuffSmem& s, const u32* __restrict__ symw, u32 m, u32 nsel, u32 ntab, u32 A) {
+__device__ __forceinline__ void recount(HuffSmem& s, const u8* nar, const unsigned long long* hmask, u32 m, u32 nsel, u32 ntab, bool any_hi) {
   const u32 tid = threadIdx.x;
-  const u32 nwords = (m + 1) >> 1;
   for (u32 i = tid; i < ntab * (HUFF_MAXSYM + 2); i += HF_THREADS) (&s.freq[0][0])[i] = 0;
   TileRegs tr;
-  tile_fetch(tr, symw, 0, nwords);
+  tile_fetch(tr, nar, hmask, 0, nsel, any_hi);
   __syncthreads();
   for (u32 g0 = 0; g0 < nsel; g0 += HF_TILE_GROUPS) {
     tile_store(tr, s.tile);
+    const unsigned long long hm = tr.hm;
     __syncthreads();
-    if (g0 + HF_TILE_GROUPS < nsel) tile_fetch(tr, symw, (g0 + HF_TILE_GROUPS) * 25, nwords);
+    if (g0 + HF_TILE_GROUPS < nsel) tile_fetch(tr, nar, hmask, g0 + HF_TILE_GROUPS, nsel, any_hi);
     const u32 g = g0 + tid;
     if (g < nsel) {
-      const u32 cnt = min(50u, m - 50u * g);
       u32* f = s.freq[s.sel[g]];
-      for (u32 k = 0; k < 25; k++) {
-        const u32 w = s.tile[tid * 25 + k];
-        if (2 * k < cnt) atomicAdd(&f[w & 0xffffu], 1u);
-        if (2 * k + 1 < cnt) atomicAdd(&f[w >> 16], 1u);
-      }
+      for_group(s.tile, min(50u, m - 50u * g), hm, [&](u32 sy) { atomicAdd(&f[sy], 1u); });
     }
     __syncthreads();
   }
-  (void)A;
+}
+
+// The prologue: the block's u16 symbols -> one byte per symbol (nar) + per group the mask of its
+// symbols >= 256 (hmask).  16-byte loads, four in flight per thread.  Returns whether the block has a
+// symbol >= 256 at all: most blocks have none, and their passes skip the masks.
+__device__ __forceinline__ bool narrow_symbols(HuffSmem& s, const u16* __restrict__ symb, u32 m, u32 nsel, u8* nar, unsigned long long* hmask) {
+  const u32 tid = threadIdx.x;
+  if (tid == 0) s.misc[7] = 0;
+  for (u32 g = tid; g < nsel; g += HF_THREADS) hmask[g] = 0;
+  __syncthreads();
+  const uint4* src = reinterpret_cast<const uint4*>(symb);
+  const u32 nv = (m + 7) >> 3;  // the tail reads past m inside the block's segment
+  for (u32 i0 = 0; i0 < nv; i0 += 4 * HF_THREADS) {
+    uint4 v[4];
+#pragma unroll
+    for (u32 q = 0; q < 4; q++) {
+      const u32 i = i0 + q * HF_THREADS + tid;
+      if (i < nv) v[q] = __ldg(src + i);
+    }
+#pragma unroll
+    for (u32 q = 0; q < 4; q++) {
+      const u32 i = i0 + q * HF_THREADS + tid;
+      if (i >= nv) continue;
+      reinterpret_cast<uint2*>(nar)[i] = make_uint2(__byte_perm(v[q].x, v[q].y, 0x6420), __byte_perm(v[q].z, v[q].w, 0x6420));
+      if ((v[q].x | v[q].y | v[q].z | v[q].w) & 0xff00ff00u) {
+        const u32 hw[4] = {v[q].x, v[q].y, v[q].z, v[q].w};
+#pragma unroll
+        for (u32 j = 0; j < 8; j++) {
+          const u32 p = 8 * i + j;
+          if (p < m && ((hw[j >> 1] >> (16 * (j & 1) + 8)) & 0xffu)) {
+            atomicOr(&hmask[p / HUFF_GROUP], 1ull << (p % HUFF_GROUP));
+            s.misc[7] = 1;
+          }
+        }
+      }
+    }
+  }
+  __syncthreads();  // the CTA's global writes are visible to all its threads
+  return s.misc[7] != 0;
 }
 
 // ---- move-to-front over <= 6 table ids, list packed as six nibbles -------------------------------
@@ -206,9 +284,9 @@ __device__ __forceinline__ u32 rec_full(u32 R) {  // R ++ (identity minus R): th
   return lst;
 }
 
-__global__ void __launch_bounds__(HF_THREADS)
+__global__ void __launch_bounds__(HF_THREADS, 2)
 k_huffman(const u16* __restrict__ sym, const u32* __restrict__ m_arr, const u32* __restrict__ freq0, const u32* __restrict__ used,
-          u8* __restrict__ sel_out, u8* __restrict__ selmtf_out, HuffBlk* __restrict__ hb_out) {
+          u8* __restrict__ sel_out, u8* __restrict__ selmtf_out, HuffBlk* __restrict__ hb_out, u8* nar_all, unsigned long long* hmask_all) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   HuffSmem& s = *reinterpret_cast<HuffSmem*>(smem_raw);
   const u32 tid = threadIdx.x;
@@ -223,16 +301,17 @@ k_huffman(const u16* __restrict__ sym, const u32* __restrict__ m_arr, const u32*
   for (int k = 0; k < 8; k++) alpha += __popc(used[blk * 8 + k]);
   const u32 A = alpha + 2;                    // RUNA, RUNB, alpha-1 MTF positions, EOB
   const u32 nsel = (m + HUFF_GROUP - 1) / HUFF_GROUP;
-  const u32* symw = reinterpret_cast<const u32*>(sym + ((size_t)blk << SEG_SHIFT));
+  u8* nar = nar_all + (size_t)blk * HF_NAR_STRIDE;
+  unsigned long long* hmask = hmask_all + (size_t)blk * SEL_STRIDE;
   u32 target;                                 // lib/Bzip2.js:826-830
   if (m >= 2400) target = 6; else if (m >= 1200) target = 5; else if (m >= 600) target = 4; else if (m >= 200) target = 3; else target = 2;
   // seed tables: global frequencies, flat frequencies (lib/Bzip2.js:835-837)
   for (u32 i = tid; i < A; i += HF_THREADS) { s.freq[0][i] = freq0[(size_t)blk * HUFF_MAXSYM + i]; s.freq[1][i] = 1; }
-  __syncthreads();
+  const bool any_hi = narrow_symbols(s, sym + ((size_t)blk << SEG_SHIFT), m, nsel, nar, hmask);
   u32 ng = 2;
   build_tables(s, ng, A);
   while (ng < target) {
-    assign_selectors(s, symw, m, nsel, ng);
+    assign_selectors(s, nar, hmask, m, nsel, ng, any_hi);
     // which table is used most? (first maximum, lib/Bzip2.js:699)
     if (tid < HUFF_MAXGROUPS) s.gcount[tid] = 0;
     for (u32 i = tid; i < 1024; i += HF_THREADS) s.chist[i] = 0;
@@ -291,10 +370,10 @@ k_huffman(const u16* __restrict__ sym, const u32* __restrict__ m_arr, const u32*
     }
     __syncthreads();
     ng++;
-    recount(s, symw, m, nsel, ng, A);
+    recount(s, nar, hmask, m, nsel, ng, any_hi);
     build_tables(s, ng, A);
   }
-  assign_selectors(s, symw, m, nsel, ng);  // lib/Bzip2.js:843
+  assign_selectors(s, nar, hmask, m, nsel, ng, any_hi);  // lib/Bzip2.js:843
   // ---- results + bit accounting ----
   // sum of the code bits
   unsigned long long bits = 0;
@@ -382,6 +461,8 @@ void huffman_batch(Ctx& c, const u16* d_sym, const u32* d_m, const u32* d_freq, 
     CUDA_CHECK(cudaFuncSetAttribute(k_huffman, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HuffSmem)));
     attr = true;
   }
-  k_huffman<<<nblk, HF_THREADS, sizeof(HuffSmem), c.stream>>>(d_sym, d_m, d_freq, d_used, d_sel, d_selmtf, d_hb);
+  DBuf<u8> nar(c, nblk * HF_NAR_STRIDE);
+  DBuf<unsigned long long> hmask(c, (size_t)nblk * SEL_STRIDE);
+  k_huffman<<<nblk, HF_THREADS, sizeof(HuffSmem), c.stream>>>(d_sym, d_m, d_freq, d_used, d_sel, d_selmtf, d_hb, nar, hmask);
   KLAUNCH(c); KCHECK();
 }
