@@ -33,6 +33,32 @@ __global__ void k_bwtc_start(BwtcState* st, u8* out, u64 cap, u32 finalByte, u32
   st->overflow = 0;
 }
 
+// The zero-run coder writes its symbols in one byte each (NarrowSyms, enc.h); the models read u16 symbols.  One thread
+// widens 16 symbols of a block; the masks of the symbols >= 256 are only read in the blocks that have one.
+#define WD_THREADS 256
+__global__ void __launch_bounds__(WD_THREADS)
+k_bwtc_widen(const u8* __restrict__ lo, const unsigned long long* __restrict__ hi, const u32* __restrict__ any_hi, const u32* __restrict__ d_m,
+             u32 tps, u16* __restrict__ sym) {
+  const u32 b = blockIdx.x / tps;
+  const u32 p0 = ((blockIdx.x % tps) * WD_THREADS + threadIdx.x) * 16;
+  const u32 m = d_m[b];
+  if (p0 >= m) return;
+  const uint4 x = *reinterpret_cast<const uint4*>(lo + ((size_t)b << SEG_SHIFT) + p0);  // inside the 1 MiB slot
+  u32 w[8] = {__byte_perm(x.x, 0, 0x4140), __byte_perm(x.x, 0, 0x4342), __byte_perm(x.y, 0, 0x4140), __byte_perm(x.y, 0, 0x4342),
+              __byte_perm(x.z, 0, 0x4140), __byte_perm(x.z, 0, 0x4342), __byte_perm(x.w, 0, 0x4140), __byte_perm(x.w, 0, 0x4342)};
+  if (any_hi[b]) {
+    const unsigned long long* h = hi + (size_t)b * SEL_STRIDE;
+#pragma unroll
+    for (u32 j = 0; j < 16; j++) {
+      const u32 p = p0 + j;
+      if (p < m && ((h[p / HUFF_GROUP] >> (p % HUFF_GROUP)) & 1u)) w[j >> 1] |= 0x100u << (16 * (j & 1));
+    }
+  }
+  uint4* dst = reinterpret_cast<uint4*>(sym + ((size_t)b << SEG_SHIFT) + p0);   // symbols past m are never read
+  dst[0] = make_uint4(w[0], w[1], w[2], w[3]);
+  dst[1] = make_uint4(w[4], w[5], w[6], w[7]);
+}
+
 // one thread per block (lane 0 of its warp): header + model -> triples
 __global__ void __launch_bounds__(32)
 k_bwtc_model(const u16* __restrict__ sym, const u32* __restrict__ d_m, const u32* __restrict__ d_n, const u32* __restrict__ d_pidx1,
@@ -225,6 +251,12 @@ void bwtc_compress_device(Ctx& c, const u8* d_in, size_t n, int level, u8* d_out
     const u32 B = (u32)std::min<size_t>(c.bwt_batch, nblocks);
     const u32 tcap = 2 * (blockSize + 1) + 1024;              // every symbol can cost an escape and a literal
     DBuf<u8> T(c, (size_t)B << SEG_SHIFT), U(c, (size_t)B << SEG_SHIFT);
+    DBuf<u8> sym_lo(c, (size_t)B << SEG_SHIFT);
+    DBuf<unsigned long long> sym_hi(c, (size_t)B * SEL_STRIDE);
+    DBuf<u32> sym_any_hi(c, B);
+    const NarrowSyms nsym{sym_lo, sym_hi, sym_any_hi};
+    CUDA_CHECK(cudaMemsetAsync(sym_hi, 0, (size_t)B * SEL_STRIDE * 8, c.stream));
+    CUDA_CHECK(cudaMemsetAsync(sym_any_hi, 0, (size_t)B * 4, c.stream));
     DBuf<u16> sym(c, (size_t)B << SEG_SHIFT);
     DBuf<u32> dn(c, B), dpidx(c, B), dm(c, B), dfreq(c, (size_t)B * HUFF_MAXSYM), dused(c, (size_t)B * 8), tcount(c, B);
     DBuf<u64> triples(c, (size_t)B * tcap);
@@ -245,7 +277,12 @@ void bwtc_compress_device(Ctx& c, const u8* d_in, size_t n, int level, u8* d_out
       }
       {
         StageScope s(c, ST_MTF);
-        mtf_rle2_batch(c, T, U, dn, hn.data(), nb, sym, dm, dfreq, dused);
+        mtf_rle2_batch(c, T, U, dn, hn.data(), nb, nsym, dm, dfreq, dused);
+        u32 mmax = 0;   // m <= n + 1
+        for (u32 b = 0; b < nb; b++) mmax = std::max(mmax, hn[b] + 1);
+        const u32 tps = (mmax + WD_THREADS * 16 - 1) / (WD_THREADS * 16);
+        k_bwtc_widen<<<nb * tps, WD_THREADS, 0, c.stream>>>(sym_lo, sym_hi, sym_any_hi, dm, tps, sym);
+        KLAUNCH(c); KCHECK();
       }
       {
         StageScope s(c, ST_HUFF);   // statistics: the model takes the slot of the Huffman stage (ms_huff) ...

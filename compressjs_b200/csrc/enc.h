@@ -36,26 +36,40 @@ void rle1_plan_ex(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan, l
 // d_n receives their lengths, d_crc their CRCs.
 void rle1_materialize(Ctx& c, const u8* d_in, size_t n, const Rle1Plan& plan, size_t first, size_t count, u8* d_T, u32* d_n, u32* d_crc);
 
-// MTF + RLE2 (lib/Bzip2.js:743-815): U (slot layout) -> symbols u16 (slot layout), m, freq, used map
-void mtf_rle2_batch(Ctx& c, const u8* d_T, const u8* d_U, const u32* d_n, const u32* h_n, u32 nblk, u16* d_sym, u32* d_m, u32* d_freq /*[nblk][258]*/,
-                    u32* d_used /*[nblk][8]*/, const u32* d_bytehist = nullptr /*[nblk][256] byte histograms of the blocks, if known*/);
-
 #define HUFF_MAXSYM 258
 #define HUFF_MAXGROUPS 6
 #define HUFF_GROUP 50
+#define SEL_STRIDE 18432  // per-block stride of the per-group arrays (>= 900001 / 50 + 1)
+
+// The zero-run coder's symbols (0..257) in one byte each.  Only symbol 256 (MTF rank 255) and 257 (the end of
+// block in a block that uses 255 or 256 byte values) do not fit; they are rare and go to a bit mask per group.
+// `hi` and `any_hi` are zeroed once when they are allocated; every batch then clears the masks of the slots whose
+// flag the batch before set (no other slot has a mask bit), so ASCII and text batches clear nothing.
+struct NarrowSyms {
+  u8* lo;                      // [nblk << SEG_SHIFT] low byte of every symbol (slot layout)
+  unsigned long long* hi;      // [nblk][SEL_STRIDE] bit j of word g: symbol 50 g + j is >= 256
+  u32* any_hi;                 // [nblk] the block has a symbol >= 256 (most have none, and skip the masks)
+};
+
+// MTF + RLE2 (lib/Bzip2.js:743-815): U (slot layout) -> symbols (slot layout), m, freq, used map
+void mtf_rle2_batch(Ctx& c, const u8* d_T, const u8* d_U, const u32* d_n, const u32* h_n, u32 nblk, const NarrowSyms& sym, u32* d_m,
+                    u32* d_freq /*[nblk][258]*/, u32* d_used /*[nblk][8]*/,
+                    const u32* d_bytehist = nullptr /*[nblk][256] byte histograms of the blocks, if known*/);
+
 // per-block result of the Huffman stage
 struct HuffBlk {
   u32 ngroups, nsel, alpha, m;
   u64 body_bits;  // bits of the block from the 48-bit magic through the last Huffman code
   u8 len[HUFF_MAXGROUPS][HUFF_MAXSYM + 6];
 };
-// Table optimisation (lib/Bzip2.js:671-733, 826-843 + HuffmanAllocator.js): selectors u8 (slot layout >> 0, stride SEL_STRIDE)
-#define SEL_STRIDE 18432
-void huffman_batch(Ctx& c, const u16* d_sym, const u32* d_m, const u32* d_freq, const u32* d_used, u32 nblk, u8* d_sel, u8* d_selmtf,
-                   HuffBlk* d_hb);
+// Table optimisation (lib/Bzip2.js:671-733, 826-843 + HuffmanAllocator.js): selectors u8 (stride SEL_STRIDE), and
+// d_goff[blk * SEL_STRIDE + g] = bit offset of group g's codes inside the block's code section (g <= nsel: the last
+// entry is the length of the section)
+void huffman_batch(Ctx& c, const NarrowSyms& sym, const u32* d_m, const u32* d_freq, const u32* d_used, u32 nblk, u8* d_sel, u8* d_selmtf,
+                   HuffBlk* d_hb, u32* d_goff);
 // bit packing of blocks at their final bit offsets (lib/Bzip2.js:740-741,749-758,847-874)
-void pack_batch(Ctx& c, const u16* d_sym, const u8* d_sel, const u8* d_selmtf, const HuffBlk* d_hb, const u32* d_used, const u32* d_pidx,
-                const u32* d_crc, const u64* d_bitoff, const u32* d_flag, u32 nblk, u32 max_m, u32* d_out_words);
+void pack_batch(Ctx& c, const NarrowSyms& sym, const u8* d_sel, const u8* d_selmtf, const HuffBlk* d_hb, const u32* d_goff, const u32* d_used,
+                const u32* d_pidx, const u32* d_crc, const u64* d_bitoff, const u32* d_flag, u32 nblk, u32 max_m, u32* d_out_words);
 
 #include <vector>
 void crc_ranges(Ctx& c, const u8* d_data, const BlkInfo* d_ranges, const std::vector<BlkInfo>& h_ranges, u32* d_crc_out);

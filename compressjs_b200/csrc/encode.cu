@@ -7,12 +7,12 @@
 // The reference pushes one bit at a time through a BitStream.  Here every block's total bit
 // length is known after the Huffman stage, so an exclusive scan gives each block its final bit
 // offset in the file and all blocks are packed in place concurrently:
-//   k_offsets     : running bit cursor + stream CRC fold (rotl1 ^ crc, lib/Bzip2.js:917)
+//   k_offsets     : one warp: running bit cursor (scan) + stream CRC fold (rotl1 ^ crc, lib/Bzip2.js:917)
 //   k_pack_header : per block: magic, CRC, pidx, symbol map, selectors (unary of the MTF'd table
 //                   ids, offsets by prefix sum), code-length tables (delta coded)
-//   k_pack_codes  : per 256 groups: per-group bit counts -> chained scan -> each thread encodes
-//                   its 50 symbols into a shared-memory staging tile that is aligned to the
-//                   global 32-bit word grid, then the tile is written out coalesced
+//   k_pack_codes  : per 128 groups: every group's bit offset comes from the Huffman stage, so each
+//                   thread encodes its 50 symbols straight into a shared-memory staging tile that is
+//                   aligned to the global 32-bit word grid, then the tile is written out coalesced
 //                   (only the two boundary words need atomics)
 #include <algorithm>
 #include <chrono>
@@ -65,20 +65,29 @@ struct BitAcc {
 };
 
 // ---- offsets ---------------------------------------------------------------------------------
-// state[0] = bit cursor, state[1] = stream crc, state[2] = overflow flag
-__global__ void k_offsets(const HuffBlk* __restrict__ hb, const u32* __restrict__ crc, u32 nblk, u64* state, u64* __restrict__ bitoff,
-                          u64 cap_bits, u32* flag) {
-  if (threadIdx.x || blockIdx.x) return;
+// state[0] = bit cursor, state[1] = stream crc.  One warp, 32 blocks per step: the bit offsets are a scan; the CRC fold
+// s' = rotl1(s) ^ crc[k] is linear, so after all nblk blocks s = rotl_nblk(s0) ^ XOR_k rotl_(nblk-1-k)(crc[k]).
+__global__ void __launch_bounds__(32) k_offsets(const HuffBlk* __restrict__ hb, const u32* __restrict__ crc, u32 nblk, u64* state,
+                                                u64* __restrict__ bitoff, u64 cap_bits, u32* flag) {
+  const u32 lane = threadIdx.x;
   u64 cur = state[0];
-  u32 scrc = (u32)state[1];
-  for (u32 k = 0; k < nblk; k++) {
-    bitoff[k] = cur;
-    cur += hb[k].body_bits;
-    scrc = ((scrc << 1) | (scrc >> 31)) ^ crc[k];
+  const u32 s0 = (u32)state[1];
+  u32 fold = 0;
+  for (u32 k0 = 0; k0 < nblk; k0 += 32) {
+    const u32 k = k0 + lane;
+    const u64 b = k < nblk ? hb[k].body_bits : 0ull;
+    if (k < nblk) fold ^= __funnelshift_l(crc[k], crc[k], (nblk - 1 - k) & 31u);
+    const u64 inc = warp_incl_add(b);
+    if (k < nblk) bitoff[k] = cur + inc - b;
+    cur += __shfl_sync(FULL_MASK, inc, 31);
   }
-  state[0] = cur;
-  state[1] = scrc;
-  if (cur + 96 + 64 > cap_bits) *flag = 1;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) fold ^= __shfl_xor_sync(FULL_MASK, fold, o);
+  if (lane == 0) {
+    state[0] = cur;
+    state[1] = __funnelshift_l(s0, s0, nblk & 31u) ^ fold;
+    if (cur + 96 + 64 > cap_bits) *flag = 1;
+  }
 }
 
 // ---- header --------------------------------------------------------------------------------
@@ -191,76 +200,94 @@ k_pack_header(const u8* __restrict__ selmtf, const HuffBlk* __restrict__ hb_arr,
 }
 
 // ---- codes ---------------------------------------------------------------------------------
-#define PC_THREADS 256
-#define PC_GROUPS 256
-#define PC_STAGE_WORDS (PC_GROUPS * 1000 / 32 + 4)
+// Accumulator of one thread's codes in the zeroed staging tile.  Every word goes in by a shared-memory atomicOr (the
+// first and last words of a thread's range are shared with its neighbours), so a put has no branch: the warp's
+// threads complete words at different symbols, and a divergent store path would run on nearly every symbol.  Bits
+// above the 32 + nb that are still pending are never read, so the accumulator is not masked.
+struct StageAcc {
+  u32* stage; u32 word, nb; unsigned long long acc;
+  __device__ __forceinline__ void init(u32* st, u32 pos) { stage = st; word = pos >> 5; nb = pos & 31; acc = 0; }
+  __device__ __forceinline__ void put(u32 cv) {  // cv = len << 24 | code
+    const u32 len = cv >> 24;
+    acc = (acc << len) | (cv & 0xffffffu);
+    nb += len;
+    if (nb >= 32) {
+      nb -= 32;
+      atomicOr(&stage[word++], bswap32((u32)(acc >> nb)));
+    }
+  }
+  __device__ __forceinline__ void flush() {
+    if (nb) atomicOr(&stage[word], bswap32((u32)acc << (32 - nb)));
+  }
+};
+
+// One thread per group, 128 groups per CTA.  The staging tile holds the worst case (every code 20 bits), so a CTA
+// needs ~29 KB of shared memory and 7 fit on an SM.
+#define PC_THREADS 128
+#define PC_GROUPS PC_THREADS
+#define PC_SYM_BYTES (PC_GROUPS * HUFF_GROUP)
+#define PC_STAGE_WORDS ((31 + PC_GROUPS * HUFF_GROUP * 20 + 31) / 32)
 
 struct PackSmem {
-  u32 tile[PC_GROUPS * 25];
+  u8 sym[PC_SYM_BYTES + 16];                  // the tile's symbols, low bytes (+ slack for a group's last word)
   u32 stage[PC_STAGE_WORDS];
   u32 code[HUFF_MAXGROUPS][HUFF_MAXSYM + 2];  // len << 24 | code
-  u32 ws[PC_THREADS / 32 + 1];
-  u32 s_tile, s_carry;
 };
 
 __global__ void __launch_bounds__(PC_THREADS)
-k_pack_codes(const u16* __restrict__ sym, const u8* __restrict__ sel, const HuffBlk* __restrict__ hb_arr, const u64* __restrict__ bitoff,
-             const u32* __restrict__ code_start, const u32* __restrict__ codes, const u32* __restrict__ flag, u32 tps, u32* ticket,
-             u64* status, u32* __restrict__ out) {
+k_pack_codes(const u8* __restrict__ sym_lo, const unsigned long long* __restrict__ sym_hi, const u32* __restrict__ any_hi,
+             const u8* __restrict__ sel, const HuffBlk* __restrict__ hb_arr, const u32* __restrict__ goff, const u64* __restrict__ bitoff,
+             const u32* __restrict__ code_start, const u32* __restrict__ codes, const u32* __restrict__ flag, u32 tps, u32* __restrict__ out) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   PackSmem& s = *reinterpret_cast<PackSmem*>(smem_raw);
   const u32 tid = threadIdx.x;
-  if (tid == 0) s.s_tile = atomicAdd(ticket, 1u);
-  __syncthreads();
-  const u32 tile = s.s_tile;
-  const u32 blk = tile / tps, lt = tile % tps;
+  const u32 blk = blockIdx.x / tps, lt = blockIdx.x % tps;
   const HuffBlk* hb = hb_arr + blk;
   const u32 nsel = hb->nsel, m = hb->m, ng = hb->ngroups, A = hb->alpha + 2;
   const u32 g0 = lt * PC_GROUPS;
   if (*flag || g0 >= nsel) return;
+  const u32 g = g0 + tid, gend = min(nsel, g0 + PC_GROUPS);
+  const u32* go = goff + (size_t)blk * SEL_STRIDE;
+  const u32 o0 = go[g0], total = go[gend] - o0;
+  const u32 my = g < nsel ? go[g] - o0 : 0u;
+  const u32 tsel = g < nsel ? sel[(size_t)blk * SEL_STRIDE + g] : 0u;
+  const unsigned long long hm = (g < nsel && any_hi[blk]) ? sym_hi[(size_t)blk * SEL_STRIDE + g] : 0ull;
+  const u64 P = bitoff[blk] + code_start[blk] + o0;  // absolute bit of this tile's first code
+  const u32 phase = (u32)(P & 31);
+  const u32 nw = (phase + total + 31) >> 5;
   for (u32 i = tid; i < ng * A; i += PC_THREADS) {
     const u32 t = i / A, sy = i % A;
     s.code[t][sy] = codes[((size_t)blk * HUFF_MAXGROUPS + t) * (HUFF_MAXSYM + 2) + sy];
   }
-  const u32* symw = reinterpret_cast<const u32*>(sym + ((size_t)blk << SEG_SHIFT));
-  const u32 nwords = (m + 1) >> 1;
-  const u32 w0 = g0 * 25;
-  for (u32 i = tid; i < PC_GROUPS * 25; i += PC_THREADS) s.tile[i] = (w0 + i < nwords) ? symw[w0 + i] : 0u;
-  for (u32 i = tid; i < PC_STAGE_WORDS; i += PC_THREADS) s.stage[i] = 0;
+  // the tile's symbols: 16-byte loads (the tile starts at byte 6400 lt of the slot); bytes past m are never coded
+  const uint4* src = reinterpret_cast<const uint4*>(sym_lo + ((size_t)blk << SEG_SHIFT) + (size_t)g0 * HUFF_GROUP);
+  for (u32 i = tid; i < PC_SYM_BYTES / 16; i += PC_THREADS) reinterpret_cast<uint4*>(s.sym)[i] = src[i];
+  for (u32 i = tid; i < nw; i += PC_THREADS) s.stage[i] = 0;
   __syncthreads();
-  const u32 g = g0 + tid;
-  u32 bits = 0, cnt = 0, tsel = 0;
   if (g < nsel) {
-    cnt = min(50u, m - 50u * g);
-    tsel = sel[(size_t)blk * SEL_STRIDE + g];
-    for (u32 k = 0; k < 25; k++) {
-      const u32 w = s.tile[tid * 25 + k];
-      if (2 * k < cnt) bits += s.code[tsel][w & 0xffffu] >> 24;
-      if (2 * k + 1 < cnt) bits += s.code[tsel][w >> 16] >> 24;
-    }
-  }
-  u32 total;
-  const u32 ex = block_excl_add<PC_THREADS, u32>(bits, s.ws, &total);
-  if (tid < 32) {
-    u32 cr = lookback_warp(status + (size_t)blk * tps, lt, total, OpAdd());
-    if (tid == 0) s.s_carry = cr;
-  }
-  __syncthreads();
-  const u64 P = bitoff[blk] + code_start[blk] + s.s_carry;  // absolute bit of this tile's first code
-  const u32 phase = (u32)(P & 31);
-  if (g < nsel) {
-    BitAcc ba;
-    ba.init(s.stage, (u64)phase + ex);
-    for (u32 k = 0; k < 25; k++) {
-      const u32 w = s.tile[tid * 25 + k];
-      if (2 * k < cnt) { const u32 cv = s.code[tsel][w & 0xffffu]; ba.put(cv >> 24, cv & 0xffffffu); }
-      if (2 * k + 1 < cnt) { const u32 cv = s.code[tsel][w >> 16]; ba.put(cv >> 24, cv & 0xffffffu); }
+    const u32* cw = s.code[tsel];
+    StageAcc ba;
+    ba.init(s.stage, phase + my);
+    const u32 cnt = min(50u, m - 50u * g), base = tid * HUFF_GROUP;
+    if (cnt == HUFF_GROUP && hm == 0) {  // all but a few groups: 13 aligned words, realigned by a funnel shift
+      const u32* wp = reinterpret_cast<const u32*>(s.sym + (base & ~3u));
+      const u32 sh = (base & 2u) * 8u;
+      u32 nxt = wp[0];
+#pragma unroll
+      for (u32 k = 0; k < 13; k++) {
+        const u32 cur = nxt;
+        nxt = wp[k + 1];
+        const u32 w = __funnelshift_r(cur, nxt, sh);
+#pragma unroll
+        for (u32 j = 0; j < (k < 12 ? 4u : 2u); j++) ba.put(cw[(w >> (8 * j)) & 0xffu]);
+      }
+    } else {
+      for (u32 j = 0; j < cnt; j++) ba.put(cw[(u32)s.sym[base + j] | (u32)((hm >> j) & 1u) << 8]);
     }
     ba.flush();
   }
   __syncthreads();
-  // stage words are already byte-swapped by BitAcc; copy out
-  const u32 nw = (phase + total + 31) >> 5;
+  // stage words are already byte-swapped; copy out
   u32* dst = out + (P >> 5);
   for (u32 i = tid; i < nw; i += PC_THREADS) {
     const u32 v = s.stage[i];
@@ -269,23 +296,20 @@ k_pack_codes(const u16* __restrict__ sym, const u8* __restrict__ sel, const Huff
   }
 }
 
-void pack_batch(Ctx& c, const u16* d_sym, const u8* d_sel, const u8* d_selmtf, const HuffBlk* d_hb, const u32* d_used, const u32* d_pidx,
-                const u32* d_crc, const u64* d_bitoff, const u32* d_flag, u32 nblk, u32 max_m, u32* d_out_words) {
+void pack_batch(Ctx& c, const NarrowSyms& sym, const u8* d_sel, const u8* d_selmtf, const HuffBlk* d_hb, const u32* d_goff, const u32* d_used,
+                const u32* d_pidx, const u32* d_crc, const u64* d_bitoff, const u32* d_flag, u32 nblk, u32 max_m, u32* d_out_words) {
   static bool attr = false;
   if (!attr) {
     CUDA_CHECK(cudaFuncSetAttribute(k_pack_codes, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PackSmem)));
     attr = true;
   }
-  DBuf<u32> code_start(c, nblk), ticket(c, 1), codes(c, (size_t)nblk * HUFF_MAXGROUPS * (HUFF_MAXSYM + 2));
+  DBuf<u32> code_start(c, nblk), codes(c, (size_t)nblk * HUFF_MAXGROUPS * (HUFF_MAXSYM + 2));
   k_pack_header<<<nblk, PH_THREADS, 0, c.stream>>>(d_selmtf, d_hb, d_used, d_pidx, d_crc, d_bitoff, d_flag, d_out_words, code_start, codes);
   KLAUNCH(c); KCHECK();
   const u32 max_sel = (max_m + HUFF_GROUP - 1) / HUFF_GROUP;
   const u32 tps = (max_sel + PC_GROUPS - 1) / PC_GROUPS;
-  DBuf<u64> status(c, (size_t)nblk * tps);
-  CUDA_CHECK(cudaMemsetAsync(status, 0, (size_t)nblk * tps * 8, c.stream));
-  CUDA_CHECK(cudaMemsetAsync(ticket, 0, 4, c.stream));
-  k_pack_codes<<<nblk * tps, PC_THREADS, sizeof(PackSmem), c.stream>>>(d_sym, d_sel, d_hb, d_bitoff, code_start, codes, d_flag, tps, ticket, status,
-                                                                      d_out_words);
+  k_pack_codes<<<nblk * tps, PC_THREADS, sizeof(PackSmem), c.stream>>>(sym.lo, sym.hi, sym.any_hi, d_sel, d_hb, d_goff, d_bitoff, code_start, codes,
+                                                                      d_flag, tps, d_out_words);
   KLAUNCH(c); KCHECK();
 }
 
@@ -319,9 +343,9 @@ struct EncSession {
   std::vector<u32> all_crc;
   std::vector<b2_block_trace> tr;
   u32 cap_blocks = 0;
-  DBuf<u8> T, U, dsel, dselmtf;
-  DBuf<u16> sym;
-  DBuf<u32> dn, dcrc, dpidx, dm, dfreq, dused, dhist;
+  DBuf<u8> T, U, dsel, dselmtf, sym_lo;
+  DBuf<unsigned long long> sym_hi;
+  DBuf<u32> dn, dcrc, dpidx, dm, dfreq, dused, dhist, sym_any_hi, dgoff;
   DBuf<HuffBlk> dhb;
   DBuf<u64> dbitoff;
   std::vector<u32> hn, hm, hp;
@@ -350,7 +374,10 @@ struct EncSession {
   void reserve(u32 nb) {
     if (nb <= cap_blocks) return;
     cap_blocks = nb;
-    T.alloc(c, (size_t)nb << SEG_SHIFT); U.alloc(c, (size_t)nb << SEG_SHIFT); sym.alloc(c, (size_t)nb << SEG_SHIFT);
+    T.alloc(c, (size_t)nb << SEG_SHIFT); U.alloc(c, (size_t)nb << SEG_SHIFT); sym_lo.alloc(c, (size_t)nb << SEG_SHIFT);
+    sym_hi.alloc(c, (size_t)nb * SEL_STRIDE); sym_any_hi.alloc(c, nb); dgoff.alloc(c, (size_t)nb * SEL_STRIDE);
+    CUDA_CHECK(cudaMemsetAsync(sym_hi, 0, (size_t)nb * SEL_STRIDE * 8, c.stream));
+    CUDA_CHECK(cudaMemsetAsync(sym_any_hi, 0, (size_t)nb * 4, c.stream));
     dn.alloc(c, nb); dcrc.alloc(c, nb); dpidx.alloc(c, nb); dm.alloc(c, nb);
     dfreq.alloc(c, (size_t)nb * HUFF_MAXSYM); dused.alloc(c, (size_t)nb * 8); dhist.alloc(c, (size_t)nb * 256);
     dsel.alloc(c, (size_t)nb * SEL_STRIDE); dselmtf.alloc(c, (size_t)nb * SEL_STRIDE);
@@ -367,6 +394,7 @@ struct EncSession {
     // all stage temporaries of one batch come to ~40 bytes per slot; size the pool for the batch class once
     const u32 half = c.bwt_batch / 2, quarter = c.bwt_batch / 4;
     if (B > quarter) c.prewarm((size_t)(B > half ? std::max<u32>(B, c.bwt_batch) : half) * 40 << SEG_SHIFT);
+    const NarrowSyms sym{sym_lo, sym_hi, sym_any_hi};
     const size_t done0 = all_crc.size();
     all_crc.resize(done0 + count);
     tr.resize(done0 + count);
@@ -389,13 +417,13 @@ struct EncSession {
       }
       {
         StageScope s(c, ST_HUFF);
-        huffman_batch(c, sym, dm, dfreq, dused, nb, dsel, dselmtf, dhb);
+        huffman_batch(c, sym, dm, dfreq, dused, nb, dsel, dselmtf, dhb, dgoff);
       }
       {
         StageScope s(c, ST_PACK);
         k_offsets<<<1, 32, 0, c.stream>>>(dhb, dcrc, nb, state, dbitoff, (u64)cap_words * 32, flag);
         KLAUNCH(c); KCHECK();
-        pack_batch(c, sym, dsel, dselmtf, dhb, dused, dpidx, dcrc, dbitoff, flag, nb, nmax + 1, reinterpret_cast<u32*>(d_out));
+        pack_batch(c, sym, dsel, dselmtf, dhb, dgoff, dused, dpidx, dcrc, dbitoff, flag, nb, nmax + 1, reinterpret_cast<u32*>(d_out));
       }
       // per-block bookkeeping for the host (trace + CRCs)
       c.to_host(hm.data(), dm, nb * 4);

@@ -9,12 +9,12 @@
 // inside a block); hundreds of blocks are in flight, two CTAs per SM, so the serial phases of one
 // block (table builds, scans) hide behind the symbol passes of others.  Inside the CTA:
 //   * the search makes 9 passes over the block's symbols (4 rounds of assign + recount, one final
-//     assign), and a batch's symbols are far larger than L2, so every pass streams from HBM.  A
-//     prologue narrows the u16 symbols once to a byte per symbol plus a 50-bit mask per group of the
-//     symbols >= 256, in a scratch buffer; the passes stream that copy (1 byte per symbol, + 8 bytes
-//     per group in the rare blocks that have a symbol >= 256), staged through shared memory a tile
-//     of 256 groups at a time.  Counting the symbols during the assign pass and re-reading only the
-//     groups the split moved measured slower (scattered per-thread loads), so recount stays a pass
+//     assign), and a batch's symbols are far larger than L2, so every pass streams from HBM.  The
+//     zero-run coder writes the symbols in one byte each plus a 50-bit mask per group of the symbols
+//     >= 256 (NarrowSyms, enc.h); the passes stream them (1 byte per symbol, + 8 bytes per group in
+//     the rare blocks that have a symbol >= 256), staged through shared memory a tile of 256 groups
+//     at a time.  Counting the symbols during the assign pass and re-reading only the groups the
+//     split moved measured slower (scattered per-thread loads), so recount stays a pass
 //   * a 50-symbol group is costed under all tables at once: the <=6 code lengths of a symbol are
 //     packed 5 bits apart into one 32-bit word, stored 16 times ([sym][lane & 15]: at most a 2-way
 //     bank conflict per lookup); even and odd fields go to two accumulators whose fields are 10 bits
@@ -23,6 +23,8 @@
 //     ordered prefix count among the groups that sit exactly on the threshold
 //   * tables are rebuilt with a rank-by-counting sort of (freq<<9|sym) and one thread per table
 //     running the exact in-place allocator
+//   * after the final assign pass the costs of the groups are still in shared memory: their scan gives
+//     every group's bit offset inside the block's code section, so the packer needs no counting pass
 #include "enc.h"
 #include "huffalloc.cuh"
 
@@ -33,7 +35,6 @@
 #define HF_TILE_REGS ((HF_TILE_VEC + HF_THREADS - 1) / HF_THREADS)
 #define HF_COPIES 16                                   // copies of the lookup table (32 would not leave room for 2 CTAs per SM)
 #define HF_EVEN 0x01F07C1Fu                            // the 5-bit fields of tables 0, 2, 4 (bits 0, 10, 20)
-#define HF_NAR_STRIDE ((size_t)SEL_STRIDE * HUFF_GROUP)  // bytes of a block's narrowed symbols
 
 struct HuffSmem {
   u8 tile[HF_TILE_BYTES + 16];         // staged low bytes of 256 groups (+ slack for the 14th word of the last group)
@@ -85,10 +86,9 @@ __device__ void build_tables(HuffSmem& s, u32 ntab, u32 A) {
   __syncthreads();
 }
 
-// The narrowed symbols are written by this kernel, so they are read through L2 (ld.global.cg), never
-// through the read-only path.  Tiles of 256 groups are staged through shared memory; the next tile's
-// loads (and each thread's own group mask) are issued into registers before the current tile is
-// consumed, so the L2/HBM latency overlaps the math.
+// Tiles of 256 groups are staged through shared memory; the next tile's loads (and each thread's own
+// group mask) are issued into registers before the current tile is consumed, so the L2/HBM latency
+// overlaps the math.  The symbols are read-only for the whole kernel.
 struct TileRegs {
   uint4 r[HF_TILE_REGS];
   unsigned long long hm;  // bit j: symbol j of the thread's group is >= 256
@@ -98,9 +98,9 @@ __device__ __forceinline__ void tile_fetch(TileRegs& t, const u8* nar, const uns
 #pragma unroll
   for (int k = 0; k < HF_TILE_REGS; k++) {
     const u32 i = k * HF_THREADS + threadIdx.x;
-    if (i < HF_TILE_VEC) t.r[k] = __ldcg(src + i);
+    if (i < HF_TILE_VEC) t.r[k] = __ldg(src + i);
   }
-  t.hm = any_hi && g0 + threadIdx.x < nsel ? __ldcg(hmask + g0 + threadIdx.x) : 0ull;
+  t.hm = any_hi && g0 + threadIdx.x < nsel ? __ldg(hmask + g0 + threadIdx.x) : 0ull;
 }
 __device__ __forceinline__ void tile_store(const TileRegs& t, u8* tile) {
 #pragma unroll
@@ -190,45 +190,6 @@ __device__ __forceinline__ void recount(HuffSmem& s, const u8* nar, const unsign
   }
 }
 
-// The prologue: the block's u16 symbols -> one byte per symbol (nar) + per group the mask of its
-// symbols >= 256 (hmask).  16-byte loads, four in flight per thread.  Returns whether the block has a
-// symbol >= 256 at all: most blocks have none, and their passes skip the masks.
-__device__ __forceinline__ bool narrow_symbols(HuffSmem& s, const u16* __restrict__ symb, u32 m, u32 nsel, u8* nar, unsigned long long* hmask) {
-  const u32 tid = threadIdx.x;
-  if (tid == 0) s.misc[7] = 0;
-  for (u32 g = tid; g < nsel; g += HF_THREADS) hmask[g] = 0;
-  __syncthreads();
-  const uint4* src = reinterpret_cast<const uint4*>(symb);
-  const u32 nv = (m + 7) >> 3;  // the tail reads past m inside the block's segment
-  for (u32 i0 = 0; i0 < nv; i0 += 4 * HF_THREADS) {
-    uint4 v[4];
-#pragma unroll
-    for (u32 q = 0; q < 4; q++) {
-      const u32 i = i0 + q * HF_THREADS + tid;
-      if (i < nv) v[q] = __ldg(src + i);
-    }
-#pragma unroll
-    for (u32 q = 0; q < 4; q++) {
-      const u32 i = i0 + q * HF_THREADS + tid;
-      if (i >= nv) continue;
-      reinterpret_cast<uint2*>(nar)[i] = make_uint2(__byte_perm(v[q].x, v[q].y, 0x6420), __byte_perm(v[q].z, v[q].w, 0x6420));
-      if ((v[q].x | v[q].y | v[q].z | v[q].w) & 0xff00ff00u) {
-        const u32 hw[4] = {v[q].x, v[q].y, v[q].z, v[q].w};
-#pragma unroll
-        for (u32 j = 0; j < 8; j++) {
-          const u32 p = 8 * i + j;
-          if (p < m && ((hw[j >> 1] >> (16 * (j & 1) + 8)) & 0xffu)) {
-            atomicOr(&hmask[p / HUFF_GROUP], 1ull << (p % HUFF_GROUP));
-            s.misc[7] = 1;
-          }
-        }
-      }
-    }
-  }
-  __syncthreads();  // the CTA's global writes are visible to all its threads
-  return s.misc[7] != 0;
-}
-
 // ---- move-to-front over <= 6 table ids, list packed as six nibbles -------------------------------
 __device__ __forceinline__ u32 mtf6_find(u32 list, u32 v) {
   u32 j = 0;
@@ -285,8 +246,9 @@ __device__ __forceinline__ u32 rec_full(u32 R) {  // R ++ (identity minus R): th
 }
 
 __global__ void __launch_bounds__(HF_THREADS, 2)
-k_huffman(const u16* __restrict__ sym, const u32* __restrict__ m_arr, const u32* __restrict__ freq0, const u32* __restrict__ used,
-          u8* __restrict__ sel_out, u8* __restrict__ selmtf_out, HuffBlk* __restrict__ hb_out, u8* nar_all, unsigned long long* hmask_all) {
+k_huffman(const u8* __restrict__ sym_lo, const unsigned long long* __restrict__ sym_hi, const u32* __restrict__ any_hi_arr,
+          const u32* __restrict__ m_arr, const u32* __restrict__ freq0, const u32* __restrict__ used, u8* __restrict__ sel_out,
+          u8* __restrict__ selmtf_out, HuffBlk* __restrict__ hb_out, u32* __restrict__ goff_out) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   HuffSmem& s = *reinterpret_cast<HuffSmem*>(smem_raw);
   const u32 tid = threadIdx.x;
@@ -301,13 +263,14 @@ k_huffman(const u16* __restrict__ sym, const u32* __restrict__ m_arr, const u32*
   for (int k = 0; k < 8; k++) alpha += __popc(used[blk * 8 + k]);
   const u32 A = alpha + 2;                    // RUNA, RUNB, alpha-1 MTF positions, EOB
   const u32 nsel = (m + HUFF_GROUP - 1) / HUFF_GROUP;
-  u8* nar = nar_all + (size_t)blk * HF_NAR_STRIDE;
-  unsigned long long* hmask = hmask_all + (size_t)blk * SEL_STRIDE;
+  const u8* nar = sym_lo + ((size_t)blk << SEG_SHIFT);
+  const unsigned long long* hmask = sym_hi + (size_t)blk * SEL_STRIDE;
+  const bool any_hi = any_hi_arr[blk] != 0;
   u32 target;                                 // lib/Bzip2.js:826-830
   if (m >= 2400) target = 6; else if (m >= 1200) target = 5; else if (m >= 600) target = 4; else if (m >= 200) target = 3; else target = 2;
   // seed tables: global frequencies, flat frequencies (lib/Bzip2.js:835-837)
   for (u32 i = tid; i < A; i += HF_THREADS) { s.freq[0][i] = freq0[(size_t)blk * HUFF_MAXSYM + i]; s.freq[1][i] = 1; }
-  const bool any_hi = narrow_symbols(s, sym + ((size_t)blk << SEG_SHIFT), m, nsel, nar, hmask);
+  __syncthreads();  // build_tables reads the seed frequencies across threads
   u32 ng = 2;
   build_tables(s, ng, A);
   while (ng < target) {
@@ -375,17 +338,34 @@ k_huffman(const u16* __restrict__ sym, const u32* __restrict__ m_arr, const u32*
   }
   assign_selectors(s, nar, hmask, m, nsel, ng, any_hi);  // lib/Bzip2.js:843
   // ---- results + bit accounting ----
-  // sum of the code bits
-  unsigned long long bits = 0;
-  for (u32 g = tid; g < nsel; g += HF_THREADS) bits += s.cost[g];
+  // bit offset of every group inside the code section: every warp scans a contiguous eighth of the groups
+  // (coalesced, lane-strided), after a block scan of the eighths' sums.  A block codes at most 900001 x 20 bits.
+  unsigned long long bits;
   {
-    // block reduce (64-bit)
-    __shared__ unsigned long long red[HF_THREADS / 32];
-    for (int o = 16; o > 0; o >>= 1) bits += __shfl_xor_sync(FULL_MASK, bits, o);
-    if ((tid & 31) == 0) red[tid >> 5] = bits;
+    const u32 w = tid >> 5, lane = tid & 31;
+    const u32 per = (nsel + HF_THREADS / 32 - 1) / (HF_THREADS / 32);
+    const u32 ga = min(nsel, w * per), gb = min(nsel, ga + per);
+    u32 part = 0;
+    for (u32 g = ga + lane; g < gb; g += 32) part += s.cost[g];
+    part = warp_reduce_add(part);
+    if (lane == 0) s.ws[w] = part;
     __syncthreads();
-    bits = 0;
-    for (int i = 0; i < HF_THREADS / 32; i++) bits += red[i];
+    u32 carry = 0, total = 0;
+    for (u32 i = 0; i < HF_THREADS / 32; i++) {
+      const u32 x = s.ws[i];
+      carry += i < w ? x : 0u;
+      total += x;
+    }
+    u32* go = goff_out + (size_t)blk * SEL_STRIDE;
+    for (u32 g0 = ga; g0 < gb; g0 += 32) {
+      const u32 g = g0 + lane;
+      const u32 c = g < gb ? (u32)s.cost[g] : 0u;
+      const u32 inc = warp_incl_add(c);
+      if (g < gb) go[g] = carry + inc - c;
+      carry += __shfl_sync(FULL_MASK, inc, 31);
+    }
+    if (tid == 0) go[nsel] = total;
+    bits = total;
     __syncthreads();
   }
   u8* so = sel_out + (size_t)blk * SEL_STRIDE;
@@ -454,15 +434,13 @@ k_huffman(const u16* __restrict__ sym, const u32* __restrict__ m_arr, const u32*
   }
 }
 
-void huffman_batch(Ctx& c, const u16* d_sym, const u32* d_m, const u32* d_freq, const u32* d_used, u32 nblk, u8* d_sel, u8* d_selmtf,
-                   HuffBlk* d_hb) {
+void huffman_batch(Ctx& c, const NarrowSyms& sym, const u32* d_m, const u32* d_freq, const u32* d_used, u32 nblk, u8* d_sel, u8* d_selmtf,
+                   HuffBlk* d_hb, u32* d_goff) {
   static bool attr = false;
   if (!attr) {
     CUDA_CHECK(cudaFuncSetAttribute(k_huffman, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HuffSmem)));
     attr = true;
   }
-  DBuf<u8> nar(c, nblk * HF_NAR_STRIDE);
-  DBuf<unsigned long long> hmask(c, (size_t)nblk * SEL_STRIDE);
-  k_huffman<<<nblk, HF_THREADS, sizeof(HuffSmem), c.stream>>>(d_sym, d_m, d_freq, d_used, d_sel, d_selmtf, d_hb, nar, hmask);
+  k_huffman<<<nblk, HF_THREADS, sizeof(HuffSmem), c.stream>>>(sym.lo, sym.hi, sym.any_hi, d_m, d_freq, d_used, d_sel, d_selmtf, d_hb, d_goff);
   KLAUNCH(c); KCHECK();
 }

@@ -18,7 +18,8 @@
 //   k_rle2_scan   : one warp per block walks the chunk summaries: output offset and carried-in run length of every chunk
 //                   (a run belongs to the chunk that holds the non-zero rank ending it); final run + EOB + m
 //   k_rle2        : zero ranks form runs -> bijective base-2 RUNA/RUNB digits (lib/Bzip2.js:783-794); every chunk knows
-//                   its offsets, so there is no chain between tiles; symbols u16 + histogram
+//                   its offsets, so there is no chain between tiles; symbols in one byte each (NarrowSyms, enc.h) +
+//                   histogram
 #include "enc.h"
 
 #define MTF_CHUNK 4096
@@ -282,7 +283,8 @@ k_mtf_ranks(const u8* __restrict__ U, const u32* __restrict__ seg_n, u32 cps, co
 // rank arrives, so the run is charged to the chunk holding that rank).  plan[chunk] = (output offset, zeros carried in).
 __global__ void __launch_bounds__(32)
 k_rle2_scan(const uint4* __restrict__ rsum, const u32* __restrict__ seg_n, u32 cps, const u32* __restrict__ used, uint2* __restrict__ plan,
-            u16* __restrict__ A, u32* __restrict__ m_out, u32* __restrict__ freq) {
+            u8* __restrict__ A, unsigned long long* __restrict__ hi, u32* __restrict__ any_hi, u32* __restrict__ m_out,
+            u32* __restrict__ freq) {
   const u32 seg = blockIdx.x, lane = threadIdx.x;
   const u32 n = seg_n[seg];
   if (n == 0) return;
@@ -308,7 +310,7 @@ k_rle2_scan(const uint4* __restrict__ rsum, const u32* __restrict__ seg_n, u32 c
     if (k < nch) plan[(size_t)seg * cps + k] = make_uint2(my_o, my_c);
   }
   if (lane == 0) {
-    u16* a = A + ((size_t)seg << SEG_SHIFT);
+    u8* a = A + ((size_t)seg << SEG_SHIFT);
     u32* fq = freq + (size_t)seg * HUFF_MAXSYM;
     u32 L = carry, f0 = 0, f1 = 0;
     while (L) {  // the run still open at the end of the block
@@ -318,12 +320,23 @@ k_rle2_scan(const uint4* __restrict__ rsum, const u32* __restrict__ seg_n, u32 c
     }
     u32 alpha = 0;
     for (int k = 0; k < 8; k++) alpha += __popc(used[seg * 8 + k]);
-    a[o] = (u16)(alpha + 1);  // end of block symbol
+    a[o] = (u8)(alpha + 1);  // end of block symbol
+    if (alpha + 1 >= 256) {
+      atomicOr(&hi[(size_t)seg * SEL_STRIDE + o / HUFF_GROUP], 1ull << (o % HUFF_GROUP));
+      any_hi[seg] = 1;
+    }
     if (f0) atomicAdd(&fq[0], f0);
     if (f1) atomicAdd(&fq[1], f1);
     atomicAdd(&fq[alpha + 1], 1u);
     m_out[seg] = o + 1;
   }
+}
+
+// The masks of the slots whose flag the previous batch set go back to zero (the masks of all other slots are zero).
+__global__ void __launch_bounds__(256) k_clear_hi(const u32* __restrict__ any_hi, unsigned long long* __restrict__ hi) {
+  if (!any_hi[blockIdx.x]) return;
+  uint4* h = reinterpret_cast<uint4*>(hi + (size_t)blockIdx.x * SEL_STRIDE);
+  for (u32 i = threadIdx.x; i < SEL_STRIDE / 2; i += 256) h[i] = make_uint4(0, 0, 0, 0);
 }
 
 // ---- RLE2 ---------------------------------------------------------------------------------
@@ -332,13 +345,13 @@ k_rle2_scan(const uint4* __restrict__ rsum, const u32* __restrict__ seg_n, u32 c
 #define R2_TILE (R2_THREADS * R2_ITEMS)   // == MTF_CHUNK: one tile per chunk summary
 
 __global__ void __launch_bounds__(R2_THREADS)
-k_rle2(const u8* __restrict__ R, const u32* __restrict__ seg_n, u32 tps, const uint2* __restrict__ plan, u16* __restrict__ A,
-       u32* __restrict__ freq) {
+k_rle2(const u8* __restrict__ R, const u32* __restrict__ seg_n, u32 tps, const uint2* __restrict__ plan, u8* __restrict__ A,
+       unsigned long long* __restrict__ hi, u32* __restrict__ any_hi, u32* __restrict__ freq) {
   __shared__ u32 hist[HUFF_MAXSYM];
   __shared__ u32 ws[R2_THREADS / 32 + 1];
-  // the tile's symbols are staged here at the alignment (mod 8 symbols = 16 bytes) they have in global memory, then
+  // the tile's symbols are staged here at the alignment (mod 16 symbols = 16 bytes) they have in global memory, then
   // copied out in 16-byte pieces: at most one symbol per rank plus the digits of the run that was carried in
-  __shared__ __align__(16) u16 stage[R2_TILE + 48];
+  __shared__ __align__(16) u8 stage[R2_TILE + 48];
   const u32 tid = threadIdx.x;
   const u32 seg = blockIdx.x / tps, lt = blockIdx.x % tps;
   const u32 n = seg_n[seg];
@@ -347,7 +360,7 @@ k_rle2(const u8* __restrict__ R, const u32* __restrict__ seg_n, u32 tps, const u
   for (u32 i = tid; i < HUFF_MAXSYM; i += R2_THREADS) hist[i] = 0;
   const uint2 pl = plan[(size_t)seg * tps + lt];
   const u8* r = R + ((size_t)seg << SEG_SHIFT);
-  u16* a = A + ((size_t)seg << SEG_SHIFT);
+  u8* a = A + ((size_t)seg << SEG_SHIFT);
   const u32 p0 = start + tid * R2_ITEMS;
   u8 v[R2_ITEMS];
   {
@@ -394,7 +407,7 @@ k_rle2(const u8* __restrict__ R, const u32* __restrict__ seg_n, u32 tps, const u
   }
   u32 tot_off;
   const u32 ex_off = block_excl_add<R2_THREADS, u32>(sum, ws, &tot_off);
-  const u32 first = pl.x & 7u;
+  const u32 first = pl.x & 15u;
   u32 o = first + ex_off;  // index into `stage`
 #pragma unroll
   for (int j = 0; j < R2_ITEMS; j++) {
@@ -407,20 +420,25 @@ k_rle2(const u8* __restrict__ R, const u32* __restrict__ seg_n, u32 tps, const u
         L >>= 1;
       }
       const u32 sy = (u32)v[j] + 1;
-      stage[o++] = (u16)sy;
+      if (sy == 256) {  // rank 255: a rare mask bit (a group can straddle two tiles, hence the atomic)
+        const u32 og = pl.x - first + o;
+        atomicOr(&hi[(size_t)seg * SEL_STRIDE + og / HUFF_GROUP], 1ull << (og % HUFF_GROUP));
+        any_hi[seg] = 1;
+      }
+      stage[o++] = (u8)sy;
       atomicAdd(&hist[sy], 1u);
     }
   }
   __syncthreads();
   {
     const u32 last = first + tot_off;
-    u16* ag = a + (pl.x - first);  // 16-byte aligned: the slot base is, and (pl.x - first) is a multiple of 8 symbols
-    for (u32 c8 = tid * 8u; c8 < last; c8 += R2_THREADS * 8u) {
-      if (c8 >= first && c8 + 8u <= last) {
-        *reinterpret_cast<uint4*>(ag + c8) = *reinterpret_cast<const uint4*>(stage + c8);
+    u8* ag = a + (pl.x - first);  // 16-byte aligned: the slot base is, and (pl.x - first) is a multiple of 16 symbols
+    for (u32 c16 = tid * 16u; c16 < last; c16 += R2_THREADS * 16u) {
+      if (c16 >= first && c16 + 16u <= last) {
+        *reinterpret_cast<uint4*>(ag + c16) = *reinterpret_cast<const uint4*>(stage + c16);
       } else {
-        const u32 e = min(c8 + 8u, last);
-        for (u32 x = max(c8, first); x < e; x++) ag[x] = stage[x];
+        const u32 e = min(c16 + 16u, last);
+        for (u32 x = max(c16, first); x < e; x++) ag[x] = stage[x];
       }
     }
   }
@@ -428,8 +446,8 @@ k_rle2(const u8* __restrict__ R, const u32* __restrict__ seg_n, u32 tps, const u
     if (hist[i]) atomicAdd(&freq[(size_t)seg * HUFF_MAXSYM + i], hist[i]);
 }
 
-void mtf_rle2_batch(Ctx& c, const u8* d_T, const u8* d_U, const u32* d_n, const u32* h_n, u32 nblk, u16* d_sym, u32* d_m, u32* d_freq,
-                    u32* d_used, const u32* d_bytehist) {
+void mtf_rle2_batch(Ctx& c, const u8* d_T, const u8* d_U, const u32* d_n, const u32* h_n, u32 nblk, const NarrowSyms& sym, u32* d_m,
+                    u32* d_freq, u32* d_used, const u32* d_bytehist) {
   (void)d_T;
   u32 n_max = 0;
   for (u32 b = 0; b < nblk; b++) n_max = h_n[b] > n_max ? h_n[b] : n_max;
@@ -438,6 +456,9 @@ void mtf_rle2_batch(Ctx& c, const u8* d_T, const u8* d_U, const u32* d_n, const 
   CUDA_CHECK(cudaMemsetAsync(d_used, 0, (size_t)nblk * 8 * 4, c.stream));
   CUDA_CHECK(cudaMemsetAsync(d_freq, 0, (size_t)nblk * HUFF_MAXSYM * 4, c.stream));
   CUDA_CHECK(cudaMemsetAsync(d_m, 0, (size_t)nblk * 4, c.stream));
+  k_clear_hi<<<nblk, 256, 0, c.stream>>>(sym.any_hi, sym.hi);
+  KLAUNCH(c); KCHECK();
+  CUDA_CHECK(cudaMemsetAsync(sym.any_hi, 0, (size_t)nblk * 4, c.stream));
   if (d_bytehist) k_used_from_hist<<<nblk, 256, 0, c.stream>>>(d_bytehist, d_used);  // the BWT column is a permutation of the block
   else k_used<<<utiles * nblk, 256, 0, c.stream>>>(d_U, d_n, utiles, d_used);
   KLAUNCH(c); KCHECK();
@@ -455,9 +476,9 @@ void mtf_rle2_batch(Ctx& c, const u8* d_T, const u8* d_U, const u32* d_n, const 
     k_mtf_ranks<<<(chunks + MR_WARPS - 1) / MR_WARPS, MR_WARPS * 32, 0, c.stream>>>(d_U, d_n, cps, lastpos, d_used, R, nblk, rsum);
     KLAUNCH(c); KCHECK();
   }
-  k_rle2_scan<<<nblk, 32, 0, c.stream>>>(rsum, d_n, cps, d_used, plan, d_sym, d_m, d_freq);
+  k_rle2_scan<<<nblk, 32, 0, c.stream>>>(rsum, d_n, cps, d_used, plan, sym.lo, sym.hi, sym.any_hi, d_m, d_freq);
   KLAUNCH(c); KCHECK();
   static_assert(R2_TILE == MTF_CHUNK, "one zero-run tile per MTF chunk");
-  k_rle2<<<cps * nblk, R2_THREADS, 0, c.stream>>>(R, d_n, cps, plan, d_sym, d_freq);
+  k_rle2<<<cps * nblk, R2_THREADS, 0, c.stream>>>(R, d_n, cps, plan, sym.lo, sym.hi, sym.any_hi, d_freq);
   KLAUNCH(c); KCHECK();
 }
