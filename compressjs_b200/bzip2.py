@@ -27,19 +27,39 @@ class Err:  # lib/Bzip2.js:62-72
     END_OF_BLOCK = -8
 
 
-def _raise(rc):
+def _error(rc):
     msg = _native.last_error()
     if rc == -100:
-        raise ValueError(msg or "Invalid block size multiplier")  # `new Error(...)` lib/Bzip2.js:888-890
+        return ValueError(msg or "Invalid block size multiplier")  # `new Error(...)` lib/Bzip2.js:888-890
     if rc in (Err.NOT_BZIP_DATA, Err.DATA_ERROR, Err.OBSOLETE_INPUT):
-        raise Bzip2Error(rc, msg)
-    raise RuntimeError("libb2bz: %s (code %d)" % (msg, rc))
+        return Bzip2Error(rc, msg)
+    return RuntimeError("libb2bz: %s (code %d)" % (msg, rc))
+
+
+def _raise(rc):
+    raise _error(rc)
 
 
 def _take(L, p, n):
     arr = np.ctypeslib.as_array(p, shape=(n.value,)).copy() if n.value else np.zeros(0, dtype=np.uint8)
     L.b2_free(p)
     return arr
+
+
+def _decode(output, call):
+    """Run a b2_bzip2_decompress*_partial call.  On a decode error the bytes the reference has written by the time it
+    throws (lib/Bzip2.js:405-448 writes as it decodes) go to `output` first, then the error is raised."""
+    L = _native.lib()
+    out, n = C.POINTER(C.c_uint8)(), C.c_size_t()
+    rc = call(C.byref(out), C.byref(n))
+    if rc and not out:
+        _raise(rc)
+    err = _error(rc) if rc else None   # before `output` can call into the library again
+    data = _take(L, out, n)
+    if err is not None:
+        deliver_output(output, data, partial=True)
+        raise err
+    return deliver_output(output, data)
 
 
 class Bzip2:
@@ -63,37 +83,36 @@ class Bzip2:
 
     @staticmethod
     def decompressFile(input, output=None, multistream=False):
-        """lib/Bzip2.js:454-481 (Bunzip.decode)."""
+        """lib/Bzip2.js:454-481 (Bunzip.decode).  On a decode error the output receives the bytes decoded before it."""
         L = _native.lib()
         data = coerce_input(input)
-        out, n = C.POINTER(C.c_uint8)(), C.c_size_t()
-        rc = L.b2_bzip2_decompress(data.ctypes.data if data.size else None, data.size, int(bool(multistream)), C.byref(out), C.byref(n))
-        if rc:
-            _raise(rc)
-        return deliver_output(output, _take(L, out, n))
+        return _decode(output, lambda out, n: L.b2_bzip2_decompress_partial(
+            data.ctypes.data if data.size else None, data.size, int(bool(multistream)), out, n))
 
     @staticmethod
     def decompressBlock(input, pos, output=None):
-        """lib/Bzip2.js:482-503 (Bunzip.decodeBlock): decode the single block whose magic starts at bit `pos`."""
+        """lib/Bzip2.js:482-503 (Bunzip.decodeBlock): decode the single block whose magic starts at bit `pos`.  A block
+        whose only failure is its CRC delivers its bytes before the error is raised."""
         L = _native.lib()
         data = coerce_input(input)
-        out, n = C.POINTER(C.c_uint8)(), C.c_size_t()
-        rc = L.b2_bzip2_decompress_block(data.ctypes.data if data.size else None, data.size, int(pos), C.byref(out), C.byref(n))
-        if rc:
-            _raise(rc)
-        return deliver_output(output, _take(L, out, n))
+        return _decode(output, lambda out, n: L.b2_bzip2_decompress_block_partial(
+            data.ctypes.data if data.size else None, data.size, int(pos), out, n))
 
     @staticmethod
     def table(input, callback, multistream=False):
-        """lib/Bzip2.js:508-548: callback(bit position, decoded bytes) once per block."""
+        """lib/Bzip2.js:508-548: callback(bit position, decoded bytes) once per block.  On a decode error the callback
+        has been called for every block in front of the failing one when the error is raised."""
         L = _native.lib()
         data = coerce_input(input)
         bp, sz, cnt = C.POINTER(C.c_uint64)(), C.POINTER(C.c_uint32)(), C.c_size_t()
-        rc = L.b2_bzip2_table(data.ctypes.data if data.size else None, data.size, int(bool(multistream)), C.byref(bp), C.byref(sz), C.byref(cnt))
-        if rc:
+        rc = L.b2_bzip2_table_partial(data.ctypes.data if data.size else None, data.size, int(bool(multistream)), C.byref(bp), C.byref(sz), C.byref(cnt))
+        if rc and not bp:
             _raise(rc)
+        err = _error(rc) if rc else None
         rows = [(int(bp[i]), int(sz[i])) for i in range(cnt.value)]
         L.b2_free(bp)
         L.b2_free(sz)
         for pos, size in rows:
             callback(pos, size)
+        if err is not None:
+            raise err

@@ -592,6 +592,8 @@ int b2_bzip2_encode_range_dev(const void* d_in, size_t n, int level, size_t firs
   });
 }
 
+// On a decode error (-2/-5/-7) the code is returned, not thrown, and *out / the table rows hold what the reference has
+// written by the time it throws; any other error throws and returns nothing.
 static int decode_common(const uint8_t* in, size_t n, int multistream, bool single, u64 bitpos, uint8_t** out, size_t* out_n,
                          std::vector<u64>* tp, std::vector<u32>* tl) {
   Ctx& c = ctx_locked();
@@ -609,8 +611,14 @@ static int decode_common(const uint8_t* in, size_t n, int multistream, bool sing
     }
     u8* dres = nullptr;
     struct DresGuard { Ctx& c; u8*& p; ~DresGuard() { if (p) { c.dfree(p); p = nullptr; } } } dres_guard{c, dres};  // also on exceptions
-    rc = bzip2_decompress_device(c, din, n, multistream, nullptr, 0, &produced, single, bitpos, tp, tl, &dres);
-    if (rc == 0 && out) {
+    try {
+      rc = bzip2_decompress_device(c, din, n, multistream, nullptr, 0, &produced, single, bitpos, tp, tl, &dres);
+    } catch (const B2Error& e) {
+      if (e.code != B2_ERR_NOT_BZIP_DATA && e.code != B2_ERR_DATA_ERROR && e.code != B2_ERR_OBSOLETE_INPUT) throw;
+      g_err = e.msg;
+      rc = e.code;
+    }
+    if (out) {
       host = pinned_alloc(produced);
       try {
         StageScope s(c, ST_D2H);
@@ -626,30 +634,55 @@ static int decode_common(const uint8_t* in, size_t n, int multistream, bool sing
   c.sync();
   c.collect();
   c.stats.raw_bytes = produced; c.stats.comp_bytes = n;
-  if (rc) return rc;
   if (out) { *out = (uint8_t*)host; *out_n = produced; }
-  return 0;
+  return rc;
 }
 
-int b2_bzip2_decompress(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n) {
+int b2_bzip2_decompress_partial(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n) {
   return guarded([&]() { return decode_common(in, n, multistream, false, 0, out, out_n, nullptr, nullptr); });
 }
 
-int b2_bzip2_decompress_block(const uint8_t* in, size_t n, uint64_t bitpos, uint8_t** out, size_t* out_n) {
+int b2_bzip2_decompress_block_partial(const uint8_t* in, size_t n, uint64_t bitpos, uint8_t** out, size_t* out_n) {
   return guarded([&]() { return decode_common(in, n, 0, true, bitpos, out, out_n, nullptr, nullptr); });
 }
 
-int b2_bzip2_table(const uint8_t* in, size_t n, int multistream, uint64_t** bitpos, uint32_t** sizes, size_t* count) {
+int b2_bzip2_table_partial(const uint8_t* in, size_t n, int multistream, uint64_t** bitpos, uint32_t** sizes, size_t* count) {
   return guarded([&]() {
     std::vector<u64> tp; std::vector<u32> tl;
-    int rc = decode_common(in, n, multistream, false, 0, nullptr, nullptr, &tp, &tl);
-    if (rc) return rc;
+    const int rc = decode_common(in, n, multistream, false, 0, nullptr, nullptr, &tp, &tl);
     *count = tp.size();
     *bitpos = (uint64_t*)malloc(sizeof(uint64_t) * (tp.size() + 1));
     *sizes = (uint32_t*)malloc(sizeof(uint32_t) * (tp.size() + 1));
     for (size_t i = 0; i < tp.size(); i++) { (*bitpos)[i] = tp[i]; (*sizes)[i] = tl[i]; }
-    return 0;
+    return rc;
   });
+}
+
+// The all-or-nothing entry points: the partial call, with what it returned on an error released here.
+static int drop_on_error(int rc, uint8_t* p, size_t pn, uint8_t** out, size_t* out_n) {
+  if (rc || !out) { b2_free(p); return rc; }
+  *out = p; *out_n = pn;
+  return 0;
+}
+
+int b2_bzip2_decompress(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n) {
+  uint8_t* p = nullptr; size_t pn = 0;
+  const int rc = b2_bzip2_decompress_partial(in, n, multistream, &p, &pn);
+  return drop_on_error(rc, p, pn, out, out_n);
+}
+
+int b2_bzip2_decompress_block(const uint8_t* in, size_t n, uint64_t bitpos, uint8_t** out, size_t* out_n) {
+  uint8_t* p = nullptr; size_t pn = 0;
+  const int rc = b2_bzip2_decompress_block_partial(in, n, bitpos, &p, &pn);
+  return drop_on_error(rc, p, pn, out, out_n);
+}
+
+int b2_bzip2_table(const uint8_t* in, size_t n, int multistream, uint64_t** bitpos, uint32_t** sizes, size_t* count) {
+  uint64_t* bp = nullptr; uint32_t* sz = nullptr; size_t cnt = 0;
+  const int rc = b2_bzip2_table_partial(in, n, multistream, &bp, &sz, &cnt);
+  if (rc) { b2_free(bp); b2_free(sz); return rc; }
+  *bitpos = bp; *sizes = sz; *count = cnt;
+  return 0;
 }
 
 int b2_bzip2_decompress_dev(const void* d_in, size_t n, int multistream, void* d_out, size_t out_cap, size_t* out_n) {

@@ -1065,7 +1065,8 @@ static std::string hexs(u32 v) {
   return b;
 }
 
-struct Event { int kind; size_t cand; u32 a, b; int code; std::string msg; };  // kind: 0 block, 1 eos, 2 error
+// kind: 0 block, 1 eos, 2 error; off: offset in the decoded stream where the event happens (a block's start)
+struct Event { int kind; size_t cand; u32 a, b; int code; std::string msg; u64 off; };
 
 // One decode in flight.  open() parses the header, finds every block candidate and decodes the share
 // [lo, hi) of them (all of them on one GPU); finish() walks the chain over ALL candidates' results
@@ -1308,7 +1309,8 @@ static void dec_open(Ctx& c, DecSession& S, const u8* d_in_user, size_t n, bool 
 
 }
 
-// fills *first_err (event index, or -1) instead of throwing when `sharded`
+// fills *first_err (event index, or -1) instead of throwing when `sharded`.  On the host path (no d_out, d_out_alloc
+// given) an error still hands over the expanded buffer, with *out_n = the bytes the reference has written by then.
 static int dec_finish(Ctx& c, DecSession& S, int multistream, u8* d_out, size_t out_cap, size_t* out_n, std::vector<u64>* tab_pos,
                       std::vector<u32>* tab_len, u8** d_out_alloc, bool sharded, u64* shard_info) {
   *out_n = 0;
@@ -1336,22 +1338,22 @@ static int dec_finish(Ctx& c, DecSession& S, int multistream, u8* d_out, size_t 
     const CandRes& r = hres[bi];
     // the member's own limits, in the reference's order: randomised bit (:143), origPointer (:146), then the body
     if (r.status != DEC_OBSOLETE && r.orig > cur_dbuf) {
-      events.push_back({2, bi, 0, 0, DEC_DATA_ERROR, "Data error: initial position out of bounds"});
+      events.push_back({2, bi, 0, 0, DEC_DATA_ERROR, "Data error: initial position out of bounds", total_out});
       return false;
     }
     if (r.status != 0) {
       std::string msg = r.status == DEC_OBSOLETE ? "Obsolete (pre 0.9.5) bzip format not supported." : "Data error";
       if (r.detail == 1) msg += ": initial position out of bounds";
-      events.push_back({2, bi, 0, 0, r.status, msg});
+      events.push_back({2, bi, 0, 0, r.status, msg, total_out});
       return false;
     }
     if (r.n > cur_dbuf) {  // dbufCount would have run over dbufSize (lib/Bzip2.js:338,354)
-      events.push_back({2, bi, 0, 0, DEC_DATA_ERROR, "Data error"});
+      events.push_back({2, bi, 0, 0, DEC_DATA_ERROR, "Data error", total_out});
       return false;
     }
     outbase[bi] = total_out;
+    events.push_back({0, bi, 0, 0, 0, "", total_out});
     total_out += r.rawlen;
-    events.push_back({0, bi, 0, 0, 0, ""});
     return true;
   };
   if (S.single) {
@@ -1362,14 +1364,14 @@ static int dec_finish(Ctx& c, DecSession& S, int multistream, u8* d_out, size_t 
     for (;;) {
       if ((pos + 7) / 8 >= n) break;  // 'eof' in inputStream && inputStream.eof() (lib/Bzip2.js:462)
       const long ci = find_cand(pos);
-      if (ci < 0) { events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data"}); break; }
+      if (ci < 0) { events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data", total_out}); break; }
       if (cands[ci].type == 1) {
         const size_t bi = (size_t)cand_to_blk[ci];
         stream_crc = cands[ci].next32 ^ ((stream_crc << 1) | (stream_crc >> 31));  // lib/Bzip2.js:138-139
         if (!block_event(bi)) break;
         pos = hres[bi].endbit;
       } else {
-        events.push_back({1, 0, stream_crc, cands[ci].next32, 0, ""});
+        events.push_back({1, 0, stream_crc, cands[ci].next32, 0, "", total_out});
         pos += 80;
         const u64 bytepos = (pos + 7) / 8;
         if (multistream && bytepos < n) {
@@ -1378,9 +1380,9 @@ static int dec_finish(Ctx& c, DecSession& S, int multistream, u8* d_out, size_t 
           const size_t avail = (size_t)std::min<u64>(4, n - bytepos);
           CUDA_CHECK(cudaMemcpyAsync(h2, S.din.p + bytepos, avail, cudaMemcpyDeviceToHost, c.stream));
           CUDA_CHECK(cudaStreamSynchronize(c.stream));
-          if (avail != 4 || h2[0] != 'B' || h2[1] != 'Z' || h2[2] != 'h') { events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data: bad magic"}); break; }
+          if (avail != 4 || h2[0] != 'B' || h2[1] != 'Z' || h2[2] != 'h') { events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data: bad magic", total_out}); break; }
           const int lv = h2[3] - 0x30;
-          if (lv < 1 || lv > 9) { events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data: level out of range"}); break; }
+          if (lv < 1 || lv > 9) { events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data: level out of range", total_out}); break; }
           cur_dbuf = (u32)lv * 100000u;
           stream_crc = 0;
           pos = (bytepos + 4) * 8;
@@ -1447,22 +1449,32 @@ static int dec_finish(Ctx& c, DecSession& S, int multistream, u8* d_out, size_t 
   S.err_event = -1;
   int err_code = 0;
   std::string err_msg;
+  u64 prefix = 0;  // bytes the reference has written when it throws: a block's own bytes go out before its CRC check
   for (size_t ei = 0; ei < events.size() && S.err_event < 0; ei++) {
     const Event& ev = events[ei];
     if (ev.kind == 0) {
       if (ev.cand >= S.lo && ev.cand < S.hi) {  // CRCs of foreign blocks are checked by their owners
         const u32 want = bc[ev.cand].next32, got = got_crc[ev.cand - S.lo];
-        if (want != got) { S.err_event = (int)ei; err_code = DEC_DATA_ERROR; err_msg = "Data error: Bad block CRC (got " + hexs(got) + " expected " + hexs(want) + ")"; }
+        if (want != got) {
+          S.err_event = (int)ei; err_code = DEC_DATA_ERROR; err_msg = "Data error: Bad block CRC (got " + hexs(got) + " expected " + hexs(want) + ")";
+          prefix = ev.off + hres[ev.cand].rawlen;
+        }
       }
       if (S.err_event < 0 && tab_pos) { tab_pos->push_back(bc[ev.cand].pos); tab_len->push_back(hres[ev.cand].rawlen); }
     } else if (ev.kind == 1) {
-      if (!tab_pos && ev.a != ev.b) { S.err_event = (int)ei; err_code = DEC_DATA_ERROR; err_msg = "Data error: Bad stream CRC (got " + hexs(ev.a) + " expected " + hexs(ev.b) + ")"; }
+      if (!tab_pos && ev.a != ev.b) {
+        S.err_event = (int)ei; err_code = DEC_DATA_ERROR; err_msg = "Data error: Bad stream CRC (got " + hexs(ev.a) + " expected " + hexs(ev.b) + ")";
+        prefix = ev.off;
+      }
     } else {
       S.err_event = (int)ei; err_code = ev.code; err_msg = ev.msg;
+      prefix = ev.off;
     }
   }
   if (shard_info) { shard_info[0] = my_off; shard_info[1] = my_len; shard_info[2] = total_out; shard_info[3] = (u64)(long long)S.err_event; shard_info[4] = (u64)(long long)err_code; }
   if (S.err_event >= 0) {
+    // the host path hands the output in front of the error to the caller with the error (b2_bzip2_decompress_partial)
+    if (!sharded && !d_out && d_out_alloc) { *out_n = (size_t)prefix; *d_out_alloc = own.p; own.p = nullptr; }
     if (!sharded) throw B2Error{err_code, err_msg};
     throw B2Error{err_code, err_msg};  // the caller (sharded) compares shard_info[3] across ranks and keeps the earliest
   }

@@ -7,13 +7,15 @@
 
 static void fin(napi_env, void* data, void*) { b2_free(data); }
 
-static napi_value fail(napi_env env, int rc) {
+// `prop` / `val`: what a failed decode had delivered (a Buffer or the table rows), attached to the error for the shim
+static napi_value fail(napi_env env, int rc, const char* prop = nullptr, napi_value val = nullptr) {
   napi_value msg, err, code;
   napi_create_string_utf8(env, b2_last_error(), NAPI_AUTO_LENGTH, &msg);
   if (rc == B2_ERR_BAD_LEVEL) napi_create_error(env, nullptr, msg, &err);        // `new Error(...)` lib/Bzip2.js:888-890
   else napi_create_type_error(env, nullptr, msg, &err);                            // `new TypeError(...)` lib/Bzip2.js:82-88
   napi_create_int32(env, rc, &code);
   napi_set_named_property(env, err, "errorCode", code);
+  if (prop && val) napi_set_named_property(env, err, prop, val);
   napi_throw(env, err);
   return nullptr;
 }
@@ -38,6 +40,13 @@ static napi_value CompressFile(napi_env env, napi_callback_info info) {
   napi_value buf; napi_create_external_buffer(env, out_n, out, fin, nullptr, &buf);
   return buf;
 }
+// result of a b2_bzip2_decompress*_partial call: the Buffer, or the error with the bytes decoded before it as .partial
+static napi_value decoded(napi_env env, int rc, uint8_t* out, size_t out_n) {
+  napi_value buf = nullptr;
+  if (out) napi_create_external_buffer(env, out_n, out, fin, nullptr, &buf);
+  if (rc) return fail(env, rc, "partial", buf);
+  return buf;
+}
 // decompressFile(buffer, multistream) -> Buffer    (Bunzip.decode, lib/Bzip2.js:454)
 static napi_value DecompressFile(napi_env env, napi_callback_info info) {
   size_t argc = 2; napi_value argv[2];
@@ -45,11 +54,9 @@ static napi_value DecompressFile(napi_env env, napi_callback_info info) {
   const uint8_t* in; size_t n; bool ms = false;
   if (!buf_arg(env, argv[0], &in, &n)) return fail(env, B2_ERR_BAD_ARG);
   if (argc > 1) napi_get_value_bool(env, argv[1], &ms);
-  uint8_t* out; size_t out_n;
-  int rc = b2_bzip2_decompress(in, n, ms ? 1 : 0, &out, &out_n);
-  if (rc) return fail(env, rc);
-  napi_value buf; napi_create_external_buffer(env, out_n, out, fin, nullptr, &buf);
-  return buf;
+  uint8_t* out = nullptr; size_t out_n = 0;
+  int rc = b2_bzip2_decompress_partial(in, n, ms ? 1 : 0, &out, &out_n);
+  return decoded(env, rc, out, out_n);
 }
 // decompressBlock(buffer, bitpos) -> Buffer        (Bunzip.decodeBlock, lib/Bzip2.js:482)
 static napi_value DecompressBlock(napi_env env, napi_callback_info info) {
@@ -58,11 +65,9 @@ static napi_value DecompressBlock(napi_env env, napi_callback_info info) {
   const uint8_t* in; size_t n; double pos = 0;
   if (!buf_arg(env, argv[0], &in, &n)) return fail(env, B2_ERR_BAD_ARG);
   napi_get_value_double(env, argv[1], &pos);
-  uint8_t* out; size_t out_n;
-  int rc = b2_bzip2_decompress_block(in, n, (uint64_t)pos, &out, &out_n);
-  if (rc) return fail(env, rc);
-  napi_value buf; napi_create_external_buffer(env, out_n, out, fin, nullptr, &buf);
-  return buf;
+  uint8_t* out = nullptr; size_t out_n = 0;
+  int rc = b2_bzip2_decompress_block_partial(in, n, (uint64_t)pos, &out, &out_n);
+  return decoded(env, rc, out, out_n);
 }
 // integer argument that must be a JS number; false (and B2_ERR_BAD_ARG thrown by the caller) otherwise
 static bool int_arg(napi_env env, napi_value v, int32_t* out) {
@@ -73,16 +78,17 @@ static bool int_arg(napi_env env, napi_value v, int32_t* out) {
 // n bytes must exist in both the source and the destination view
 static bool len_ok(int32_t n, size_t a, size_t b) { return n >= 0 && (size_t)n <= a && (size_t)n <= b; }
 
-// table(buffer, multistream) -> [[bitpos, size], ...]   (Bunzip.table, lib/Bzip2.js:508)
+// table(buffer, multistream) -> [[bitpos, size], ...]   (Bunzip.table, lib/Bzip2.js:508); on a decode error the rows
+// of the blocks before it go with the error as .rows
 static napi_value Table(napi_env env, napi_callback_info info) {
   size_t argc = 2; napi_value argv[2];
   napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr);
   const uint8_t* in; size_t n; bool ms = false;
   if (!buf_arg(env, argv[0], &in, &n)) return fail(env, B2_ERR_BAD_ARG);
   if (argc > 1) napi_get_value_bool(env, argv[1], &ms);
-  uint64_t* bp; uint32_t* sz; size_t cnt;
-  int rc = b2_bzip2_table(in, n, ms ? 1 : 0, &bp, &sz, &cnt);
-  if (rc) return fail(env, rc);
+  uint64_t* bp = nullptr; uint32_t* sz = nullptr; size_t cnt = 0;
+  int rc = b2_bzip2_table_partial(in, n, ms ? 1 : 0, &bp, &sz, &cnt);
+  if (rc && !bp) return fail(env, rc);
   napi_value arr; napi_create_array_with_length(env, cnt, &arr);
   for (size_t i = 0; i < cnt; i++) {
     napi_value row, a, b;
@@ -92,6 +98,7 @@ static napi_value Table(napi_env env, napi_callback_info info) {
     napi_set_element(env, arr, (uint32_t)i, row);
   }
   b2_free(bp); b2_free(sz);
+  if (rc) return fail(env, rc, "rows", arr);
   return arr;
 }
 // bwtransform2(T, U, n) -> pidx                     (BWT.bwtransform2, lib/BWT.js:372)

@@ -13,21 +13,33 @@ function drain(input) {                       // Util.coerceInputStream semantic
   }
   return Buffer.isBuffer(input) ? input : Buffer.from(input);
 }
-function deliver(output, data) {              // Util.coerceOutputStream + retval semantics
+// partial: data is what a failed decode had written; a stream gets all of it, a buffer what fits (a typed array drops
+// writes past its end), a size nothing, as the reference's output stream when it throws
+function deliver(output, data, partial) {     // Util.coerceOutputStream + retval semantics
   if (output && typeof output === 'object' && typeof output.writeByte === 'function') {
     for (var i = 0; i < data.length; i++) { output.writeByte(data[i]); }
     return output;
   }
   if (typeof output === 'number') {
+    if (partial) { return output; }
     if (output !== data.length) { throw new TypeError('outputsize does not match decoded input'); }
     return new Uint8Array(data);
   }
   if (output) {
-    if (output.length !== data.length) { throw new TypeError('outputsize does not match decoded input'); }
-    for (var j = 0; j < data.length; j++) { output[j] = data[j]; }
+    if (!partial && output.length !== data.length) { throw new TypeError('outputsize does not match decoded input'); }
+    for (var j = 0; j < data.length && j < output.length; j++) { output[j] = data[j]; }
     return output;
   }
   return new Uint8Array(data);
+}
+// a decode whose error carries the bytes decoded before it (addon.cc): deliver those, then rethrow
+function decode(output, call) {
+  var data;
+  try { data = call(); } catch (e) {
+    if (e.partial) { deliver(output, e.partial, true); }
+    throw e;
+  }
+  return deliver(output, data);
 }
 
 var Bzip2 = Object.create(null);
@@ -37,13 +49,20 @@ Bzip2.compressFile = function(inStream, outStream, props) {
   return deliver(outStream, native.compressFile(drain(inStream), level));
 };
 Bzip2.decompressFile = function(input, output, multistream) {
-  return deliver(output, native.decompressFile(drain(input), !!multistream));
+  var data = drain(input);
+  return decode(output, function() { return native.decompressFile(data, !!multistream); });
 };
 Bzip2.decompressBlock = function(input, pos, output) {
-  return deliver(output, native.decompressBlock(drain(input), pos));
+  var data = drain(input);
+  return decode(output, function() { return native.decompressBlock(data, pos); });
 };
 Bzip2.table = function(input, callback, multistream) {
-  native.table(drain(input), !!multistream).forEach(function(r) { callback(r[0], r[1]); });
+  var rows;
+  try { rows = native.table(drain(input), !!multistream); } catch (e) {
+    (e.rows || []).forEach(function(r) { callback(r[0], r[1]); });
+    throw e;
+  }
+  rows.forEach(function(r) { callback(r[0], r[1]); });
 };
 
 var BWT = Object.create(null);

@@ -46,14 +46,26 @@ void b2_free(void* p);
 /* Bzip2.compressFile(input, output, level)            lib/Bzip2.js:879-929 */
 int b2_bzip2_compress(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n);
 /* Bzip2.decompressFile(input, output, multistream)    lib/Bzip2.js:454-481
- * Members of a multistream file may have different levels.  On an error nothing is returned (the reference hands the
- * blocks in front of the error to its output stream first); one call keeps ~2 MiB per block of the file on the device. */
+ * Members of a multistream file may have different levels.  On an error nothing is returned and nothing needs freeing;
+ * one call keeps ~2 MiB per block of the file on the device. */
 int b2_bzip2_decompress(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n);
 /* Bzip2.decompressBlock(input, bitPos, output)        lib/Bzip2.js:482-503 */
 int b2_bzip2_decompress_block(const uint8_t* in, size_t n, uint64_t bitpos, uint8_t** out, size_t* out_n);
 /* Bzip2.table(input, callback, multistream)           lib/Bzip2.js:508-548
  * (the callback is replayed by the host shim from the two arrays) */
 int b2_bzip2_table(const uint8_t* in, size_t n, int multistream, uint64_t** bitpos, uint32_t** sizes, size_t* count);
+/* The same three calls with the reference's output on error: it writes every decoded byte to its output stream as it
+ * goes (lib/Bzip2.js:405-448) and calls table's callback once per good block, so the bytes and blocks in front of an
+ * error are already out when it throws.  On a decode error (-2 / -5 / -7) these return that code and the message of
+ * the calls above, and *out / *out_n (the row arrays and *count) hold that prefix, to be released with b2_free():
+ *   - a block whose CRC fails: the blocks before it and all of its own bytes (they are written before the check);
+ *   - any other error inside a block, a bad magic, truncation: the blocks before it;
+ *   - a bad stream CRC: every block of the member; a bad header of a later member: all earlier members;
+ *   - table: the rows of the blocks before the failing one (the stream CRC is not checked, as there).
+ * On any other error (CUDA failure, bad argument) nothing is returned.  On success they equal the calls above. */
+int b2_bzip2_decompress_partial(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n);
+int b2_bzip2_decompress_block_partial(const uint8_t* in, size_t n, uint64_t bitpos, uint8_t** out, size_t* out_n);
+int b2_bzip2_table_partial(const uint8_t* in, size_t n, int multistream, uint64_t** bitpos, uint32_t** sizes, size_t* count);
 
 /* ---- compressjs.BWT (lib/BWT.js) ------------------------------------------------- */
 /* BWT.bwtransform2(T, U, n, 256) -> pidx  (cyclic)    lib/BWT.js:372-417
