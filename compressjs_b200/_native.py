@@ -13,7 +13,7 @@ _LIB = None
 EXPORTS = [
     "b2_init", "b2_shutdown", "b2_last_error", "b2_free",
     "b2_bzip2_compress", "b2_bzip2_decompress", "b2_bzip2_decompress_block", "b2_bzip2_table",
-    "b2_bzip2_decompress_partial", "b2_bzip2_decompress_block_partial", "b2_bzip2_table_partial",
+    "b2_bzip2_decompress_partial", "b2_bzip2_decompress_block_partial", "b2_bzip2_table_partial", "b2_bzip2_decompress_blocks",
     "b2_bwt_cyclic", "b2_bwt_cyclic_batch", "b2_suffixsort", "b2_bwt_sentinel", "b2_bwt_inverse", "b2_bwtc_compress", "b2_bwtc_decompress", "b2_crc32_bzip2",
     "b2_bzip2_bound", "b2_bzip2_compress_dev", "b2_bzip2_decompress_dev",
     "b2_bzip2_plan", "b2_bzip2_plan_spec", "b2_bzip2_share_summary", "b2_bzip2_plan_share", "b2_bitshift_dev", "b2_dec_shard_open", "b2_dec_shard_export", "b2_dec_shard_finish", "b2_bzip2_encode_range_dev", "b2_get_stats", "b2_last_trace",
@@ -59,6 +59,8 @@ def lib():
         getattr(L, "b2_bzip2_decompress_block" + sfx).argtypes = [C.c_void_p, C.c_size_t, C.c_uint64, u8pp, szp]
         getattr(L, "b2_bzip2_table" + sfx).argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.POINTER(C.POINTER(C.c_uint64)),
                                                       C.POINTER(C.POINTER(C.c_uint32)), szp]
+    L.b2_bzip2_decompress_blocks.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, u8pp, szp,
+                                             C.POINTER(C.POINTER(C.c_uint64)), szp]
     L.b2_bwt_cyclic.restype = C.c_int32
     L.b2_bwt_cyclic.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
     L.b2_bwt_cyclic_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]

@@ -1,4 +1,5 @@
-"""compressjs.Bzip2 on the GPU: same four entry points as lib/Bzip2.js:879-933."""
+"""compressjs.Bzip2 on the GPU: same four entry points as lib/Bzip2.js:879-933, and decompressBlocks (decompressBlock at
+many positions in one pass)."""
 import ctypes as C
 
 import numpy as np
@@ -97,6 +98,36 @@ class Bzip2:
         data = coerce_input(input)
         return _decode(output, lambda out, n: L.b2_bzip2_decompress_block_partial(
             data.ctypes.data if data.size else None, data.size, int(pos), out, n))
+
+    @staticmethod
+    def decompressBlocks(input, positions, output=None):
+        """GPU extension: decompressBlock at every bit position of `positions`, in one pass.  The result is that of
+        ``[decompressBlock(input, p) for p in positions]`` (output None: a list of bytes), or of
+        ``for p in positions: decompressBlock(input, p, output)`` with a writeByte stream, which is returned.  On an error
+        the stream first receives what that loop would have written, then the first failing position's error is raised.
+        Positions may repeat and come in any order; every block is held to the dbufSize of the file's first header."""
+        if output is not None and not hasattr(output, "writeByte"):
+            raise TypeError("decompressBlocks writes to a stream (writeByte) or returns a list: output must be one or None")
+        L = _native.lib()
+        data = coerce_input(input)
+        pos = np.array([int(p) & 0xFFFFFFFFFFFFFFFF for p in positions], dtype=np.uint64)   # as c_uint64 takes decompressBlock's pos
+        out, n = C.POINTER(C.c_uint8)(), C.c_size_t()
+        ends, done = C.POINTER(C.c_uint64)(), C.c_size_t()
+        rc = L.b2_bzip2_decompress_blocks(data.ctypes.data if data.size else None, data.size, pos.ctypes.data if pos.size else None,
+                                          pos.size, C.byref(out), C.byref(n), C.byref(ends), C.byref(done))
+        if rc and not out:
+            _raise(rc)
+        err = _error(rc) if rc else None
+        stops = [int(ends[i]) for i in range(done.value)]
+        L.b2_free(ends)
+        buf = _take(L, out, n)
+        if output is not None:
+            deliver_output(output, buf, partial=err is not None)
+        if err is not None:
+            raise err
+        if output is not None:
+            return output
+        return [buf[s:e].tobytes() for s, e in zip([0] + stops[:-1], stops)]
 
     @staticmethod
     def table(input, callback, multistream=False):

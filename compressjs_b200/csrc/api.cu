@@ -30,7 +30,7 @@ void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* 
 void dec_shard_export(u64* buf);
 int dec_shard_finish(Ctx& c, const u64* all, int multistream, u8* d_out, size_t out_cap, u64* res);
 int bzip2_decompress_device(Ctx& c, const u8* d_in, size_t n, int multistream, u8* d_out, size_t out_cap, size_t* out_n,
-                            bool single_block, u64 bitpos, std::vector<u64>* tab_pos, std::vector<u32>* tab_len,
+                            const std::vector<u64>* positions, std::vector<u64>* ends, std::vector<u64>* tab_pos, std::vector<u32>* tab_len,
                             u8** d_out_alloc);
 
 static std::mutex g_mu;
@@ -593,9 +593,10 @@ int b2_bzip2_encode_range_dev(const void* d_in, size_t n, int level, size_t firs
 }
 
 // On a decode error (-2/-5/-7) the code is returned, not thrown, and *out / the table rows hold what the reference has
-// written by the time it throws; any other error throws and returns nothing.
-static int decode_common(const uint8_t* in, size_t n, int multistream, bool single, u64 bitpos, uint8_t** out, size_t* out_n,
-                         std::vector<u64>* tp, std::vector<u32>* tl) {
+// written by the time it throws; any other error throws and returns nothing.  positions / ends: a position list
+// (bzip2_decompress_device).
+static int decode_common(const uint8_t* in, size_t n, int multistream, const std::vector<u64>* positions, std::vector<u64>* ends,
+                         uint8_t** out, size_t* out_n, std::vector<u64>* tp, std::vector<u32>* tl) {
   Ctx& c = ctx_locked();
   c.reset_call();
   size_t produced = 0;
@@ -612,7 +613,7 @@ static int decode_common(const uint8_t* in, size_t n, int multistream, bool sing
     u8* dres = nullptr;
     struct DresGuard { Ctx& c; u8*& p; ~DresGuard() { if (p) { c.dfree(p); p = nullptr; } } } dres_guard{c, dres};  // also on exceptions
     try {
-      rc = bzip2_decompress_device(c, din, n, multistream, nullptr, 0, &produced, single, bitpos, tp, tl, &dres);
+      rc = bzip2_decompress_device(c, din, n, multistream, nullptr, 0, &produced, positions, ends, tp, tl, &dres);
     } catch (const B2Error& e) {
       if (e.code != B2_ERR_NOT_BZIP_DATA && e.code != B2_ERR_DATA_ERROR && e.code != B2_ERR_OBSOLETE_INPUT) throw;
       g_err = e.msg;
@@ -639,17 +640,40 @@ static int decode_common(const uint8_t* in, size_t n, int multistream, bool sing
 }
 
 int b2_bzip2_decompress_partial(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n) {
-  return guarded([&]() { return decode_common(in, n, multistream, false, 0, out, out_n, nullptr, nullptr); });
+  return guarded([&]() { return decode_common(in, n, multistream, nullptr, nullptr, out, out_n, nullptr, nullptr); });
 }
 
+int b2_bzip2_decompress_blocks(const uint8_t* in, size_t n, const uint64_t* bitpos, size_t count, uint8_t** out, size_t* out_n,
+                               uint64_t** ends, size_t* done) {
+  return guarded([&]() {
+    if (count && !bitpos) throw B2Error{B2_ERR_BAD_ARG, "bitpos is null"};
+    if (!out || !out_n || !ends || !done) throw B2Error{B2_ERR_BAD_ARG, "null output argument"};
+    struct HostBuf { void* p; ~HostBuf() { free(p); } } ep{malloc(sizeof(uint64_t) * (count + 1))};
+    if (!ep.p) throw B2Error{B2_ERR_CUDA, "out of host memory"};
+    std::vector<u64> pos(bitpos, bitpos + count), e;
+    int rc = 0;
+    uint8_t* o = nullptr; size_t on = 0;
+    if (count) rc = decode_common(in, n, 0, &pos, &e, &o, &on, nullptr, nullptr);
+    else if (!(o = (uint8_t*)malloc(1))) throw B2Error{B2_ERR_CUDA, "out of host memory"};  // no position: nothing is read, not even the header
+    for (size_t i = 0; i < e.size(); i++) ((uint64_t*)ep.p)[i] = e[i];
+    *out = o; *out_n = on; *ends = (uint64_t*)ep.p; *done = e.size();
+    ep.p = nullptr;
+    return rc;
+  });
+}
+
+// one-element position lists
 int b2_bzip2_decompress_block_partial(const uint8_t* in, size_t n, uint64_t bitpos, uint8_t** out, size_t* out_n) {
-  return guarded([&]() { return decode_common(in, n, 0, true, bitpos, out, out_n, nullptr, nullptr); });
+  uint64_t* ends = nullptr; size_t done = 0;
+  const int rc = b2_bzip2_decompress_blocks(in, n, &bitpos, 1, out, out_n, &ends, &done);
+  b2_free(ends);
+  return rc;
 }
 
 int b2_bzip2_table_partial(const uint8_t* in, size_t n, int multistream, uint64_t** bitpos, uint32_t** sizes, size_t* count) {
   return guarded([&]() {
     std::vector<u64> tp; std::vector<u32> tl;
-    const int rc = decode_common(in, n, multistream, false, 0, nullptr, nullptr, &tp, &tl);
+    const int rc = decode_common(in, n, multistream, nullptr, nullptr, nullptr, nullptr, &tp, &tl);
     *count = tp.size();
     *bitpos = (uint64_t*)malloc(sizeof(uint64_t) * (tp.size() + 1));
     *sizes = (uint32_t*)malloc(sizeof(uint32_t) * (tp.size() + 1));
@@ -692,7 +716,7 @@ int b2_bzip2_decompress_dev(const void* d_in, size_t n, int multistream, void* d
     int rc;
     {
       StageScope tot(c, ST_TOTAL);
-      rc = bzip2_decompress_device(c, (const u8*)d_in, n, multistream, (u8*)d_out, out_cap, out_n, false, 0, nullptr, nullptr, nullptr);
+      rc = bzip2_decompress_device(c, (const u8*)d_in, n, multistream, (u8*)d_out, out_cap, out_n, nullptr, nullptr, nullptr, nullptr, nullptr);
     }
     c.sync();
     c.collect();

@@ -5,6 +5,7 @@
 //
 //   k_scan_magic   : every bit offset is tested for the 48-bit block / end-of-stream magics
 //                    (blocks start at arbitrary bit positions and a .bz2 has no index)
+//   k_magic_at     : the same test at caller-given bit positions only (decompressBlock / decompressBlocks)
 //   k_hdec         : one CTA (4 warps) per candidate block: header parse (symbol map, selectors, code
 //                    length tables -- lib/Bzip2.js:137-275), canonical decode tables exactly as the
 //                    reference builds them (limit/base/permute) plus a 9-bit LUT derived from them,
@@ -27,7 +28,8 @@
 //                    offsets from tile sums + one warp scan per block, tiles expanded in shared
 //                    memory, CRC32 per block
 //   host           : walks the block chain (a block must start exactly where the previous one
-//                    ended), folds/validates CRCs and raises the reference's errors in stream order.
+//                    ended), folds/validates CRCs and raises the reference's errors in stream order;
+//                    a position list is taken in list order instead, without a chain.
 #include <algorithm>
 #include <vector>
 #include "enc.h"
@@ -61,38 +63,64 @@ struct CandRes {
   u8 sym_to_byte[256];
 };
 
-// ---- magic scan ---------------------------------------------------------------------------
-// One thread per aligned 32-bit word of the stream = 32 bit offsets: the words w, w+1, w+2 (big endian) hold the 80 bits
-// that a candidate starting in word w can span (48-bit magic + the 32 bits behind it need w+3 as well).  The first 32
-// bits of the magic are tested with one funnel shift and one compare per offset.
-__global__ void k_scan_magic(const u8* __restrict__ in, u64 n, Cand* __restrict__ cands, u32* count, u32 cap) {
-  const u64 wi = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-  const u64 nwords = (n + 3) / 4;      // the private copy of the input is zero padded (dec_open): reads up to n + 31 are safe
-  if (wi >= nwords) return;
+// ---- magic test -----------------------------------------------------------------------------
+// The words wi .. wi+3 of the stream (big endian) hold the 80 bits that a candidate starting in word wi can span: the
+// 48-bit magic and the 32 bits behind it.  The private copy of the input is zero padded (dec_open): for wi < (n + 3) / 4
+// the reads stay below n + 32.
+struct MagicWords { u32 w0, w1, w2, w3; };
+__device__ __forceinline__ MagicWords magic_words(const u8* __restrict__ in, u64 wi) {
   const u32* words = reinterpret_cast<const u32*>(in);
-  const u32 w0 = __byte_perm(words[wi], 0, 0x0123), w1 = __byte_perm(words[wi + 1], 0, 0x0123), w2 = __byte_perm(words[wi + 2], 0, 0x0123),
-            w3 = __byte_perm(words[wi + 3], 0, 0x0123);
+  return {__byte_perm(words[wi], 0, 0x0123), __byte_perm(words[wi + 1], 0, 0x0123), __byte_perm(words[wi + 2], 0, 0x0123),
+          __byte_perm(words[wi + 3], 0, 0x0123)};
+}
+// Is there a magic at bit pos = 32 wi + b of an n-byte stream?  If so, found(type, next32): type 1 = block, 2 = end of
+// stream, next32 = the 32 bits behind it.  The first 32 bits of the magic are tested with one funnel shift and one compare;
+// the rest, rarely reached, sits inside that branch (a callback rather than a return value keeps the scan loop free of
+// a second branch per offset).
+template <class F>
+__device__ __forceinline__ void magic_test(const MagicWords& w, u32 b, u64 pos, u64 n, F&& found) {
   const u32 M1 = (u32)(WHOLEPI >> 16), M2 = (u32)(SQRTPI >> 16);
-#pragma unroll 8
-  for (u32 b = 0; b < 32; b++) {
-    const u32 h = __funnelshift_l(w1, w0, b);            // stream bits [b, b + 32) of this word pair
-    if (h == M1 || h == M2) {
-      const u32 mid = __funnelshift_l(w2, w1, b);        // bits [b + 32, b + 64)
-      const u64 v = ((u64)h << 16) | (mid >> 16);
-      const u64 pos = wi * 32 + b;
-      if ((v == WHOLEPI || v == SQRTPI) && pos < n * 8) {
-        const u32 idx = atomicAdd(count, 1u);
-        if (idx < cap) {
-          Cand c;
-          c.pos = pos;
-          c.type = v == WHOLEPI ? 1u : 2u;
-          const u32 lo = __funnelshift_l(w3, w2, b);     // bits [b + 64, b + 96)
-          c.next32 = (mid << 16) | (lo >> 16);           // the 32 bits behind the 48-bit magic
-          cands[idx] = c;
-        }
-      }
+  const u32 h = __funnelshift_l(w.w1, w.w0, b);          // stream bits [b, b + 32) of this word pair
+  if (h == M1 || h == M2) {
+    const u32 mid = __funnelshift_l(w.w2, w.w1, b);      // bits [b + 32, b + 64)
+    const u64 v = ((u64)h << 16) | (mid >> 16);
+    if ((v == WHOLEPI || v == SQRTPI) && pos < n * 8) {
+      const u32 lo = __funnelshift_l(w.w3, w.w2, b);     // bits [b + 64, b + 96)
+      found(v == WHOLEPI ? 1u : 2u, (mid << 16) | (lo >> 16));
     }
   }
+}
+
+// ---- magic scan ---------------------------------------------------------------------------
+// One thread per aligned 32-bit word of the stream = 32 bit offsets.
+__global__ void k_scan_magic(const u8* __restrict__ in, u64 n, Cand* __restrict__ cands, u32* count, u32 cap) {
+  const u64 wi = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (wi >= (n + 3) / 4) return;
+  const MagicWords w = magic_words(in, wi);
+#pragma unroll 8
+  for (u32 b = 0; b < 32; b++) {
+    const u64 pos = wi * 32 + b;
+    magic_test(w, b, pos, n, [&](u32 type, u32 next32) {
+      const u32 idx = atomicAdd(count, 1u);
+      if (idx < cap) {
+        Cand c;
+        c.pos = pos; c.type = type; c.next32 = next32;
+        cands[idx] = c;
+      }
+    });
+  }
+}
+
+// ---- magic at given positions -----------------------------------------------------------------
+// One thread per requested bit position (a list decode: no scan of the whole stream).  type 0: no magic there.
+__global__ void k_magic_at(const u8* __restrict__ in, u64 n, const u64* __restrict__ pos, u64 count, Cand* __restrict__ cands) {
+  const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  Cand c;
+  c.pos = pos[i]; c.type = 0; c.next32 = 0;
+  if (c.pos < n * 8)  // no reads past the stream
+    magic_test(magic_words(in, c.pos >> 5), (u32)(c.pos & 31), c.pos, n, [&](u32 type, u32 next32) { c.type = type; c.next32 = next32; });
+  cands[i] = c;
 }
 
 // ---- bit reader (one thread) ----------------------------------------------------------------
@@ -1065,24 +1093,26 @@ static std::string hexs(u32 v) {
   return b;
 }
 
-// kind: 0 block, 1 eos, 2 error; off: offset in the decoded stream where the event happens (a block's start)
+// kind: 0 block, 1 eos, 2 error, 3 an end-of-stream magic in a position list (no bytes, no stream CRC);
+// off: offset in the decoded stream where the event happens (a block's start)
 struct Event { int kind; size_t cand; u32 a, b; int code; std::string msg; u64 off; };
 
 // One decode in flight.  open() parses the header, finds every block candidate and decodes the share
 // [lo, hi) of them (all of them on one GPU); finish() walks the chain over ALL candidates' results
 // (imported from the other ranks when sharded), expands + CRC-checks the blocks of the own share and
-// raises the reference's errors in stream order.
+// raises the reference's errors in stream order.  A position list (decompressBlock once per position) has no chain:
+// its candidates are the magics at the given positions, in list order, and finish() takes them in that order.
 struct DecSession {
   Ctx* c = nullptr;
   size_t n = 0;
   u32 dbuf_size = 0;
   DBuf<u8> din;
-  std::vector<Cand> cands;         // every magic found, sorted by position
+  std::vector<Cand> cands;         // every magic found, sorted by position; for a list: one per position (type 0 = none)
   std::vector<size_t> blk_idx;     // block candidates (index into cands)
   std::vector<Cand> bc;            // the same as Cand records
   std::vector<CandRes> hres;       // per block candidate (valid for [lo,hi) after open, for all after import)
   size_t lo = 0, hi = 0;           // own share of the block candidates
-  bool single = false, eos_single = false;
+  bool listed = false;             // cands come from a position list
   DBuf<Cand> dcand;
   DBuf<CandRes> dres;              // own share only
   DBuf<u8> rle, cls;               // cls (count-byte classes) is kept for the whole share only while that is cheap (keep_cls)
@@ -1103,8 +1133,9 @@ static u32 dec_keep_cls_limit() {
   return DEC_KEEP_CLS;
 }
 
-static void dec_open(Ctx& c, DecSession& S, const u8* d_in_user, size_t n, bool single_block, u64 bitpos, int rank, int world) {
-  S.c = &c; S.n = n; S.single = single_block;
+// positions: decode the blocks at these bit positions (in this order) instead of the stream's chain
+static void dec_open(Ctx& c, DecSession& S, const u8* d_in_user, size_t n, const std::vector<u64>* positions, int rank, int world) {
+  S.c = &c; S.n = n; S.listed = positions != nullptr;
   // padded private copy of the input (aligned word reads past the end must be safe)
   S.din.alloc(c, n + 32);
   CUDA_CHECK(cudaMemsetAsync(S.din.p + (n & ~(size_t)3), 0, (n + 32) - (n & ~(size_t)3), c.stream));
@@ -1125,7 +1156,27 @@ static void dec_open(Ctx& c, DecSession& S, const u8* d_in_user, size_t n, bool 
 
   // ---- 1. candidates ----
   std::vector<Cand>& cands = S.cands;
-  {
+  std::vector<size_t>& blk_idx = S.blk_idx;
+  if (positions) {
+    // lib/Bzip2.js:482-503 once per position: seekBit(pos), then one _get_next_block.  Only the given positions are
+    // tested; the first one without a magic raises "Not bzip data", so nothing behind it is decoded.
+    StageScope ss(c, ST_SCAN);
+    const size_t np = positions->size();
+    DBuf<u64> dpos(c, np ? np : 1);
+    DBuf<Cand> dc(c, np ? np : 1);
+    cands.resize(np);
+    if (np) {
+      CUDA_CHECK(cudaMemcpyAsync(dpos, positions->data(), 8 * np, cudaMemcpyHostToDevice, c.stream));
+      k_magic_at<<<(unsigned)((np + 255) / 256), 256, 0, c.stream>>>(din, n, dpos, np, dc);
+      KLAUNCH(c); KCHECK();
+      CUDA_CHECK(cudaMemcpyAsync(cands.data(), dc, sizeof(Cand) * np, cudaMemcpyDeviceToHost, c.stream));
+    }
+    CUDA_CHECK(cudaStreamSynchronize(c.stream));
+    for (size_t i = 0; i < np; i++) {
+      if (cands[i].type == 0) { cands.resize(i + 1); break; }
+      if (cands[i].type == 1) blk_idx.push_back(i);
+    }
+  } else {
     StageScope ss(c, ST_SCAN);
     // Highly repetitive input compresses to a few dozen bytes per block (and multistream files may hold thousands of
     // tiny members), so the number of magics is not bounded by the usual ~100 KB per block: when the first guess is too
@@ -1149,16 +1200,6 @@ static void dec_open(Ctx& c, DecSession& S, const u8* d_in_user, size_t n, bool 
     if (cnt) CUDA_CHECK(cudaMemcpyAsync(cands.data(), dc, sizeof(Cand) * cnt, cudaMemcpyDeviceToHost, c.stream));
     CUDA_CHECK(cudaStreamSynchronize(c.stream));
     std::sort(cands.begin(), cands.end(), [](const Cand& a, const Cand& b) { return a.pos < b.pos; });
-  }
-  std::vector<size_t>& blk_idx = S.blk_idx;
-  if (single_block) {
-    // lib/Bzip2.js:482-503: seekBit(pos) then one _get_next_block
-    const Cand* hit = nullptr;
-    for (auto& cd : cands) if (cd.pos == bitpos) hit = &cd;
-    if (!hit) throw B2Error{DEC_NOT_BZIP, "Not bzip data"};
-    if (hit->type == 2) { S.eos_single = true; return; }
-    blk_idx.push_back((size_t)(hit - cands.data()));
-  } else {
     for (size_t i = 0; i < cands.size(); i++) if (cands[i].type == 1) blk_idx.push_back(i);
   }
   const size_t nb_all = blk_idx.size();
@@ -1190,7 +1231,7 @@ static void dec_open(Ctx& c, DecSession& S, const u8* d_in_user, size_t n, bool 
         if (need > free_b + spare) {
           char msg[256];
           snprintf(msg, sizeof msg, "stream of %zu blocks needs about %zu MiB of device memory for one call (%zu MiB free): decode it in parts "
-                                    "(Bzip2.table + decompressBlock) or over several GPUs (decompress_file_sharded)", nb, need >> 20, free_b >> 20);
+                                    "(Bzip2.table + decompressBlocks) or over several GPUs (decompress_file_sharded)", nb, need >> 20, free_b >> 20);
           throw B2Error{B2_ERR_CUDA, msg};
         }
       } else cudaGetLastError();
@@ -1311,11 +1352,11 @@ static void dec_open(Ctx& c, DecSession& S, const u8* d_in_user, size_t n, bool 
 
 // fills *first_err (event index, or -1) instead of throwing when `sharded`.  On the host path (no d_out, d_out_alloc
 // given) an error still hands over the expanded buffer, with *out_n = the bytes the reference has written by then.
+// ends (position list): the end offset of every position's bytes that were delivered in full.
 static int dec_finish(Ctx& c, DecSession& S, int multistream, u8* d_out, size_t out_cap, size_t* out_n, std::vector<u64>* tab_pos,
-                      std::vector<u32>* tab_len, u8** d_out_alloc, bool sharded, u64* shard_info) {
+                      std::vector<u32>* tab_len, u8** d_out_alloc, bool sharded, u64* shard_info, std::vector<u64>* ends = nullptr) {
   *out_n = 0;
   if (d_out_alloc) *d_out_alloc = nullptr;
-  if (S.eos_single) return 0;
   const size_t n = S.n;
   const size_t nb_all = S.blk_idx.size();
   std::vector<Cand>& cands = S.cands;
@@ -1356,8 +1397,14 @@ static int dec_finish(Ctx& c, DecSession& S, int multistream, u8* d_out, size_t 
     total_out += r.rawlen;
     return true;
   };
-  if (S.single) {
-    block_event(0);
+  if (S.listed) {
+    // one event per position, in list order; dec_open ended the list at the first position without a magic
+    size_t bi = 0;
+    for (const Cand& cd : cands) {
+      if (cd.type == 0) { events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data", total_out}); break; }
+      if (cd.type == 2) { events.push_back({3, 0, 0, 0, 0, "", total_out}); continue; }
+      if (!block_event(bi++)) break;
+    }
   } else {
     u64 pos = 32;
     u32 stream_crc = 0;
@@ -1466,10 +1513,11 @@ static int dec_finish(Ctx& c, DecSession& S, int multistream, u8* d_out, size_t 
         S.err_event = (int)ei; err_code = DEC_DATA_ERROR; err_msg = "Data error: Bad stream CRC (got " + hexs(ev.a) + " expected " + hexs(ev.b) + ")";
         prefix = ev.off;
       }
-    } else {
+    } else if (ev.kind == 2) {
       S.err_event = (int)ei; err_code = ev.code; err_msg = ev.msg;
       prefix = ev.off;
     }
+    if (ends && S.err_event < 0) ends->push_back(ev.kind == 0 ? ev.off + hres[ev.cand].rawlen : ev.off);
   }
   if (shard_info) { shard_info[0] = my_off; shard_info[1] = my_len; shard_info[2] = total_out; shard_info[3] = (u64)(long long)S.err_event; shard_info[4] = (u64)(long long)err_code; }
   if (S.err_event >= 0) {
@@ -1483,13 +1531,16 @@ static int dec_finish(Ctx& c, DecSession& S, int multistream, u8* d_out, size_t 
   return 0;
 }
 
-int bzip2_decompress_device(Ctx& c, const u8* d_in_user, size_t n, int multistream, u8* d_out, size_t out_cap, size_t* out_n, bool single_block,
-                            u64 bitpos, std::vector<u64>* tab_pos, std::vector<u32>* tab_len, u8** d_out_alloc) {
+// positions: decode the blocks at these bit positions, back to back in list order (ends: see dec_finish), instead of the
+// stream's chain
+int bzip2_decompress_device(Ctx& c, const u8* d_in_user, size_t n, int multistream, u8* d_out, size_t out_cap, size_t* out_n,
+                            const std::vector<u64>* positions, std::vector<u64>* ends, std::vector<u64>* tab_pos, std::vector<u32>* tab_len,
+                            u8** d_out_alloc) {
   *out_n = 0;
   if (d_out_alloc) *d_out_alloc = nullptr;
   DecSession S;
-  dec_open(c, S, d_in_user, n, single_block, bitpos, 0, 1);
-  return dec_finish(c, S, multistream, d_out, out_cap, out_n, tab_pos, tab_len, d_out_alloc, false, nullptr);
+  dec_open(c, S, d_in_user, n, positions, 0, 1);
+  return dec_finish(c, S, multistream, d_out, out_cap, out_n, tab_pos, tab_len, d_out_alloc, false, nullptr, ends);
 }
 
 // ---- sharded decode (SURVEY.md section 8e): open on every rank, exchange results, finish ------------
@@ -1497,7 +1548,7 @@ static DecSession* g_shard = nullptr;
 void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* info) {
   delete g_shard;
   g_shard = new DecSession();
-  dec_open(c, *g_shard, d_in, n, false, 0, rank, world);
+  dec_open(c, *g_shard, d_in, n, nullptr, rank, world);
   info[0] = g_shard->blk_idx.size(); info[1] = g_shard->lo; info[2] = g_shard->hi;
 }
 void dec_shard_export(u64* buf) {

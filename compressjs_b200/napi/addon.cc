@@ -7,8 +7,10 @@
 
 static void fin(napi_env, void* data, void*) { b2_free(data); }
 
-// `prop` / `val`: what a failed decode had delivered (a Buffer or the table rows), attached to the error for the shim
-static napi_value fail(napi_env env, int rc, const char* prop = nullptr, napi_value val = nullptr) {
+// `prop` / `val`, `prop2` / `val2`: what a failed decode had delivered (a Buffer, the table rows, end offsets), attached
+// to the error for the shim
+static napi_value fail(napi_env env, int rc, const char* prop = nullptr, napi_value val = nullptr, const char* prop2 = nullptr,
+                       napi_value val2 = nullptr) {
   napi_value msg, err, code;
   napi_create_string_utf8(env, b2_last_error(), NAPI_AUTO_LENGTH, &msg);
   if (rc == B2_ERR_BAD_LEVEL) napi_create_error(env, nullptr, msg, &err);        // `new Error(...)` lib/Bzip2.js:888-890
@@ -16,6 +18,7 @@ static napi_value fail(napi_env env, int rc, const char* prop = nullptr, napi_va
   napi_create_int32(env, rc, &code);
   napi_set_named_property(env, err, "errorCode", code);
   if (prop && val) napi_set_named_property(env, err, prop, val);
+  if (prop2 && val2) napi_set_named_property(env, err, prop2, val2);
   napi_throw(env, err);
   return nullptr;
 }
@@ -68,6 +71,37 @@ static napi_value DecompressBlock(napi_env env, napi_callback_info info) {
   uint8_t* out = nullptr; size_t out_n = 0;
   int rc = b2_bzip2_decompress_block_partial(in, n, (uint64_t)pos, &out, &out_n);
   return decoded(env, rc, out, out_n);
+}
+// decompressBlocks(buffer, positions /* Float64Array */) -> [Buffer, [end offset of each position's bytes]]
+// (decompressBlock at every position, one GPU pass); on a decode error the bytes delivered before it go with the error as
+// .partial and the end offsets of the positions delivered in full as .ends
+static napi_value DecompressBlocks(napi_env env, napi_callback_info info) {
+  size_t argc = 2; napi_value argv[2];
+  napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr);
+  const uint8_t* in; size_t n;
+  napi_typedarray_type ty; size_t count = 0; void* pv = nullptr; napi_value ab; size_t off;
+  if (!buf_arg(env, argv[0], &in, &n)) return fail(env, B2_ERR_BAD_ARG);
+  if (argc < 2 || napi_get_typedarray_info(env, argv[1], &ty, &count, &pv, &ab, &off) != napi_ok || ty != napi_float64_array)
+    return fail(env, B2_ERR_BAD_ARG);
+  uint64_t* pos = new uint64_t[count + 1];
+  for (size_t i = 0; i < count; i++) pos[i] = (uint64_t)((const double*)pv)[i];
+  uint8_t* out = nullptr; size_t out_n = 0; uint64_t* ends = nullptr; size_t done = 0;
+  int rc = b2_bzip2_decompress_blocks(in, n, pos, count, &out, &out_n, &ends, &done);
+  delete[] pos;
+  if (rc && !out) return fail(env, rc);
+  napi_value buf, e;
+  napi_create_external_buffer(env, out_n, out, fin, nullptr, &buf);
+  napi_create_array_with_length(env, done, &e);
+  for (size_t i = 0; i < done; i++) {
+    napi_value v;
+    napi_create_double(env, (double)ends[i], &v);
+    napi_set_element(env, e, (uint32_t)i, v);
+  }
+  b2_free(ends);
+  if (rc) return fail(env, rc, "partial", buf, "ends", e);
+  napi_value r; napi_create_array_with_length(env, 2, &r);
+  napi_set_element(env, r, 0, buf); napi_set_element(env, r, 1, e);
+  return r;
 }
 // integer argument that must be a JS number; false (and B2_ERR_BAD_ARG thrown by the caller) otherwise
 static bool int_arg(napi_env env, napi_value v, int32_t* out) {
@@ -184,6 +218,7 @@ static napi_value Init(napi_env env, napi_value exports) {
       {"compressFile", nullptr, CompressFile, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"decompressFile", nullptr, DecompressFile, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"decompressBlock", nullptr, DecompressBlock, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"decompressBlocks", nullptr, DecompressBlocks, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"table", nullptr, Table, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"bwtransform2", nullptr, Bwtransform2, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"suffixsort", nullptr, Suffixsort, nullptr, nullptr, nullptr, napi_default, nullptr},

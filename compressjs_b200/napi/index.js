@@ -56,6 +56,24 @@ Bzip2.decompressBlock = function(input, pos, output) {
   var data = drain(input);
   return decode(output, function() { return native.decompressBlock(data, pos); });
 };
+// GPU extension: decompressBlock at every position, in one pass.  No output: an array of Uint8Arrays, one per position;
+// a writeByte stream receives every position's bytes in order (on an error, what the per-position loop would have
+// written) and is returned.  A size or a buffer has no meaning for several blocks.
+Bzip2.decompressBlocks = function(input, positions, output) {
+  var stream = !!output && typeof output === 'object' && typeof output.writeByte === 'function';
+  if (output !== undefined && output !== null && !stream) {
+    throw new TypeError('decompressBlocks writes to a stream or returns an array');
+  }
+  var data = drain(input), r;
+  try { r = native.decompressBlocks(data, Float64Array.from(positions)); } catch (e) {
+    if (stream && e.partial) { deliver(output, e.partial, true); }
+    throw e;
+  }
+  if (stream) { return deliver(output, r[0]); }
+  var blocks = [], s = 0;
+  r[1].forEach(function(e) { blocks.push(new Uint8Array(r[0].subarray(s, e))); s = e; });
+  return blocks;
+};
 Bzip2.table = function(input, callback, multistream) {
   var rows;
   try { rows = native.table(drain(input), !!multistream); } catch (e) {

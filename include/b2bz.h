@@ -66,6 +66,19 @@ int b2_bzip2_table(const uint8_t* in, size_t n, int multistream, uint64_t** bitp
 int b2_bzip2_decompress_partial(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n);
 int b2_bzip2_decompress_block_partial(const uint8_t* in, size_t n, uint64_t bitpos, uint8_t** out, size_t* out_n);
 int b2_bzip2_table_partial(const uint8_t* in, size_t n, int multistream, uint64_t** bitpos, uint32_t** sizes, size_t* count);
+/* GPU extension: Bzip2.decompressBlock at every position of a list, in one pass (the input is uploaded once and only
+ * the given positions are tested for a magic).  The result equals b2_bzip2_decompress_block_partial called once per
+ * position, in list order, until the first error: positions may repeat and come in any order, an end-of-stream magic
+ * gives 0 bytes, a position without a magic fails with -2 "Not bzip data", and every block is held to the dbufSize of
+ * the file's first header.  *out holds the positions' bytes back to back; ends[k] is the end offset of position k's.
+ *   - success: 0, *done == count, ends has count entries;
+ *   - decode error (-2 / -5 / -7): the first failing position's code and message; *done = the positions delivered in
+ *     full before it, ends has *done entries, and *out_n also counts the failing position's own bytes when only its CRC
+ *     failed (b2_bzip2_decompress_block_partial);
+ *   - count == 0: 0 and nothing decoded, whatever the input holds;  count > 0 with bitpos == NULL: B2_ERR_BAD_ARG.
+ * *out and *ends are released with b2_free(); on any other error nothing is returned. */
+int b2_bzip2_decompress_blocks(const uint8_t* in, size_t n, const uint64_t* bitpos, size_t count, uint8_t** out, size_t* out_n,
+                               uint64_t** ends, size_t* done);
 
 /* ---- compressjs.BWT (lib/BWT.js) ------------------------------------------------- */
 /* BWT.bwtransform2(T, U, n, 256) -> pidx  (cyclic)    lib/BWT.js:372-417
