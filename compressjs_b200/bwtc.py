@@ -17,22 +17,36 @@ def _take(L, p, n):
     return arr
 
 
+def _level(props):
+    """props: block size in units of 100 000 bytes, 1..9; anything else means 9 (lib/BWTC.js:16-19)."""
+    if isinstance(props, (int, float)) and not isinstance(props, bool) and 1 <= props <= 9:
+        return int(props)
+    return 9
+
+
+def _compress(entry, input, props):
+    L = _native.lib()
+    data = coerce_input(input)
+    out, n = C.POINTER(C.c_uint8)(), C.c_size_t()
+    rc = getattr(L, entry)(data.ctypes.data if data.size else None, data.size, _level(props), C.byref(out), C.byref(n))
+    if rc:
+        raise RuntimeError("libb2bz: %s (code %d)" % (_native.last_error(), rc))
+    return _take(L, out, n)
+
+
+def _compress_unsized(input, props=None):
+    """BWTC.compressFile of an input stream without a size (lib/Util.js:119-124): the header says "size unknown".  The
+    command line writes this for a pipe or an empty file, as bin/compressjs does.  Returns bytes."""
+    return _compress("b2_bwtc_compress_unsized", input, props).tobytes()
+
+
 class BWTC:
     MAGIC = "bwtc"  # lib/BWTC.js:11
 
     @staticmethod
     def compressFile(input, output=None, props=None):
         """lib/BWTC.js:12-139.  props: block size in units of 100 000 bytes, 1..9; anything else means 9 (:16-19)."""
-        L = _native.lib()
-        data = coerce_input(input)
-        level = 9
-        if isinstance(props, (int, float)) and not isinstance(props, bool) and 1 <= props <= 9:
-            level = int(props)
-        out, n = C.POINTER(C.c_uint8)(), C.c_size_t()
-        rc = L.b2_bwtc_compress(data.ctypes.data if data.size else None, data.size, level, C.byref(out), C.byref(n))
-        if rc:
-            raise RuntimeError("libb2bz: %s (code %d)" % (_native.last_error(), rc))
-        return deliver_output(output, _take(L, out, n))
+        return deliver_output(output, _compress("b2_bwtc_compress", input, props))
 
     @staticmethod
     def decompressFile(input, output=None):

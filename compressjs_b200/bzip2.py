@@ -47,16 +47,34 @@ def _take(L, p, n):
     return arr
 
 
-def _decode(output, call):
-    """Run a b2_bzip2_decompress*_partial call.  On a decode error the bytes the reference has written by the time it
-    throws (lib/Bzip2.js:405-448 writes as it decodes) go to `output` first, then the error is raised."""
+def _partial(call):
+    """Run a b2_bzip2_decompress*_partial call: (decoded bytes, None), or on a decode error (the bytes the reference has
+    written by the time it throws -- lib/Bzip2.js:405-448 writes as it decodes --, the error)."""
     L = _native.lib()
     out, n = C.POINTER(C.c_uint8)(), C.c_size_t()
     rc = call(C.byref(out), C.byref(n))
     if rc and not out:
         _raise(rc)
     err = _error(rc) if rc else None   # before `output` can call into the library again
-    data = _take(L, out, n)
+    return _take(L, out, n), err
+
+
+def _file(input, multistream=False):
+    L = _native.lib()
+    data = coerce_input(input)
+    return _partial(lambda out, n: L.b2_bzip2_decompress_partial(
+        data.ctypes.data if data.size else None, data.size, int(bool(multistream)), out, n))
+
+
+def _block(input, pos):
+    L = _native.lib()
+    data = coerce_input(input)
+    return _partial(lambda out, n: L.b2_bzip2_decompress_block_partial(
+        data.ctypes.data if data.size else None, data.size, int(pos), out, n))
+
+
+def _deliver(output, data, err):
+    """On a decode error `output` gets the bytes decoded before it first, then the error is raised."""
     if err is not None:
         deliver_output(output, data, partial=True)
         raise err
@@ -85,19 +103,13 @@ class Bzip2:
     @staticmethod
     def decompressFile(input, output=None, multistream=False):
         """lib/Bzip2.js:454-481 (Bunzip.decode).  On a decode error the output receives the bytes decoded before it."""
-        L = _native.lib()
-        data = coerce_input(input)
-        return _decode(output, lambda out, n: L.b2_bzip2_decompress_partial(
-            data.ctypes.data if data.size else None, data.size, int(bool(multistream)), out, n))
+        return _deliver(output, *_file(input, multistream))
 
     @staticmethod
     def decompressBlock(input, pos, output=None):
         """lib/Bzip2.js:482-503 (Bunzip.decodeBlock): decode the single block whose magic starts at bit `pos`.  A block
         whose only failure is its CRC delivers its bytes before the error is raised."""
-        L = _native.lib()
-        data = coerce_input(input)
-        return _decode(output, lambda out, n: L.b2_bzip2_decompress_block_partial(
-            data.ctypes.data if data.size else None, data.size, int(pos), out, n))
+        return _deliver(output, *_block(input, pos))
 
     @staticmethod
     def decompressBlocks(input, positions, output=None):

@@ -1,0 +1,228 @@
+"""The compressjs command line (bin/compressjs) for the compressors this package has: ``python -m compressjs_b200``.
+
+    python -m compressjs_b200 -z -t bzip2 -9 < file > file.bz2
+    python -m compressjs_b200 -d -t bzip2 file.bz2 file
+
+Options, rules and messages are those of bin/compressjs:1-58.  What differs is the choice of compressor: -t takes
+``bzip2`` (or ``bzip``) and ``bwtc``; the reference's other compressors, including its default lzp3 (what an absent -t
+means), fail with a message instead of writing something the user did not ask for.
+
+As in the reference, BWTC writes the input's size into its header when ``fstat`` of the input gives a non-zero size
+(a regular file), and "size unknown" otherwise (a pipe, an empty file): bin/compressjs:60-65 with lib/Util.js:119-124.
+The reference writes its output through a 4096-byte buffer that is flushed only when the next byte arrives, and
+nothing flushes it when a decode throws (bin/compressjs:103-115): so on a decode error the output holds the bytes
+decoded before the error, cut down to a multiple of 4096.
+
+Usage errors are found before the GPU library is loaded, so they work on a machine without a GPU.
+"""
+import math
+import mmap
+import os
+import stat
+import sys
+
+VERSION = "0.0.1"  # main.js:5
+
+HELP = """
+  Usage: python -m compressjs_b200 -d|-z [infile] [outfile]
+
+  Options:
+
+    -h, --help        output usage information
+    -V, --version     output the version number
+    -d, --decompress  Decompress stdin to stdout
+    -z, --compress    Compress stdin to stdout
+    -b, --block <n>   Extract a single block, starting at <n> bits.
+    -t <compressor>   Select compressor type (bzip2 or bwtc)
+    -1                Fastest/largest compression
+    -2
+    -3
+    -4
+    -5
+    -6
+    -7
+    -8
+    -9                Slowest/smallest compression
+
+  If <infile> is omitted, reads from stdin.
+  If <outfile> is omitted, writes to stdout.
+"""
+
+# the compressors of bin/compressjs:133-156 that this package does not have
+OTHER_COMPRESSORS = ("defsum", "fenwick", "mtf", "context1", "no", "huff", "huffman", "dmc", "lzjb", "lzjbr", "lzp3",
+                     "ppm", "simple")
+FLUSH = 4096  # bin/compressjs:103-115
+
+
+class UsageError(Exception):
+    pass
+
+
+def _number(s):
+    """JavaScript's unary + on an option string (NaN for anything that is not a number)."""
+    s = s.strip()
+    if not s:
+        return 0.0
+    try:
+        return float(int(s, 0)) if s[:2].lower() in ("0x", "0o", "0b") else float(s)
+    except ValueError:
+        return math.nan
+
+
+def parse(argv):
+    """Returns a dict of the options, or raises UsageError.  --help and --version are returned as 'help'/'version'."""
+    opts = {"decompress": False, "compress": False, "block": "-1", "T": None, "levels": set(), "args": []}
+    i = 0
+    only_args = False
+    while i < len(argv):
+        a = argv[i]
+        i += 1
+        if only_args or a == "-" or not a.startswith("-"):
+            opts["args"].append(a)
+            continue
+        if a == "--":
+            only_args = True
+            continue
+        if a.startswith("--"):
+            name, eq, val = a[2:].partition("=")
+            if name in ("help", "version"):
+                return {name: True}
+            if name in ("decompress", "compress") and not eq:
+                opts[name] = True
+            elif name == "block":
+                if not eq:
+                    if i >= len(argv):
+                        raise UsageError("error: option `-b, --block <n>' argument missing")
+                    val = argv[i]
+                    i += 1
+                opts["block"] = val
+            else:
+                raise UsageError("error: unknown option `%s'" % a)
+            continue
+        # short options, possibly grouped (-dz, -9z, -tbzip2)
+        j = 1
+        while j < len(a):
+            f = a[j]
+            j += 1
+            if f == "h":
+                return {"help": True}
+            if f == "V":
+                return {"version": True}
+            if f == "d":
+                opts["decompress"] = True
+            elif f == "z":
+                opts["compress"] = True
+            elif f.isdigit() and f != "0":
+                opts["levels"].add(int(f))
+            elif f in ("b", "t"):
+                val = a[j:]
+                if not val:
+                    if i >= len(argv):
+                        raise UsageError("error: option `%s' argument missing" % ("-b, --block <n>" if f == "b" else "-t <compressor>"))
+                    val = argv[i]
+                    i += 1
+                opts["block" if f == "b" else "T"] = val
+                break
+            else:
+                raise UsageError("error: unknown option `-%s'" % f)
+    return opts
+
+
+def check(opts):
+    """bin/compressjs:32-58: returns (decompress, level, block) or raises UsageError with the reference's message."""
+    decompress = opts["decompress"]
+    compress = opts["compress"] or not decompress
+    if decompress and compress:
+        raise UsageError("Must specify either -d or -z.")
+    block = _number(opts["block"])
+    if compress and block >= 0:
+        raise UsageError("--block can only be used with decompression")
+    level = None
+    for l in range(1, 10):
+        if l in opts["levels"]:
+            if level:
+                raise UsageError("Can't specify both -%d and -%d" % (level, l))
+            level = l
+    if level and decompress:
+        raise UsageError("Compression level has no effect when decompressing.")
+    return decompress, level or 7, block
+
+
+def compressor(name):
+    """bin/compressjs:131-158, for the compressors this package has: 'bzip2' or 'bwtc', else UsageError."""
+    key = (name if name is not None else "lzp3").lower()
+    if key in ("bzip", "bzip2"):
+        return "bzip2"
+    if key == "bwtc":
+        return "bwtc"
+    if key in OTHER_COMPRESSORS:
+        raise UsageError("Compressor %s is not available in compressjs_b200: use -t bzip2 or -t bwtc" % key)
+    raise UsageError("Unknown compressor: %s" % name)
+
+
+def read_input(fd):
+    """(the input's bytes, the size fstat gives): a regular file is mapped, anything else read to its end."""
+    st = os.fstat(fd)
+    if stat.S_ISREG(st.st_mode) and st.st_size > 0:
+        return memoryview(mmap.mmap(fd, 0, access=mmap.ACCESS_READ)), st.st_size
+    chunks = []
+    while True:
+        b = os.read(fd, 1 << 20)
+        if not b:
+            break
+        chunks.append(b)
+    return b"".join(chunks), st.st_size
+
+
+def run(kind, decompress, level, block, data, size):
+    """(output bytes, error or None).  On a decode error the bytes are those decoded before it."""
+    from . import bwtc, bzip2
+    from .bwtc import BWTC
+    from .bzip2 import Bzip2
+    if not decompress:
+        if kind == "bzip2":
+            return Bzip2.compressFile(data, None, level), None
+        if size > 0:
+            return BWTC.compressFile(data, None, level), None
+        return bwtc._compress_unsized(data, level), None
+    if kind == "bzip2":
+        # Bzip2.decompressBlock / decompressFile (without multistream, as bin/compressjs:160-164 calls it)
+        out, err = bzip2._block(data, int(block)) if block >= 0 else bzip2._file(data)
+        return out.tobytes(), err
+    if block >= 0:
+        raise UsageError("--block needs -t bzip2: compressjs has no BWTC.decompressBlock")
+    try:
+        return BWTC.decompressFile(data), None
+    except (RuntimeError, ValueError) as e:
+        return b"", e
+
+
+def main(argv=None):
+    argv = sys.argv[1:] if argv is None else argv
+    try:
+        opts = parse(argv)
+        if opts.get("help"):
+            sys.stdout.write(HELP + "\n")
+            return 0
+        if opts.get("version"):
+            sys.stdout.write(VERSION + "\n")
+            return 0
+        decompress, level, block = check(opts)
+        args = opts["args"]
+        in_fd = os.open(args[0], os.O_RDONLY) if len(args) > 0 else sys.stdin.fileno()
+        out = open(args[1], "wb") if len(args) > 1 else sys.stdout.buffer
+        kind = compressor(opts["T"])
+        data, size = read_input(in_fd)
+        result, err = run(kind, decompress, level, block, data, size)
+        if err is not None:
+            k = len(result)
+            out.write(result[:FLUSH * ((k - 1) // FLUSH)] if k else b"")
+            out.flush()
+            sys.stderr.write("%s\n" % err)
+            return 1
+        out.write(result)
+        out.flush()
+        return 0
+    except Exception as e:   # usage errors, files that cannot be opened, the library's own errors (no GPU, ...)
+        sys.stderr.write("%s\n" % e)
+        return 1

@@ -20,10 +20,11 @@ void bzip2_compress_device(Ctx& c, const u8* d_in, size_t n, int level, u8* d_ou
 void bitshift_device(Ctx& c, const void* src, u64 nbits, int phase, void* dst);
 void bzip2_share_summary(Ctx& c, const u8* d_in, size_t n, u64* out);
 void bzip2_plan_share(Ctx& c, const u8* d_buf, size_t n, int level, u64 st0, u64 W0, size_t first, size_t count, u64* info);
-void bwt_inverse_sentinel(Ctx& c, const u8* d_L, u32 n, u32 pidx, u8* d_out);
+void bwt_inverse_sentinel_batch(Ctx& c, const u8* d_L, const u32* h_n, const u32* h_pidx, u32 nb, u8* d_out);
 size_t bwtc_bound(size_t n);
-void bwtc_compress_device(Ctx& c, const u8* d_in, size_t n, int level, u8* d_out, size_t out_cap, size_t* out_n);
-void bwtc_decompress_device(Ctx& c, const u8* d_in, size_t n, const u8* h_head, size_t head_n, u8* d_out, size_t out_cap, size_t* out_n);
+void bwtc_compress_device(Ctx& c, const u8* d_in, size_t n, int level, u64 file_size, u8* d_out, size_t out_cap, size_t* out_n);
+u64 bwtc_parse_header(const u8* in, size_t n, size_t* pos);
+void bwtc_decompress(Ctx& c, const u8* d_in, size_t n, size_t pos, u64 fs, void* (*alloc_host)(size_t), u8** h_out, size_t* out_n);
 void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, int level, u8* d_in, size_t win, u8* d_out, size_t out_cap, u8* h_out,
                          size_t h_out_cap, size_t* out_n, bool pinned_in);
 void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* info);
@@ -353,9 +354,10 @@ int b2_bwt_inverse(const uint8_t* L, uint8_t* out, int32_t n, int32_t pidx) {
     c.reset_call();
     {
       StageScope tot(c, ST_TOTAL);
-      DBuf<u8> dL(c, n), dO(c, n);
+      DBuf<u8> dL(c, SEG_SIZE), dO(c, n);
       CUDA_CHECK(cudaMemcpyAsync(dL.p, L, n, cudaMemcpyHostToDevice, c.stream));
-      bwt_inverse_sentinel(c, dL, (u32)n, (u32)pidx, dO);
+      const u32 hn = (u32)n, hp = (u32)pidx;
+      bwt_inverse_sentinel_batch(c, dL, &hn, &hp, 1, dO);
       CUDA_CHECK(cudaMemcpyAsync(out, dO.p, n, cudaMemcpyDeviceToHost, c.stream));
     }
     c.sync();
@@ -365,7 +367,8 @@ int b2_bwt_inverse(const uint8_t* L, uint8_t* out, int32_t n, int32_t pidx) {
 }
 
 // ---- BWTC container (experimental, see bwtc.cu) ----------------------------------------------
-int b2_bwtc_compress(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n) {
+// file_size: the header's size field, n or (u64)-1 for a stream without a size (lib/Util.js:118-124)
+static int bwtc_compress_common(const uint8_t* in, size_t n, int level, u64 file_size, uint8_t** out, size_t* out_n) {
   return guarded([&]() {
     Ctx& c = ctx_locked();
     c.reset_call();
@@ -376,7 +379,7 @@ int b2_bwtc_compress(const uint8_t* in, size_t n, int level, uint8_t** out, size
       StageScope tot(c, ST_TOTAL);
       DBuf<u8> din(c, n ? n : 1), dout(c, cap);
       if (n) CUDA_CHECK(cudaMemcpyAsync(din.p, in, n, cudaMemcpyHostToDevice, c.stream));
-      bwtc_compress_device(c, din, n, level, dout, cap, &produced);
+      bwtc_compress_device(c, din, n, level, file_size, dout, cap, &produced);
       host = pinned_alloc(produced);
       CUDA_CHECK(cudaMemcpyAsync(host, dout.p, produced, cudaMemcpyDeviceToHost, c.stream));
     }
@@ -387,35 +390,34 @@ int b2_bwtc_compress(const uint8_t* in, size_t n, int level, uint8_t** out, size
     return 0;
   });
 }
+int b2_bwtc_compress(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n) {
+  return bwtc_compress_common(in, n, level, n, out, out_n);
+}
+int b2_bwtc_compress_unsized(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n) {
+  return bwtc_compress_common(in, n, level, ~(u64)0, out, out_n);
+}
 int b2_bwtc_decompress(const uint8_t* in, size_t n, uint8_t** out, size_t* out_n) {
   return guarded([&]() {
     Ctx& c = ctx_locked();
     c.reset_call();
     size_t produced = 0;
-    void* host = nullptr;
-    {
+    u8* host = nullptr;   // pinned (size known) or malloc'ed (size unknown): b2_free releases either
+    try {
       StageScope tot(c, ST_TOTAL);
-      // the decoded size is in the header: parse it before any device work
-      size_t pos = 4; uint64_t fs = 0;
-      if (n < 5 || memcmp(in, "bwtc", 4)) throw B2Error{B2_ERR_BAD_MAGIC, "Bad magic"};
-      for (;;) {
-        if (pos >= n || pos > 4 + 9) throw B2Error{B2_ERR_DATA_ERROR, "truncated or oversized BWTC header"};
-        const uint32_t ch = in[pos++];
-        if (ch & 0x80) { fs += ch & 0x7F; break; }
-        fs = (fs + ch) * 128;
-      }
-      if (fs == 0) throw B2Error{B2_ERR_BAD_ARG, "BWTC streams of unknown size are not supported"};
-      const size_t size = (size_t)(fs - 1);
-      DBuf<u8> din(c, n), dout(c, size ? size : 1);
+      size_t pos = 0;
+      const u64 fs = bwtc_parse_header(in, n, &pos);   // before any device work
+      DBuf<u8> din(c, n);
       CUDA_CHECK(cudaMemcpyAsync(din.p, in, n, cudaMemcpyHostToDevice, c.stream));
-      bwtc_decompress_device(c, din, n, in, std::min<size_t>(n, 16), dout, size, &produced);
-      host = pinned_alloc(produced);
-      if (produced) CUDA_CHECK(cudaMemcpyAsync(host, dout.p, produced, cudaMemcpyDeviceToHost, c.stream));
+      bwtc_decompress(c, din, n, pos, fs, pinned_alloc, &host, &produced);
+    } catch (...) {
+      if (g_pinned_live.count(host)) pinned_release(host); else free(host);
+      throw;
     }
+    if (!host && !(host = (u8*)malloc(1))) throw B2Error{B2_ERR_CUDA, "out of host memory"};   // an empty stream of unknown size
     c.sync();
     c.collect();
     c.stats.raw_bytes = produced; c.stats.comp_bytes = n;
-    *out = (uint8_t*)host; *out_n = produced;
+    *out = host; *out_n = produced;
     return 0;
   });
 }

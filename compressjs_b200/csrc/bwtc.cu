@@ -11,14 +11,17 @@
 // bzip2 merely appends an end-of-block symbol).  The model is a serial chain per block (k_bwtc_model: one thread per
 // block, blocks in parallel), the coder a serial chain per file (k_bwtc_code: one thread; its `range` recurrence
 // needs an integer division per symbol and nothing shortens it).  Decode cannot even split model and coder:
-// k_bwtc_decode is one thread for the whole stream, followed by the inverse sentinel BWT per block (decode.cu).
+// k_bwtc_decode is one thread that decodes a batch of blocks at a time, followed by one batched inverse sentinel BWT
+// (decode.cu), so device memory is bounded by the batch.
 #include <algorithm>
+#include <cstdlib>
+#include <cstring>
 #include <vector>
 #include "enc.h"
 #include "bwtc_core.cuh"
 
 void bwt_forward_batch(Ctx& c, const u8* d_T, u8* d_U, const u32* d_n, const u32* h_n, u32 nblk, u32* d_pidx, bool sentinel, u32* d_sa_out, u32* d_hist_out = nullptr);
-void bwt_inverse_sentinel(Ctx& c, const u8* d_L, u32 n, u32 pidx, u8* d_out);
+void bwt_inverse_sentinel_batch(Ctx& c, const u8* d_L, const u32* h_n, const u32* h_pidx, u32 nb, u8* d_out);
 
 struct BwtcState {
   bc_enc rc;
@@ -232,16 +235,16 @@ __global__ void k_bwtc_finish(BwtcState* st) {
 
 size_t bwtc_bound(size_t n) { return n + n / 8 + (n / 100000 + 2) * 1024 + 64; }
 
-// BWTC.compressFile on device buffers; the size of the input is written into the header (Util.js:118-134: a buffer
-// input has a known size).  out_cap >= bwtc_bound(n).
-void bwtc_compress_device(Ctx& c, const u8* d_in, size_t n, int level, u8* d_out, size_t out_cap, size_t* out_n) {
+// BWTC.compressFile on device buffers.  file_size is the size field of the header (Util.js:118-124): n for an input of
+// known size, or (u64)-1 (a single size byte 0x80) for a stream without a size.  out_cap >= bwtc_bound(n).
+void bwtc_compress_device(Ctx& c, const u8* d_in, size_t n, int level, u64 file_size, u8* d_out, size_t out_cap, size_t* out_n) {
   if (level < 1 || level > 9) level = 9;                      // lib/BWTC.js:16-19
   const u32 blockSize = (u32)level * 100000u;
   const int fast = level <= 5;                                // :22
   if (out_cap < 32) throw B2Error{B2_ERR_BAD_ARG, "output buffer too small"};
   u8 hdr[24];
   u32 finalByte = 0;
-  const u32 hlen = bc_file_header(hdr, n, &finalByte);
+  const u32 hlen = bc_file_header(hdr, file_size, &finalByte);
   c.to_device(d_out, hdr, hlen);
   DBuf<BwtcState> st(c, 1);
   k_bwtc_start<<<1, 1, 0, c.stream>>>(st, d_out + hlen, out_cap - hlen, finalByte, (u32)level);
@@ -309,95 +312,150 @@ void bwtc_compress_device(Ctx& c, const u8* d_in, size_t n, int level, u8* d_out
 }
 
 // ---- decode ---------------------------------------------------------------------------------------------------
-struct BwtcDecResult {
-  int status;       // 0 ok, negative: the stream is nonsense
-  u32 nblocks;
+// The range decoder and the level are all that carries from one block to the next (the block models start afresh in
+// bc_decode_block, the length model is stateless), so the decode stops after a batch of blocks and resumes from here.
+#define BD_MORE 0      // more blocks may follow
+#define BD_END 1       // "no more blocks" has been read
+#define BD_CORRUPT (-1)
+#define BD_SIZE (-2)   // the blocks add up to more than the size field
+struct BwtcDecState {
+  bc_dec rc;
+  u64 total;        // bytes in the blocks decoded so far
+  u64 limit;        // the size field's size; ~0 when the stream has no size
+  u64 maxblocks;
   u32 level;
-  u32 pad;
+  u32 nblocks;      // blocks decoded so far
+  u32 nb;           // blocks decoded by the last launch
+  int status;       // BD_*
 };
 
-// one thread: the whole stream down to the L columns (inverse MTF folded in), block b at slot b << 20
-__global__ void k_bwtc_decode(const u8* __restrict__ in, u64 n, u64 pos, u32 maxblocks, u8* __restrict__ L, u32* __restrict__ lengths,
-                              u32* __restrict__ pidx1, BwtcDecResult* res) {
+__global__ void k_bwtc_dec_start(BwtcDecState* st, const u8* __restrict__ in, u64 n, u64 pos, u64 limit, u64 maxblocks) {
   if (threadIdx.x || blockIdx.x) return;
-  bc_dec rc;
-  bc_dec_start(&rc, in, n, pos);                                // lib/BWTC.js:142-143
-  const u32 level = bc_dec_cul(&rc, 256);                       // decoder.decodeByte(), :144
-  bc_dec_update(&rc, 1, level, 256);
-  res->level = level;
-  res->nblocks = 0;
-  if (level < 1 || level > 9) { res->status = B2_ERR_DATA_ERROR; return; }
+  bc_dec_start(&st->rc, in, n, pos);                            // lib/BWTC.js:142-143
+  st->level = bc_dec_cul(&st->rc, 256);                         // decoder.decodeByte(), :144
+  bc_dec_update(&st->rc, 1, st->level, 256);
+  st->total = 0; st->limit = limit; st->maxblocks = maxblocks;
+  st->nblocks = 0; st->nb = 0;
+  st->status = st->level >= 1 && st->level <= 9 ? BD_MORE : BD_CORRUPT;
+}
+
+// one thread: up to B more blocks down to their L columns (inverse MTF folded in), block b of the launch at slot b << 20
+__global__ void k_bwtc_decode(BwtcDecState* st, u32 B, u8* __restrict__ L, u32* __restrict__ lengths, u32* __restrict__ pidx1) {
+  if (threadIdx.x || blockIdx.x) return;
+  st->nb = 0;
+  if (st->status != BD_MORE) return;
+  bc_dec rc = st->rc;
+  const u32 level = st->level;
+  const bool unsized = st->limit == ~0ull;
+  u64 total = st->total;
   bc_model model;
   u32 nb = 0;
-  int r = 0;
-  for (;;) {
-    if (nb >= maxblocks) {
+  int status = BD_MORE;
+  while (nb < B) {
+    if (st->nblocks + nb >= st->maxblocks) {
       // only "no more blocks" may follow
-      const u32 ind = bc_dec_cul(&rc, 3);
-      r = ind == 2 ? 1 : B2_ERR_DATA_ERROR;
+      status = bc_dec_cul(&rc, 3) == 2 ? BD_END : BD_CORRUPT;
       break;
     }
     u32 len = 0, p1 = 0;
-    r = bc_decode_block(&rc, &model, level * 100000u, level <= 5, L + ((size_t)nb << SEG_SHIFT), &len, &p1);
-    if (r) break;
+    const int r = bc_decode_block(&rc, &model, level * 100000u, level <= 5, L + ((size_t)nb << SEG_SHIFT), &len, &p1);
+    if (r) { status = r == 1 ? BD_END : BD_CORRUPT; break; }
+    if (total + len > st->limit) { status = BD_SIZE; break; }
+    total += len;
     lengths[nb] = len; pidx1[nb] = p1;
     nb++;
   }
-  res->nblocks = nb;
-  res->status = r == 1 ? 0 : B2_ERR_DATA_ERROR;
+  // Without a size, the end of the input is the only bound.  A whole stream is never read past its end (the coder's
+  // trailer is longer than the decoder's look-ahead), so a decoder that has read past it (its last byte read is EOF)
+  // is decoding a cut stream: an error, where the reference has no check and decodes on.
+  if (unsized && status >= 0 && rc.buffer == 0xFFFFFFFFu) status = BD_CORRUPT;
+  st->rc = rc;
+  st->total = total;
+  st->nblocks += nb;
+  st->nb = nb;
+  st->status = status;
 }
 
-// BWTC.decompressFile on device buffers.  h_head = the first bytes of the stream on the host (>= 16 or all of it).
-void bwtc_decompress_device(Ctx& c, const u8* d_in, size_t n, const u8* h_head, size_t head_n, u8* d_out, size_t out_cap, size_t* out_n) {
-  if (head_n < 5 || h_head[0] != 'b' || h_head[1] != 'w' || h_head[2] != 't' || h_head[3] != 'c')
-    throw B2Error{B2_ERR_BAD_MAGIC, "Bad magic"};             // lib/Util.js:151-153
-  size_t pos = 4;
+// blocks per decode batch ($B2_BWTC_DEC_BATCH: test hook, small batches exercise the batch seams on small inputs)
+static u32 bwtc_dec_batch(const Ctx& c) {
+  if (const char* e = getenv("B2_BWTC_DEC_BATCH")) { const int v = atoi(e); if (v >= 1) return (u32)v; }
+  return c.bwt_batch;
+}
+
+// lib/Util.js:211-220 readUnsignedNumber after the magic.  Returns the size field (0 = unknown size, else size + 1) and
+// sets *pos behind it: its last byte is the range coder's first.
+u64 bwtc_parse_header(const u8* in, size_t n, size_t* pos) {
+  if (n < 5 || memcmp(in, "bwtc", 4)) throw B2Error{B2_ERR_BAD_MAGIC, "Bad magic"};   // lib/Util.js:151-153
+  size_t p = 4;
   u64 fs = 0;
-  for (;;) {                                                   // lib/Util.js:211-220 readUnsignedNumber
+  for (;;) {
     // nine 7-bit groups hold any size below 2^63; a longer number cannot be the size of a real file and would overflow
-    if (pos >= head_n || pos > 4 + 9) throw B2Error{B2_ERR_DATA_ERROR, "truncated or oversized BWTC header"};
-    const u32 ch = h_head[pos++];
+    if (p >= n || p > 4 + 9) throw B2Error{B2_ERR_DATA_ERROR, "truncated or oversized BWTC header"};
+    const u32 ch = in[p++];
     if (ch & 0x80) { fs += ch & 0x7F; break; }
     fs = (fs + ch) * 128;
   }
-  if (fs == 0) throw B2Error{B2_ERR_BAD_ARG, "BWTC streams of unknown size are not supported"};
-  const u64 size = fs - 1;
-  *out_n = (size_t)size;
-  if (size > out_cap) throw B2Error{B2_ERR_BAD_ARG, "output buffer too small"};
-  // the level is inside the coded stream: size the buffers for the smallest block size
+  if (fs != 0 && fs - 1 > ((u64)1 << 40)) throw B2Error{B2_ERR_DATA_ERROR, "Data error: implausible BWTC size field"};
+  *pos = p;
+  return fs;
+}
+
+// BWTC.decompressFile: d_in = the stream on the device, pos and fs from bwtc_parse_header.  The decoded bytes go to the
+// host, batch by batch, into *h_out (null on entry; the caller owns it afterwards, also when this throws).  Size field
+// known: one buffer from alloc_host, allocated up front.  Size unknown (fs == 0): a malloc'ed buffer that grows as the
+// batches arrive.  *out_n = the bytes decoded.  Device memory: one batch of blocks, whatever the size of the file.
+void bwtc_decompress(Ctx& c, const u8* d_in, size_t n, size_t pos, u64 fs, void* (*alloc_host)(size_t), u8** h_out, size_t* out_n) {
+  *out_n = 0;
+  const bool unsized = fs == 0;
+  const u64 limit = unsized ? ~0ull : fs - 1;
+  // the level is inside the coded stream: bound the block count for the smallest block size
   // (the header is not trusted: a block costs at least a few coded bytes, so n compressed bytes cannot hold more than
-  // n / 2 blocks, and the decoded size must be something this GPU can hold)
-  if (size > ((u64)1 << 40)) throw B2Error{B2_ERR_DATA_ERROR, "Data error: implausible BWTC size field"};
-  const u64 mb64 = std::min<u64>(size / 100000u + 2, (u64)n / 2 + 2);
-  const u32 maxblocks = (u32)mb64;
-  DBuf<u8> L(c, (size_t)maxblocks << SEG_SHIFT);
-  DBuf<u32> lengths(c, maxblocks), pidx1(c, maxblocks);
-  DBuf<BwtcDecResult> res(c, 1);
-  {
-    StageScope s(c, ST_HDEC);
-    k_bwtc_decode<<<1, 1, 0, c.stream>>>(d_in, n, pos, maxblocks, L, lengths, pidx1, res);
-    KLAUNCH(c); KCHECK();
-  }
-  BwtcDecResult h;
-  c.to_host(&h, res, sizeof h);
-  c.sync();
-  if (h.status) throw B2Error{B2_ERR_DATA_ERROR, "Data error: BWTC stream is corrupt"};
-  std::vector<u32> hl(h.nblocks), hp(h.nblocks);
-  if (h.nblocks) {
-    c.to_host(hl.data(), lengths, 4 * h.nblocks);
-    c.to_host(hp.data(), pidx1, 4 * h.nblocks);
-    c.sync();
-  }
-  u64 total = 0;
-  for (u32 b = 0; b < h.nblocks; b++) total += hl[b];
-  if (total != size) throw B2Error{B2_ERR_DATA_ERROR, "outputsize does not match decoded input"};   // lib/Util.js:69-71
+  // n / 2 blocks)
+  const u64 maxblocks = unsized ? (u64)n / 2 + 2 : std::min<u64>(limit / 100000u + 2, (u64)n / 2 + 2);
+  const u32 B = (u32)std::min<u64>(bwtc_dec_batch(c), maxblocks);
+  DBuf<u8> L(c, (size_t)B << SEG_SHIFT), dout(c, (size_t)B * 900000u);
+  DBuf<u32> lengths(c, B), pidx1(c, B);
+  DBuf<BwtcDecState> st(c, 1);
+  k_bwtc_dec_start<<<1, 1, 0, c.stream>>>(st, d_in, n, pos, limit, maxblocks);
+  KLAUNCH(c); KCHECK();
+  std::vector<u32> hl(B), hp(B);
+  // a known size gets all of its buffer now, up to what maxblocks blocks can hold (more would fail the size check)
+  size_t cap = unsized ? 0 : (size_t)std::min<u64>(limit, maxblocks * 900000u);
+  if (!unsized) *h_out = (u8*)alloc_host(cap);
   u64 off = 0;
-  StageScope s(c, ST_IBWT);
-  for (u32 b = 0; b < h.nblocks; b++) {                         // BWT.unbwtransform per block, lib/BWTC.js:224
-    const u8* Lb = L.p + ((size_t)b << SEG_SHIFT);
-    if (hl[b] == 1) CUDA_CHECK(cudaMemcpyAsync(d_out + off, Lb, 1, cudaMemcpyDeviceToDevice, c.stream));
-    else bwt_inverse_sentinel(c, Lb, hl[b], hp[b], d_out + off);
-    off += hl[b];
+  for (;;) {
+    {
+      StageScope s(c, ST_HDEC);
+      k_bwtc_decode<<<1, 1, 0, c.stream>>>(st, B, L, lengths, pidx1);
+      KLAUNCH(c); KCHECK();
+    }
+    BwtcDecState h;
+    c.to_host(&h, st, sizeof h);
+    c.to_host(hl.data(), lengths, 4 * B);
+    c.to_host(hp.data(), pidx1, 4 * B);
+    c.sync();   // also ends the previous batch's copy to the host
+    if (h.status == BD_CORRUPT) throw B2Error{B2_ERR_DATA_ERROR, "Data error: BWTC stream is corrupt"};
+    if (h.status == BD_SIZE) throw B2Error{B2_ERR_DATA_ERROR, "outputsize does not match decoded input"};   // lib/Util.js:69-71
+    u64 bytes = 0;
+    for (u32 b = 0; b < h.nb; b++) bytes += hl[b];
+    if (unsized && off + bytes > cap) {
+      const size_t ncap = std::max<size_t>(off + bytes, cap * 2);
+      u8* p = (u8*)realloc(*h_out, ncap);
+      if (!p) throw B2Error{B2_ERR_CUDA, "out of host memory"};
+      *h_out = p; cap = ncap;
+    }
+    if (h.nb) {
+      {
+        StageScope s(c, ST_IBWT);   // BWT.unbwtransform of every block of the batch, lib/BWTC.js:224
+        bwt_inverse_sentinel_batch(c, L, hl.data(), hp.data(), h.nb, dout);
+      }
+      CUDA_CHECK(cudaMemcpyAsync(*h_out + off, dout, bytes, cudaMemcpyDeviceToHost, c.stream));
+      off += bytes;
+      c.stats.blocks += h.nb;
+    }
+    if (h.status == BD_END) break;
   }
-  c.stats.blocks += h.nblocks;
+  c.sync();
+  if (!unsized && off != limit) throw B2Error{B2_ERR_DATA_ERROR, "outputsize does not match decoded input"};
+  *out_n = (size_t)off;
 }

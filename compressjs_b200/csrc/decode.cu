@@ -22,7 +22,7 @@
 //                    it passes, a serial pass over the 7000 walk summaries orders them, and the block
 //                    is assembled by copies (only what lies behind a walk's 512-byte record is
 //                    walked again)
-//   bwt_inverse_sentinel: BWT.unbwtransform (lib/BWT.js:352-363) on the same walk kernels
+//   bwt_inverse_sentinel_batch: BWT.unbwtransform (lib/BWT.js:352-363) of a batch of blocks on the same walk kernels
 //   k_unrle_*      : RLE1 decode (lib/Bzip2.js:424-436): count bytes are identified from local
 //                    synchronisation points (8 bytes per thread, decided in registers), output
 //                    offsets from tile sums + one warp scan per block, tiles expanded in shared
@@ -651,11 +651,6 @@ k_unmtf_map(const u16* __restrict__ sym, const u8* __restrict__ symb, const Cand
 }
 
 // ---- inverse BWT ------------------------------------------------------------------------------
-__global__ void k_ibwt_keys(const u8* __restrict__ tt, const u32* __restrict__ seg_n, u32 nslots, u32* __restrict__ key) {
-  const u32 g = blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= nslots) return;
-  if ((g & SEG_MASK) < seg_n[g >> SEG_SHIFT]) key[g] = tt[g];
-}
 #define IB_SHIFT 7
 #define IB_STEP (1u << IB_SHIFT)
 #define IB_SEGS (SEG_SIZE / IB_STEP + 1)  // sampled rows per block + the start row
@@ -831,20 +826,30 @@ static void dec_attr_once();
 // Reference walk: t = 0; for i = n-1..0: U[i] = T[t]; t = LF[t] + C[T[t]]; t += (t < pidx).  LF[t] + C[T[t]] is
 // the rank x of position t in the stable order by byte, i.e. the inverse of the sorted-position vector that one
 // radix pass produces.  P[t] = next(t) << 8 | T[t] feeds the same sampled-row walks as the bzip2 decoder; the
-// spare slot 2^20-1 holds the pseudo start entry (orig) whose successor is row 0.
-__global__ void k_unbwt_pack(const u8* __restrict__ L, const u32* __restrict__ sorted_pos, u32 n, u32 pidx, u32* __restrict__ P) {
-  const u32 x = blockIdx.x * blockDim.x + threadIdx.x;
-  if (x == 0) P[SEG_SIZE - 1] = 0;
+// spare slot 2^20-1 holds the pseudo start entry (orig) whose successor is row 0.  The walk reaches row n only when
+// pidx == n (the reference then reads T[n], undefined, as 0): P[n] = 0 reproduces that.  Block = blockIdx.y.
+__global__ void k_unbwt_pack(const u8* __restrict__ L, const u32* __restrict__ sorted_pos, const u32* __restrict__ d_n,
+                             const u32* __restrict__ d_pidx, u32* __restrict__ P) {
+  const u32 x = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+  const u32 n = d_n[b], pidx = d_pidx[b];
+  const size_t base = (size_t)b << SEG_SHIFT;
+  if (x == 0) { P[base + SEG_SIZE - 1] = 0; P[base + n] = 0; }
   if (x >= n) return;
-  const u32 t = sorted_pos[x] & SEG_MASK;
-  P[t] = ((x + (x < pidx ? 1u : 0u)) << 8) | L[t];
+  const u32 t = sorted_pos[base + x] & SEG_MASK;
+  P[base + t] = ((x + (x < pidx ? 1u : 0u)) << 8) | L[base + t];
 }
-__global__ void k_unbwt_setup(CandRes* r, u32 n) {
+__global__ void k_unbwt_setup(CandRes* res, const u32* __restrict__ d_n, u32 nb) {
+  const u32 b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= nb) return;
+  CandRes* r = res + b;
+  const u32 n = d_n[b];
   r->status = 0; r->detail = 0; r->m = 0; r->orig = SEG_SIZE - 1; r->sym_total = 0; r->n = n; r->rawlen = n; r->pad = 0; r->endbit = 0;
 }
-__global__ void k_reverse_bytes(const u8* __restrict__ in, u32 n, u8* __restrict__ out) {
-  const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[n - 1 - i] = in[i];
+// the walks write each block back to front into its slot; the blocks go out front to back and back to back
+__global__ void k_reverse_blocks(const u8* __restrict__ in, const u32* __restrict__ d_n, const u64* __restrict__ d_off, u8* __restrict__ out) {
+  const u32 i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+  const u32 n = d_n[b];
+  if (i < n) out[d_off[b] + n - 1 - i] = in[((size_t)b << SEG_SHIFT) + i];
 }
 static void dec_attr_once() {
   static bool attr = false;
@@ -855,39 +860,51 @@ static void dec_attr_once() {
   CUDA_CHECK(cudaFuncSetAttribute(k_ibwt_chain, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(Seg) * IB_SEGS)));
   attr = true;
 }
-// d_L, d_out: device buffers of n bytes; 2 <= n <= 2^20 - 2; 0 <= pidx <= n
-void bwt_inverse_sentinel(Ctx& c, const u8* d_L, u32 n, u32 pidx, u8* d_out) {
+// nb blocks at once: block b is the L column in slot b of d_L (d_L + (b << SEG_SHIFT)), h_n[b] bytes (1 <= n <= 2^20 - 2)
+// with primary index h_pidx[b] (0 <= pidx <= n).  The decoded blocks go to d_out back to back, in block order.
+// Scratch: about 14 MiB per block.
+void bwt_inverse_sentinel_batch(Ctx& c, const u8* d_L, const u32* h_n, const u32* h_pidx, u32 nb, u8* d_out) {
+  if (!nb) return;
   dec_attr_once();
-  DBuf<u32> keyA(c, SEG_SIZE), keyB(c, SEG_SIZE), valA(c, SEG_SIZE), valB(c, SEG_SIZE), dn(c, 1), nvis(c, 1);
-  DBuf<u8> tmp(c, SEG_SIZE);
-  DBuf<CandRes> res(c, 1);
-  DBuf<Seg> segs(c, IB_SEGS);
-  DBuf<Visit> visits(c, IB_VCAP);
-  DBuf<u32> capr(c, IB_SEGS), tails(c, IB_VCAP), ntails(c, 1);
-  DBuf<u8> slots(c, (size_t)SEG_SIZE * 4 + IB_CAP);  // slotA; the start row's slot sits behind it
-  c.to_device(dn, &n, 4);
-  k_ibwt_keys<<<(SEG_SIZE + 255) / 256, 256, 0, c.stream>>>(d_L, dn, SEG_SIZE, keyA);
+  u32 nmax = 0; u64 ntot = 0;
+  std::vector<u64> hoff(nb);
+  for (u32 b = 0; b < nb; b++) { hoff[b] = ntot; ntot += h_n[b]; nmax = std::max(nmax, h_n[b]); }
+  const size_t slots = (size_t)nb << SEG_SHIFT;
+  DBuf<u32> valA(c, slots), valB(c, slots), slotA(c, slots), dn(c, nb), dpidx(c, nb), nvis(c, nb), ntails(c, nb);
+  DBuf<u8> kout(c, slots), tmp(c, slots);
+  DBuf<u64> doff(c, nb);
+  DBuf<CandRes> res(c, nb);
+  DBuf<Seg> segs(c, (size_t)nb * IB_SEGS);
+  DBuf<Visit> visits(c, (size_t)nb * IB_VCAP);
+  DBuf<u32> capr(c, (size_t)nb * IB_SEGS), tails(c, (size_t)nb * IB_VCAP);
+  c.to_device(dn, h_n, 4 * nb);
+  c.to_device(dpidx, h_pidx, 4 * nb);
+  c.to_device(doff, hoff.data(), 8 * nb);
+  // one stable counting-sort pass per block over the L column's bytes: vin = the positions in sorted order
+  u8* kin = const_cast<u8*>(d_L);   // read only: a single pass writes kout
+  u8* ko = kout.p;
+  u32 *vin = valA.p, *vout = valB.p;
+  radix_sort<u8>(c, kin, vin, ko, vout, dn.p, nb, SEG_SHIFT, nmax, 0, 1, true, ntot);
+  u32* P = vout;    // the iota pass never read its value buffer
+  const dim3 grid((nmax + 255) / 256, nb);
+  k_unbwt_pack<<<grid, 256, 0, c.stream>>>(d_L, vin, dn, dpidx, P);
   KLAUNCH(c); KCHECK();
-  u32 *kin = keyA.p, *kout = keyB.p, *vin = valA.p, *vout = valB.p;
-  radix_sort<u32>(c, kin, vin, kout, vout, dn.p, 1, SEG_SHIFT, n, 0, 1, true, n);  // swaps the pairs: vin = sorted positions
-  u32* P = kout;  // the other key buffer is free now
-  CUDA_CHECK(cudaMemsetAsync(P, 0, (size_t)SEG_SIZE * 4, c.stream));  // rows >= n lead back to row 0: the walks stay in bounds
-  k_unbwt_pack<<<(n + 255) / 256, 256, 0, c.stream>>>(d_L, vin, n, pidx, P);
+  k_unbwt_setup<<<(nb + 127) / 128, 128, 0, c.stream>>>(res, dn, nb);
   KLAUNCH(c); KCHECK();
-  k_unbwt_setup<<<1, 1, 0, c.stream>>>(res, n);
+  // the walks record into slotA (4 MiB per block); the start row's slot goes to the head of the block's 4 MiB of the
+  // sorted positions, which k_unbwt_pack has consumed
+  u8* sA = reinterpret_cast<u8*>(slotA.p);
+  u8* sB = reinterpret_cast<u8*>(vin);
+  k_ibwt_walk1<<<(nb * IB_SEGS + 127) / 128, 128, 0, c.stream>>>(P, res, nb, segs, capr, sA, sB);
   KLAUNCH(c); KCHECK();
-  u8* slotA = slots.p; u8* slotB = slots.p + (size_t)SEG_SIZE * 4;
-  k_ibwt_walk1<<<(IB_SEGS + 127) / 128, 128, 0, c.stream>>>(P, res, 1, segs, capr, slotA, slotB);
+  k_ibwt_chain<<<nb, 128, sizeof(Seg) * IB_SEGS, c.stream>>>(P, res, nb, segs, visits, nvis, tails, ntails);
   KLAUNCH(c); KCHECK();
-  k_ibwt_chain<<<1, 128, sizeof(Seg) * IB_SEGS, c.stream>>>(P, res, 1, segs, visits, nvis, tails, ntails);
+  k_ibwt_place<<<nb * IB_PLACE_CTAS, IB_PLACE_THREADS, 0, c.stream>>>(P, res, nb, visits, nvis, sA, sB, tmp);
   KLAUNCH(c); KCHECK();
-  k_ibwt_place<<<IB_PLACE_CTAS, IB_PLACE_THREADS, 0, c.stream>>>(P, res, 1, visits, nvis, slotA, slotB, tmp);
+  k_ibwt_tail<<<(nb * IB_VCAP + 127) / 128, 128, 0, c.stream>>>(P, res, nb, visits, nvis, tails, ntails, capr, tmp);
   KLAUNCH(c); KCHECK();
-  k_ibwt_tail<<<(IB_VCAP + 127) / 128, 128, 0, c.stream>>>(P, res, 1, visits, nvis, tails, ntails, capr, tmp);
+  k_reverse_blocks<<<grid, 256, 0, c.stream>>>(tmp, dn, doff, d_out);
   KLAUNCH(c); KCHECK();
-  k_reverse_bytes<<<(n + 255) / 256, 256, 0, c.stream>>>(tmp, n, d_out);
-  KLAUNCH(c); KCHECK();
-  c.sync();
 }
 
 // ---- RLE1 decode ------------------------------------------------------------------------------

@@ -100,7 +100,14 @@ int b2_bwt_inverse(const uint8_t* L, uint8_t* out, int32_t n, int32_t pidx);
 /* ---- compressjs.BWTC (lib/BWTC.js) -- new, bound by one serial coder thread: see compressjs_b200/csrc/bwtc.cu -----
  * BWTC.compressFile(input, output, level)             lib/BWTC.js:12-139 (level outside 1..9 means 9, as there) */
 int b2_bwtc_compress(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n);
-/* BWTC.decompressFile(input, output)                  lib/BWTC.js:141-231 (streams that carry their size) */
+/* BWTC.compressFile of an input stream without a size  lib/Util.js:119-124: the header's size field is "unknown" (the
+ * single byte 0x80, which the range coder takes as its first byte); everything else is b2_bwtc_compress.  This is what
+ * the compressjs command line writes for a pipe or an empty file. */
+int b2_bwtc_compress_unsized(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n);
+/* BWTC.decompressFile(input, output)                  lib/BWTC.js:141-231, for streams with a size field and for
+ * streams of unknown size (decoded up to the "no more blocks" marker).  Blocks are decoded a batch at a time
+ * ($B2_BWTC_DEC_BATCH, default two per SM) and each batch goes to the host, so device memory is bounded by one batch
+ * (about 17 MiB per block) for any file size.  A stream whose blocks exceed its size field fails as soon as they do. */
 int b2_bwtc_decompress(const uint8_t* in, size_t n, uint8_t** out, size_t* out_n);
 /* CRC32 helper object of lib/CRC32.js:72-103 (bzip2 polynomial, MSB first) */
 uint32_t b2_crc32_bzip2(const uint8_t* p, size_t n);
