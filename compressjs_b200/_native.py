@@ -27,7 +27,10 @@ class Stats(C.Structure):
                [(n, C.c_uint64) for n in
                 ("radix_launches", "radix_bytes", "bwt_bytes", "bwt_rounds", "kernel_launches", "blocks",
                  "raw_bytes", "comp_bytes", "msd_launches", "msd_scatter_bytes", "msd_bucket_bytes")] + \
-               [(n, C.c_float) for n in ("ms_msd_scatter", "ms_msd_bucket")]
+               [(n, C.c_float) for n in ("ms_msd_scatter", "ms_msd_bucket")] + \
+               [(n, C.c_uint64) for n in
+                ("bwt_msd_done", "bwt_direct_done", "bwt_rounds_batches", "bwt_wide_batches",
+                 "bwt_msd_fallback_why", "bwt_direct_fallback_why")]
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}

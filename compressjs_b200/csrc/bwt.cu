@@ -422,6 +422,8 @@ k_emit_detect(const u64* __restrict__ rec, const u8* __restrict__ T, const u32* 
 
 #define RD_MAXGROUP 16  // larger groups and rotations equal over RD_DEPTH more bytes go to the doubling rounds
 #define RD_DEPTH 64
+#define RD_FAIL_GROUP 1u  // *fail bits: a group larger than RD_MAXGROUP,
+#define RD_FAIL_DEPTH 2u  // two rotations equal over h0 + RD_DEPTH bytes
 __global__ void k_resolve_direct(const u32* __restrict__ head, const u32* __restrict__ idx, u32 M, const u8* __restrict__ T,
                                  const u32* __restrict__ seg_n, u32 h0, u8* __restrict__ U, u32* __restrict__ pidx, u32* fail) {
   const u32 q = blockIdx.x * blockDim.x + threadIdx.x;
@@ -431,7 +433,7 @@ __global__ void k_resolve_direct(const u32* __restrict__ head, const u32* __rest
   u32 mem[RD_MAXGROUP];
   u32 cnt = 0;
   while (q + cnt < M && head[q + cnt] == hd) {
-    if (cnt == RD_MAXGROUP) { atomicOr(fail, 1u); return; }
+    if (cnt == RD_MAXGROUP) { atomicOr(fail, RD_FAIL_GROUP); return; }
     mem[cnt] = idx[q + cnt] & SEG_MASK;
     cnt++;
   }
@@ -448,7 +450,7 @@ __global__ void k_resolve_direct(const u32* __restrict__ head, const u32* __rest
         const u32 wx = word_at(Tb, n, x, d), wy = word_at(Tb, n, y, d);
         if (wx != wy) { less = wx < wy ? 1 : 0; break; }
       }
-      if (less < 0) { atomicOr(fail, 1u); return; }
+      if (less < 0) { atomicOr(fail, RD_FAIL_DEPTH); return; }
       if (!less) break;
       mem[pos] = y;
       pos--;
@@ -514,6 +516,9 @@ __global__ void k_emit_sentinel(const u32* __restrict__ SA, const u8* __restrict
 }
 
 // host side: radix_sort<> lives in radix_host.cuh
+// why a direct finish gave up (b2_stats.bwt_msd_fallback_why / bwt_direct_fallback_why)
+enum : u32 { WHY_BUCKET = 1, WHY_CELL = 2, WHY_TIES = 4, WHY_GROUP = 8, WHY_DEPTH = 16 };
+static u32 resolve_why(u32 fail) { return (fail & RD_FAIL_GROUP ? WHY_GROUP : 0u) | (fail & RD_FAIL_DEPTH ? WHY_DEPTH : 0u); }
 static u32 bits_for(u32 maxval) {  // number of bits needed to represent values 0..maxval
   u32 b = 0;
   while (maxval) { b++; maxval >>= 1; }
@@ -566,6 +571,7 @@ void bwt_forward_batch(Ctx& c, const u8* d_T, u8* d_U, const u32* d_n, const u32
     c.bwt_mode_known = true;
   }
   const bool wide = sentinel ? false : c.bwt_wide;
+  if (wide) c.stats.bwt_wide_batches++;
   if (!wide && !sentinel && c.bwt_msd) {
     // sparse-tie batches: one MSD pass + shared-memory bucket sorts (bwt_msd.cu); ties on 5 bytes are ordered directly
     CUDA_CHECK(cudaMemsetAsync(cnt, 0, 16, c.stream));
@@ -576,19 +582,22 @@ void bwt_forward_batch(Ctx& c, const u8* d_T, u8* d_U, const u32* d_n, const u32
     c.to_host(&score, dscore, 4);
     c.sync();
     if (!c.bwt_wide_forced) c.bwt_wide = score > 0.5f;  // next batch of this call
-    if (!h_ctl[2] && !h_ctl[1]) {
+    u32 why = (h_ctl[2] ? WHY_BUCKET : 0u) | (h_ctl[1] ? WHY_CELL : 0u);
+    if (!why) {
       const u32 Mt = h_ctl[0];
       u32 failed = 0;
-      if (Mt > n_total / 8) failed = 1;
+      if (Mt > n_total / 8) why = WHY_TIES;
       else if (Mt) {
         k_resolve_direct<<<(Mt + 127) / 128, 128, 0, c.stream>>>(headA, idxA, Mt, d_T, d_n, 5, d_U, d_pidx, cnt.p + 1);
         KLAUNCH(c); KCHECK();
         c.stats.bwt_bytes += (u64)Mt * 80;
         c.to_host(&failed, cnt.p + 1, 4);
         c.sync();
+        why = resolve_why(failed);
       }
-      if (!failed) return;
+      if (!why) { c.stats.bwt_msd_done++; return; }
     }
+    c.stats.bwt_msd_fallback_why |= why;
     // an oversized bucket or long repeats after all: the LSD path below redoes the batch
   }
   k_build_keys<<<bk_tps * nblk, BK_THREADS, 0, c.stream>>>(d_T, d_n, bk_tps, kin, nullptr, wide ? 4u : 0u, sentinel ? 1 : 0);
@@ -621,18 +630,21 @@ void bwt_forward_batch(Ctx& c, const u8* d_T, u8* d_U, const u32* d_n, const u32
     c.to_host(&score, dscore, 4);
     c.sync();
     if (!c.bwt_wide_forced) c.bwt_wide = score > 0.5f;  // next batch of this call
-    u32 failed = 0;
-    if (Mt > n_total / 8) failed = 1;
+    u32 failed = 0, why = 0;
+    if (Mt > n_total / 8) why = WHY_TIES;
     else if (Mt) {
       k_resolve_direct<<<(Mt + 127) / 128, 128, 0, c.stream>>>(headA, idxA, Mt, d_T, d_n, 4, d_U, d_pidx, cnt.p + 1);
       KLAUNCH(c); KCHECK();
       c.stats.bwt_bytes += (u64)Mt * 80;
       c.to_host(&failed, cnt.p + 1, 4);
       c.sync();
+      why = resolve_why(failed);
     }
-    if (!failed) return;
+    if (!why) { c.stats.bwt_direct_done++; return; }
+    c.stats.bwt_direct_fallback_why |= why;
     // long repeats after all: fall through to the rank-based rounds (the sorted records are still intact)
   }
+  c.stats.bwt_rounds_batches++;
   CUDA_CHECK(cudaMemsetAsync(st, 0, (size_t)3 * rr_tiles_init * 8, c.stream));
   CUDA_CHECK(cudaMemsetAsync(ticket, 0, 4, c.stream));
   CUDA_CHECK(cudaMemsetAsync(cnt, 0, 4, c.stream));

@@ -19,7 +19,7 @@ struct MsdBlk {
   u64 S;      // floor(2^64 / a^4): scaled key = (key * S) >> 32
 };
 
-// d_ctl: u32[4] zeroed by the caller: [0] = members of tie groups written to the tie list, [1] = resolver failure,
+// d_ctl: u32[4] zeroed by the caller: [0] = members of tie groups written to the tie list, [1] = a cell exceeds MB_MAXCELL,
 // [2] = a bucket exceeds MB_CAP (nothing was done), [3] = non-empty buckets (length of the work list).
 void bwt_msd_launch(Ctx& c, const u8* d_T, u8* d_U, const u32* d_n, u32 nblk, u32 n_max, u64 n_total, const u32* d_hist, u64* d_rec,
                     u32* d_pidx, u32* d_tie_head, u32* d_tie_idx, u32* d_ctl);

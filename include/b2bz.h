@@ -183,6 +183,14 @@ typedef struct b2_stats {
   uint64_t msd_scatter_bytes;  /* algorithmic bytes of k_msd_scatter (text in, records out) */
   uint64_t msd_bucket_bytes;   /* algorithmic bytes of k_msd_bucket (records in, column out) */
   float ms_msd_scatter, ms_msd_bucket;
+  /* How each forward-BWT batch finished (bwt.cu).  Every non-empty batch counts in exactly one of the first three. */
+  uint64_t bwt_msd_done;             /* finished by the MSD path (5-byte ties ordered directly) */
+  uint64_t bwt_direct_done;          /* finished by the 4-byte LSD sort + direct tie resolve */
+  uint64_t bwt_rounds_batches;       /* finished by the rank-based prefix-doubling rounds (sentinel calls included) */
+  uint64_t bwt_wide_batches;         /* sorted on 8-byte prefixes first (text-like mode) */
+  uint64_t bwt_msd_fallback_why;     /* OR over batches of why the MSD path gave up: 1 = bucket > MB_CAP, 2 = cell >
+                                        MB_MAXCELL, 4 = tie list > n/8, 8 = tie group > 16, 16 = tie deeper than the resolver */
+  uint64_t bwt_direct_fallback_why;  /* the same bits 4 / 8 / 16 for the LSD direct resolve */
 } b2_stats;
 void b2_get_stats(b2_stats* s);
 
