@@ -30,9 +30,9 @@ void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, int level, u8* d_in, 
 void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* info);
 void dec_shard_export(u64* buf);
 int dec_shard_finish(Ctx& c, const u64* all, int multistream, u8* d_out, size_t out_cap, u64* res);
-int bzip2_decompress_device(Ctx& c, const u8* d_in, size_t n, int multistream, u8* d_out, size_t out_cap, size_t* out_n,
-                            const std::vector<u64>* positions, std::vector<u64>* ends, std::vector<u64>* tab_pos, std::vector<u32>* tab_len,
-                            u8** d_out_alloc);
+int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multistream, u8* d_out, size_t out_cap, size_t* out_n,
+                     const std::vector<u64>* positions, std::vector<u64>* ends, std::vector<u64>* tab_pos, std::vector<u32>* tab_len,
+                     void* (*alloc_host)(size_t), void (*free_host)(void*), u8** h_out);
 
 static std::mutex g_mu;
 static Ctx* g_ctx = nullptr;
@@ -58,6 +58,9 @@ void Ctx::collect() {
     float ms = 0.f;
     if (copy_used[w] && cudaEventElapsedTime(&ms, copy_ev[w][0], copy_ev[w][1]) == cudaSuccess) (w ? stats.ms_d2h : stats.ms_h2d) += ms;
   }
+  uint64_t high = 0;
+  if (pool && cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemHigh, &high) == cudaSuccess) stats.dev_peak_bytes = high;
+  else cudaGetLastError();
 }
 
 // ---- small control transfers through mapped pinned memory ----------------------------------
@@ -139,6 +142,7 @@ static Ctx& ctx_locked() {
     CUDA_CHECK(cudaDeviceGetDefaultMemPool(&pool, dev));
     uint64_t thr = UINT64_MAX;
     CUDA_CHECK(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr));
+    c->pool = pool;
     int sms = 0;
     CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     c->bwt_batch = 2u * (u32)sms;
@@ -596,43 +600,29 @@ int b2_bzip2_encode_range_dev(const void* d_in, size_t n, int level, size_t firs
 
 // On a decode error (-2/-5/-7) the code is returned, not thrown, and *out / the table rows hold what the reference has
 // written by the time it throws; any other error throws and returns nothing.  positions / ends: a position list
-// (bzip2_decompress_device).
+// (bzip2_decompress).  The input stays on the host; the decoder uploads it a window at a time.
 static int decode_common(const uint8_t* in, size_t n, int multistream, const std::vector<u64>* positions, std::vector<u64>* ends,
                          uint8_t** out, size_t* out_n, std::vector<u64>* tp, std::vector<u32>* tl) {
   Ctx& c = ctx_locked();
   c.reset_call();
   size_t produced = 0;
-  void* host = nullptr;
+  u8* host = nullptr;
   int rc = 0;
-  {
+  try {
     StageScope tot(c, ST_TOTAL);
-    DBuf<u8> din(c, n + 16);
-    {
-      StageScope s(c, ST_H2D);
-      CUDA_CHECK(cudaMemsetAsync(din.p + n, 0, 16, c.stream));
-      if (n) CUDA_CHECK(cudaMemcpyAsync(din, in, n, cudaMemcpyHostToDevice, c.stream));
-    }
-    u8* dres = nullptr;
-    struct DresGuard { Ctx& c; u8*& p; ~DresGuard() { if (p) { c.dfree(p); p = nullptr; } } } dres_guard{c, dres};  // also on exceptions
     try {
-      rc = bzip2_decompress_device(c, din, n, multistream, nullptr, 0, &produced, positions, ends, tp, tl, &dres);
+      rc = bzip2_decompress(c, in, nullptr, n, multistream, nullptr, 0, &produced, positions, ends, tp, tl, pinned_alloc, pinned_release,
+                            out ? &host : nullptr);
     } catch (const B2Error& e) {
       if (e.code != B2_ERR_NOT_BZIP_DATA && e.code != B2_ERR_DATA_ERROR && e.code != B2_ERR_OBSOLETE_INPUT) throw;
       g_err = e.msg;
       rc = e.code;
     }
-    if (out) {
-      host = pinned_alloc(produced);
-      try {
-        StageScope s(c, ST_D2H);
-        if (produced) CUDA_CHECK(cudaMemcpyAsync(host, dres, produced, cudaMemcpyDeviceToHost, c.stream));
-        c.sync();
-      } catch (...) {
-        pinned_release(host);
-        throw;
-      }
-    }
+    if (out && !host) host = (u8*)pinned_alloc(produced);
     c.sync();
+  } catch (...) {
+    if (host) pinned_release(host);
+    throw;
   }
   c.sync();
   c.collect();
@@ -718,7 +708,8 @@ int b2_bzip2_decompress_dev(const void* d_in, size_t n, int multistream, void* d
     int rc;
     {
       StageScope tot(c, ST_TOTAL);
-      rc = bzip2_decompress_device(c, (const u8*)d_in, n, multistream, (u8*)d_out, out_cap, out_n, nullptr, nullptr, nullptr, nullptr, nullptr);
+      rc = bzip2_decompress(c, nullptr, (const u8*)d_in, n, multistream, (u8*)d_out, out_cap, out_n, nullptr, nullptr, nullptr, nullptr,
+                            nullptr, nullptr, nullptr);
     }
     c.sync();
     c.collect();

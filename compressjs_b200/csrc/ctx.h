@@ -70,7 +70,12 @@ struct Ctx {
   // first / last copy of a call on a copy stream (which: 0 = host to device, 1 = device to host)
   void copy_begin(cudaStream_t s, int which) { CUDA_CHECK(cudaEventRecord(copy_ev[which][0], s)); copy_used[which] = true; }
   void copy_end(cudaStream_t s, int which) { CUDA_CHECK(cudaEventRecord(copy_ev[which][1], s)); }
+  cudaMemPool_t pool = nullptr;  // the device's default pool: every dalloc comes from it (b2_stats.dev_peak_bytes)
   void reset_call() {
+    if (pool) {
+      uint64_t zero = 0;  // the high-water mark restarts from what is in use now
+      CUDA_CHECK(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrUsedMemHigh, &zero));
+    }
     copy_used[0] = copy_used[1] = false;
     fetches.clear();  // a call that failed half way may have left some behind
     stage_used = 0;

@@ -27,9 +27,11 @@
 //                    synchronisation points (8 bytes per thread, decided in registers), output
 //                    offsets from tile sums + one warp scan per block, tiles expanded in shared
 //                    memory, CRC32 per block
-//   host           : walks the block chain (a block must start exactly where the previous one
-//                    ended), folds/validates CRCs and raises the reference's errors in stream order;
-//                    a position list is taken in list order instead, without a chain.
+//   host           : one rolling loop over windows of the compressed input and batches of blocks
+//                    (bzip2_decompress): walks the block chain (a block must start exactly where the previous
+//                    one ended) after every batch, folds/validates CRCs, delivers the settled blocks and
+//                    raises the reference's errors in stream order; a position list is taken in list order
+//                    instead, without a chain.
 #include <algorithm>
 #include <vector>
 #include "enc.h"
@@ -58,14 +60,14 @@ struct CandRes {
   u32 sym_total;   // distinct bytes
   u32 n;           // block length after un-MTF (filled later)
   u32 rawlen;      // bytes after RLE1 decode (filled later)
-  u32 pad;
+  u32 open;        // 1 = decoding it read up to the end of an input window that is not the end of the file: not final
   u64 endbit;      // bit position just behind the EOB code
   u8 sym_to_byte[256];
 };
 
 // ---- magic test -----------------------------------------------------------------------------
 // The words wi .. wi+3 of the stream (big endian) hold the 80 bits that a candidate starting in word wi can span: the
-// 48-bit magic and the 32 bits behind it.  The private copy of the input is zero padded (dec_open): for wi < (n + 3) / 4
+// 48-bit magic and the 32 bits behind it.  The device copy of the input (window) is zero padded: for wi < (n + 3) / 4
 // the reads stay below n + 32.
 struct MagicWords { u32 w0, w1, w2, w3; };
 __device__ __forceinline__ MagicWords magic_words(const u8* __restrict__ in, u64 wi) {
@@ -73,18 +75,18 @@ __device__ __forceinline__ MagicWords magic_words(const u8* __restrict__ in, u64
   return {__byte_perm(words[wi], 0, 0x0123), __byte_perm(words[wi + 1], 0, 0x0123), __byte_perm(words[wi + 2], 0, 0x0123),
           __byte_perm(words[wi + 3], 0, 0x0123)};
 }
-// Is there a magic at bit pos = 32 wi + b of an n-byte stream?  If so, found(type, next32): type 1 = block, 2 = end of
-// stream, next32 = the 32 bits behind it.  The first 32 bits of the magic are tested with one funnel shift and one compare;
-// the rest, rarely reached, sits inside that branch (a callback rather than a return value keeps the scan loop free of
-// a second branch per offset).
+// Is there a magic at bit pos = 32 wi + b of the buffer, pos < lim?  If so, found(type, next32): type 1 = block, 2 = end
+// of stream, next32 = the 32 bits behind it.  The first 32 bits of the magic are tested with one funnel shift and one
+// compare; the rest, rarely reached, sits inside that branch (a callback rather than a return value keeps the scan loop
+// free of a second branch per offset).
 template <class F>
-__device__ __forceinline__ void magic_test(const MagicWords& w, u32 b, u64 pos, u64 n, F&& found) {
+__device__ __forceinline__ void magic_test(const MagicWords& w, u32 b, u64 pos, u64 lim, F&& found) {
   const u32 M1 = (u32)(WHOLEPI >> 16), M2 = (u32)(SQRTPI >> 16);
   const u32 h = __funnelshift_l(w.w1, w.w0, b);          // stream bits [b, b + 32) of this word pair
   if (h == M1 || h == M2) {
     const u32 mid = __funnelshift_l(w.w2, w.w1, b);      // bits [b + 32, b + 64)
     const u64 v = ((u64)h << 16) | (mid >> 16);
-    if ((v == WHOLEPI || v == SQRTPI) && pos < n * 8) {
+    if ((v == WHOLEPI || v == SQRTPI) && pos < lim) {
       const u32 lo = __funnelshift_l(w.w3, w.w2, b);     // bits [b + 64, b + 96)
       found(v == WHOLEPI ? 1u : 2u, (mid << 16) | (lo >> 16));
     }
@@ -92,19 +94,20 @@ __device__ __forceinline__ void magic_test(const MagicWords& w, u32 b, u64 pos, 
 }
 
 // ---- magic scan ---------------------------------------------------------------------------
-// One thread per aligned 32-bit word of the stream = 32 bit offsets.
-__global__ void k_scan_magic(const u8* __restrict__ in, u64 n, Cand* __restrict__ cands, u32* count, u32 cap) {
+// One thread per aligned 32-bit word of the n-byte window = 32 bit offsets.  The window starts at bit base_bit of the
+// file (a multiple of 32); magics at window offsets below lim are recorded, with their position in the file.
+__global__ void k_scan_magic(const u8* __restrict__ in, u64 n, u64 base_bit, u64 lim, Cand* __restrict__ cands, u32* count, u32 cap) {
   const u64 wi = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (wi >= (n + 3) / 4) return;
   const MagicWords w = magic_words(in, wi);
 #pragma unroll 8
   for (u32 b = 0; b < 32; b++) {
     const u64 pos = wi * 32 + b;
-    magic_test(w, b, pos, n, [&](u32 type, u32 next32) {
+    magic_test(w, b, pos, lim, [&](u32 type, u32 next32) {
       const u32 idx = atomicAdd(count, 1u);
       if (idx < cap) {
         Cand c;
-        c.pos = pos; c.type = type; c.next32 = next32;
+        c.pos = base_bit + pos; c.type = type; c.next32 = next32;
         cands[idx] = c;
       }
     });
@@ -119,7 +122,7 @@ __global__ void k_magic_at(const u8* __restrict__ in, u64 n, const u64* __restri
   Cand c;
   c.pos = pos[i]; c.type = 0; c.next32 = 0;
   if (c.pos < n * 8)  // no reads past the stream
-    magic_test(magic_words(in, c.pos >> 5), (u32)(c.pos & 31), c.pos, n, [&](u32 type, u32 next32) { c.type = type; c.next32 = next32; });
+    magic_test(magic_words(in, c.pos >> 5), (u32)(c.pos & 31), c.pos, n * 8, [&](u32 type, u32 next32) { c.type = type; c.next32 = next32; });
   cands[i] = c;
 }
 
@@ -197,16 +200,19 @@ __device__ __noinline__ u32 hdec_slow(const HdecWarp& s, u32 g, u32 bits20, int 
 // 128 threads: 10 CTAs per SM (45 registers, 19 KB of shared memory each), so that the ~1200 blocks of a 1 GiB file are
 // resident at once on the 132 SMs of an H100.  At 9 per SM (1188 slots) the last blocks ran as a second wave: 66 ms
 // instead of 44 ms per GiB (H100 SXM, 400 W power limit).
+// The input is a window of nbytes bytes that starts at bit base_bit of the file (a multiple of 32) and is zero padded
+// behind; candidate positions and endbit are bits of the file.  A result that depends on no bit at or past the window's
+// end is what the whole file gives; any other is marked open unless the window ends where the file does (`last`).
 template <int HD_T>
 __global__ void __launch_bounds__(HD_T, HD_T == 128 ? 10 : 1152 / HD_T)
-k_hdec(const u8* __restrict__ in, u64 nbytes, const Cand* __restrict__ cands, u32 first, u32 count, u32 dbuf_size, u8* __restrict__ sel_buf,
-       u16* __restrict__ sym_out, CandRes* __restrict__ res) {
+k_hdec(const u8* __restrict__ in, u64 nbytes, u64 base_bit, u32 last, const Cand* __restrict__ cands, u32 count, u32 dbuf_size,
+       u8* __restrict__ sel_buf, u16* __restrict__ sym_out, CandRes* __restrict__ res) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   HdecWarp& s = *reinterpret_cast<HdecWarp*>(smem_raw);
   const u32 lane = threadIdx.x;  // 0..HD_T-1: one CTA per candidate block
   const u32 ci = blockIdx.x;
   if (ci >= count) return;
-  const Cand cd = cands[first + ci];
+  const Cand cd = cands[ci];
   CandRes* r = res + ci;
   u8* sel = sel_buf + (size_t)ci * SEL_CAP;
   u16* so = sym_out + ((size_t)ci << SEG_SHIFT);
@@ -215,7 +221,7 @@ k_hdec(const u8* __restrict__ in, u64 nbytes, const Cand* __restrict__ cands, u3
   if (lane == 0) {
     s.status = 0;
     r->detail = 0; r->m = 0; r->n = 0; r->rawlen = 0; r->endbit = 0;
-    br.init(in, nbytes, cd.pos + 48 + 32);
+    br.init(in, nbytes, cd.pos - base_bit + 48 + 32);
     do {
       if (br.get(1)) { s.status = DEC_OBSOLETE; break; }           // lib/Bzip2.js:143
       const u32 orig = br.get(24);
@@ -266,7 +272,8 @@ k_hdec(const u8* __restrict__ in, u64 nbytes, const Cand* __restrict__ cands, u3
   }
   __syncthreads();
   if (s.status != 0) {
-    if (lane == 0) r->status = s.status;
+    // a header error is decided by the bits read so far
+    if (lane == 0) { r->status = s.status; r->open = !last && br.tell() > nbytes * 8; }
     return;
   }
   const u32 gc = s.ngroups, symCount = s.symcount;
@@ -454,7 +461,11 @@ k_hdec(const u8* __restrict__ in, u64 nbytes, const Cand* __restrict__ cands, u3
     if (lane == 0) {
       r->status = status;
       r->m = m;
-      r->endbit = P;
+      r->endbit = base_bit + P;
+      // a block that ends well is decided by the bits in front of its end; a failure by at most a window of codes
+      // behind P (the speculative decode reads HD_WIN + 20 bits ahead)
+      const u64 hi = status == 0 ? P : P + HD_WIN + 32;
+      r->open = !last && hi > nbytes * 8;
     }
   }
 }
@@ -843,7 +854,7 @@ __global__ void k_unbwt_setup(CandRes* res, const u32* __restrict__ d_n, u32 nb)
   if (b >= nb) return;
   CandRes* r = res + b;
   const u32 n = d_n[b];
-  r->status = 0; r->detail = 0; r->m = 0; r->orig = SEG_SIZE - 1; r->sym_total = 0; r->n = n; r->rawlen = n; r->pad = 0; r->endbit = 0;
+  r->status = 0; r->detail = 0; r->m = 0; r->orig = SEG_SIZE - 1; r->sym_total = 0; r->n = n; r->rawlen = n; r->open = 0; r->endbit = 0;
 }
 // the walks write each block back to front into its slot; the blocks go out front to back and back to back
 __global__ void k_reverse_blocks(const u8* __restrict__ in, const u32* __restrict__ d_n, const u64* __restrict__ d_off, u8* __restrict__ out) {
@@ -1111,32 +1122,9 @@ static std::string hexs(u32 v) {
 }
 
 // kind: 0 block, 1 eos, 2 error, 3 an end-of-stream magic in a position list (no bytes, no stream CRC);
-// off: offset in the decoded stream where the event happens (a block's start)
-struct Event { int kind; size_t cand; u32 a, b; int code; std::string msg; u64 off; };
-
-// One decode in flight.  open() parses the header, finds every block candidate and decodes the share
-// [lo, hi) of them (all of them on one GPU); finish() walks the chain over ALL candidates' results
-// (imported from the other ranks when sharded), expands + CRC-checks the blocks of the own share and
-// raises the reference's errors in stream order.  A position list (decompressBlock once per position) has no chain:
-// its candidates are the magics at the given positions, in list order, and finish() takes them in that order.
-struct DecSession {
-  Ctx* c = nullptr;
-  size_t n = 0;
-  u32 dbuf_size = 0;
-  DBuf<u8> din;
-  std::vector<Cand> cands;         // every magic found, sorted by position; for a list: one per position (type 0 = none)
-  std::vector<size_t> blk_idx;     // block candidates (index into cands)
-  std::vector<Cand> bc;            // the same as Cand records
-  std::vector<CandRes> hres;       // per block candidate (valid for [lo,hi) after open, for all after import)
-  size_t lo = 0, hi = 0;           // own share of the block candidates
-  bool listed = false;             // cands come from a position list
-  DBuf<Cand> dcand;
-  DBuf<CandRes> dres;              // own share only
-  DBuf<u8> rle, cls;               // cls (count-byte classes) is kept for the whole share only while that is cheap (keep_cls)
-  bool keep_cls = true;
-  DBuf<u32> tileoff;
-  int err_event = -1;              // index of the first failing event (sharded mode)
-};
+// off: offset in the decoded stream where the event happens (a block's start).  A block event carries its bit position,
+// its stored CRC (a), its decoded length and the slot of its results (in the batch; in the file for the sharded decode).
+struct Event { int kind; size_t slot; u32 a, b; int code; std::string msg; u64 off; u64 pos; u32 len; };
 
 static const u32 UR_TPS = SEG_SIZE / UR_TILE;
 #define DEC_KEEP_CLS 16384u
@@ -1149,10 +1137,524 @@ static u32 dec_keep_cls_limit() {
   if (const char* e = getenv("B2_DEC_KEEP_CLS")) { const int v = atoi(e); if (v >= 0) return (u32)v; }  // test hook
   return DEC_KEEP_CLS;
 }
+// bytes of compressed input on the device at a time, which also caps the output staged for the host ($B2_DEC_WINDOW,
+// default 4 GiB: most files are one window; down to 64 KiB as a test hook)
+static size_t dec_window() {
+  if (const char* e = getenv("B2_DEC_WINDOW")) { const long long v = atoll(e); if (v >= (64 << 10)) return (size_t)v; }
+  return (size_t)4 << 30;
+}
 
-// positions: decode the blocks at these bit positions (in this order) instead of the stream's chain
-static void dec_open(Ctx& c, DecSession& S, const u8* d_in_user, size_t n, const std::vector<u64>* positions, int rank, int world) {
-  S.c = &c; S.n = n; S.listed = positions != nullptr;
+// Scratch of one decode batch, allocated for the largest batch of a call and reused by every batch: about 20 MiB per block
+// (the radix sort's keys and values, 16 MiB, are most of it).
+struct DecScratch {
+  u32 cap = 0;
+  DBuf<u16> sym;
+  DBuf<u8> selbuf, tt, symb, perms, lists;
+  DBuf<ChunkSum> sums;
+  DBuf<ChunkStart> starts;
+  DBuf<u32> keyA, keyB, valA, valB, dn, nvis, tilesum, capr, tails, ntails;
+  DBuf<Seg> segs;
+  DBuf<Visit> visits;
+  std::vector<u32> hn;
+  void alloc(Ctx& c, u32 nbm) {
+    if (nbm <= cap) return;
+    cap = nbm;
+    const size_t cps = SEG_SIZE / UM_CHUNK, slots = (size_t)nbm << SEG_SHIFT;
+    sym.alloc(c, slots);
+    selbuf.alloc(c, (size_t)nbm * SEL_CAP); tt.alloc(c, slots); symb.alloc(c, slots);
+    sums.alloc(c, nbm * cps); perms.alloc(c, nbm * cps * 256); lists.alloc(c, nbm * cps * 256); starts.alloc(c, nbm * cps);
+    keyA.alloc(c, slots); keyB.alloc(c, slots); valA.alloc(c, slots); valB.alloc(c, slots);
+    dn.alloc(c, nbm); nvis.alloc(c, nbm); tilesum.alloc(c, (size_t)nbm * UR_TPS);
+    segs.alloc(c, (size_t)nbm * IB_SEGS); visits.alloc(c, (size_t)nbm * IB_VCAP);
+    capr.alloc(c, (size_t)nbm * IB_SEGS); tails.alloc(c, (size_t)nbm * IB_VCAP); ntails.alloc(c, nbm);
+    hn.resize(nbm);
+  }
+};
+
+// One decode batch: the cnt block candidates dcand[0, cnt) of the input window `in` (wbytes bytes from bit base_bit of the
+// file; `last`: the window ends with the file) through the Huffman stage, un-MTF, the inverse BWT (into the slots at rle)
+// and the RLE1 length scan (count-byte classes into the slots at cls, tile offsets into tileoff).  Results in rb on the
+// device and in hres on the host.
+static void dec_batch(Ctx& c, DecScratch& B, const u8* in, u64 wbytes, u64 base_bit, bool last, const Cand* dcand, u32 cnt,
+                      CandRes* rb, CandRes* hres, u8* rle, u8* cls, u32* tileoff) {
+  // The kernels decode every candidate under the largest block size: the members of a multistream file may have
+  // different levels (lib/Bzip2.js:105-124 re-reads the level per member), and which member a candidate belongs to is
+  // only known when the host walks the chain, where the member's own limit is applied (block_event).
+  const u32 dbuf_size = 900000u;
+  const u32 cps = SEG_SIZE / UM_CHUNK, ur_tps = UR_TPS;
+  B.alloc(c, cnt);
+  dec_attr_once();
+  {
+    // the per-block Huffman stage is one CTA per block and latency bound: it gets the whole batch at once
+    StageScope ss(c, ST_HDEC);
+    static int sms = 0;
+    if (!sms) CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c.device));
+    if (cnt <= 2u * (u32)sms) k_hdec<512><<<cnt, 512, sizeof(HdecWarp), c.stream>>>(in, wbytes, base_bit, last, dcand, cnt, dbuf_size, B.selbuf, B.sym, rb);
+    else if (cnt <= 4u * (u32)sms) k_hdec<256><<<cnt, 256, sizeof(HdecWarp), c.stream>>>(in, wbytes, base_bit, last, dcand, cnt, dbuf_size, B.selbuf, B.sym, rb);
+    else k_hdec<HD_THREADS><<<cnt, HD_THREADS, sizeof(HdecWarp), c.stream>>>(in, wbytes, base_bit, last, dcand, cnt, dbuf_size, B.selbuf, B.sym, rb);
+    KLAUNCH(c); KCHECK();
+  }
+  {
+    StageScope ss(c, ST_UNMTF);
+    const u32 chunks = cnt * cps;
+    k_unmtf_a<<<(chunks + UA_THREADS - 1) / UA_THREADS, UA_THREADS, 0, c.stream>>>(B.sym, rb, cnt, cps, B.sums, B.perms, B.symb);
+    KLAUNCH(c); KCHECK();
+    k_unmtf_scan<<<cnt, 32, 0, c.stream>>>(rb, cnt, cps, dbuf_size, B.sums, B.perms, B.lists, B.starts);
+    KLAUNCH(c); KCHECK();
+    k_unmtf_map<<<(chunks + UM_WARPS - 1) / UM_WARPS, UM_WARPS * 32, 0, c.stream>>>(B.sym, B.symb, rb, cnt, cps, B.lists, B.starts, B.tt);
+    KLAUNCH(c); KCHECK();
+  }
+  CUDA_CHECK(cudaMemcpyAsync(hres, rb, sizeof(CandRes) * cnt, cudaMemcpyDeviceToHost, c.stream));
+  CUDA_CHECK(cudaStreamSynchronize(c.stream));
+  u32 nmax = 0; u64 ntot = 0;
+  for (u32 i = 0; i < cnt; i++) { B.hn[i] = hres[i].status == 0 ? hres[i].n : 0; nmax = std::max(nmax, B.hn[i]); ntot += B.hn[i]; }
+  if (nmax) {
+    StageScope ss(c, ST_IBWT);
+    CUDA_CHECK(cudaMemcpyAsync(B.dn, B.hn.data(), cnt * 4, cudaMemcpyHostToDevice, c.stream));
+    // T-vector: one stable counting-sort pass over the L column itself (byte keys, the values are the row numbers);
+    // the pass writes P[row] = successor << 8 | L[row] directly (radix.cuh: pack epilogue)
+    u8* kin = B.tt.p; u8* kout = nullptr;
+    u32 *vin = B.valA, *vout = B.valB;
+    u32* Pp = B.keyB;
+    radix_sort<u8>(c, kin, vin, kout, vout, B.dn, cnt, SEG_SHIFT, nmax, 0, 1, true, ntot, nullptr, B.tt.p, Pp);
+    // all blocks of the batch walk together: the launch lasts as long as its longest segment walk, so fewer,
+    // bigger launches win over keeping the packed T-vectors L2 resident (measured: 75 ms -> 36 ms per GiB).
+    // The walks record into the free key / value buffers of the sort (4 MiB per block each).
+    u8* slotA = reinterpret_cast<u8*>(B.keyA.p);
+    u8* slotB = reinterpret_cast<u8*>(B.valA.p);
+    k_ibwt_walk1<<<(cnt * IB_SEGS + 127) / 128, 128, 0, c.stream>>>(Pp, rb, cnt, B.segs, B.capr, slotA, slotB);
+    KLAUNCH(c); KCHECK();
+    k_ibwt_chain<<<cnt, 128, sizeof(Seg) * IB_SEGS, c.stream>>>(Pp, rb, cnt, B.segs, B.visits, B.nvis, B.tails, B.ntails);
+    KLAUNCH(c); KCHECK();
+    k_ibwt_place<<<cnt * IB_PLACE_CTAS, IB_PLACE_THREADS, 0, c.stream>>>(Pp, rb, cnt, B.visits, B.nvis, slotA, slotB, rle);
+    KLAUNCH(c); KCHECK();
+    k_ibwt_tail<<<(cnt * IB_VCAP + 127) / 128, 128, 0, c.stream>>>(Pp, rb, cnt, B.visits, B.nvis, B.tails, B.ntails, B.capr, rle);
+    KLAUNCH(c); KCHECK();
+  }
+  if (nmax) {
+    StageScope ss(c, ST_UNRLE);
+    const u32 nslots = cnt << SEG_SHIFT;
+    k_unrle_classify<<<(nslots / 8 + 255) / 256, 256, 0, c.stream>>>(rle, rb, cnt, cls);
+    KLAUNCH(c); KCHECK();
+    k_unrle_tilesum<<<cnt * ur_tps, UR_THREADS, 0, c.stream>>>(rle, cls, rb, ur_tps, B.tilesum);
+    KLAUNCH(c); KCHECK();
+    k_unrle_tileoff<<<cnt, 32, 0, c.stream>>>(rb, ur_tps, B.tilesum, tileoff);
+    KLAUNCH(c); KCHECK();
+    CUDA_CHECK(cudaMemcpyAsync(hres, rb, sizeof(CandRes) * cnt, cudaMemcpyDeviceToHost, c.stream));
+  }
+  CUDA_CHECK(cudaStreamSynchronize(c.stream));
+  c.stats.blocks += cnt;
+}
+
+// Expand the results [0, cnt) whose ob[i] is not ~0 (RLE1 decode of their slots at rle) to dout + ob[i], and CRC each
+// into got[i].  classify: the count-byte classes were not kept; find them again, into cls.
+static void dec_expand(Ctx& c, const u8* rle, u8* cls, bool classify, const CandRes* d_res, const CandRes* h_res, const u32* tileoff, u32 cnt,
+                       const u64* ob, u8* dout, u32* got) {
+  if (!cnt) return;
+  StageScope ss(c, ST_UNRLE);
+  DBuf<u64> dob(c, cnt);
+  CUDA_CHECK(cudaMemcpyAsync(dob, ob, 8 * (size_t)cnt, cudaMemcpyHostToDevice, c.stream));
+  if (classify) {
+    k_unrle_classify<<<(unsigned)((((size_t)cnt << SEG_SHIFT) / 8 + 255) / 256), 256, 0, c.stream>>>(rle, d_res, cnt, cls);
+    KLAUNCH(c); KCHECK();
+  }
+  k_unrle_emit<<<(unsigned)((size_t)cnt * UR_TPS), UR_THREADS, 0, c.stream>>>(rle, cls, d_res, UR_TPS, tileoff, dob, dout);
+  KLAUNCH(c); KCHECK();
+  std::vector<BlkInfo> ranges(cnt);
+  for (u32 i = 0; i < cnt; i++) {
+    memset(&ranges[i], 0, sizeof(BlkInfo));
+    if (ob[i] != ~0ull) { ranges[i].s = ob[i]; ranges[i].e = ob[i] + h_res[i].rawlen; }
+  }
+  DBuf<BlkInfo> dr(c, cnt);
+  DBuf<u32> dcrc(c, cnt);
+  CUDA_CHECK(cudaMemcpyAsync(dr, ranges.data(), sizeof(BlkInfo) * cnt, cudaMemcpyHostToDevice, c.stream));
+  crc_ranges(c, dout, dr, ranges, dcrc);
+  CUDA_CHECK(cudaMemcpyAsync(got, dcrc, 4 * (size_t)cnt, cudaMemcpyDeviceToHost, c.stream));
+  CUDA_CHECK(cudaStreamSynchronize(c.stream));
+}
+
+// ---- the block chain (lib/Bzip2.js:454-481 / 508-548) ----
+struct Chain {
+  size_t n = 0;             // bytes of the file
+  int multistream = 0;
+  u32 cur_dbuf = 0;         // dbufSize of the member the walk is in (lib/Bzip2.js:121)
+  u64 pos = 32;             // bit position of the next magic
+  u32 stream_crc = 0;
+  u64 total_out = 0;        // decoded bytes of the blocks walked
+  size_t li = 0;            // position list: the next entry
+  bool done = false;        // end of the stream reached, or an error recorded
+  std::vector<Event> events;
+};
+
+// a block on the chain; false when it ends the walk (its error is recorded)
+static bool block_event(Chain& ch, const Cand& cd, const CandRes& r, size_t slot) {
+  // the member's own limits, in the reference's order: randomised bit (:143), origPointer (:146), then the body
+  if (r.status != DEC_OBSOLETE && r.orig > ch.cur_dbuf) {
+    ch.events.push_back({2, slot, 0, 0, DEC_DATA_ERROR, "Data error: initial position out of bounds", ch.total_out, 0, 0});
+    return false;
+  }
+  if (r.status != 0) {
+    std::string msg = r.status == DEC_OBSOLETE ? "Obsolete (pre 0.9.5) bzip format not supported." : "Data error";
+    if (r.detail == 1) msg += ": initial position out of bounds";
+    ch.events.push_back({2, slot, 0, 0, r.status, msg, ch.total_out, 0, 0});
+    return false;
+  }
+  if (r.n > ch.cur_dbuf) {  // dbufCount would have run over dbufSize (lib/Bzip2.js:338,354)
+    ch.events.push_back({2, slot, 0, 0, DEC_DATA_ERROR, "Data error", ch.total_out, 0, 0});
+    return false;
+  }
+  ch.events.push_back({0, slot, cd.next32, 0, 0, "", ch.total_out, cd.pos, r.rawlen});
+  ch.total_out += r.rawlen;
+  return true;
+}
+
+// What the caller knows of the magic at a bit position.  kind: -1 nothing final yet (walk on later), 0 no magic,
+// 1 block (cd, its results r in slot), 2 end of stream (cd).
+struct At { int kind; const Cand* cd; const CandRes* r; size_t slot; };
+
+// Walk the chain from ch.pos as far as look() has final results.  head(bytepos, h) reads up to 4 bytes of the file at
+// bytepos for a member header and returns how many there are.
+template <class Look, class Head>
+static void chain_walk(Chain& ch, Look look, Head head) {
+  while (!ch.done) {
+    if ((ch.pos + 7) / 8 >= ch.n) { ch.done = true; break; }  // 'eof' in inputStream && inputStream.eof() (lib/Bzip2.js:462)
+    const At at = look(ch.pos);
+    if (at.kind < 0) return;
+    if (at.kind == 0) { ch.events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data", ch.total_out, 0, 0}); ch.done = true; break; }
+    if (at.kind == 1) {
+      ch.stream_crc = at.cd->next32 ^ ((ch.stream_crc << 1) | (ch.stream_crc >> 31));  // lib/Bzip2.js:138-139
+      if (!block_event(ch, *at.cd, *at.r, at.slot)) { ch.done = true; break; }
+      ch.pos = at.r->endbit;
+      continue;
+    }
+    ch.events.push_back({1, 0, ch.stream_crc, at.cd->next32, 0, "", ch.total_out, 0, 0});
+    ch.pos += 80;
+    const u64 bytepos = (ch.pos + 7) / 8;
+    if (!ch.multistream || bytepos >= ch.n) { ch.done = true; break; }
+    // _start_bunzip on the byte stream (resyncs to the next byte)
+    u8 h2[4] = {0, 0, 0, 0};
+    const size_t avail = head(bytepos, h2);
+    if (avail != 4 || h2[0] != 'B' || h2[1] != 'Z' || h2[2] != 'h') {
+      ch.events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data: bad magic", ch.total_out, 0, 0}); ch.done = true; break;
+    }
+    const int lv = h2[3] - 0x30;
+    if (lv < 1 || lv > 9) { ch.events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data: level out of range", ch.total_out, 0, 0}); ch.done = true; break; }
+    ch.cur_dbuf = (u32)lv * 100000u;
+    ch.stream_crc = 0;
+    ch.pos = (bytepos + 4) * 8;
+  }
+}
+
+// The same for a position list (lib/Bzip2.js:482-503 once per position), in list order: cands[i] is the magic at the
+// i-th position (type 0: none).  look(i, &r, &slot) gives a block's results, or false when they are not decoded yet.
+template <class Look>
+static void list_walk(Chain& ch, const std::vector<Cand>& cands, Look look) {
+  while (!ch.done) {
+    if (ch.li >= cands.size()) { ch.done = true; break; }
+    const Cand& cd = cands[ch.li];
+    if (cd.type == 0) { ch.events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data", ch.total_out, 0, 0}); ch.done = true; break; }
+    if (cd.type == 2) { ch.events.push_back({3, 0, 0, 0, 0, "", ch.total_out, 0, 0}); ch.li++; continue; }
+    const CandRes* r = nullptr; size_t slot = 0;
+    if (!look(ch.li, &r, &slot)) return;
+    if (!block_event(ch, cd, *r, slot)) { ch.done = true; break; }
+    ch.li++;
+  }
+}
+
+// The first failure in stream order: event index, code, message, and the bytes the reference has written when it throws
+// (a block's own bytes go out before its CRC check).
+struct DecErr { long ev = -1; int code = 0; std::string msg; u64 prefix = 0; };
+
+// Replay events [e0, e1) up to the first failure, which goes to E: block CRCs against got(slot) = {known, crc} (a block
+// whose CRC is not known here passes: another rank checks it), stream CRCs unless for a table; the table rows and list
+// ends of everything in front of the failure.
+template <class Got>
+static void replay(const Chain& ch, size_t e0, size_t e1, Got got, std::vector<u64>* tab_pos, std::vector<u32>* tab_len,
+                   std::vector<u64>* ends, DecErr& E) {
+  for (size_t ei = e0; ei < e1 && E.ev < 0; ei++) {
+    const Event& ev = ch.events[ei];
+    if (ev.kind == 0) {
+      const std::pair<bool, u32> g = got(ev.slot);
+      if (g.first && g.second != ev.a) {
+        E.ev = (long)ei; E.code = DEC_DATA_ERROR; E.msg = "Data error: Bad block CRC (got " + hexs(g.second) + " expected " + hexs(ev.a) + ")";
+        E.prefix = ev.off + ev.len;
+      }
+      if (E.ev < 0 && tab_pos) { tab_pos->push_back(ev.pos); tab_len->push_back(ev.len); }
+    } else if (ev.kind == 1) {
+      if (!tab_pos && ev.a != ev.b) {
+        E.ev = (long)ei; E.code = DEC_DATA_ERROR; E.msg = "Data error: Bad stream CRC (got " + hexs(ev.a) + " expected " + hexs(ev.b) + ")";
+        E.prefix = ev.off;
+      }
+    } else if (ev.kind == 2) {
+      E.ev = (long)ei; E.code = ev.code; E.msg = ev.msg; E.prefix = ev.off;
+    }
+    if (ends && E.ev < 0) ends->push_back(ev.kind == 0 ? ev.off + ev.len : ev.off);
+  }
+}
+
+static void read_level(const u8* hdr, size_t n, u32* dbuf_size) {
+  // lib/Bzip2.js:105-124 _start_bunzip
+  if (n < 4 || hdr[0] != 'B' || hdr[1] != 'Z' || hdr[2] != 'h') throw B2Error{DEC_NOT_BZIP, "Not bzip data: bad magic"};
+  const int level = hdr[3] - 0x30;
+  if (level < 1 || level > 9) throw B2Error{DEC_NOT_BZIP, "Not bzip data: level out of range"};
+  *dbuf_size = 100000u * (u32)level;
+}
+
+// Every magic of the window `in` (wbytes bytes from bit base_bit of the file) below window bit lim, sorted by position.
+static void scan_window(Ctx& c, const u8* in, u64 wbytes, u64 base_bit, u64 lim, std::vector<Cand>& cands) {
+  StageScope ss(c, ST_SCAN);
+  // Highly repetitive input compresses to a few dozen bytes per block (and multistream files may hold thousands of
+  // tiny members), so the number of magics is not bounded by the usual ~100 KB per block: when the first guess is too
+  // small the scan counts them all and runs once more with exactly that capacity.
+  u32 cap = (u32)(wbytes / 8000 + 1024);
+  DBuf<Cand> dc(c, cap);
+  DBuf<u32> dcount(c, 1);
+  u32 cnt = 0;
+  for (int attempt = 0; attempt < 2; attempt++) {
+    CUDA_CHECK(cudaMemsetAsync(dcount, 0, 4, c.stream));
+    k_scan_magic<<<(unsigned)(((wbytes + 3) / 4 + 255) / 256), 256, 0, c.stream>>>(in, wbytes, base_bit, lim, dc, dcount, cap);
+    KLAUNCH(c); KCHECK();
+    CUDA_CHECK(cudaMemcpyAsync(&cnt, dcount, 4, cudaMemcpyDeviceToHost, c.stream));
+    CUDA_CHECK(cudaStreamSynchronize(c.stream));
+    if (cnt <= cap) break;
+    cap = cnt;
+    dc.alloc(c, cap);
+  }
+  if (cnt > cap) throw B2Error{B2_ERR_CUDA, "magic scan did not settle"};
+  cands.resize(cnt);
+  if (cnt) CUDA_CHECK(cudaMemcpyAsync(cands.data(), dc, sizeof(Cand) * cnt, cudaMemcpyDeviceToHost, c.stream));
+  CUDA_CHECK(cudaStreamSynchronize(c.stream));
+  std::sort(cands.begin(), cands.end(), [](const Cand& a, const Cand& b) { return a.pos < b.pos; });
+}
+
+// ---- single-GPU decode: one rolling loop over input windows and decode batches --------------------------------------
+// The compressed input is h_in (host) or d_in (device), n bytes.  Only the window [a, a + W) of it is on the device
+// (W = dec_window(); a is the chain's position, rounded down to 256 bytes).  The window's magics are decoded in position
+// order, a batch at a time; after each batch the host walks the chain as far as final results allow, and the blocks that
+// walk settled are expanded, CRC-checked and delivered.  The first chain position without a final result starts the next
+// window; a window that would start where this one did is twice as long, so a block longer than W still decodes.
+// Delivery: d_out (device, absolute offsets, nothing past out_cap), or the table rows (tab_pos / tab_len: expanded only
+// for the CRCs), or else *h_out (host, grown from alloc_host / free_host; owned by the caller, also when this throws),
+// through a device staging buffer of at most max(W, one block) bytes.
+// positions: decode the blocks at these bit positions, back to back in list order (ends: the end offset of every
+// position delivered in full), with the whole input on the device.
+int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multistream, u8* d_out, size_t out_cap, size_t* out_n,
+                     const std::vector<u64>* positions, std::vector<u64>* ends, std::vector<u64>* tab_pos, std::vector<u32>* tab_len,
+                     void* (*alloc_host)(size_t), void (*free_host)(void*), u8** h_out) {
+  *out_n = 0;
+  // with neither d_out nor h_out (a table, or a device call without a buffer) the blocks are expanded only for their CRCs
+  const bool dev = d_out != nullptr, listed = positions != nullptr;
+  auto read_in = [&](u8* dst, u64 off, size_t len) {
+    if (!len) return;
+    if (h_in) { memcpy(dst, h_in + off, len); return; }
+    CUDA_CHECK(cudaMemcpyAsync(dst, d_in + off, len, cudaMemcpyDeviceToHost, c.stream));
+    CUDA_CHECK(cudaStreamSynchronize(c.stream));
+  };
+  Chain ch;
+  {
+    u8 hdr[4] = {0, 0, 0, 0};
+    read_in(hdr, 0, std::min<size_t>(n, 4));
+    read_level(hdr, n, &ch.cur_dbuf);
+  }
+  ch.n = n;
+  ch.multistream = listed ? 0 : multistream;
+  const size_t W = dec_window();
+  const u32 DB = dec_batch_blocks(c);
+  DecScratch B;
+  DBuf<u8> win, rle, cls, stage;
+  DBuf<u32> tileoff;
+  DBuf<CandRes> dres;
+  DBuf<Cand> dcand;
+  size_t win_cap = 0, slots = 0, stage_cap = 0, h_cap = 0;
+  std::vector<Cand> cands;
+  std::vector<size_t> blk;      // block candidates of the window (index into cands)
+  std::vector<CandRes> hres;    // results of the batch
+  std::vector<u32> got;
+  std::vector<u64> ob;
+  std::vector<size_t> settled;  // block events of the batch
+  DecErr E;
+  u64 prev_a = ~0ull;
+  size_t wcur = W;
+  auto head = [&](u64 bytepos, u8* h) -> size_t {
+    const size_t avail = (size_t)std::min<u64>(4, n - bytepos);
+    read_in(h, bytepos, avail);
+    return avail;
+  };
+  // *h_out must hold the decoded bytes [0, need), of which `have` are there: it doubles, or gets the exact size when the
+  // stream is known to end there (a call of one batch: one buffer, one copy)
+  auto host_reserve = [&](u64 need, u64 have, bool final_size) {
+    if (need <= h_cap) return;
+    const size_t cap = final_size ? (size_t)need : std::max<size_t>((size_t)need, 2 * h_cap);
+    u8* p = (u8*)alloc_host(cap);
+    if (*h_out) {
+      CUDA_CHECK(cudaStreamSynchronize(c.stream));
+      memcpy(p, *h_out, (size_t)have);
+      free_host(*h_out);
+    }
+    *h_out = p; h_cap = cap;
+  };
+  u64 h_have = 0;  // bytes delivered to *h_out
+  while (!ch.done && (E.ev < 0 || dev)) {
+    // ---- 1. the input window ----
+    const u64 a = listed ? 0 : (ch.pos >> 3) & ~(u64)255;
+    wcur = a == prev_a ? wcur * 2 : W;
+    prev_a = a;
+    const u64 wl = listed ? n : std::min<u64>(wcur, n - a);
+    const bool last = a + wl == n;
+    if (wl + 32 > win_cap) { win.alloc(c, wl + 32); win_cap = wl + 32; }
+    // zero padded (aligned word reads past the end must be safe)
+    CUDA_CHECK(cudaMemsetAsync(win.p + (wl & ~(u64)3), 0, 32 + (wl & 3), c.stream));
+    if (h_in) {
+      StageScope s(c, ST_H2D);
+      if (wl) CUDA_CHECK(cudaMemcpyAsync(win, h_in + a, wl, cudaMemcpyHostToDevice, c.stream));
+    } else if (wl) {
+      CUDA_CHECK(cudaMemcpyAsync(win, d_in + a, wl, cudaMemcpyDeviceToDevice, c.stream));
+    }
+    cands.clear(); blk.clear();
+    if (listed) {
+      // only the given positions are tested; the first one without a magic raises "Not bzip data", so nothing behind it
+      // is decoded
+      StageScope ss(c, ST_SCAN);
+      const size_t np = positions->size();
+      DBuf<u64> dpos(c, np ? np : 1);
+      DBuf<Cand> dc(c, np ? np : 1);
+      cands.resize(np);
+      if (np) {
+        CUDA_CHECK(cudaMemcpyAsync(dpos, positions->data(), 8 * np, cudaMemcpyHostToDevice, c.stream));
+        k_magic_at<<<(unsigned)((np + 255) / 256), 256, 0, c.stream>>>(win, n, dpos, np, dc);
+        KLAUNCH(c); KCHECK();
+        CUDA_CHECK(cudaMemcpyAsync(cands.data(), dc, sizeof(Cand) * np, cudaMemcpyDeviceToHost, c.stream));
+      }
+      CUDA_CHECK(cudaStreamSynchronize(c.stream));
+      for (size_t i = 0; i < np; i++) if (cands[i].type == 0) { cands.resize(i + 1); break; }
+    } else {
+      // a magic whose 80 bits (magic + CRC) run past the window's end belongs to the next window
+      const u64 lim = last ? wl * 8 : (wl * 8 >= 80 ? wl * 8 - 79 : 0);
+      scan_window(c, win, wl, a * 8, lim, cands);
+    }
+    for (size_t i = 0; i < cands.size(); i++) if (cands[i].type == 1) blk.push_back(i);
+    const size_t nbm = std::min<size_t>(DB, blk.size());
+    if (nbm > slots) {
+      // per-batch state, kept for the largest batch of the call
+      rle.alloc(c, nbm << SEG_SHIFT); cls.alloc(c, nbm << SEG_SHIFT); tileoff.alloc(c, nbm * UR_TPS);
+      dres.alloc(c, nbm); dcand.alloc(c, nbm);
+      slots = nbm;
+    }
+    auto first_blk_from = [&](u64 pos) {
+      return (size_t)(std::lower_bound(blk.begin(), blk.end(), pos, [&](size_t ci, u64 p) { return cands[ci].pos < p; }) - blk.begin());
+    };
+    size_t kb = listed ? 0 : first_blk_from(ch.pos);
+    // ---- 2. batches ----
+    for (;;) {
+      const u32 cnt = (u32)std::min<size_t>(DB, blk.size() - kb);
+      if (cnt) {
+        std::vector<Cand> bc(cnt);
+        for (u32 i = 0; i < cnt; i++) bc[i] = cands[blk[kb + i]];
+        CUDA_CHECK(cudaMemcpyAsync(dcand, bc.data(), sizeof(Cand) * cnt, cudaMemcpyHostToDevice, c.stream));
+        hres.resize(cnt);
+        dec_batch(c, B, win, wl, a * 8, last, dcand, cnt, dres, hres.data(), rle, cls, tileoff);
+      }
+      // ---- 3. walk ----
+      bool need_window = false;
+      const size_t e0 = ch.events.size();
+      if (listed) {
+        list_walk(ch, cands, [&](size_t li, const CandRes** r, size_t* slot) {
+          const size_t j = (size_t)(std::lower_bound(blk.begin(), blk.end(), li) - blk.begin());
+          if (j >= kb + cnt) return false;
+          *r = &hres[j - kb]; *slot = j - kb;
+          return true;
+        });
+      } else {
+        chain_walk(ch, [&](u64 pos) -> At {
+          const auto it = std::lower_bound(cands.begin(), cands.end(), pos, [](const Cand& x, u64 p) { return x.pos < p; });
+          if (it == cands.end() || it->pos != pos) {
+            if (!last && pos + 80 > (a + wl) * 8) { need_window = true; return {-1, nullptr, nullptr, 0}; }
+            return {0, nullptr, nullptr, 0};
+          }
+          if (it->type == 2) return {2, &*it, nullptr, 0};
+          const size_t j = first_blk_from(pos);
+          if (j >= kb + cnt) return {-1, nullptr, nullptr, 0};  // in a later batch of this window
+          const CandRes& r = hres[j - kb];
+          if (r.open) { need_window = true; return {-1, nullptr, nullptr, 0}; }
+          return {1, &*it, &r, j - kb};
+        }, head);
+      }
+      const size_t e1 = ch.events.size();
+      // ---- 4. expand and deliver the blocks this walk settled ----
+      settled.clear();
+      for (size_t ei = e0; ei < e1; ei++) if (ch.events[ei].kind == 0) settled.push_back(ei);
+      got.assign(cnt ? cnt : 1, 0);
+      ob.assign(cnt ? cnt : 1, ~0ull);
+      if (dev) {
+        // straight to the caller's buffer; a block that does not fit is only counted (the needed size is returned)
+        for (size_t ei : settled) { const Event& ev = ch.events[ei]; if (ev.off + ev.len <= out_cap) ob[ev.slot] = ev.off; }
+        if (!settled.empty()) dec_expand(c, rle, cls, false, dres, hres.data(), tileoff, cnt, ob.data(), d_out, got.data());
+      } else {
+        // through the staging buffer, groups of consecutive blocks of at most max(W, one block) bytes
+        for (size_t g0 = 0; g0 < settled.size();) {
+          const Event& f = ch.events[settled[g0]];
+          u64 bytes = f.len;
+          size_t g1 = g0 + 1;
+          while (g1 < settled.size() && bytes + ch.events[settled[g1]].len <= W) bytes += ch.events[settled[g1++]].len;
+          const size_t s0 = f.slot, s1 = ch.events[settled[g1 - 1]].slot + 1;
+          for (size_t g = g0; g < g1; g++) { const Event& ev = ch.events[settled[g]]; ob[ev.slot] = ev.off - f.off; }
+          if (bytes > stage_cap) { stage.alloc(c, bytes); stage_cap = bytes; }
+          dec_expand(c, rle.p + (s0 << SEG_SHIFT), cls.p + (s0 << SEG_SHIFT), false, dres.p + s0, hres.data() + s0, tileoff.p + s0 * UR_TPS,
+                     (u32)(s1 - s0), ob.data() + s0, stage, got.data() + s0);
+          if (h_out && bytes) {
+            host_reserve(f.off + bytes, h_have, ch.done && g1 == settled.size());
+            StageScope s(c, ST_D2H);
+            CUDA_CHECK(cudaMemcpyAsync(*h_out + f.off, stage, bytes, cudaMemcpyDeviceToHost, c.stream));
+            h_have = f.off + bytes;
+          }
+          g0 = g1;
+        }
+      }
+      // ---- replay: the first failure in stream order ends the call (the device path walks on for the needed size) ----
+      if (E.ev < 0)
+        replay(ch, e0, e1, [&](size_t slot) { return std::make_pair(ob[slot] != ~0ull, got[slot]); }, tab_pos, tab_len, ends, E);
+      if (ch.done || (E.ev >= 0 && !dev) || need_window) break;
+      const size_t nk = listed ? kb + cnt : first_blk_from(ch.pos);
+      if (nk <= kb) throw B2Error{B2_ERR_CUDA, "bzip2 decode: the chain walk made no progress"};
+      kb = nk;
+    }
+  }
+  CUDA_CHECK(cudaStreamSynchronize(c.stream));
+  if (dev && ch.total_out > out_cap) {
+    *out_n = (size_t)ch.total_out;
+    throw B2Error{B2_ERR_BAD_ARG, "output buffer too small"};
+  }
+  if (E.ev >= 0) {
+    // the host path hands the output in front of the error to the caller with the error (b2_bzip2_decompress_partial)
+    if (h_out) *out_n = (size_t)E.prefix;
+    throw B2Error{E.code, E.msg};
+  }
+  *out_n = (size_t)ch.total_out;
+  return 0;
+}
+
+// ---- sharded decode (SURVEY.md section 8e): open on every rank, exchange results, finish ------------
+// open() parses the header, finds every block candidate of the whole file and decodes the share [lo, hi) of them;
+// finish() walks the chain over ALL candidates' results (imported from the other ranks), expands + CRC-checks the blocks
+// of the own share and raises the reference's errors in stream order.  A rank keeps its share's results until the
+// all-gather, so its device memory grows with its share of the file.
+struct DecSession {
+  size_t n = 0;
+  u32 dbuf_size = 0;
+  DBuf<u8> din;                    // the whole file, zero padded
+  std::vector<Cand> cands;         // every magic found, sorted by position
+  std::vector<size_t> blk_idx;     // block candidates (index into cands)
+  std::vector<CandRes> hres;       // per block candidate (valid for [lo,hi) after open, for all after import)
+  size_t lo = 0, hi = 0;           // own share of the block candidates
+  DBuf<Cand> dcand;
+  DBuf<CandRes> dres;              // own share only
+  DBuf<u8> rle, cls;               // cls (count-byte classes) is kept for the whole share only while that is cheap (keep_cls)
+  bool keep_cls = true;
+  DBuf<u32> tileoff;
+};
+
+static void dec_open(Ctx& c, DecSession& S, const u8* d_in_user, size_t n, int rank, int world) {
+  S.n = n;
   // padded private copy of the input (aligned word reads past the end must be safe)
   S.din.alloc(c, n + 32);
   CUDA_CHECK(cudaMemsetAsync(S.din.p + (n & ~(size_t)3), 0, (n + 32) - (n & ~(size_t)3), c.stream));
@@ -1160,78 +1662,23 @@ static void dec_open(Ctx& c, DecSession& S, const u8* d_in_user, size_t n, const
   u8 hdr[4] = {0, 0, 0, 0};
   if (n >= 4) CUDA_CHECK(cudaMemcpyAsync(hdr, S.din, 4, cudaMemcpyDeviceToHost, c.stream));
   CUDA_CHECK(cudaStreamSynchronize(c.stream));
-  // lib/Bzip2.js:105-124 _start_bunzip
-  if (n < 4 || hdr[0] != 'B' || hdr[1] != 'Z' || hdr[2] != 'h') throw B2Error{DEC_NOT_BZIP, "Not bzip data: bad magic"};
-  int level = hdr[3] - 0x30;
-  if (level < 1 || level > 9) throw B2Error{DEC_NOT_BZIP, "Not bzip data: level out of range"};
-  S.dbuf_size = 100000u * (u32)level;
-  // The kernels decode every candidate under the largest block size: the members of a multistream file may have
-  // different levels (lib/Bzip2.js:105-124 re-reads the level per member), and which member a candidate belongs to is
-  // only known when the host walks the chain, where the member's own limit is applied (dec_finish).
-  const u32 dbuf_size = 900000u;
-  const u8* din = S.din;
-
-  // ---- 1. candidates ----
-  std::vector<Cand>& cands = S.cands;
-  std::vector<size_t>& blk_idx = S.blk_idx;
-  if (positions) {
-    // lib/Bzip2.js:482-503 once per position: seekBit(pos), then one _get_next_block.  Only the given positions are
-    // tested; the first one without a magic raises "Not bzip data", so nothing behind it is decoded.
-    StageScope ss(c, ST_SCAN);
-    const size_t np = positions->size();
-    DBuf<u64> dpos(c, np ? np : 1);
-    DBuf<Cand> dc(c, np ? np : 1);
-    cands.resize(np);
-    if (np) {
-      CUDA_CHECK(cudaMemcpyAsync(dpos, positions->data(), 8 * np, cudaMemcpyHostToDevice, c.stream));
-      k_magic_at<<<(unsigned)((np + 255) / 256), 256, 0, c.stream>>>(din, n, dpos, np, dc);
-      KLAUNCH(c); KCHECK();
-      CUDA_CHECK(cudaMemcpyAsync(cands.data(), dc, sizeof(Cand) * np, cudaMemcpyDeviceToHost, c.stream));
-    }
-    CUDA_CHECK(cudaStreamSynchronize(c.stream));
-    for (size_t i = 0; i < np; i++) {
-      if (cands[i].type == 0) { cands.resize(i + 1); break; }
-      if (cands[i].type == 1) blk_idx.push_back(i);
-    }
-  } else {
-    StageScope ss(c, ST_SCAN);
-    // Highly repetitive input compresses to a few dozen bytes per block (and multistream files may hold thousands of
-    // tiny members), so the number of magics is not bounded by the usual ~100 KB per block: when the first guess is too
-    // small the scan counts them all and runs once more with exactly that capacity.
-    u32 cap = (u32)(n / 8000 + 1024);
-    DBuf<Cand> dc(c, cap);
-    DBuf<u32> dcount(c, 1);
-    u32 cnt = 0;
-    for (int attempt = 0; attempt < 2; attempt++) {
-      CUDA_CHECK(cudaMemsetAsync(dcount, 0, 4, c.stream));
-      k_scan_magic<<<(unsigned)(((n + 3) / 4 + 255) / 256), 256, 0, c.stream>>>(din, n, dc, dcount, cap);
-      KLAUNCH(c); KCHECK();
-      CUDA_CHECK(cudaMemcpyAsync(&cnt, dcount, 4, cudaMemcpyDeviceToHost, c.stream));
-      CUDA_CHECK(cudaStreamSynchronize(c.stream));
-      if (cnt <= cap) break;
-      cap = cnt;
-      dc.alloc(c, cap);
-    }
-    if (cnt > cap) throw B2Error{B2_ERR_CUDA, "magic scan did not settle"};
-    cands.resize(cnt);
-    if (cnt) CUDA_CHECK(cudaMemcpyAsync(cands.data(), dc, sizeof(Cand) * cnt, cudaMemcpyDeviceToHost, c.stream));
-    CUDA_CHECK(cudaStreamSynchronize(c.stream));
-    std::sort(cands.begin(), cands.end(), [](const Cand& a, const Cand& b) { return a.pos < b.pos; });
-    for (size_t i = 0; i < cands.size(); i++) if (cands[i].type == 1) blk_idx.push_back(i);
-  }
-  const size_t nb_all = blk_idx.size();
-  S.bc.resize(nb_all);
-  for (size_t i = 0; i < nb_all; i++) S.bc[i] = cands[blk_idx[i]];
+  read_level(hdr, n, &S.dbuf_size);
+  scan_window(c, S.din, n, 0, n * 8, S.cands);
+  for (size_t i = 0; i < S.cands.size(); i++) if (S.cands[i].type == 1) S.blk_idx.push_back(i);
+  const size_t nb_all = S.blk_idx.size();
+  std::vector<Cand> bc(nb_all);
+  for (size_t i = 0; i < nb_all; i++) bc[i] = S.cands[S.blk_idx[i]];
   S.hres.assign(nb_all, CandRes());
   for (auto& r : S.hres) { memset(&r, 0, sizeof r); r.status = DEC_DATA_ERROR; }
   S.lo = (size_t)rank * nb_all / (size_t)world;
   S.hi = (size_t)(rank + 1) * nb_all / (size_t)world;
   const size_t nb = S.hi - S.lo;
+  const u32 DB = dec_batch_blocks(c);
   {
     // every block of the own share keeps 2 MiB (L column + count-byte classes; 1 MiB beyond DEC_KEEP_CLS blocks) until the
     // stream is assembled, and a batch of up to 2048 blocks needs ~20 MiB of scratch per block: say so instead of failing
     // inside an allocation
-    const size_t need = nb * ((size_t)(nb <= dec_keep_cls_limit() ? 2 : 1) << 20) + std::min<size_t>(nb, dec_batch_blocks(c)) * ((size_t)20 << 20) + n;
+    const size_t need = nb * ((size_t)(nb <= dec_keep_cls_limit() ? 2 : 1) << 20) + std::min<size_t>(nb, DB) * ((size_t)20 << 20) + n;
     // memory the stream-ordered pool holds but does not use is available too: when that covers the call (every call
     // after the first of a kind) the driver is not asked at all -- cudaMemGetInfo takes milliseconds on a busy context
     uint64_t reserved = 0, used = 0;
@@ -1247,8 +1694,8 @@ static void dec_open(Ctx& c, DecSession& S, const u8* d_in_user, size_t n, const
       if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess) {
         if (need > free_b + spare) {
           char msg[256];
-          snprintf(msg, sizeof msg, "stream of %zu blocks needs about %zu MiB of device memory for one call (%zu MiB free): decode it in parts "
-                                    "(Bzip2.table + decompressBlocks) or over several GPUs (decompress_file_sharded)", nb, need >> 20, free_b >> 20);
+          snprintf(msg, sizeof msg, "stream of %zu blocks needs about %zu MiB of device memory for one sharded call (%zu MiB free): decode it "
+                                    "on more GPUs, or on one (decompressFile), whose device memory does not grow with the file", nb, need >> 20, free_b >> 20);
           throw B2Error{B2_ERR_CUDA, msg};
         }
       } else cudaGetLastError();
@@ -1258,314 +1705,87 @@ static void dec_open(Ctx& c, DecSession& S, const u8* d_in_user, size_t n, const
   S.dres.alloc(c, nb ? nb : 1);
   S.rle.alloc(c, (nb ? nb : 1) << SEG_SHIFT);
   // The count-byte classes of a block are needed twice (length scan here, expansion in dec_finish).  Up to DEC_KEEP_CLS
-  // blocks they stay on the device in between; a stream of more blocks (tens of GB of level-1 data) keeps only the L
+  // blocks they stay on the device in between; a share of more blocks (tens of GB of level-1 data) keeps only the L
   // columns (1 MiB per block) and classifies a second time, batch by batch, when it expands them.
   S.keep_cls = nb <= dec_keep_cls_limit();
-  const u32 DBc = dec_batch_blocks(c);
-  S.cls.alloc(c, (size_t)(S.keep_cls ? (nb ? nb : 1) : std::min<size_t>(nb, DBc)) << SEG_SHIFT);
+  S.cls.alloc(c, (size_t)(S.keep_cls ? (nb ? nb : 1) : std::min<size_t>(nb, DB)) << SEG_SHIFT);
   S.tileoff.alloc(c, (nb ? nb : 1) * (size_t)UR_TPS);
-  if (nb_all) CUDA_CHECK(cudaMemcpyAsync(S.dcand, S.bc.data(), sizeof(Cand) * nb_all, cudaMemcpyHostToDevice, c.stream));
-  CUDA_CHECK(cudaStreamSynchronize(c.stream));
-  CandRes* hres = S.hres.data() + S.lo;  // own share
-  Cand* dcand = S.dcand.p + S.lo;
-  DBuf<CandRes>& dres = S.dres;
-  DBuf<u8>& rle = S.rle; DBuf<u8>& cls = S.cls; DBuf<u32>& tileoff = S.tileoff;
-  const u32 ur_tps = UR_TPS;
-
-  // ---- 2. decode the own share of the candidate blocks, in batches ----
-  // the per-block Huffman stage is one CTA per block and latency bound: give it every block at once
-  // (about 19 MB of scratch per block: a batch of 2048 takes about half of an 80 GB H100)
-  const u32 DB = dec_batch_blocks(c);
-  dec_attr_once();
-  if (nb) {
-    const u32 nbm = (u32)std::min<size_t>(DB, nb);
-    DBuf<u16> sym(c, (size_t)nbm << SEG_SHIFT);
-    DBuf<u8> selbuf(c, (size_t)nbm * SEL_CAP), tt(c, (size_t)nbm << SEG_SHIFT), symb(c, (size_t)nbm << SEG_SHIFT);
-    const u32 cps = SEG_SIZE / UM_CHUNK;
-    DBuf<ChunkSum> sums(c, (size_t)nbm * cps);
-    DBuf<u8> perms(c, (size_t)nbm * cps * 256), lists(c, (size_t)nbm * cps * 256);
-    DBuf<ChunkStart> starts(c, (size_t)nbm * cps);
-    DBuf<u32> keyA(c, (size_t)nbm << SEG_SHIFT), keyB(c, (size_t)nbm << SEG_SHIFT), valA(c, (size_t)nbm << SEG_SHIFT), valB(c, (size_t)nbm << SEG_SHIFT);
-    DBuf<u32> dn(c, nbm), nvis(c, nbm), tilesum(c, (size_t)nbm * ur_tps);
-    DBuf<Seg> segs(c, (size_t)nbm * IB_SEGS);
-    DBuf<Visit> visits(c, (size_t)nbm * IB_VCAP);
-    DBuf<u32> capr(c, (size_t)nbm * IB_SEGS), tails(c, (size_t)nbm * IB_VCAP), ntails(c, nbm);
-    std::vector<u32> hn(nbm);
-    for (size_t k0 = 0; k0 < nb; k0 += DB) {
-      const u32 cnt = (u32)std::min<size_t>(DB, nb - k0);
-      CandRes* rb = dres.p + k0;
-      {
-        StageScope ss(c, ST_HDEC);
-        static int sms = 0;
-        if (!sms) CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c.device));
-        if (cnt <= 2u * (u32)sms) k_hdec<512><<<cnt, 512, sizeof(HdecWarp), c.stream>>>(din, n, dcand, (u32)k0, cnt, dbuf_size, selbuf, sym, rb);
-        else if (cnt <= 4u * (u32)sms) k_hdec<256><<<cnt, 256, sizeof(HdecWarp), c.stream>>>(din, n, dcand, (u32)k0, cnt, dbuf_size, selbuf, sym, rb);
-        else k_hdec<HD_THREADS><<<cnt, HD_THREADS, sizeof(HdecWarp), c.stream>>>(din, n, dcand, (u32)k0, cnt, dbuf_size, selbuf, sym, rb);
-        KLAUNCH(c); KCHECK();
-      }
-      {
-        StageScope ss(c, ST_UNMTF);
-        const u32 chunks = cnt * cps;
-        k_unmtf_a<<<(chunks + UA_THREADS - 1) / UA_THREADS, UA_THREADS, 0, c.stream>>>(sym, rb, cnt, cps, sums, perms, symb);
-        KLAUNCH(c); KCHECK();
-        k_unmtf_scan<<<cnt, 32, 0, c.stream>>>(rb, cnt, cps, dbuf_size, sums, perms, lists, starts);
-        KLAUNCH(c); KCHECK();
-        k_unmtf_map<<<(chunks + UM_WARPS - 1) / UM_WARPS, UM_WARPS * 32, 0, c.stream>>>(sym, symb, rb, cnt, cps, lists, starts, tt);
-        KLAUNCH(c); KCHECK();
-      }
-      CUDA_CHECK(cudaMemcpyAsync(hres + k0, rb, sizeof(CandRes) * cnt, cudaMemcpyDeviceToHost, c.stream));
-      CUDA_CHECK(cudaStreamSynchronize(c.stream));
-      u32 nmax = 0; u64 ntot = 0;
-      for (u32 i = 0; i < cnt; i++) { hn[i] = hres[k0 + i].status == 0 ? hres[k0 + i].n : 0; nmax = std::max(nmax, hn[i]); ntot += hn[i]; }
-      if (nmax) {
-        StageScope ss(c, ST_IBWT);
-        CUDA_CHECK(cudaMemcpyAsync(dn, hn.data(), cnt * 4, cudaMemcpyHostToDevice, c.stream));
-        // T-vector: one stable counting-sort pass over the L column itself (byte keys, the values are the row numbers);
-        // the pass writes P[row] = successor << 8 | L[row] directly (radix.cuh: pack epilogue)
-        u8* kin = tt.p; u8* kout = nullptr;
-        u32 *vin = valA, *vout = valB;
-        u32* Pp = keyB;
-        radix_sort<u8>(c, kin, vin, kout, vout, dn, cnt, SEG_SHIFT, nmax, 0, 1, true, ntot, nullptr, tt.p, Pp);
-        // all blocks of the batch walk together: the launch lasts as long as its longest segment walk, so fewer,
-        // bigger launches win over keeping the packed T-vectors L2 resident (measured: 75 ms -> 36 ms per GiB)
-        const u32 ib_sub = cnt;
-        for (u32 s0 = 0; s0 < cnt; s0 += ib_sub) {
-          const u32 sc = std::min<u32>(ib_sub, cnt - s0);
-          const u32* Ps = Pp + ((size_t)s0 << SEG_SHIFT);
-          // the walks record into the free key / value buffers of the sort (4 MiB per block each)
-          u8* slotA = reinterpret_cast<u8*>(keyA.p) + ((size_t)s0 << (SEG_SHIFT + 2));
-          u8* slotB = reinterpret_cast<u8*>(valA.p) + ((size_t)s0 << (SEG_SHIFT + 2));
-          k_ibwt_walk1<<<(sc * IB_SEGS + 127) / 128, 128, 0, c.stream>>>(Ps, rb + s0, sc, segs.p + (size_t)s0 * IB_SEGS, capr.p + (size_t)s0 * IB_SEGS, slotA, slotB);
-          KLAUNCH(c); KCHECK();
-          k_ibwt_chain<<<sc, 128, sizeof(Seg) * IB_SEGS, c.stream>>>(Ps, rb + s0, sc, segs.p + (size_t)s0 * IB_SEGS, visits.p + (size_t)s0 * IB_VCAP, nvis.p + s0,
-                                                                   tails.p + (size_t)s0 * IB_VCAP, ntails.p + s0);
-          KLAUNCH(c); KCHECK();
-          u8* ob = rle.p + ((k0 + s0) << SEG_SHIFT);
-          k_ibwt_place<<<sc * IB_PLACE_CTAS, IB_PLACE_THREADS, 0, c.stream>>>(Ps, rb + s0, sc, visits.p + (size_t)s0 * IB_VCAP, nvis.p + s0, slotA, slotB, ob);
-          KLAUNCH(c); KCHECK();
-          k_ibwt_tail<<<(sc * IB_VCAP + 127) / 128, 128, 0, c.stream>>>(Ps, rb + s0, sc, visits.p + (size_t)s0 * IB_VCAP, nvis.p + s0,
-                                                                      tails.p + (size_t)s0 * IB_VCAP, ntails.p + s0, capr.p + (size_t)s0 * IB_SEGS, ob);
-          KLAUNCH(c); KCHECK();
-        }
-      }
-      if (nmax) {
-        StageScope ss(c, ST_UNRLE);
-        const u32 nslots = cnt << SEG_SHIFT;
-        u8* clsb = cls.p + (S.keep_cls ? (k0 << SEG_SHIFT) : 0);
-        k_unrle_classify<<<(nslots / 8 + 255) / 256, 256, 0, c.stream>>>(rle.p + (k0 << SEG_SHIFT), rb, cnt, clsb);
-        KLAUNCH(c); KCHECK();
-        k_unrle_tilesum<<<cnt * ur_tps, UR_THREADS, 0, c.stream>>>(rle.p + (k0 << SEG_SHIFT), clsb, rb, ur_tps, tilesum);
-        KLAUNCH(c); KCHECK();
-        k_unrle_tileoff<<<cnt, 32, 0, c.stream>>>(rb, ur_tps, tilesum, tileoff.p + k0 * ur_tps);
-        KLAUNCH(c); KCHECK();
-        CUDA_CHECK(cudaMemcpyAsync(hres + k0, rb, sizeof(CandRes) * cnt, cudaMemcpyDeviceToHost, c.stream));
-      }
-      CUDA_CHECK(cudaStreamSynchronize(c.stream));
-      c.stats.blocks += cnt;
-    }
+  if (nb_all) CUDA_CHECK(cudaMemcpyAsync(S.dcand, bc.data(), sizeof(Cand) * nb_all, cudaMemcpyHostToDevice, c.stream));
+  DecScratch B;
+  for (size_t k0 = 0; k0 < nb; k0 += DB) {
+    const u32 cnt = (u32)std::min<size_t>(DB, nb - k0);
+    dec_batch(c, B, S.din, n, 0, true, S.dcand.p + S.lo + k0, cnt, S.dres.p + k0, S.hres.data() + S.lo + k0, S.rle.p + (k0 << SEG_SHIFT),
+              S.cls.p + (S.keep_cls ? (k0 << SEG_SHIFT) : 0), S.tileoff.p + k0 * UR_TPS);
   }
-
+  CUDA_CHECK(cudaStreamSynchronize(c.stream));
 }
 
-// fills *first_err (event index, or -1) instead of throwing when `sharded`.  On the host path (no d_out, d_out_alloc
-// given) an error still hands over the expanded buffer, with *out_n = the bytes the reference has written by then.
-// ends (position list): the end offset of every position's bytes that were delivered in full.
-static int dec_finish(Ctx& c, DecSession& S, int multistream, u8* d_out, size_t out_cap, size_t* out_n, std::vector<u64>* tab_pos,
-                      std::vector<u32>* tab_len, u8** d_out_alloc, bool sharded, u64* shard_info, std::vector<u64>* ends = nullptr) {
-  *out_n = 0;
-  if (d_out_alloc) *d_out_alloc = nullptr;
-  const size_t n = S.n;
-  const size_t nb_all = S.blk_idx.size();
-  std::vector<Cand>& cands = S.cands;
-  std::vector<Cand>& bc = S.bc;
-  std::vector<CandRes>& hres = S.hres;
-  u32 cur_dbuf = S.dbuf_size;  // dbufSize of the member the walk is in (lib/Bzip2.js:121)
-  const u32 ur_tps = UR_TPS;
-  // ---- 3. walk the chain in stream order (lib/Bzip2.js:454-481 / 508-548) ----
-  std::vector<Event> events;
-  std::vector<u64> outbase(nb_all ? nb_all : 1, ~0ull);
-  u64 total_out = 0;
-  auto find_cand = [&](u64 pos) -> long {
-    size_t lo = 0, hi = cands.size();
-    while (lo < hi) { size_t mid = (lo + hi) / 2; if (cands[mid].pos < pos) lo = mid + 1; else hi = mid; }
-    return (lo < cands.size() && cands[lo].pos == pos) ? (long)lo : -1;
-  };
+// Walks the chain over every rank's results, expands the own blocks into d_out, and fills shard_info.  Throws the first
+// failure in stream order; shard_info[3] tells the ranks which failure is the earliest.
+static int dec_finish(Ctx& c, DecSession& S, int multistream, u8* d_out, size_t out_cap, u64* shard_info) {
+  const std::vector<Cand>& cands = S.cands;
+  Chain ch;
+  ch.n = S.n; ch.multistream = multistream; ch.cur_dbuf = S.dbuf_size;
   std::vector<long> cand_to_blk(cands.size(), -1);
-  for (size_t i = 0; i < nb_all; i++) cand_to_blk[S.blk_idx[i]] = (long)i;
-  auto block_event = [&](size_t bi) -> bool {  // returns false when the walk must stop (error recorded)
-    const CandRes& r = hres[bi];
-    // the member's own limits, in the reference's order: randomised bit (:143), origPointer (:146), then the body
-    if (r.status != DEC_OBSOLETE && r.orig > cur_dbuf) {
-      events.push_back({2, bi, 0, 0, DEC_DATA_ERROR, "Data error: initial position out of bounds", total_out});
-      return false;
-    }
-    if (r.status != 0) {
-      std::string msg = r.status == DEC_OBSOLETE ? "Obsolete (pre 0.9.5) bzip format not supported." : "Data error";
-      if (r.detail == 1) msg += ": initial position out of bounds";
-      events.push_back({2, bi, 0, 0, r.status, msg, total_out});
-      return false;
-    }
-    if (r.n > cur_dbuf) {  // dbufCount would have run over dbufSize (lib/Bzip2.js:338,354)
-      events.push_back({2, bi, 0, 0, DEC_DATA_ERROR, "Data error", total_out});
-      return false;
-    }
-    outbase[bi] = total_out;
-    events.push_back({0, bi, 0, 0, 0, "", total_out});
-    total_out += r.rawlen;
-    return true;
-  };
-  if (S.listed) {
-    // one event per position, in list order; dec_open ended the list at the first position without a magic
-    size_t bi = 0;
-    for (const Cand& cd : cands) {
-      if (cd.type == 0) { events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data", total_out}); break; }
-      if (cd.type == 2) { events.push_back({3, 0, 0, 0, 0, "", total_out}); continue; }
-      if (!block_event(bi++)) break;
-    }
-  } else {
-    u64 pos = 32;
-    u32 stream_crc = 0;
-    for (;;) {
-      if ((pos + 7) / 8 >= n) break;  // 'eof' in inputStream && inputStream.eof() (lib/Bzip2.js:462)
-      const long ci = find_cand(pos);
-      if (ci < 0) { events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data", total_out}); break; }
-      if (cands[ci].type == 1) {
-        const size_t bi = (size_t)cand_to_blk[ci];
-        stream_crc = cands[ci].next32 ^ ((stream_crc << 1) | (stream_crc >> 31));  // lib/Bzip2.js:138-139
-        if (!block_event(bi)) break;
-        pos = hres[bi].endbit;
-      } else {
-        events.push_back({1, 0, stream_crc, cands[ci].next32, 0, "", total_out});
-        pos += 80;
-        const u64 bytepos = (pos + 7) / 8;
-        if (multistream && bytepos < n) {
-          // _start_bunzip on the byte stream (resyncs to the next byte)
-          u8 h2[4] = {0, 0, 0, 0};
-          const size_t avail = (size_t)std::min<u64>(4, n - bytepos);
-          CUDA_CHECK(cudaMemcpyAsync(h2, S.din.p + bytepos, avail, cudaMemcpyDeviceToHost, c.stream));
-          CUDA_CHECK(cudaStreamSynchronize(c.stream));
-          if (avail != 4 || h2[0] != 'B' || h2[1] != 'Z' || h2[2] != 'h') { events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data: bad magic", total_out}); break; }
-          const int lv = h2[3] - 0x30;
-          if (lv < 1 || lv > 9) { events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data: level out of range", total_out}); break; }
-          cur_dbuf = (u32)lv * 100000u;
-          stream_crc = 0;
-          pos = (bytepos + 4) * 8;
-        } else break;
-      }
-    }
-  }
-
-  // ---- 4. expand the chain blocks of the own share, CRC them ----
+  for (size_t i = 0; i < S.blk_idx.size(); i++) cand_to_blk[S.blk_idx[i]] = (long)i;
+  chain_walk(ch, [&](u64 pos) -> At {
+    const auto it = std::lower_bound(cands.begin(), cands.end(), pos, [](const Cand& x, u64 p) { return x.pos < p; });
+    if (it == cands.end() || it->pos != pos) return {0, nullptr, nullptr, 0};
+    if (it->type == 2) return {2, &*it, nullptr, 0};
+    const size_t bi = (size_t)cand_to_blk[it - cands.begin()];
+    return {1, &*it, &S.hres[bi], bi};
+  }, [&](u64 bytepos, u8* h) -> size_t {
+    const size_t avail = (size_t)std::min<u64>(4, S.n - bytepos);
+    CUDA_CHECK(cudaMemcpyAsync(h, S.din.p + bytepos, avail, cudaMemcpyDeviceToHost, c.stream));
+    CUDA_CHECK(cudaStreamSynchronize(c.stream));
+    return avail;
+  });
   // own output window: [my_off, my_off + my_len) of the decoded stream
-  u64 my_off = 0, my_len = 0;
-  {
-    bool first = true;
-    for (size_t i = S.lo; i < S.hi; i++)
-      if (outbase[i] != ~0ull) {
-        if (first) { my_off = outbase[i]; first = false; }
-        my_len = outbase[i] + hres[i].rawlen - my_off;
-      }
-  }
   const size_t nb = S.hi - S.lo;
+  std::vector<u64> ob(nb ? nb : 1, ~0ull);
+  u64 my_off = 0, my_len = 0;
+  bool first = true;
+  for (const Event& ev : ch.events)
+    if (ev.kind == 0 && ev.slot >= S.lo && ev.slot < S.hi) {
+      if (first) { my_off = ev.off; first = false; }
+      ob[ev.slot - S.lo] = ev.off - my_off;
+      my_len = ev.off + ev.len - my_off;
+    }
   u8* dout = d_out;
   DBuf<u8> own;
   if (!d_out) {
     own.alloc(c, my_len ? my_len : 1);
     dout = own.p;
   } else if (my_len > out_cap) {
-    *out_n = (size_t)my_len;
     throw B2Error{B2_ERR_BAD_ARG, "output buffer too small"};
   }
-  std::vector<u32> got_crc(nb ? nb : 1, 0);
-  if (nb) {
-    StageScope ss(c, ST_UNRLE);
-    std::vector<u64> ob(nb);
-    for (size_t i = 0; i < nb; i++) ob[i] = outbase[S.lo + i] == ~0ull ? ~0ull : outbase[S.lo + i] - my_off;
-    DBuf<u64> dob(c, nb);
-    CUDA_CHECK(cudaMemcpyAsync(dob, ob.data(), 8 * nb, cudaMemcpyHostToDevice, c.stream));
-    if (S.keep_cls) {
-      k_unrle_emit<<<(unsigned)(nb * ur_tps), UR_THREADS, 0, c.stream>>>(S.rle, S.cls, S.dres, ur_tps, S.tileoff, dob, dout);
-      KLAUNCH(c); KCHECK();
-    } else {
-      const size_t DBc = dec_batch_blocks(c);
-      for (size_t k0 = 0; k0 < nb; k0 += DBc) {
-        const u32 cnt = (u32)std::min<size_t>(DBc, nb - k0);
-        k_unrle_classify<<<(unsigned)((((size_t)cnt << SEG_SHIFT) / 8 + 255) / 256), 256, 0, c.stream>>>(S.rle.p + (k0 << SEG_SHIFT), S.dres.p + k0, cnt, S.cls);
-        KLAUNCH(c); KCHECK();
-        k_unrle_emit<<<(unsigned)(cnt * ur_tps), UR_THREADS, 0, c.stream>>>(S.rle.p + (k0 << SEG_SHIFT), S.cls, S.dres.p + k0, ur_tps, S.tileoff.p + k0 * ur_tps,
-                                                                            dob.p + k0, dout);
-        KLAUNCH(c); KCHECK();
-      }
+  std::vector<u32> got(nb ? nb : 1, 0);
+  if (S.keep_cls) {
+    dec_expand(c, S.rle, S.cls, false, S.dres, S.hres.data() + S.lo, S.tileoff, (u32)nb, ob.data(), dout, got.data());
+  } else {
+    const size_t DBc = dec_batch_blocks(c);
+    for (size_t k0 = 0; k0 < nb; k0 += DBc) {
+      const u32 cnt = (u32)std::min<size_t>(DBc, nb - k0);
+      dec_expand(c, S.rle.p + (k0 << SEG_SHIFT), S.cls, true, S.dres.p + k0, S.hres.data() + S.lo + k0, S.tileoff.p + k0 * UR_TPS, cnt,
+                 ob.data() + k0, dout, got.data() + k0);
     }
-    std::vector<BlkInfo> ranges(nb);
-    for (size_t i = 0; i < nb; i++) {
-      memset(&ranges[i], 0, sizeof(BlkInfo));
-      if (ob[i] != ~0ull) { ranges[i].s = ob[i]; ranges[i].e = ob[i] + hres[S.lo + i].rawlen; }
-    }
-    DBuf<BlkInfo> dr(c, nb);
-    DBuf<u32> dcrc(c, nb);
-    CUDA_CHECK(cudaMemcpyAsync(dr, ranges.data(), sizeof(BlkInfo) * nb, cudaMemcpyHostToDevice, c.stream));
-    crc_ranges(c, dout, dr, ranges, dcrc);
-    CUDA_CHECK(cudaMemcpyAsync(got_crc.data(), dcrc, 4 * nb, cudaMemcpyDeviceToHost, c.stream));
-    CUDA_CHECK(cudaStreamSynchronize(c.stream));
   }
-  // ---- 5. replay the events: first failure in stream order wins ----
-  S.err_event = -1;
-  int err_code = 0;
-  std::string err_msg;
-  u64 prefix = 0;  // bytes the reference has written when it throws: a block's own bytes go out before its CRC check
-  for (size_t ei = 0; ei < events.size() && S.err_event < 0; ei++) {
-    const Event& ev = events[ei];
-    if (ev.kind == 0) {
-      if (ev.cand >= S.lo && ev.cand < S.hi) {  // CRCs of foreign blocks are checked by their owners
-        const u32 want = bc[ev.cand].next32, got = got_crc[ev.cand - S.lo];
-        if (want != got) {
-          S.err_event = (int)ei; err_code = DEC_DATA_ERROR; err_msg = "Data error: Bad block CRC (got " + hexs(got) + " expected " + hexs(want) + ")";
-          prefix = ev.off + hres[ev.cand].rawlen;
-        }
-      }
-      if (S.err_event < 0 && tab_pos) { tab_pos->push_back(bc[ev.cand].pos); tab_len->push_back(hres[ev.cand].rawlen); }
-    } else if (ev.kind == 1) {
-      if (!tab_pos && ev.a != ev.b) {
-        S.err_event = (int)ei; err_code = DEC_DATA_ERROR; err_msg = "Data error: Bad stream CRC (got " + hexs(ev.a) + " expected " + hexs(ev.b) + ")";
-        prefix = ev.off;
-      }
-    } else if (ev.kind == 2) {
-      S.err_event = (int)ei; err_code = ev.code; err_msg = ev.msg;
-      prefix = ev.off;
-    }
-    if (ends && S.err_event < 0) ends->push_back(ev.kind == 0 ? ev.off + hres[ev.cand].rawlen : ev.off);
-  }
-  if (shard_info) { shard_info[0] = my_off; shard_info[1] = my_len; shard_info[2] = total_out; shard_info[3] = (u64)(long long)S.err_event; shard_info[4] = (u64)(long long)err_code; }
-  if (S.err_event >= 0) {
-    // the host path hands the output in front of the error to the caller with the error (b2_bzip2_decompress_partial)
-    if (!sharded && !d_out && d_out_alloc) { *out_n = (size_t)prefix; *d_out_alloc = own.p; own.p = nullptr; }
-    if (!sharded) throw B2Error{err_code, err_msg};
-    throw B2Error{err_code, err_msg};  // the caller (sharded) compares shard_info[3] across ranks and keeps the earliest
-  }
-  *out_n = (size_t)my_len;
-  if (!d_out && d_out_alloc) { *d_out_alloc = own.p; own.p = nullptr; }
+  DecErr E;
+  replay(ch, 0, ch.events.size(), [&](size_t slot) {
+    // CRCs of foreign blocks are checked by their owners
+    return slot >= S.lo && slot < S.hi ? std::make_pair(true, got[slot - S.lo]) : std::make_pair(false, 0u);
+  }, nullptr, nullptr, nullptr, E);
+  shard_info[0] = my_off; shard_info[1] = my_len; shard_info[2] = ch.total_out; shard_info[3] = (u64)(long long)E.ev; shard_info[4] = (u64)(long long)E.code;
+  // the caller compares shard_info[3] across ranks and keeps the earliest
+  if (E.ev >= 0) throw B2Error{E.code, E.msg};
   return 0;
 }
 
-// positions: decode the blocks at these bit positions, back to back in list order (ends: see dec_finish), instead of the
-// stream's chain
-int bzip2_decompress_device(Ctx& c, const u8* d_in_user, size_t n, int multistream, u8* d_out, size_t out_cap, size_t* out_n,
-                            const std::vector<u64>* positions, std::vector<u64>* ends, std::vector<u64>* tab_pos, std::vector<u32>* tab_len,
-                            u8** d_out_alloc) {
-  *out_n = 0;
-  if (d_out_alloc) *d_out_alloc = nullptr;
-  DecSession S;
-  dec_open(c, S, d_in_user, n, positions, 0, 1);
-  return dec_finish(c, S, multistream, d_out, out_cap, out_n, tab_pos, tab_len, d_out_alloc, false, nullptr, ends);
-}
-
-// ---- sharded decode (SURVEY.md section 8e): open on every rank, exchange results, finish ------------
 static DecSession* g_shard = nullptr;
 void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* info) {
   delete g_shard;
   g_shard = new DecSession();
-  dec_open(c, *g_shard, d_in, n, nullptr, rank, world);
+  dec_open(c, *g_shard, d_in, n, rank, world);
   info[0] = g_shard->blk_idx.size(); info[1] = g_shard->lo; info[2] = g_shard->hi;
 }
 void dec_shard_export(u64* buf) {
@@ -1585,7 +1805,6 @@ int dec_shard_finish(Ctx& c, const u64* all, int multistream, u8* d_out, size_t 
     CandRes& r = S.hres[i];
     r.status = (int)(long long)o[0]; r.detail = (u32)o[1]; r.endbit = o[2]; r.n = (u32)o[3]; r.rawlen = (u32)o[4]; r.orig = (u32)o[5];
   }
-  size_t out_n = 0;
   struct Closer { ~Closer() { delete g_shard; g_shard = nullptr; } } closer;
-  return dec_finish(c, S, multistream, d_out, out_cap, &out_n, nullptr, nullptr, nullptr, true, res);
+  return dec_finish(c, S, multistream, d_out, out_cap, res);
 }

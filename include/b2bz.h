@@ -46,8 +46,14 @@ void b2_free(void* p);
 /* Bzip2.compressFile(input, output, level)            lib/Bzip2.js:879-929 */
 int b2_bzip2_compress(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n);
 /* Bzip2.decompressFile(input, output, multistream)    lib/Bzip2.js:454-481
- * Members of a multistream file may have different levels.  On an error nothing is returned and nothing needs freeing;
- * one call keeps ~2 MiB per block of the file on the device. */
+ * Members of a multistream file may have different levels.  On an error nothing is returned and nothing needs freeing.
+ * Device memory does not grow with the file: the input goes to the device a window of W bytes at a time
+ * ($B2_DEC_WINDOW, default 4 GiB), its blocks are decoded B at a time ($B2_DEC_BATCH, default 2048; B counts only the
+ * blocks of the largest batch), and the decoded bytes leave through a staging buffer of at most max(W, one block) bytes.
+ * A window grows past W only for a block longer than W.  For W >= 64 KiB, one call of this family (table and
+ * decompress_block[s] too; b2_bzip2_decompress_dev has no staging buffer) keeps at most
+ *     2 * max(W, 48 MiB) + B * 24 MiB + 16 bytes per magic in a window
+ * on the device (b2_stats.dev_peak_bytes).  A position list keeps the whole input on the device instead of a window. */
 int b2_bzip2_decompress(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n);
 /* Bzip2.decompressBlock(input, bitPos, output)        lib/Bzip2.js:482-503 */
 int b2_bzip2_decompress_block(const uint8_t* in, size_t n, uint64_t bitpos, uint8_t** out, size_t* out_n);
@@ -191,6 +197,7 @@ typedef struct b2_stats {
   uint64_t bwt_msd_fallback_why;     /* OR over batches of why the MSD path gave up: 1 = bucket > MB_CAP, 2 = cell >
                                         MB_MAXCELL, 4 = tie list > n/8, 8 = tie group > 16, 16 = tie deeper than the resolver */
   uint64_t bwt_direct_fallback_why;  /* the same bits 4 / 8 / 16 for the LSD direct resolve */
+  uint64_t dev_peak_bytes;           /* high-water mark of the library's device allocations during the last call */
 } b2_stats;
 void b2_get_stats(b2_stats* s);
 
