@@ -30,7 +30,8 @@ class Stats(C.Structure):
                [(n, C.c_float) for n in ("ms_msd_scatter", "ms_msd_bucket")] + \
                [(n, C.c_uint64) for n in
                 ("bwt_msd_done", "bwt_direct_done", "bwt_rounds_batches", "bwt_wide_batches",
-                 "bwt_msd_fallback_why", "bwt_direct_fallback_why", "dev_peak_bytes")]
+                 "bwt_msd_fallback_why", "bwt_direct_fallback_why", "dev_peak_bytes",
+                 "rle_group_scans", "rle_walk_parallel", "rle_walk_serial")]
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}

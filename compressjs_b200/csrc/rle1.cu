@@ -918,6 +918,7 @@ void rle1_plan_ex(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan, l
       k_rle_scan<<<1, RS_THREADS, 0, c.stream>>>(sums, ntiles, n, plan.tile_carry, plan.tile_prefix, st0, W0, dagg);
       KLAUNCH(c); KCHECK();
     } else {
+      c.stats.rle_group_scans++;
       const u32 ng = (u32)((ntiles + RG_TILES - 1) / RG_TILES);
       DBuf<u64> gagg(c, ng), gstart(c, ng + 1), gsum(c, ng), gbase(c, ng + 1);
       k_rle_scan_g1<<<ng, RG_THREADS, 0, c.stream>>>(sums, ntiles, n, gagg);
@@ -978,10 +979,11 @@ void rle1_plan_ex(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan, l
       // exact plans must cover the input; range plans are checked against their neighbours by the caller
       ok = !exact || (plan.h_blocks[0].s == 0 && plan.h_blocks[nb - 1].e == n);
       for (u32 k = 0; k + 1 < nb && ok; k++) ok = plan.h_blocks[k].e == plan.h_blocks[k + 1].s;
-      if (ok) { plan.nblocks = nb; return; }
+      if (ok) { plan.nblocks = nb; c.stats.rle_walk_parallel++; return; }
       plan.h_blocks.clear();
     }
   }
+  c.stats.rle_walk_serial++;
   DBuf<u32> dnb(c, 1);
   k_rle_blocks<<<1, RT_THREADS, 0, c.stream>>>(d_in, n, BS, plan.tile_carry, plan.tile_prefix, ntiles, plan.blocks, dnb, maxblocks, u_start, 0, 0, 0);
   KLAUNCH(c); KCHECK();

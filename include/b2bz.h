@@ -198,6 +198,10 @@ typedef struct b2_stats {
                                         MB_MAXCELL, 4 = tie list > n/8, 8 = tie group > 16, 16 = tie deeper than the resolver */
   uint64_t bwt_direct_fallback_why;  /* the same bits 4 / 8 / 16 for the LSD direct resolve */
   uint64_t dev_peak_bytes;           /* high-water mark of the library's device allocations during the last call */
+  /* How the RLE1 stage (rle1.cu) planned, summed over the plans of the last call */
+  uint64_t rle_group_scans;    /* plans whose tile scan ran as the multi-CTA group scan (> 8192 tiles, or B2_RLE_SCAN_GROUPS) */
+  uint64_t rle_walk_parallel;  /* speculative parallel block walks that chained up and were accepted */
+  uint64_t rle_walk_serial;    /* single-CTA block walks: the fallback of a rejected parallel walk, or the only walk */
 } b2_stats;
 void b2_get_stats(b2_stats* s);
 

@@ -959,10 +959,15 @@ ORC_EXPORT int orc_bzip2_compress_mt(const uint8_t* in, size_t n, int level, int
   crc_init();
   if (level < 1 || level > 9) return -100;
   size_t stride = (size_t)level * 100000;
-  size_t cap = n / (size_t)(level * 100000 - 19) + 2;
+  /* a block holds at least 4/5 of blockSize raw bytes (runs of exactly four: 5 RLE1 bytes per 4 raw bytes) */
+  size_t cap = n / ((size_t)(level * 100000 - 19) * 4 / 5) + 2;
   uint64_t* starts = (uint64_t*)malloc(8 * cap); uint32_t* lens = (uint32_t*)malloc(4 * cap); uint32_t* crcs = (uint32_t*)malloc(4 * cap);
   uint8_t* blocks = (uint8_t*)malloc(stride * cap);
   size_t nb = orc_rle1_split(in, n, level, starts, lens, crcs, cap, blocks, stride);
+  if (nb > cap) { /* the split kept only `cap` blocks: fail rather than compress a truncated list */
+    free(starts); free(lens); free(crcs); free(blocks);
+    return -101;
+  }
   mt_job_t job; job.blocks = blocks; job.stride = stride; job.lens = lens; job.nb = nb; job.next = 0;
   pthread_mutex_init(&job.mu, NULL);
   job.bits = (uint8_t**)calloc(nb + 1, sizeof(uint8_t*)); job.nbits = (size_t*)calloc(nb + 1, sizeof(size_t));

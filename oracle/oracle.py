@@ -120,6 +120,13 @@ def huffman_code_lengths(freqs, maxlen):
     return arr.tolist()
 
 
+def block_cap(n, level):
+    """Upper bound on the number of blocks of an n-byte input: a block holds at least 4/5 of blockSize raw bytes
+    (runs of exactly four give 5 RLE1 bytes per 4 raw bytes), the last one may be short."""
+    bs = max(level * 100000 - 19, 1)
+    return n // max(bs * 4 // 5, 1) + 2
+
+
 def bzip2_compress(data, level=9, legacy_sort=False, trace=False, threads=0):
     L = lib()
     a, p = _buf(data)
@@ -127,9 +134,9 @@ def bzip2_compress(data, level=9, legacy_sort=False, trace=False, threads=0):
     if threads and not trace and not legacy_sort:
         rc = L.orc_bzip2_compress_mt(p, a.size, level, threads, C.byref(out), C.byref(n))
         if rc:
-            raise OracleError(rc, "Invalid block size multiplier")
+            raise OracleError(rc, "more blocks than the block arrays hold" if rc == -101 else "Invalid block size multiplier")
         return _take(L, out, n)
-    cap = a.size // max(level * 100000 - 19, 1) + 2
+    cap = block_cap(a.size, level)
     tr = (BlockTrace * cap)()
     nt = C.c_size_t()
     rc = L.orc_bzip2_compress_ex(p, a.size, level, int(legacy_sort), C.byref(out), C.byref(n), tr, cap, C.byref(nt))
@@ -178,9 +185,8 @@ def rle1_split(data, level=9, stride=None):
     """Returns (raw_starts, lens, crcs, blocks[nb, stride])."""
     L = lib()
     a, p = _buf(data)
-    bs = level * 100000 - 19
     stride = stride or level * 100000
-    cap = a.size // bs + 2
+    cap = block_cap(a.size, level)
     starts = np.zeros(cap, dtype=np.uint64)
     lens = np.zeros(cap, dtype=np.uint32)
     crcs = np.zeros(cap, dtype=np.uint32)
