@@ -7,26 +7,15 @@
 #include <mutex>
 #include <string>
 #include <vector>
-#include "ctx.h"
+#include "enc.h"
 
 // stages implemented in the other translation units
-void bwt_forward_batch(Ctx& c, const u8* d_T, u8* d_U, const u32* d_n, const u32* h_n, u32 nblk, u32* d_pidx, bool sentinel = false,
-                       u32* d_sa_out = nullptr, u32* d_hist_out = nullptr);
-u32 crc32_device(Ctx& c, const u8* d_p, size_t n);
-void bzip2_compress_device(Ctx& c, const u8* d_in, size_t n, int level, u8* d_out, size_t out_cap, size_t* out_n,
-                           size_t first_block, size_t block_count, int bit_phase, bool whole_file, u64* out_bits,
-                           std::vector<u32>* crcs_out, size_t* total_blocks, long long spec_first = -2, size_t spec_count = 0,
-                           u64* spec_range = nullptr);
-void bitshift_device(Ctx& c, const void* src, u64 nbits, int phase, void* dst);
-void bzip2_share_summary(Ctx& c, const u8* d_in, size_t n, u64* out);
-void bzip2_plan_share(Ctx& c, const u8* d_buf, size_t n, int level, u64 st0, u64 W0, size_t first, size_t count, u64* info);
 void bwt_inverse_sentinel_batch(Ctx& c, const u8* d_L, const u32* h_n, const u32* h_pidx, u32 nb, u8* d_out);
 size_t bwtc_bound(size_t n);
 void bwtc_compress_device(Ctx& c, const u8* d_in, size_t n, int level, u64 file_size, u8* d_out, size_t out_cap, size_t* out_n);
 u64 bwtc_parse_header(const u8* in, size_t n, size_t* pos);
 void bwtc_decompress(Ctx& c, const u8* d_in, size_t n, size_t pos, u64 fs, void* (*alloc_host)(size_t), u8** h_out, size_t* out_n);
-void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, int level, u8* d_in, size_t win, u8* d_out, size_t out_cap, u8* h_out,
-                         size_t h_out_cap, size_t* out_n, bool pinned_in);
+void dec_shard_release();
 void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* info);
 void dec_shard_export(u64* buf);
 int dec_shard_finish(Ctx& c, const u64* all, int multistream, u8* d_out, size_t out_cap, u64* res);
@@ -221,6 +210,9 @@ void b2_shutdown(void) {
   std::lock_guard<std::mutex> lk(g_mu);
   if (!g_ctx) return;
   cudaSetDevice(g_ctx->device);
+  // state kept across calls holds device buffers of this context: free it while the context is alive
+  bzip2_release_plan();
+  dec_shard_release();
   cudaStreamSynchronize(g_ctx->stream);
   for (auto& kv : g_pinned_free) cudaFreeHost(kv.second);
   g_pinned_free.clear();
@@ -456,7 +448,7 @@ int b2_bzip2_compress_dev(const void* d_in, size_t n, int level, void* d_out, si
     c.reset_call();
     {
       StageScope tot(c, ST_TOTAL);
-      bzip2_compress_device(c, (const u8*)d_in, n, level, (u8*)d_out, out_cap, out_n, 0, (size_t)-1, 0, true, nullptr, nullptr, nullptr);
+      bzip2_compress_dev(c, (const u8*)d_in, n, level, (u8*)d_out, out_cap, out_n);
     }
     c.sync();
     c.collect();
@@ -503,8 +495,8 @@ int b2_bzip2_plan(const void* d_in, size_t n, int level, size_t* total_blocks) {
     if (level < 1 || level > 9) throw B2Error{B2_ERR_BAD_LEVEL, "Invalid block size multiplier"};
     Ctx& c = ctx_locked();
     c.reset_call();
-    size_t dummy = 0;
-    bzip2_compress_device(c, (const u8*)d_in, n, level, nullptr, 0, &dummy, 0, 0, 0, false, nullptr, nullptr, total_blocks);
+    const size_t nb = bzip2_plan(c, (const u8*)d_in, n, level);
+    if (total_blocks) *total_blocks = nb;
     c.sync();
     return 0;
   });
@@ -549,9 +541,7 @@ int b2_bzip2_plan_spec(const void* d_in, size_t n, int level, int rank, int worl
     if (world < 1 || rank < 0 || rank >= world) throw B2Error{B2_ERR_BAD_ARG, "bad rank/world"};
     Ctx& c = ctx_locked();
     c.reset_call();
-    size_t dummy = 0;
-    bzip2_compress_device(c, (const u8*)d_in, n, level, nullptr, 0, &dummy, 0, 0, 0, false, nullptr, nullptr, nullptr, -1,
-                          ((size_t)rank << 32) | (size_t)world, info);
+    bzip2_plan_spec(c, (const u8*)d_in, n, level, rank, world, info);
     c.sync();
     return 0;
   });
@@ -585,15 +575,12 @@ int b2_bzip2_encode_range_dev(const void* d_in, size_t n, int level, size_t firs
     if (bit_phase < 0 || bit_phase > 7) throw B2Error{B2_ERR_BAD_ARG, "bit_phase must be 0..7"};
     Ctx& c = ctx_locked();
     c.reset_call();
-    size_t bytes = 0;
-    std::vector<u32> crcs;
     {
       StageScope tot(c, ST_TOTAL);
-      bzip2_compress_device(c, (const u8*)d_in, n, level, (u8*)d_out, out_cap, &bytes, first, count, bit_phase, false, out_bits, &crcs, nullptr);
+      bzip2_encode_range(c, (const u8*)d_in, n, level, first, count, bit_phase, (u8*)d_out, out_cap, out_bits, block_crcs);
     }
     c.sync();
     c.collect();
-    if (block_crcs) for (size_t i = 0; i < crcs.size(); i++) block_crcs[i] = crcs[i];
     return 0;
   });
 }

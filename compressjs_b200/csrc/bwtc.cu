@@ -20,7 +20,6 @@
 #include "enc.h"
 #include "bwtc_core.cuh"
 
-void bwt_forward_batch(Ctx& c, const u8* d_T, u8* d_U, const u32* d_n, const u32* h_n, u32 nblk, u32* d_pidx, bool sentinel, u32* d_sa_out, u32* d_hist_out = nullptr);
 void bwt_inverse_sentinel_batch(Ctx& c, const u8* d_L, const u32* h_n, const u32* h_pidx, u32 nb, u8* d_out);
 
 struct BwtcState {

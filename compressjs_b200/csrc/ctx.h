@@ -25,8 +25,6 @@ struct Ctx {
   bool timing = true;
   bool bwt_msd = true;  // MSD + shared-memory bucket sort for sparse-tie batches (bwt_msd.cu); B2_BWT_MSD=0 disables it
   bool bwt_wide = false, bwt_wide_forced = false, bwt_mode_known = false;  // 8-byte initial sort for text-like batches (see bwt.cu)
-  // plan handed from b2_bzip2_plan to the next b2_bzip2_encode_range_dev on the same (unchanged) buffer
-  void* plan_cache = nullptr; const void* plan_ptr = nullptr; size_t plan_n = 0; int plan_level = 0;
 
   void* dalloc(size_t bytes) {
     void* p = nullptr;

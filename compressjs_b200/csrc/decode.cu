@@ -1782,6 +1782,8 @@ static int dec_finish(Ctx& c, DecSession& S, int multistream, u8* d_out, size_t 
 }
 
 static DecSession* g_shard = nullptr;
+// frees an open sharded decode (b2_shutdown, while the context its buffers belong to is alive)
+void dec_shard_release() { delete g_shard; g_shard = nullptr; }
 void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* info) {
   delete g_shard;
   g_shard = new DecSession();

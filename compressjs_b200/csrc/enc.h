@@ -12,6 +12,8 @@ struct BlkInfo {
   u32 n;    // post-RLE1 length of the block (<= blockSize)
 };
 
+inline u32 rle1_block_size(int level) { return (u32)level * 100000 - 19; }  // lib/Bzip2.js:892-900
+
 struct Rle1Plan {
   DBuf<u32> tile_carry;   // per raw tile: length (mod 255) of the run entering the tile
   DBuf<u64> tile_prefix;  // per raw tile: W(tile start)
@@ -20,18 +22,20 @@ struct Rle1Plan {
   std::vector<BlkInfo> h_blocks;
   size_t nblocks = 0;      // entries of h_blocks
   size_t first_index = 0;  // global block index of h_blocks[0] (range plans)
-  size_t total_guess = 0;  // ceil(W(N) / blockSize)
-  u64 w_total = 0;         // W at the end of the buffer (RLE1 bytes of the whole input up to there)
-  u64 ntiles = 0;
+  u64 w_total = 0;         // W at the end of the buffer (RLE1 bytes of the whole input up to there); total_guess = ceil(W / BS)
+  size_t total_guess(int level) const { return (size_t)((w_total + rle1_block_size(level) - 1) / rle1_block_size(level)); }
 };
 
 #define RLE_TILE 4096
 
+// Tile scan (tile_*, w_total).  st0 / W0: run state and RLE1 output in front of the buffer when it is a share of a larger
+// input; summary (host, optional): receives the aggregate run state of the buffer and the length of its leading run.
+void rle1_scan_tiles(Ctx& c, const u8* d_in, size_t n, Rle1Plan& plan, u64 st0 = 0, u64 W0 = 0, u64* summary = nullptr);
+// Cut of blocks [first, first+count) of the whole input from the speculative boundary W = first * blockSize, over a
+// plan whose tiles are scanned (exact unless a run-phase slip happened earlier in the input).
+void rle1_cut_range(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan, size_t first, size_t count);
+// Tile scan and exact cut of every block of d_in[0, n).
 void rle1_plan(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan);
-// st0 / W0: run state and RLE1 output in front of the buffer when it is a share of a larger input (0, 0 for a whole file);
-// agg_state (host, 2 x u64, optional): receives the aggregate run state of the buffer and the length of its leading run.
-void rle1_plan_ex(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan, long long spec_first, size_t spec_count, bool tiles_only,
-                  u64 st0 = 0, u64 W0 = 0, u64* agg_state = nullptr);
 // materialise blocks [first, first+count) of the plan into the slot layout at d_T (u8[count<<20]);
 // d_n receives their lengths, d_crc their CRCs.
 void rle1_materialize(Ctx& c, const u8* d_in, size_t n, const Rle1Plan& plan, size_t first, size_t count, u8* d_T, u32* d_n, u32* d_crc);
@@ -73,3 +77,19 @@ void pack_batch(Ctx& c, const NarrowSyms& sym, const u8* d_sel, const u8* d_selm
 
 #include <vector>
 void crc_ranges(Ctx& c, const u8* d_data, const BlkInfo* d_ranges, const std::vector<BlkInfo>& h_ranges, u32* d_crc_out);
+u32 crc32_device(Ctx& c, const u8* d_p, size_t n);
+void bwt_forward_batch(Ctx& c, const u8* d_T, u8* d_U, const u32* d_n, const u32* h_n, u32 nblk, u32* d_pidx, bool sentinel = false,
+                       u32* d_sa_out = nullptr, u32* d_hist_out = nullptr);
+
+// ---- bzip2 encode drivers (encode.cu), one per entry point of include/b2bz.h ----
+void bzip2_compress_dev(Ctx& c, const u8* d_in, size_t n, int level, u8* d_out, size_t out_cap, size_t* out_n);
+void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, int level, u8* d_in, size_t win, u8* d_out, size_t out_cap, u8* h_out,
+                         size_t h_out_cap, size_t* out_n, bool pinned_in);
+size_t bzip2_plan(Ctx& c, const u8* d_in, size_t n, int level);
+void bzip2_plan_spec(Ctx& c, const u8* d_in, size_t n, int level, int rank, int world, u64* info);
+void bzip2_share_summary(Ctx& c, const u8* d_in, size_t n, u64* out);
+void bzip2_plan_share(Ctx& c, const u8* d_buf, size_t n, int level, u64 st0, u64 W0, size_t first, size_t count, u64* info);
+void bzip2_encode_range(Ctx& c, const u8* d_in, size_t n, int level, size_t first, size_t count, int bit_phase, u8* d_out, size_t out_cap,
+                        u64* out_bits, u32* block_crcs);
+void bitshift_device(Ctx& c, const void* src, u64 nbits, int phase, void* dst);
+void bzip2_release_plan();  // the plan kept for b2_bzip2_encode_range_dev

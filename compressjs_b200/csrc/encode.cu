@@ -19,11 +19,9 @@
 #include <cstdio>
 #include <cstdlib>
 #include <functional>
+#include <optional>
 #include <vector>
 #include "enc.h"
-
-void bwt_forward_batch(Ctx& c, const u8* d_T, u8* d_U, const u32* d_n, const u32* h_n, u32 nblk, u32* d_pidx, bool sentinel = false,
-                       u32* d_sa_out = nullptr, u32* d_hist_out = nullptr);
 
 // ---- bit writers (stream is MSB first; words are stored big-endian) ----------------------
 __device__ __forceinline__ u32 bswap32(u32 v) { return __byte_perm(v, 0, 0x0123); }
@@ -332,10 +330,9 @@ __global__ void k_rebase(u32* out, u64 word_index, u64* state, u32 bits_in_word)
   state[0] = bits_in_word;
 }
 
-// compressFile on device buffers.  whole_file: header + all blocks + trailer.  Otherwise encodes
-// blocks [first_block, first_block+block_count) starting at bit `bit_phase` of d_out.
 // One output stream being written: the running bit position lives on the device (state[0]); blocks of one or more
 // RLE1 plans are appended batch by batch.  Shared by the device-resident entry points and the pipelined host path.
+// whole_file: file header + blocks + trailer; otherwise the blocks alone, from bit `bit_phase` of d_out.
 struct EncSession {
   Ctx& c;
   int level; u8* d_out; size_t cap_words; bool whole_file; int bit_phase;
@@ -476,59 +473,80 @@ struct EncSession {
   }
 };
 
-void bzip2_compress_device(Ctx& c, const u8* d_in, size_t n, int level, u8* d_out, size_t out_cap, size_t* out_n, size_t first_block,
-                           size_t block_count, int bit_phase, bool whole_file, u64* out_bits, std::vector<u32>* crcs_out,
-                           size_t* total_blocks, long long spec_first, size_t spec_count, u64* spec_range) {
-  // b2_bzip2_plan() leaves its plan for the encode_range call that follows on the same buffer
-  Rle1Plan* planp = nullptr;
-  const bool plan_only = !whole_file && block_count == 0;
-  if (!whole_file && !plan_only && c.plan_cache && c.plan_ptr == d_in && c.plan_n == n && c.plan_level == level) {
-    planp = static_cast<Rle1Plan*>(c.plan_cache);
-    c.plan_cache = nullptr;
-  } else {
-    if (c.plan_cache) { delete static_cast<Rle1Plan*>(c.plan_cache); c.plan_cache = nullptr; }
-    planp = new Rle1Plan();
-    StageScope s(c, ST_RLE1);
-    if (spec_first >= -1 && plan_only && spec_range) {
-      // speculative range plan (multi-GPU): total guess first, then only this rank's blocks
-      rle1_plan_ex(c, d_in, n, level, *planp, -1, 0, true);
-      const size_t total = planp->total_guess;
-      size_t f = (size_t)spec_first, cnt = spec_count;
-      if (spec_first == -1) {  // caller passes (rank, world) in spec_count's two halves
-        const size_t rank = spec_count >> 32, world = spec_count & 0xffffffffu;
-        f = rank * total / world;
-        cnt = (rank + 1) * total / world - f;
-      }
-      rle1_plan_ex(c, d_in, n, level, *planp, (long long)f, cnt, false);
-      spec_range[0] = planp->nblocks ? planp->h_blocks.front().s : 0;
-      spec_range[1] = planp->nblocks ? planp->h_blocks.back().e : 0;
-      spec_range[2] = f;
-      spec_range[3] = cnt;
-      spec_range[4] = planp->nblocks;
-      spec_range[5] = total;
-    } else {
-      rle1_plan(c, d_in, n, level, *planp);
-    }
+// ---- device-resident entry points ------------------------------------------------------------------------------
+// The plan of b2_bzip2_plan, _plan_spec or _plan_share, kept for the next b2_bzip2_encode_range_dev.  That call takes
+// it if (buffer, length, level) match; the cache is empty afterwards either way.  compress_dev drops it too.
+struct PlanCache {
+  std::optional<Rle1Plan> plan;
+  const u8* ptr = nullptr; size_t n = 0; int level = 0;
+  std::optional<Rle1Plan> take(const u8* p, size_t n_, int level_) {
+    std::optional<Rle1Plan> r;
+    if (plan && p == ptr && n_ == n && level_ == level) r = std::move(plan);
+    plan.reset();
+    return r;
   }
-  struct PlanOwner { Rle1Plan* p; bool keep; ~PlanOwner() { if (!keep) delete p; } } owner{planp, false};
-  Rle1Plan& plan = *planp;
-  const size_t nb_all = plan.first_index + plan.nblocks;  // exact plans: first_index == 0
-  if (total_blocks) *total_blocks = nb_all;
+  void put(Rle1Plan&& p, const u8* p_, size_t n_, int level_) { plan = std::move(p); ptr = p_; n = n_; level = level_; }
+};
+static PlanCache g_plan;
+void bzip2_release_plan() { g_plan.plan.reset(); }
+
+void bzip2_compress_dev(Ctx& c, const u8* d_in, size_t n, int level, u8* d_out, size_t out_cap, size_t* out_n) {
+  g_plan.plan.reset();
+  Rle1Plan plan;
+  rle1_plan(c, d_in, n, level, plan);
   c.trace.clear();
-  if (plan_only) {
-    *out_n = 0;
-    c.plan_cache = planp; c.plan_ptr = d_in; c.plan_n = n; c.plan_level = level;
-    owner.keep = true;
-    return;
-  }
-  size_t first = whole_file ? 0 : std::min(first_block, nb_all);
-  size_t count = whole_file ? nb_all : std::min(block_count, nb_all - first);
-  if (first < plan.first_index) throw B2Error{B2_ERR_BAD_ARG, "block range is not covered by the cached range plan"};
-  EncSession S(c, level, d_out, out_cap, whole_file, bit_phase);
-  S.encode(d_in, n, plan, first - plan.first_index, count, 0);  // h_blocks[k] is global block first_index + k
-  const u64 bits = S.finish(out_n);
-  if (!whole_file && out_bits) *out_bits = bits - (u64)bit_phase;
-  if (crcs_out) *crcs_out = S.all_crc;
+  EncSession S(c, level, d_out, out_cap, true, 0);
+  S.encode(d_in, n, plan, 0, plan.nblocks, 0);
+  S.finish(out_n);
+}
+
+size_t bzip2_plan(Ctx& c, const u8* d_in, size_t n, int level) {
+  g_plan.plan.reset();
+  Rle1Plan plan;
+  rle1_plan(c, d_in, n, level, plan);
+  c.trace.clear();
+  const size_t nb = plan.nblocks;
+  g_plan.put(std::move(plan), d_in, n, level);
+  return nb;
+}
+
+// info = {raw start, raw end of the blocks cut, first, planned, cut, last}
+static void range_info(const Rle1Plan& plan, size_t first, size_t count, u64 last, u64* info) {
+  info[0] = plan.nblocks ? plan.h_blocks.front().s : 0;
+  info[1] = plan.nblocks ? plan.h_blocks.back().e : 0;
+  info[2] = first; info[3] = count; info[4] = plan.nblocks; info[5] = last;
+}
+
+// Speculative range plan (multi-GPU, whole input on every rank): the blocks of rank `rank` of `world` among the
+// total guess, cut from the speculative boundary.  info[5] = the total guess.
+void bzip2_plan_spec(Ctx& c, const u8* d_in, size_t n, int level, int rank, int world, u64* info) {
+  g_plan.plan.reset();
+  Rle1Plan plan;
+  rle1_scan_tiles(c, d_in, n, plan);
+  const size_t total = plan.total_guess(level);
+  const size_t first = (size_t)rank * total / world, count = (size_t)(rank + 1) * total / world - first;
+  rle1_cut_range(c, d_in, n, level, plan, first, count);
+  c.trace.clear();
+  range_info(plan, first, count, total, info);
+  g_plan.put(std::move(plan), d_in, n, level);
+}
+
+// Blocks [first, first+count) without file header and trailer, from bit `bit_phase` of d_out.
+void bzip2_encode_range(Ctx& c, const u8* d_in, size_t n, int level, size_t first, size_t count, int bit_phase, u8* d_out, size_t out_cap,
+                        u64* out_bits, u32* block_crcs) {
+  std::optional<Rle1Plan> plan = g_plan.take(d_in, n, level);
+  if (!plan) rle1_plan(c, d_in, n, level, plan.emplace());
+  c.trace.clear();
+  const size_t nb_all = plan->first_index + plan->nblocks;  // exact plans: first_index == 0
+  first = std::min(first, nb_all);
+  count = std::min(count, nb_all - first);
+  if (first < plan->first_index) throw B2Error{B2_ERR_BAD_ARG, "block range is not covered by the cached range plan"};
+  EncSession S(c, level, d_out, out_cap, false, bit_phase);
+  S.encode(d_in, n, *plan, first - plan->first_index, count, 0);  // h_blocks[k] is global block first_index + k
+  size_t bytes = 0;
+  const u64 bits = S.finish(&bytes);
+  if (out_bits) *out_bits = bits - (u64)bit_phase;
+  if (block_crcs) std::copy(S.all_crc.begin(), S.all_crc.end(), block_crcs);
 }
 
 // ---- multi-GPU: every rank holds a share of the input (plus some bytes of the next share) ---------------------
@@ -536,12 +554,9 @@ void bzip2_compress_device(Ctx& c, const u8* d_in, size_t n, int level, u8* d_ou
 // RLE1 bytes of the share when no run enters it, share length}
 void bzip2_share_summary(Ctx& c, const u8* d_in, size_t n, u64* out) {
   out[0] = out[1] = out[2] = 0; out[3] = n;
-  if (!n) return;
   Rle1Plan plan;
-  u64 agg[2] = {0, 0};
-  StageScope s(c, ST_RLE1);
-  rle1_plan_ex(c, d_in, n, 9, plan, -1, 0, true, 0, 0, agg);  // tiles only: the level does not matter
-  out[0] = agg[0]; out[1] = agg[1]; out[2] = plan.w_total;
+  rle1_scan_tiles(c, d_in, n, plan, 0, 0, out);
+  out[2] = plan.w_total;
 }
 // Cut blocks [first, first+count) of the whole input inside this rank's buffer (share + halo): st0 / W0 = run state
 // and RLE1 output in front of the buffer (from the summaries of the ranks before).  The blocks are located by the
@@ -549,21 +564,12 @@ void bzip2_share_summary(Ctx& c, const u8* d_in, size_t n, u64* out) {
 // checks that the pieces of all ranks chain up.  info = {raw start, raw end (buffer offsets), first, planned, cut,
 // W at the end of the buffer}.  The plan is kept for the b2_bzip2_encode_range_dev call that follows.
 void bzip2_plan_share(Ctx& c, const u8* d_buf, size_t n, int level, u64 st0, u64 W0, size_t first, size_t count, u64* info) {
-  if (c.plan_cache) { delete static_cast<Rle1Plan*>(c.plan_cache); c.plan_cache = nullptr; }
-  Rle1Plan* planp = new Rle1Plan();
-  struct Owner { Rle1Plan* p; bool keep; ~Owner() { if (!keep) delete p; } } owner{planp, false};
-  {
-    StageScope s(c, ST_RLE1);
-    rle1_plan_ex(c, d_buf, n, level, *planp, (long long)first, count, false, st0, W0, nullptr);
-  }
-  info[0] = planp->nblocks ? planp->h_blocks.front().s : 0;
-  info[1] = planp->nblocks ? planp->h_blocks.back().e : 0;
-  info[2] = first;
-  info[3] = count;
-  info[4] = planp->nblocks;
-  info[5] = planp->w_total;
-  c.plan_cache = planp; c.plan_ptr = d_buf; c.plan_n = n; c.plan_level = level;
-  owner.keep = true;
+  g_plan.plan.reset();
+  Rle1Plan plan;
+  rle1_scan_tiles(c, d_buf, n, plan, st0, W0);
+  rle1_cut_range(c, d_buf, n, level, plan, first, count);
+  range_info(plan, first, count, plan.w_total, info);
+  g_plan.put(std::move(plan), d_buf, n, level);
 }
 
 // Bzip2.compressFile with HOST buffers (b2_bzip2_compress).  With a pinned input the upload is cut into chunks
@@ -643,10 +649,7 @@ void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, int level, u8* d_in, 
       const bool last = avail == wlen;
       mark("chunks arrived", have);
       Rle1Plan plan;
-      {
-        StageScope s(c, ST_RLE1);
-        rle1_plan(c, d_in + resume, avail - resume, level, plan);
-      }
+      rle1_plan(c, d_in + resume, avail - resume, level, plan);
       // only the very end of the FILE closes a short block; the last block of any other prefix may still grow
       const size_t nfinal = (last && last_window) ? plan.nblocks : (plan.nblocks ? plan.nblocks - 1 : 0);
       mark("planned, final blocks", nfinal);

@@ -876,9 +876,6 @@ u32 crc32_device(Ctx& c, const u8* d_p, size_t n) {
 }
 
 // ---- host drivers ---------------------------------------------------------------------------
-// spec_first < 0: exact plan of the whole input.  Otherwise only blocks [spec_first, spec_first+spec_count) are
-// walked, starting from the speculative boundary W(s) = spec_first * BS (see k_rle_blocks); plan.first_index
-// records the global index of h_blocks[0] and plan.total_guess = ceil(W(N) / BS).
 // length of the run the buffer starts with (in bytes, not reduced): tiles of one and the same byte, then the lead of
 // the first tile that is not
 __global__ void k_share_lead(const TileSum* __restrict__ sums, u64 ntiles, u64* __restrict__ out) {
@@ -894,70 +891,65 @@ __global__ void k_share_lead(const TileSum* __restrict__ sums, u64 ntiles, u64* 
   *out = lead;
 }
 
-void rle1_plan_ex(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan, long long spec_first, size_t spec_count, bool tiles_only,
-                  u64 st0, u64 W0, u64* agg_state) {
+void rle1_scan_tiles(Ctx& c, const u8* d_in, size_t n, Rle1Plan& plan, u64 st0, u64 W0, u64* summary) {
   crc_setup();
-  plan.nblocks = 0;
-  plan.h_blocks.clear();
-  plan.first_index = 0;
-  plan.total_guess = 0;
+  StageScope s(c, ST_RLE1);
   if (n == 0) return;
-  const u32 BS = (u32)level * 100000 - 19;  // lib/Bzip2.js:892-900
   const u64 ntiles = (n + RLE_TILE - 1) / RLE_TILE;
-  if (plan.ntiles != ntiles || !plan.tile_prefix.p) {
-    plan.ntiles = ntiles;
-    DBuf<TileSum> sums(c, ntiles);
-    DBuf<u64> dagg(c, 4);
-    plan.tile_carry.alloc(c, ntiles);
-    plan.tile_prefix.alloc(c, ntiles + 1);
-    plan.tile_plain.alloc(c, ntiles);
-    k_rle_summary<<<(unsigned)ntiles, RT_THREADS, 0, c.stream>>>(d_in, n, sums, plan.tile_plain);
+  DBuf<TileSum> sums(c, ntiles);
+  DBuf<u64> dagg(c, 4);
+  plan.tile_carry.alloc(c, ntiles);
+  plan.tile_prefix.alloc(c, ntiles + 1);
+  plan.tile_plain.alloc(c, ntiles);
+  k_rle_summary<<<(unsigned)ntiles, RT_THREADS, 0, c.stream>>>(d_in, n, sums, plan.tile_plain);
+  KLAUNCH(c); KCHECK();
+  static const bool force_groups = getenv("B2_RLE_SCAN_GROUPS") != nullptr;  // test hook: multi-CTA scan on small inputs too
+  if (ntiles <= 4 * RG_TILES && !force_groups) {
+    k_rle_scan<<<1, RS_THREADS, 0, c.stream>>>(sums, ntiles, n, plan.tile_carry, plan.tile_prefix, st0, W0, dagg);
     KLAUNCH(c); KCHECK();
-    static const bool force_groups = getenv("B2_RLE_SCAN_GROUPS") != nullptr;  // test hook: multi-CTA scan on small inputs too
-    if (ntiles <= 4 * RG_TILES && !force_groups) {
-      k_rle_scan<<<1, RS_THREADS, 0, c.stream>>>(sums, ntiles, n, plan.tile_carry, plan.tile_prefix, st0, W0, dagg);
-      KLAUNCH(c); KCHECK();
-    } else {
-      c.stats.rle_group_scans++;
-      const u32 ng = (u32)((ntiles + RG_TILES - 1) / RG_TILES);
-      DBuf<u64> gagg(c, ng), gstart(c, ng + 1), gsum(c, ng), gbase(c, ng + 1);
-      k_rle_scan_g1<<<ng, RG_THREADS, 0, c.stream>>>(sums, ntiles, n, gagg);
-      KLAUNCH(c); KCHECK();
-      k_rle_scan_groups<true><<<1, RS_THREADS, 0, c.stream>>>(gagg, ng, gstart, st0, dagg);
-      KLAUNCH(c); KCHECK();
-      k_rle_scan_g3<<<ng, RG_THREADS, 0, c.stream>>>(sums, ntiles, n, gstart, plan.tile_carry, plan.tile_prefix, gsum);
-      KLAUNCH(c); KCHECK();
-      k_rle_scan_groups<false><<<1, RS_THREADS, 0, c.stream>>>(gsum, ng, gbase, W0, nullptr);
-      KLAUNCH(c); KCHECK();
-      k_rle_scan_g5<<<ng, RG_THREADS, 0, c.stream>>>(ntiles, gbase, ng, plan.tile_prefix);
-      KLAUNCH(c); KCHECK();
-    }
-    if (agg_state) {
-      // share summary for the multi-GPU planner: aggregate run state, length of the leading run, (W total follows below)
-      k_share_lead<<<1, 32, 0, c.stream>>>(sums, ntiles, dagg.p + 1);
-      KLAUNCH(c); KCHECK();
-      c.to_host(agg_state, dagg, 16);
-    }
+  } else {
+    c.stats.rle_group_scans++;
+    const u32 ng = (u32)((ntiles + RG_TILES - 1) / RG_TILES);
+    DBuf<u64> gagg(c, ng), gstart(c, ng + 1), gsum(c, ng), gbase(c, ng + 1);
+    k_rle_scan_g1<<<ng, RG_THREADS, 0, c.stream>>>(sums, ntiles, n, gagg);
+    KLAUNCH(c); KCHECK();
+    k_rle_scan_groups<true><<<1, RS_THREADS, 0, c.stream>>>(gagg, ng, gstart, st0, dagg);
+    KLAUNCH(c); KCHECK();
+    k_rle_scan_g3<<<ng, RG_THREADS, 0, c.stream>>>(sums, ntiles, n, gstart, plan.tile_carry, plan.tile_prefix, gsum);
+    KLAUNCH(c); KCHECK();
+    k_rle_scan_groups<false><<<1, RS_THREADS, 0, c.stream>>>(gsum, ng, gbase, W0, nullptr);
+    KLAUNCH(c); KCHECK();
+    k_rle_scan_g5<<<ng, RG_THREADS, 0, c.stream>>>(ntiles, gbase, ng, plan.tile_prefix);
+    KLAUNCH(c); KCHECK();
   }
-  u64 wtotal = 0;
-  c.to_host(&wtotal, plan.tile_prefix.p + ntiles, 8);
+  if (summary) {
+    k_share_lead<<<1, 32, 0, c.stream>>>(sums, ntiles, dagg.p + 1);
+    KLAUNCH(c); KCHECK();
+    c.to_host(summary, dagg, 16);
+  }
+  c.to_host(&plan.w_total, plan.tile_prefix.p + ntiles, 8);
   c.sync();
-  plan.total_guess = (size_t)((wtotal + BS - 1) / BS);
-  plan.w_total = wtotal;
-  if (tiles_only) return;
+}
+
+// exact: every block of the buffer.  Otherwise blocks [first, first+count) of the whole input, walked from the
+// speculative boundary W = first * BS (see k_rle_blocks); plan.first_index records the global index of h_blocks[0].
+static void cut_blocks(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan, bool exact, size_t first, size_t count) {
+  StageScope s(c, ST_RLE1);
+  if (n == 0) return;
+  const u32 BS = rle1_block_size(level);
+  const u64 ntiles = (n + RLE_TILE - 1) / RLE_TILE;
   u32 maxblocks = (u32)(n / ((u64)BS * 4 / 5) + 2);
   u64 u_start = 0;
-  if (spec_first >= 0) {
-    maxblocks = (u32)std::min<size_t>(maxblocks, spec_count);
-    u_start = (u64)spec_first * BS;
-    plan.first_index = (size_t)spec_first;
+  if (!exact) {
+    maxblocks = (u32)std::min<size_t>(maxblocks, count);
+    u_start = (u64)first * BS;
+    plan.first_index = first;
     if (maxblocks == 0) return;
   }
   plan.blocks.alloc(c, maxblocks);
   // many blocks: walk P segments in parallel first (see k_rle_blocks)
-  const u32 total = (u32)plan.total_guess;
-  const bool exact = spec_first < 0;
-  const u32 rfirst = exact ? 0u : (u32)spec_first, rcount = exact ? total : maxblocks;
+  const u32 total = (u32)plan.total_guess(level);
+  const u32 rfirst = exact ? 0u : (u32)first, rcount = exact ? total : maxblocks;
   const u32 P = std::min<u32>(64, rcount / 8);
   if (P > 1 && (!exact || total < maxblocks)) {
     DBuf<u32> dnb(c, P);
@@ -995,7 +987,13 @@ void rle1_plan_ex(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan, l
   if (nb) c.to_host(plan.h_blocks.data(), plan.blocks, sizeof(BlkInfo) * nb);
   c.sync();
 }
-void rle1_plan(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan) { rle1_plan_ex(c, d_in, n, level, plan, -1, 0, false, 0, 0, nullptr); }
+void rle1_cut_range(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan, size_t first, size_t count) {
+  cut_blocks(c, d_in, n, level, plan, false, first, count);
+}
+void rle1_plan(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan) {
+  rle1_scan_tiles(c, d_in, n, plan);
+  cut_blocks(c, d_in, n, level, plan, true, 0, 0);
+}
 void rle1_materialize(Ctx& c, const u8* d_in, size_t n, const Rle1Plan& plan, size_t first, size_t count, u8* d_T, u32* d_n, u32* d_crc) {
   if (count == 0) return;
   std::vector<u64> tbase(count + 1), pbase(count + 1);

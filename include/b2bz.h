@@ -129,18 +129,17 @@ int b2_bzip2_compress_dev(const void* d_in, size_t n, int level, void* d_out, si
 int b2_bzip2_decompress_dev(const void* d_in, size_t n, int multistream, void* d_out, size_t out_cap, size_t* out_n);
 
 /* ---- block-range encode for multi-GPU sharding (SURVEY.md section 8e) ------------- */
-/* Encodes blocks [first, first+count) of the stream that b2_bzip2_compress would produce
- * for (d_in, n, level) WITHOUT file header/trailer: the fragment starts at bit offset
- * (*bit_phase in 0..7, chosen by the caller = global bit offset mod 8) inside d_out and is
- * *out_bits long.  block_crcs (host, cap entries) receives the per-block CRCs so the
- * caller can fold the stream CRC.  total_blocks receives the number of blocks in the file. */
+/* Plan cache: b2_bzip2_plan, _plan_spec and _plan_share keep their plan, replacing the one kept before.  The next
+ * b2_bzip2_encode_range_dev takes it if it names the same (buffer, n, level), else plans the buffer exactly; either way
+ * the cache is empty afterwards.  b2_bzip2_compress_dev empties it, no other call touches it.  The buffer must not
+ * change in between. */
+/* Exact plan of the whole buffer; total_blocks receives the number of blocks in the file. */
 int b2_bzip2_plan(const void* d_in, size_t n, int level, size_t* total_blocks);
 /* Speculative range plan for rank `rank` of `world`: cuts only this rank's share of the blocks, starting from
  * the boundary implied by W-space arithmetic (exact unless a run-phase slip happened earlier in the file).
  * info[0..5] = raw start, raw end, first block, planned count, blocks actually cut, total block guess.
  * The ranks must verify end(r) == start(r+1), start(0) == 0, end(last) == n and cut == planned on every rank
- * (compressjs_b200/sharded.py does); otherwise fall back to b2_bzip2_plan.  The plan is cached for the next
- * b2_bzip2_encode_range_dev on the same buffer. */
+ * (compressjs_b200/sharded.py does); otherwise fall back to b2_bzip2_plan. */
 int b2_bzip2_plan_spec(const void* d_in, size_t n, int level, int rank, int world, uint64_t* info);
 /* Sharded input: every rank holds only a contiguous share of the input (followed by a halo: the first bytes of the
  * next share, so that a block that starts in the share can be finished).
@@ -150,12 +149,15 @@ int b2_bzip2_plan_spec(const void* d_in, size_t n, int level, int rank, int worl
 int b2_bzip2_share_summary(const void* d_share, size_t n, uint64_t* summary);
 /* Cuts blocks [first, first+count) of the whole input inside the buffer d_buf[0, n) = share + halo, given the run state
  * and RLE1 output in front of it.  Speculative like b2_bzip2_plan_spec (same checks by the caller); info[0..5] = raw
- * start, raw end (offsets inside d_buf), first, planned, blocks cut, RLE1 output up to the end of the buffer.  The plan
- * is cached for the next b2_bzip2_encode_range_dev(d_buf, n, level, first, count, ...). */
+ * start, raw end (offsets inside d_buf), first, planned, blocks cut, RLE1 output up to the end of the buffer. */
 int b2_bzip2_plan_share(const void* d_buf, size_t n, int level, uint64_t state_in, uint64_t w_in, size_t first, size_t count, uint64_t* info);
 /* dst := the first nbits of src moved to start at bit `phase` (0..7, MSB first), zero outside; dst must hold
  * ceil((phase+nbits)/32)*4 bytes and may not overlap src.  Used to align a fragment to its global bit offset. */
 int b2_bitshift_dev(const void* d_src, uint64_t nbits, int phase, void* d_dst);
+/* Encodes blocks [first, first+count) of the stream that b2_bzip2_compress would produce for (d_in, n, level)
+ * WITHOUT file header/trailer: the fragment starts at bit offset bit_phase (0..7, chosen by the caller = global bit
+ * offset mod 8) inside d_out (4-byte aligned, >= 32 bytes, zeroed first) and is *out_bits long (0 without blocks).
+ * block_crcs (host, one entry per block) receives the per-block CRCs so the caller can fold the stream CRC. */
 int b2_bzip2_encode_range_dev(const void* d_in, size_t n, int level, size_t first, size_t count, int bit_phase,
                               void* d_out, size_t out_cap, uint64_t* out_bits, uint32_t* block_crcs);
 
