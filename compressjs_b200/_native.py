@@ -10,10 +10,15 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B2_LIB") or os.path.join(_HERE, "libb2bz.so")
 _LIB = None
 
+# the callbacks of the stream entry points (b2_read_fn / b2_write_fn of include/b2bz.h)
+READ_FN = C.CFUNCTYPE(C.c_int64, C.c_void_p, C.POINTER(C.c_uint8), C.c_size_t)
+WRITE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_uint8), C.c_size_t)
+
 EXPORTS = [
     "b2_init", "b2_shutdown", "b2_last_error", "b2_free",
     "b2_bzip2_compress", "b2_bzip2_decompress", "b2_bzip2_decompress_block", "b2_bzip2_table",
     "b2_bzip2_decompress_partial", "b2_bzip2_decompress_block_partial", "b2_bzip2_table_partial", "b2_bzip2_decompress_blocks",
+    "b2_bzip2_compress_stream", "b2_bzip2_decompress_stream",
     "b2_bwt_cyclic", "b2_bwt_cyclic_batch", "b2_suffixsort", "b2_bwt_sentinel", "b2_bwt_inverse", "b2_bwtc_compress", "b2_bwtc_compress_unsized", "b2_bwtc_decompress", "b2_crc32_bzip2",
     "b2_bzip2_bound", "b2_bzip2_compress_dev", "b2_bzip2_decompress_dev",
     "b2_bzip2_plan", "b2_bzip2_plan_spec", "b2_bzip2_share_summary", "b2_bzip2_plan_share", "b2_bitshift_dev", "b2_dec_shard_open", "b2_dec_shard_export", "b2_dec_shard_finish", "b2_bzip2_encode_range_dev", "b2_get_stats", "b2_last_trace",
@@ -65,6 +70,8 @@ def lib():
                                                       C.POINTER(C.POINTER(C.c_uint32)), szp]
     L.b2_bzip2_decompress_blocks.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, u8pp, szp,
                                              C.POINTER(C.POINTER(C.c_uint64)), szp]
+    L.b2_bzip2_compress_stream.argtypes = [READ_FN, WRITE_FN, C.c_void_p, C.c_int]
+    L.b2_bzip2_decompress_stream.argtypes = [READ_FN, WRITE_FN, C.c_void_p, C.c_int]
     L.b2_bwt_cyclic.restype = C.c_int32
     L.b2_bwt_cyclic.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
     L.b2_bwt_cyclic_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]

@@ -5,6 +5,7 @@ import ctypes as C
 import numpy as np
 
 from . import _native
+from ._pump import Pump, is_stream_pair
 from ._streams import coerce_input, deliver_output
 
 
@@ -39,6 +40,16 @@ def _error(rc):
 
 def _raise(rc):
     raise _error(rc)
+
+
+def _level(props):
+    """compressFile's block size multiplier: props if it is a number (9 otherwise), 1..9 (lib/Bzip2.js:881-890)."""
+    level = 9
+    if isinstance(props, (int, float)) and not isinstance(props, bool):
+        level = props
+    if level < 1 or level > 9 or int(level) != level:
+        raise ValueError("Invalid block size multiplier")
+    return int(level)
 
 
 def _take(L, p, n):
@@ -86,14 +97,17 @@ class Bzip2:
 
     @staticmethod
     def compressFile(input, output=None, props=None):
-        """lib/Bzip2.js:879-929.  props: block size multiplier 1..9 (default 9)."""
+        """lib/Bzip2.js:879-929.  props: block size multiplier 1..9 (default 9).  When input has readByte and output
+        has writeByte, the input is read and the output written as the encode goes, in bounded memory."""
+        if is_stream_pair(input, output):
+            level = _level(props)   # before anything is read
+            pump = Pump(input, output)
+            rc = _native.lib().b2_bzip2_compress_stream(pump.read_fn, pump.write_fn, None, level)
+            pump.check(rc, _error)
+            return output
         L = _native.lib()
         data = coerce_input(input)
-        level = 9
-        if isinstance(props, (int, float)) and not isinstance(props, bool):
-            level = props
-        if level < 1 or level > 9 or int(level) != level:
-            raise ValueError("Invalid block size multiplier")
+        level = _level(props)
         out, n = C.POINTER(C.c_uint8)(), C.c_size_t()
         rc = L.b2_bzip2_compress(data.ctypes.data if data.size else None, data.size, int(level), C.byref(out), C.byref(n))
         if rc:
@@ -102,7 +116,14 @@ class Bzip2:
 
     @staticmethod
     def decompressFile(input, output=None, multistream=False):
-        """lib/Bzip2.js:454-481 (Bunzip.decode).  On a decode error the output receives the bytes decoded before it."""
+        """lib/Bzip2.js:454-481 (Bunzip.decode).  On a decode error the output receives the bytes decoded before it.
+        When input has readByte and output has writeByte, the input is read and the output written as the decode goes,
+        in bounded memory."""
+        if is_stream_pair(input, output):
+            pump = Pump(input, output)
+            rc = _native.lib().b2_bzip2_decompress_stream(pump.read_fn, pump.write_fn, None, int(bool(multistream)))
+            pump.check(rc, _error)
+            return output
         return _deliver(output, *_file(input, multistream))
 
     @staticmethod

@@ -13,6 +13,11 @@ The reference writes its output through a 4096-byte buffer that is flushed only 
 nothing flushes it when a decode throws (bin/compressjs:103-115): so on a decode error the output holds the bytes
 decoded before the error, cut down to a multiple of 4096.
 
+For -t bzip2 (without -b) the command line is a pipe filter, as the reference is: the input is read a chunk at a time
+and the output written as the library produces it (InStream / OutStream, the makeInStream / makeOutStream of
+bin/compressjs:60-120), so memory does not grow with the stream (include/b2bz.h gives the bound).  -b (the reference
+seeks in its input) and BWTC read the whole input first.
+
 Usage errors are found before the GPU library is loaded, so they work on a machine without a GPU.
 """
 import math
@@ -174,6 +179,74 @@ def read_input(fd):
     return b"".join(chunks), st.st_size
 
 
+class InStream:
+    """makeInStream of bin/compressjs:60-98: the descriptor read a chunk at a time, straight into the caller's buffer."""
+
+    def __init__(self, fd):
+        self.fd = fd
+
+    def read(self, buf, bufOffset, length):
+        """buf: a writable bytes-like object.  Returns the bytes read, 0 at the end of the input."""
+        return os.readv(self.fd, [memoryview(buf)[bufOffset:bufOffset + length]]) if length > 0 else 0
+
+    def readByte(self):
+        b = os.read(self.fd, 1)
+        return b[0] if b else -1
+
+
+class OutStream:
+    """makeOutStream of bin/compressjs:100-116: a FLUSH-byte buffer in front of the binary file `f`, flushed only when
+    the next byte arrives (or by flush()).  After T >= 1 bytes, the file has the first FLUSH * ((T - 1) // FLUSH)."""
+
+    def __init__(self, f):
+        self.f = f
+        self.pending = bytearray()
+
+    def writeByte(self, b):
+        if len(self.pending) >= FLUSH:
+            self.f.write(self.pending)
+            self.pending = bytearray()
+        self.pending.append(b & 0xFF)
+
+    def write(self, buf, bufOffset, length):
+        """writeByte of each of buf[bufOffset:bufOffset + length], with whole buffers written at once."""
+        data = memoryview(bytes(buf) if isinstance(buf, list) else buf).cast("B")[bufOffset:bufOffset + length]
+        total = len(self.pending) + len(data)
+        cut = total - ((total - 1) % FLUSH + 1) if total else 0   # what goes to the file: whole buffers
+        if cut:
+            head = cut - len(self.pending)   # >= 0: the pending buffer is at most FLUSH bytes
+            self.f.write(self.pending)
+            self.f.write(data[:head])
+            self.pending = bytearray(data[head:])
+        else:
+            self.pending += data
+        return length
+
+    def flush(self):
+        self.f.write(self.pending)
+        self.pending = bytearray()
+        self.f.flush()
+
+
+def stream_bzip2(decompress, level, in_fd, out):
+    """-t bzip2 without -b: Bzip2.compressFile / decompressFile from the descriptor to the binary file `out` through
+    the streams of bin/compressjs, in bounded memory.  The exit status; on an error its message is on stderr and `out`
+    has what went out before it (on a decode error: the decoded bytes cut down to a multiple of FLUSH)."""
+    from .bzip2 import Bzip2
+    src, dst = InStream(in_fd), OutStream(out)
+    try:
+        if decompress:
+            Bzip2.decompressFile(src, dst)   # without multistream, as bin/compressjs:160-164 calls it
+        else:
+            Bzip2.compressFile(src, dst, level)
+    except Exception as e:
+        out.flush()
+        sys.stderr.write("%s\n" % e)
+        return 1
+    dst.flush()
+    return 0
+
+
 def run(kind, decompress, level, block, data, size):
     """(output bytes, error or None).  On a decode error the bytes are those decoded before it."""
     from . import bwtc, bzip2
@@ -212,6 +285,8 @@ def main(argv=None):
         in_fd = os.open(args[0], os.O_RDONLY) if len(args) > 0 else sys.stdin.fileno()
         out = open(args[1], "wb") if len(args) > 1 else sys.stdout.buffer
         kind = compressor(opts["T"])
+        if kind == "bzip2" and block < 0:
+            return stream_bzip2(decompress, level, in_fd, out)
         data, size = read_input(in_fd)
         result, err = run(kind, decompress, level, block, data, size)
         if err is not None:

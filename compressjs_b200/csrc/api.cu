@@ -21,11 +21,21 @@ void dec_shard_export(u64* buf);
 int dec_shard_finish(Ctx& c, const u64* all, int multistream, u8* d_out, size_t out_cap, u64* res);
 int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multistream, u8* d_out, size_t out_cap, size_t* out_n,
                      const std::vector<u64>* positions, std::vector<u64>* ends, std::vector<u64>* tab_pos, std::vector<u32>* tab_len,
-                     void* (*alloc_host)(size_t), void (*free_host)(void*), u8** h_out);
+                     void* (*alloc_host)(size_t), void (*free_host)(void*), u8** h_out, StreamIn* sin = nullptr,
+                     StreamOut* sout = nullptr);
 
 static std::mutex g_mu;
 static Ctx* g_ctx = nullptr;
 static thread_local std::string g_err;
+// Set while a stream call runs one of its callbacks on this thread.  That thread holds g_mu, so a library call from the
+// callback would wait for itself: it fails at once instead.
+static thread_local bool t_in_callback = false;
+static const char* const IN_CALLBACK = "called from inside a stream callback";
+struct InCallback {
+  std::string err;  // the call's own error state, which the callback's library calls may overwrite
+  InCallback() : err(g_err) { t_in_callback = true; }
+  ~InCallback() { t_in_callback = false; g_err = err; }
+};
 static std::map<void*, size_t> g_pinned_live;                  // pointers handed to the caller
 static std::multimap<size_t, void*> g_pinned_free;             // cached pinned buffers by capacity
 
@@ -178,6 +188,7 @@ static void pinned_release(void* p) {
 
 template <typename F>
 static int guarded(F f) {
+  if (t_in_callback) { g_err = IN_CALLBACK; return B2_ERR_BAD_ARG; }
   std::lock_guard<std::mutex> lk(g_mu);
   try {
     g_err.clear();
@@ -207,6 +218,7 @@ int b2_init(int device) {
 }
 
 void b2_shutdown(void) {
+  if (t_in_callback) { g_err = IN_CALLBACK; return; }
   std::lock_guard<std::mutex> lk(g_mu);
   if (!g_ctx) return;
   cudaSetDevice(g_ctx->device);
@@ -230,17 +242,20 @@ const char* b2_last_error(void) { return g_err.c_str(); }
 
 void b2_free(void* p) {
   if (!p) return;
+  if (t_in_callback) { g_err = IN_CALLBACK; return; }
   std::lock_guard<std::mutex> lk(g_mu);
   if (g_pinned_live.find(p) == g_pinned_live.end()) { free(p); return; }
   pinned_release(p);
 }
 
 void b2_get_stats(b2_stats* s) {
+  if (t_in_callback) { g_err = IN_CALLBACK; memset(s, 0, sizeof *s); return; }
   std::lock_guard<std::mutex> lk(g_mu);
   if (g_ctx) *s = g_ctx->stats; else memset(s, 0, sizeof *s);
 }
 
 size_t b2_last_trace(b2_block_trace* out, size_t cap) {
+  if (t_in_callback) { g_err = IN_CALLBACK; return 0; }
   std::lock_guard<std::mutex> lk(g_mu);
   if (!g_ctx) return 0;
   size_t n = g_ctx->trace.size();
@@ -419,6 +434,7 @@ int b2_bwtc_decompress(const uint8_t* in, size_t n, uint8_t** out, size_t* out_n
 }
 
 uint32_t b2_crc32_bzip2(const uint8_t* p, size_t n) {
+  if (t_in_callback) { g_err = IN_CALLBACK; return (uint32_t)B2_ERR_BAD_ARG; }
   uint32_t crc = 0;
   int rc = guarded([&]() {
     Ctx& c = ctx_locked();
@@ -439,6 +455,139 @@ size_t b2_bzip2_bound(size_t n) {
   // RLE1 can expand the block stream by 5/4.  Use a comfortable 1.5x + per-block headers.
   size_t blocks = n / 99981 + 2;
   return n + n / 2 + blocks * 4096 + 64;
+}
+
+}  // extern "C"
+
+// Inputs above the streaming window pass through the device in windows (bounded device memory: files larger than HBM);
+// $B2_STREAM_WINDOW sets the window in bytes (default 8 GiB, at least 64 MiB -- a test hook allows less).
+static size_t stream_window() {
+  size_t win = (size_t)8 << 30;
+  if (const char* e = getenv("B2_STREAM_WINDOW")) { const long long v = atoll(e); if (v >= (1 << 20)) win = (size_t)v; }
+  return win;
+}
+
+// ---- the callbacks of the stream entry points ----
+StreamIn::~StreamIn() {
+  if (buf) { cudaStreamSynchronize(busy); free(buf); }
+}
+size_t StreamIn::fill(size_t end) {
+  while (base + have < end && !eof) {
+    if (have == cap) {
+      // double (from 64 KiB), but never past what is asked for: memory follows the data that has arrived.  Pageable:
+      // pinning every size a growing buffer passes through costs more than the driver's staged copies out of it
+      const size_t ncap = std::max<size_t>((size_t)64 << 10, std::min(2 * cap, end - base));
+      CUDA_CHECK(cudaStreamSynchronize(busy));
+      u8* nb = (u8*)realloc(buf, ncap);
+      if (!nb) throw B2Error{B2_ERR_CUDA, "out of host memory"};
+      buf = nb; cap = ncap;
+    }
+    int64_t got;
+    {
+      InCallback in;
+      got = rd(user, buf + have, cap - have);
+    }
+    if (got < 0) throw B2Error{B2_ERR_STREAM, "the read callback aborted the stream"};
+    if ((uint64_t)got > cap - have) throw B2Error{B2_ERR_BAD_ARG, "the read callback returned more bytes than it was asked for"};
+    if (got == 0) eof = true;
+    have += (size_t)got;
+  }
+  return base + have;
+}
+void StreamIn::drop(size_t pos) {
+  const size_t k = std::min(pos > base ? pos - base : 0, have);
+  if (!k) return;
+  CUDA_CHECK(cudaStreamSynchronize(busy));
+  memmove(buf, buf + k, have - k);
+  base += k; have -= k;
+}
+// the output buffer comes from (and goes back to) the pinned buffers b2_free recycles: a second call reuses it
+StreamOut::~StreamOut() {
+  if (buf) pinned_release(buf);
+}
+void StreamOut::reserve(size_t bytes, size_t limit) {
+  if (bytes <= cap) return;
+  const size_t ncap = std::max(bytes, std::min(2 * cap, limit));
+  if (buf) pinned_release(buf);
+  buf = nullptr; cap = 0;
+  buf = (u8*)pinned_alloc(ncap);
+  cap = ncap;
+}
+void StreamOut::put(const u8* p, size_t n) {
+  if (!n) return;
+  int r;
+  {
+    InCallback in;
+    r = wr(user, p, n);
+  }
+  if (r != 0) throw B2Error{B2_ERR_STREAM, "the write callback aborted the stream"};
+  written += n;
+}
+
+extern "C" {
+
+int b2_bzip2_compress_stream(b2_read_fn rd, b2_write_fn wr, void* user, int level) {
+  return guarded([&]() {
+    if (level < 1 || level > 9) throw B2Error{B2_ERR_BAD_LEVEL, "Invalid block size multiplier"};
+    if (!rd || !wr) throw B2Error{B2_ERR_BAD_ARG, "null callback"};
+    Ctx& c = ctx_locked();
+    c.reset_call();
+    StreamIn in(rd, user, c.h2d_stream);
+    StreamOut out(wr, user);
+    size_t produced = 0;
+    try {
+      StageScope tot(c, ST_TOTAL);
+      // the first window sizes the buffers as the input's size does in b2_bzip2_compress: an input that ends inside it
+      // is one window of exactly its size
+      size_t win = stream_window();
+      const size_t first = in.fill(win + 1);
+      const bool whole = in.eof && first <= win;
+      if (whole) win = first;
+      const size_t dcap = whole ? b2_bzip2_bound(first) : b2_bzip2_bound(win) + 64;
+      out.reserve(dcap, dcap);
+      DBuf<u8> din(c, win ? win : 1), dout(c, dcap);
+      c.sync();  // the buffers are used from the copy streams as well
+      bzip2_compress_host(c, nullptr, 0, &in, level, din, win, dout, dcap, nullptr, 0, &out, &produced, false);
+    } catch (...) {
+      cudaStreamSynchronize(c.stream);  // nothing of this call may still be running when the next one starts
+      throw;
+    }
+    c.sync();
+    c.collect();
+    c.stats.raw_bytes = in.base + in.have; c.stats.comp_bytes = produced;
+    return 0;
+  });
+}
+
+int b2_bzip2_decompress_stream(b2_read_fn rd, b2_write_fn wr, void* user, int multistream) {
+  return guarded([&]() {
+    if (!rd || !wr) throw B2Error{B2_ERR_BAD_ARG, "null callback"};
+    Ctx& c = ctx_locked();
+    c.reset_call();
+    StreamIn in(rd, user, c.stream);
+    StreamOut out(wr, user);
+    size_t produced = 0;
+    int rc = 0;
+    try {
+      StageScope tot(c, ST_TOTAL);
+      try {
+        rc = bzip2_decompress(c, nullptr, nullptr, 0, multistream, nullptr, 0, &produced, nullptr, nullptr, nullptr, nullptr, nullptr,
+                              nullptr, nullptr, &in, &out);
+      } catch (const B2Error& e) {
+        if (e.code != B2_ERR_NOT_BZIP_DATA && e.code != B2_ERR_DATA_ERROR && e.code != B2_ERR_OBSOLETE_INPUT) throw;
+        g_err = e.msg;
+        rc = e.code;
+      }
+      c.sync();
+    } catch (...) {
+      cudaStreamSynchronize(c.stream);
+      throw;
+    }
+    c.sync();
+    c.collect();
+    c.stats.raw_bytes = produced; c.stats.comp_bytes = in.base + in.have;
+    return rc;
+  });
 }
 
 int b2_bzip2_compress_dev(const void* d_in, size_t n, int level, void* d_out, size_t out_cap, size_t* out_n) {
@@ -466,10 +615,7 @@ int b2_bzip2_compress(const uint8_t* in, size_t n, int level, uint8_t** out, siz
     void* host = pinned_alloc(cap);
     try {
       StageScope tot(c, ST_TOTAL);
-      // Inputs above the streaming window pass through the device in windows (bounded device memory: files larger than
-      // HBM); $B2_STREAM_WINDOW sets the window in bytes (default 8 GiB, at least 64 MiB -- a test hook allows less).
-      size_t win = (size_t)8 << 30;
-      if (const char* e = getenv("B2_STREAM_WINDOW")) { const long long v = atoll(e); if (v >= (1 << 20)) win = (size_t)v; }
+      size_t win = stream_window();
       if (win > n) win = n;
       const size_t dcap = win < n ? b2_bzip2_bound(win) + 64 : cap;
       DBuf<u8> din(c, win ? win : 1), dout(c, dcap);
@@ -477,7 +623,7 @@ int b2_bzip2_compress(const uint8_t* in, size_t n, int level, uint8_t** out, siz
       cudaPointerAttributes pa;
       const bool pinned_in = n && cudaPointerGetAttributes(&pa, in) == cudaSuccess && pa.type == cudaMemoryTypeHost;
       cudaGetLastError();
-      bzip2_compress_host(c, in, n, level, din, win, dout, dcap, (u8*)host, cap, &produced, pinned_in);
+      bzip2_compress_host(c, in, n, nullptr, level, din, win, dout, dcap, (u8*)host, cap, nullptr, &produced, pinned_in);
     } catch (...) {
       pinned_release(host);
       throw;

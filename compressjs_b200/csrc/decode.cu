@@ -1438,9 +1438,14 @@ static void scan_window(Ctx& c, const u8* in, u64 wbytes, u64 base_bit, u64 lim,
 // through a device staging buffer of at most max(W, one block) bytes.
 // positions: decode the blocks at these bit positions, back to back in list order (ends: the end offset of every
 // position delivered in full), with the whole input on the device.
+// Stream calls (b2_bzip2_decompress_stream): the input comes from `sin` instead (h_in, d_in and n are unused), which keeps
+// the bytes from the window's start on.  Every window is read one byte past its end, so the stream's end is known exactly
+// when b2_bzip2_decompress would know it (n stays unknown until then, and no window is the last one).  The staged blocks
+// go out through `sout`, each group only as far as the replay allows, so nothing past the prefix of
+// b2_bzip2_decompress_partial is ever written.
 int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multistream, u8* d_out, size_t out_cap, size_t* out_n,
                      const std::vector<u64>* positions, std::vector<u64>* ends, std::vector<u64>* tab_pos, std::vector<u32>* tab_len,
-                     void* (*alloc_host)(size_t), void (*free_host)(void*), u8** h_out) {
+                     void* (*alloc_host)(size_t), void (*free_host)(void*), u8** h_out, StreamIn* sin, StreamOut* sout) {
   *out_n = 0;
   // with neither d_out nor h_out (a table, or a device call without a buffer) the blocks are expanded only for their CRCs
   const bool dev = d_out != nullptr, listed = positions != nullptr;
@@ -1451,12 +1456,23 @@ int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multi
     CUDA_CHECK(cudaStreamSynchronize(c.stream));
   };
   Chain ch;
-  {
+  // stream calls: the input's length, once read has returned 0
+  auto learn_end = [&]() {
+    if (sin->eof) ch.n = n = sin->base + sin->have;
+  };
+  if (sin) {
+    n = SIZE_MAX;
+    const size_t end = sin->fill(5);  // the header, and whether anything follows it
+    u8 hdr[4] = {0, 0, 0, 0};
+    memcpy(hdr, sin->at(0), std::min<size_t>(end, 4));
+    read_level(hdr, end, &ch.cur_dbuf);
+  } else {
     u8 hdr[4] = {0, 0, 0, 0};
     read_in(hdr, 0, std::min<size_t>(n, 4));
     read_level(hdr, n, &ch.cur_dbuf);
   }
   ch.n = n;
+  if (sin) learn_end();
   ch.multistream = listed ? 0 : multistream;
   const size_t W = dec_window();
   const u32 DB = dec_batch_blocks(c);
@@ -1476,6 +1492,14 @@ int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multi
   u64 prev_a = ~0ull;
   size_t wcur = W;
   auto head = [&](u64 bytepos, u8* h) -> size_t {
+    if (sin) {
+      // the header may lie past the window; one byte more tells whether the file ends behind it
+      const size_t end = sin->fill(bytepos + 5);
+      learn_end();
+      const size_t avail = (size_t)std::min<u64>(4, end - bytepos);
+      memcpy(h, sin->at(bytepos), avail);
+      return avail;
+    }
     const size_t avail = (size_t)std::min<u64>(4, n - bytepos);
     read_in(h, bytepos, avail);
     return avail;
@@ -1499,14 +1523,19 @@ int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multi
     const u64 a = listed ? 0 : (ch.pos >> 3) & ~(u64)255;
     wcur = a == prev_a ? wcur * 2 : W;
     prev_a = a;
-    const u64 wl = listed ? n : std::min<u64>(wcur, n - a);
+    if (sin) {
+      sin->drop(a);
+      sin->fill(a + wcur + 1);
+      learn_end();
+    }
+    const u64 wl = listed ? n : std::min<u64>(wcur, (sin ? sin->base + sin->have : n) - a);
     const bool last = a + wl == n;
     if (wl + 32 > win_cap) { win.alloc(c, wl + 32); win_cap = wl + 32; }
     // zero padded (aligned word reads past the end must be safe)
     CUDA_CHECK(cudaMemsetAsync(win.p + (wl & ~(u64)3), 0, 32 + (wl & 3), c.stream));
-    if (h_in) {
+    if (h_in || sin) {
       StageScope s(c, ST_H2D);
-      if (wl) CUDA_CHECK(cudaMemcpyAsync(win, h_in + a, wl, cudaMemcpyHostToDevice, c.stream));
+      if (wl) CUDA_CHECK(cudaMemcpyAsync(win, h_in ? h_in + a : sin->at(a), wl, cudaMemcpyHostToDevice, c.stream));
     } else if (wl) {
       CUDA_CHECK(cudaMemcpyAsync(win, d_in + a, wl, cudaMemcpyDeviceToDevice, c.stream));
     }
@@ -1585,6 +1614,8 @@ int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multi
       for (size_t ei = e0; ei < e1; ei++) if (ch.events[ei].kind == 0) settled.push_back(ei);
       got.assign(cnt ? cnt : 1, 0);
       ob.assign(cnt ? cnt : 1, ~0ull);
+      auto got_fn = [&](size_t slot) { return std::make_pair(ob[slot] != ~0ull, got[slot]); };
+      size_t er = e0;  // events replayed so far (stream calls replay group by group)
       if (dev) {
         // straight to the caller's buffer; a block that does not fit is only counted (the needed size is returned)
         for (size_t ei : settled) { const Event& ev = ch.events[ei]; if (ev.off + ev.len <= out_cap) ob[ev.slot] = ev.off; }
@@ -1607,12 +1638,28 @@ int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multi
             CUDA_CHECK(cudaMemcpyAsync(*h_out + f.off, stage, bytes, cudaMemcpyDeviceToHost, c.stream));
             h_have = f.off + bytes;
           }
+          if (sout) {
+            // the group's events say how much of it the reference writes before it throws
+            const size_t g_end = settled[g1 - 1] + 1;
+            replay(ch, er, g_end, got_fn, tab_pos, tab_len, ends, E);
+            er = g_end;
+            const u64 keep = E.ev < 0 ? bytes : (E.prefix > f.off ? std::min<u64>(bytes, E.prefix - f.off) : 0);
+            if (keep) {
+              sout->reserve((size_t)keep, std::max<size_t>(W, (size_t)keep));
+              {
+                StageScope s(c, ST_D2H);
+                CUDA_CHECK(cudaMemcpyAsync(sout->buf, stage, keep, cudaMemcpyDeviceToHost, c.stream));
+              }
+              CUDA_CHECK(cudaStreamSynchronize(c.stream));
+              sout->put(sout->buf, (size_t)keep);
+            }
+            if (E.ev >= 0) break;
+          }
           g0 = g1;
         }
       }
       // ---- replay: the first failure in stream order ends the call (the device path walks on for the needed size) ----
-      if (E.ev < 0)
-        replay(ch, e0, e1, [&](size_t slot) { return std::make_pair(ob[slot] != ~0ull, got[slot]); }, tab_pos, tab_len, ends, E);
+      if (E.ev < 0) replay(ch, er, e1, got_fn, tab_pos, tab_len, ends, E);
       if (ch.done || (E.ev >= 0 && !dev) || need_window) break;
       const size_t nk = listed ? kb + cnt : first_blk_from(ch.pos);
       if (nk <= kb) throw B2Error{B2_ERR_CUDA, "bzip2 decode: the chain walk made no progress"};
@@ -1626,7 +1673,7 @@ int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multi
   }
   if (E.ev >= 0) {
     // the host path hands the output in front of the error to the caller with the error (b2_bzip2_decompress_partial)
-    if (h_out) *out_n = (size_t)E.prefix;
+    if (h_out || sout) *out_n = (size_t)E.prefix;
     throw B2Error{E.code, E.msg};
   }
   *out_n = (size_t)ch.total_out;

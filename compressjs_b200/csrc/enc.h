@@ -81,10 +81,41 @@ u32 crc32_device(Ctx& c, const u8* d_p, size_t n);
 void bwt_forward_batch(Ctx& c, const u8* d_T, u8* d_U, const u32* d_n, const u32* h_n, u32 nblk, u32* d_pidx, bool sentinel = false,
                        u32* d_sa_out = nullptr, u32* d_hist_out = nullptr);
 
+// ---- the callbacks of the stream entry points (b2_bzip2_*_stream; implemented in api.cu) ----
+// The input: the stream's bytes [base, base + have) in a host buffer that doubles as data arrives.  A callback that
+// aborts throws B2Error{B2_ERR_STREAM}.
+struct StreamIn {
+  b2_read_fn rd; void* user;
+  cudaStream_t busy;  // copies out of buf may be queued here: they are waited for before buf changes
+  u8* buf = nullptr;
+  size_t cap = 0, base = 0, have = 0;
+  bool eof = false;   // read returned 0: the stream is base + have bytes long
+  StreamIn(b2_read_fn rd_, void* user_, cudaStream_t busy_) : rd(rd_), user(user_), busy(busy_) {}
+  StreamIn(const StreamIn&) = delete;
+  ~StreamIn();
+  size_t fill(size_t end);  // read until the bytes in front of `end` are here or the input ends; returns base + have
+  void drop(size_t pos);    // forget the bytes in front of pos
+  const u8* at(size_t pos) const { return buf + (pos - base); }
+};
+// The output: pieces are staged in a pinned buffer (from the library's pinned pool) and handed to the write callback.
+struct StreamOut {
+  b2_write_fn wr; void* user;
+  u8* buf = nullptr;
+  size_t cap = 0;
+  u64 written = 0;
+  StreamOut(b2_write_fn wr_, void* user_) : wr(wr_), user(user_) {}
+  StreamOut(const StreamOut&) = delete;
+  ~StreamOut();
+  void reserve(size_t bytes, size_t limit);  // buf holds >= bytes (doubling up to `limit`); its contents are not kept
+  void put(const u8* p, size_t n);
+};
+
 // ---- bzip2 encode drivers (encode.cu), one per entry point of include/b2bz.h ----
 void bzip2_compress_dev(Ctx& c, const u8* d_in, size_t n, int level, u8* d_out, size_t out_cap, size_t* out_n);
-void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, int level, u8* d_in, size_t win, u8* d_out, size_t out_cap, u8* h_out,
-                         size_t h_out_cap, size_t* out_n, bool pinned_in);
+// b2_bzip2_compress (h_in, n; output to h_out) and b2_bzip2_compress_stream (input from `sin`; output through `sout`,
+// staged in sout->buf, which holds out_cap bytes)
+void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, StreamIn* sin, int level, u8* d_in, size_t win, u8* d_out, size_t out_cap,
+                         u8* h_out, size_t h_out_cap, StreamOut* sout, size_t* out_n, bool pinned_in);
 size_t bzip2_plan(Ctx& c, const u8* d_in, size_t n, int level);
 void bzip2_plan_spec(Ctx& c, const u8* d_in, size_t n, int level, int rank, int world, u64* info);
 void bzip2_share_summary(Ctx& c, const u8* d_in, size_t n, u64* out);

@@ -576,14 +576,19 @@ void bzip2_plan_share(Ctx& c, const u8* d_buf, size_t n, int level, u64 st0, u64
 // on a copy stream; block boundaries only depend on the bytes before them (lib/Bzip2.js:636-667 consumes its
 // input strictly forward), so every block but the last of a plan over the prefix that has arrived is final
 // and is encoded while the rest is still in flight.  Finished words of the output go back on a second copy
-// stream after every batch.  h_out must hold out_cap bytes (pinned).
-void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, int level, u8* d_in, size_t win, u8* d_out, size_t out_cap, u8* h_out,
-                         size_t h_out_cap, size_t* out_n, bool pinned_in) {
+// stream after every batch.  h_out must hold h_out_cap bytes (pinned).
+// Stream calls: the input comes from `sin` (h_in and n are unused) and the output goes out through `sout`.  sin keeps
+// the bytes from the window's start on and reads until it holds more than a window or the input ends, so every window
+// is the one b2_bzip2_compress would see for the whole input: the same blocks, the same stream.  Each window's output
+// is staged in sout->buf (it holds out_cap bytes, like d_out) and written after every batch.
+void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, StreamIn* sin, int level, u8* d_in, size_t win, u8* d_out, size_t out_cap,
+                         u8* h_out, size_t h_out_cap, StreamOut* sout, size_t* out_n, bool pinned_in) {
   // d_in holds `win` bytes, d_out `out_cap` bytes (>= b2_bzip2_bound(win)).  win >= n: the whole file in one window (the
   // usual case).  win < n: the input STREAMS through the device in windows -- every window is uploaded, planned and
   // encoded like a small file whose last block is kept back (it may go on in the next window), the next window starts at
   // the first raw byte that has not been consumed, and the output window is drained and rebased in between: device
   // memory is bounded by the window, not by the file (lib/Bzip2.js:879-929 reads its input strictly forward, too).
+  if (sout) { h_out = sout->buf; h_out_cap = sout->cap; }
   size_t CH = (size_t)64 << 20;
   if (const char* e = getenv("B2_H2D_CHUNK")) {  // test hook: small chunks exercise the prefix planning on small inputs
     const long long v = atoll(e);
@@ -594,7 +599,7 @@ void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, int level, u8* d_in, 
   auto mark = [&](const char* what, size_t v) {
     if (trace_host) fprintf(stderr, "[b2 host] %8.2f ms  %s %zu\n", std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count(), what, v);
   };
-  const size_t max_ch = (std::min(win, n) + CH - 1) / CH + 1;
+  const size_t max_ch = ((sin ? win : std::min(win, n)) + CH - 1) / CH + 1;
   std::vector<cudaEvent_t> ev(max_ch);
   struct Cleanup {
     std::vector<cudaEvent_t>& ev; Ctx& c;
@@ -608,11 +613,21 @@ void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, int level, u8* d_in, 
   EncSession S(c, level, d_out, out_cap, true, 0);
   mark("session ready", 0);
   size_t copied = 0;       // bytes of the current output window already on their way to the host
-  size_t host_base = 0;    // offset in h_out of the window's byte 0
+  size_t host_base = 0;    // offset in h_out of the window's byte 0 (stream calls: always 0)
+  size_t out_base = 0;     // offset in the output of the window's byte 0
+  size_t sent = 0;         // stream calls: bytes of the current output window written
   bool d2h_started = false, h2d_started = false;
+  // stream calls: write what the copies queued so far have brought to the host
+  auto drain = [&]() {
+    if (!sout || copied == sent) return;
+    CUDA_CHECK(cudaStreamSynchronize(c.d2h_stream));
+    sout->put(h_out + sent, copied - sent);
+    sent = copied;
+  };
   S.on_batch = [&](u64 bit_end) {
     const size_t ready = (size_t)(bit_end / 32) * 4;  // whole words below the one still being filled
     if (ready > copied) {
+      drain();  // the previous batch's words: their copy has had a batch's time to land
       if (host_base + ready > h_out_cap) throw B2Error{B2_ERR_BAD_ARG, "output buffer too small for the compressed stream"};
       if (!d2h_started) { c.copy_begin(c.d2h_stream, 1); d2h_started = true; }
       CUDA_CHECK(cudaMemcpyAsync(h_out + host_base + copied, d_out + copied, ready - copied, cudaMemcpyDeviceToHost, c.d2h_stream));
@@ -620,21 +635,36 @@ void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, int level, u8* d_in, 
     }
   };
   size_t file_pos = 0;  // raw bytes consumed by finished blocks
-  for (bool first_window = true; first_window || file_pos < n; first_window = false) {
-    const size_t wlen = std::min(win, n - file_pos);
-    const bool last_window = file_pos + wlen == n;
+  for (bool first_window = true;; first_window = false) {
+    const u8* src;        // the window's input on the host
+    size_t wlen;
+    bool last_window;
+    if (sin) {
+      // the window and one byte more when there is one: a window that holds the rest of the input is the last one
+      sin->drop(file_pos);
+      const size_t end = sin->fill(file_pos + win + 1);
+      wlen = std::min(win, end - file_pos);
+      last_window = sin->eof && file_pos + wlen == end;
+      src = sin->at(file_pos);
+    } else {
+      wlen = std::min(win, n - file_pos);
+      last_window = file_pos + wlen == n;
+      src = h_in + file_pos;
+    }
     if (!first_window) {
       // the previous window's output is on its way: wait for it, then reuse both windows
       CUDA_CHECK(cudaStreamSynchronize(c.d2h_stream));
+      drain();
       S.rebase(copied + 8);
-      host_base += copied;
-      copied = 0;
+      out_base += copied;
+      if (!sout) host_base += copied;
+      copied = sent = 0;
     }
     const size_t nch = (pinned_in && wlen > CH) ? (wlen + CH - 1) / CH : (wlen ? 1 : 0);
     if (!h2d_started) { c.copy_begin(c.h2d_stream, 0); h2d_started = true; }
     for (size_t i = 0; i < nch; i++) {
       const size_t o = nch == 1 ? 0 : i * CH, len = nch == 1 ? wlen : std::min(CH, wlen - o);
-      CUDA_CHECK(cudaMemcpyAsync(d_in + o, h_in + file_pos + o, len, cudaMemcpyHostToDevice, c.h2d_stream));
+      CUDA_CHECK(cudaMemcpyAsync(d_in + o, src + o, len, cudaMemcpyHostToDevice, c.h2d_stream));
       CUDA_CHECK(cudaEventRecord(ev[i], c.h2d_stream));
     }
     c.copy_end(c.h2d_stream, 0);
@@ -671,13 +701,15 @@ void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, int level, u8* d_in, 
   size_t total = 0;
   S.finish(&total);
   *out_n = total;
-  if (*out_n > h_out_cap) throw B2Error{B2_ERR_BAD_ARG, "output buffer too small for the compressed stream"};
+  const size_t tail = *out_n - out_base;  // bytes of the last window, trailer included
+  if (host_base + tail > h_out_cap) throw B2Error{B2_ERR_BAD_ARG, "output buffer too small for the compressed stream"};
   if (!d2h_started) c.copy_begin(c.d2h_stream, 1);
-  const size_t tail = *out_n - host_base;  // bytes of the last window, trailer included
   CUDA_CHECK(cudaMemcpyAsync(h_out + host_base + copied, d_out + copied, tail - copied, cudaMemcpyDeviceToHost, c.d2h_stream));
   c.copy_end(c.d2h_stream, 1);
   mark("finished, bytes left to download", tail - copied);
+  copied = tail;
   CUDA_CHECK(cudaStreamSynchronize(c.d2h_stream));
+  drain();
   mark("download done", *out_n);
 }
 

@@ -14,7 +14,8 @@
  *     library in pinned host memory and released with b2_free().
  *   - all work runs on the GPU selected by b2_init(); there is NO CPU fallback: if no
  *     CUDA device is usable every call fails with B2_ERR_CUDA.
- *   - calls are synchronous and serialised by an internal mutex.
+ *   - calls are synchronous and serialised by an internal mutex.  A call made from inside a stream callback (below)
+ *     fails with B2_ERR_BAD_ARG instead of waiting for that mutex.
  */
 #ifndef B2BZ_H
 #define B2BZ_H
@@ -33,6 +34,7 @@ extern "C" {
 #define B2_ERR_BAD_LEVEL (-100)   /* lib/Bzip2.js:888-890 "Invalid block size multiplier" */
 #define B2_ERR_BAD_ARG (-101)
 #define B2_ERR_BAD_MAGIC (-102)   /* lib/Util.js:151-153 Error("Bad magic") of the BWTC container */
+#define B2_ERR_STREAM (-103)      /* a read or write callback of a stream call asked to abort */
 #define B2_ERR_CUDA (-200)        /* CUDA runtime failure or no device: never falls back to CPU */
 
 /* Select the CUDA device (ordinal) used by this process and create the context.
@@ -85,6 +87,39 @@ int b2_bzip2_table_partial(const uint8_t* in, size_t n, int multistream, uint64_
  * *out and *ends are released with b2_free(); on any other error nothing is returned. */
 int b2_bzip2_decompress_blocks(const uint8_t* in, size_t n, const uint64_t* bitpos, size_t count, uint8_t** out, size_t* out_n,
                                uint64_t** ends, size_t* done);
+
+/* ---- streams: Bzip2.compressFile / decompressFile over readByte / writeByte streams (lib/Bzip2.js:405-448, 879-929) ----
+ * The input is pulled through a read callback and the output pushed through a write callback as the call goes, so host
+ * memory does not grow with the stream.  Both callbacks run on the calling thread, in stream order.
+ *   read:  puts 1..cap bytes into buf and returns how many; 0 = end of input; < 0 = abort.  A short read is not the end:
+ *          only a read that returns 0 ends the input.  Returning more than cap fails the call with B2_ERR_BAD_ARG.
+ *   write: takes n > 0 bytes of output; returns 0 to go on, anything else to abort.
+ * After an abort no further callback runs and the call returns B2_ERR_STREAM, with a message naming the callback.  Any
+ * call of this library made from inside a callback fails with B2_ERR_BAD_ARG ("called from inside a stream callback";
+ * b2_crc32_bzip2 returns (uint32_t)B2_ERR_BAD_ARG there, and b2_free, b2_get_stats, b2_last_trace and b2_shutdown do
+ * nothing). */
+typedef int64_t (*b2_read_fn)(void* user, uint8_t* buf, size_t cap);
+typedef int (*b2_write_fn)(void* user, const uint8_t* buf, size_t n);
+/* Compress: everything passed to write, concatenated, is the *out of b2_bzip2_compress on everything read returned, at
+ * the same level, however the input is split into reads; b2_last_trace and b2_get_stats report the call as they do
+ * there.  An empty input gives the 14-byte file.  A bad level returns B2_ERR_BAD_LEVEL before any callback runs.  The
+ * input goes through the device in the windows of b2_bzip2_compress (W = $B2_STREAM_WINDOW): the same device memory. */
+int b2_bzip2_compress_stream(b2_read_fn rd, b2_write_fn wr, void* user, int level);
+/* Decompress: the bytes passed to write, the return code and b2_last_error() are those of b2_bzip2_decompress_partial on
+ * the same input (data errors, CRC failures, truncation, bad members, "Not bzip data"): no byte past the prefix that
+ * call returns is ever written, because a block's bytes are written only once the blocks and stream CRCs in front of
+ * them have checked out.  The input is read only as far as the decode needs (a member's trailer ends a stream read
+ * without multistream).  Device memory is that of b2_bzip2_decompress ($B2_DEC_WINDOW, $B2_DEC_BATCH, the formula
+ * above).
+ * Host memory: a stream call holds one input buffer, which starts at 64 KiB and doubles as data arrives, and one pinned
+ * output buffer (compress: b2_bzip2_bound of the first window's input; decompress: the most bytes written at once).
+ * The input buffer is freed when the call returns, the output buffer goes back to the pinned buffers the library
+ * recycles (as b2_free does).  Whatever the stream's length, they stay within
+ *     compress:    W + 1 bytes of input and b2_bzip2_bound(W) + 64 of output: under 3 W + 1 MiB in all;
+ *     decompress:  the input window plus 5 bytes, and max(W, 48 MiB) of output: under 3 max(W, 48 MiB) in all
+ * (the input window is W, wider only for a block longer than W, as in b2_bzip2_decompress; a compressed block is
+ * under 2 MiB). */
+int b2_bzip2_decompress_stream(b2_read_fn rd, b2_write_fn wr, void* user, int multistream);
 
 /* ---- compressjs.BWT (lib/BWT.js) ------------------------------------------------- */
 /* BWT.bwtransform2(T, U, n, 256) -> pidx  (cyclic)    lib/BWT.js:372-417
