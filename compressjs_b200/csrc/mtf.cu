@@ -110,6 +110,7 @@ __global__ void __launch_bounds__(256) k_mtf_prefix(const u32* __restrict__ seg_
 struct MtfWarp {
   u16 K[256];                       // recency key of every byte value (larger = used more recently)
   __align__(16) u32 bm[MB_BUCKETS][4];  // bitmap of the key values that are currently somebody's key
+  u32 nz[MTF_CHUNK / 32];           // bit i of word s: rank 32 s + i of the chunk is not zero
 };
 // MTF rank of a byte = number of byte values used more recently than it.  Every byte value carries
 // a 13-bit recency key: (list position at the chunk start, 0 = back of the list) until it is used inside
@@ -119,8 +120,11 @@ struct MtfWarp {
 //   * T_i = time of the previous use of lane i's byte on a 9-bit scale that keeps the order of those times:
 //     255 - r0_i for a first use, 256 + prev_i for a byte an earlier lane prev_i of the window holds
 //   * rank_i = (r0_i for a first use) + #{k in (prev_i, i) : T_k < T_i}   (bytes first used after T_i inside the
-//     window), with the T_k < T_i lane mask built by a 9-round ballot radix compare
+//     window), with the T_k < T_i lane mask built by a 9-round ballot radix compare, low bit first (no equal-so-far
+//     mask to carry)
 //   * only the last use of a byte inside the window rewrites its key.
+// The zero-run summary of the chunk is not kept step by step: every step stores the ballot of its non-zero ranks, and
+// the warp reads the chunk's 4096 bits once at the end.
 __global__ void __launch_bounds__(MR_WARPS * 32)
 k_mtf_ranks(const u8* __restrict__ U, const u32* __restrict__ seg_n, u32 cps, const u32* __restrict__ lastpos,
             const u32* __restrict__ used, u8* __restrict__ R, u32 nblk, uint4* __restrict__ rsum) {
@@ -186,9 +190,6 @@ k_mtf_ranks(const u8* __restrict__ U, const u32* __restrict__ seg_n, u32 cps, co
   __syncwarp();
   const u8* src = U + ((size_t)seg << SEG_SHIFT) + start;
   u8* dst = R + ((size_t)seg << SEG_SHIFT) + start;
-  // zero-run summary of the chunk (warp-uniform state + a per-lane count of emitted symbols)
-  u32 z_open = 0, z_lead = 0, z_acc = 0;
-  bool z_seen = false;
   for (u32 base = 0; base < count; base += 32) {
     const bool valid = base + lane < count;
     const u32 c = valid ? (u32)src[base + lane] : (256u + lane);
@@ -232,35 +233,21 @@ k_mtf_ranks(const u8* __restrict__ U, const u32* __restrict__ seg_n, u32 cps, co
     }
     // ---- bytes first used after T_i inside the window: k in (prev_i, i) with T_k < T_i ----
     {
-      u32 lt = 0, eq = FULL_MASK;
+      // after bits 0..b: lt = lanes whose T is below mine in those bits.  Where my bit is 1, every lane with a 0 there
+      // is below me; where it is 0, only lanes that were below and have a 0 there stay below.
+      u32 lt = 0;
 #pragma unroll
-      for (int bit = 8; bit >= 0; bit--) {
-        const bool one = (T >> bit) & 1u;
-        const u32 B = __ballot_sync(FULL_MASK, one);
-        if (one) { lt |= eq & ~B; eq &= B; }
-        else eq &= ~B;
+      for (int bit = 0; bit <= 8; bit++) {
+        const bool one = T & (1u << bit);
+        const u32 nB = ~__ballot_sync(FULL_MASK, one);
+        lt = one ? (lt | nB) : (lt & nB);
       }
       rank += __popc(lt & lanemask_lt() & (FULL_MASK << (u32)(prev + 1)));
     }
     if (valid) dst[base + lane] = (u8)rank;
     {
       const u32 nzm = __ballot_sync(FULL_MASK, valid && rank != 0);
-      const u32 nvalid = min(32u, count - base);
-      if (valid && rank != 0) {
-        const u32 below = nzm & lanemask_lt();
-        if (below) {
-          const u32 L = lane - (31 - __clz(below)) - 1;          // zeros since the previous non-zero of this step
-          z_acc += 1 + (L ? 31 - __clz(L + 1) : 0);
-        } else if (z_seen) {
-          const u32 L = z_open + lane;
-          z_acc += 1 + (L ? 31 - __clz(L + 1) : 0);
-        } else {
-          z_lead = z_open + lane;                                 // the run that reaches back to the chunk start is not ours to count
-          z_acc += 1;
-        }
-      }
-      if (nzm) { z_seen = true; z_open = nvalid - 1 - (31 - __clz(nzm)); }
-      else z_open += nvalid;
+      if (lane == 0) s.nz[base >> 5] = nzm;
     }
     // ---- the last use of every byte in the window rewrites its key ----
     if (valid && is_last) {
@@ -272,10 +259,41 @@ k_mtf_ranks(const u8* __restrict__ U, const u32* __restrict__ seg_n, u32 cps, co
     if (lane == 0) s.bm[tb >> 7][(tb & 127u) >> 5] = newbits;
     __syncwarp();
   }
+  // ---- zero-run summary: leading zeros, trailing zeros, symbols emitted by the non-zero ranks and interior runs ----
+  // Lane l reads the bits of ranks [128 l, 128 l + 128).  A non-zero rank emits itself and, unless it is the first of
+  // the chunk (the run in front of that one is carried in by the block scan), the digits of the zero run before it.
   {
-    const u32 inner = warp_reduce_add(z_acc);
-    const u32 lead = z_seen ? warp_reduce_max(z_lead) : count;
-    if (lane == 0) rsum[gchunk] = make_uint4(lead, z_seen ? z_open : count, inner, z_seen ? 0u : 1u);
+    u32 nzw[4], mylast = 0;  // mylast: position + 1 of the lane's last non-zero rank, 0 if none
+    const u32 nw = (count + 31) >> 5;
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+      nzw[k] = lane * 4 + k < nw ? s.nz[lane * 4 + k] : 0u;
+      if (nzw[k]) mylast = lane * 128 + 32 * k + 32 - __clz(nzw[k]);
+    }
+    const u32 inc = warp_incl_max(mylast);
+    u32 pp = __shfl_up_sync(FULL_MASK, inc, 1);  // position + 1 of the last non-zero rank before the lane's bits
+    if (lane == 0) pp = 0;
+    u32 acc = 0, lead = 0;
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+      const u32 x = nzw[k], p0 = lane * 128 + 32 * k;
+      acc += __popc(x);
+      // non-zero ranks with a zero rank right in front of them (or, at p0 = 0, the chunk start)
+      u32 y = x & ~((x << 1) | (pp == p0 ? 1u : 0u));
+      while (y) {
+        const u32 bit = __ffs(y) - 1;
+        y &= y - 1;
+        const u32 low = x & ((1u << bit) - 1u);
+        const u32 q = low ? p0 + 32 - __clz(low) : pp;
+        if (q == 0) lead = p0 + bit;
+        else acc += 31 - __clz(p0 + bit - q + 1);
+      }
+      if (x) pp = p0 + 32 - __clz(x);
+    }
+    const u32 inner = warp_reduce_add(acc);
+    const u32 last = __shfl_sync(FULL_MASK, inc, 31);
+    lead = warp_reduce_max(lead);
+    if (lane == 0) rsum[gchunk] = last ? make_uint4(lead, count - last, inner, 0u) : make_uint4(count, count, 0u, 1u);
   }
 }
 
@@ -348,11 +366,11 @@ __global__ void __launch_bounds__(R2_THREADS)
 k_rle2(const u8* __restrict__ R, const u32* __restrict__ seg_n, u32 tps, const uint2* __restrict__ plan, u8* __restrict__ A,
        unsigned long long* __restrict__ hi, u32* __restrict__ any_hi, u32* __restrict__ freq) {
   __shared__ u32 hist[HUFF_MAXSYM];
-  __shared__ u32 ws[R2_THREADS / 32 + 1];
+  __shared__ uint4 wrec[R2_THREADS / 32];
   // the tile's symbols are staged here at the alignment (mod 16 symbols = 16 bytes) they have in global memory, then
   // copied out in 16-byte pieces: at most one symbol per rank plus the digits of the run that was carried in
   __shared__ __align__(16) u8 stage[R2_TILE + 48];
-  const u32 tid = threadIdx.x;
+  const u32 tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const u32 seg = blockIdx.x / tps, lt = blockIdx.x % tps;
   const u32 n = seg_n[seg];
   const u32 start = lt * R2_TILE;
@@ -362,64 +380,62 @@ k_rle2(const u8* __restrict__ R, const u32* __restrict__ seg_n, u32 tps, const u
   const u8* r = R + ((size_t)seg << SEG_SHIFT);
   u8* a = A + ((size_t)seg << SEG_SHIFT);
   const u32 p0 = start + tid * R2_ITEMS;
-  u8 v[R2_ITEMS];
-  {
-    const uint4 x = *reinterpret_cast<const uint4*>(r + p0);  // inside the 1 MiB slot; bytes past n are ignored below
-    const u32 xw[4] = {x.x, x.y, x.z, x.w};
-#pragma unroll
-    for (int j = 0; j < R2_ITEMS; j++) v[j] = (u8)(xw[j >> 2] >> (8 * (j & 3)));
-  }
-  // last non-zero position (+1) among this thread's items
-  u32 lastnz = 0;
-#pragma unroll
-  for (int j = 0; j < R2_ITEMS; j++)
-    if (p0 + j < n && v[j] != 0) lastnz = p0 + j + 1;
-  // exclusive max scan over threads
-  u32 inc = warp_incl_max(lastnz);
-  u32 exw = __shfl_up_sync(FULL_MASK, inc, 1);
-  if (lane_id() == 0) exw = 0;
-  if (lane_id() == 31) ws[tid >> 5] = inc;
-  __syncthreads();
-  if (tid < 32) {
-    u32 x = (tid < R2_THREADS / 32) ? ws[tid] : 0u;
-    u32 xi = warp_incl_max(x);
-    u32 xe = __shfl_up_sync(FULL_MASK, xi, 1);
-    if (tid == 0) xe = 0;
-    if (tid < R2_THREADS / 32) ws[tid] = xe;
-  }
-  __syncthreads();
-  const u32 ex_run = max(exw, ws[tid >> 5]);
-  __syncthreads();
-  u32 rs = max(start - pl.y, ex_run);  // position after the last non-zero before p (pl.y zeros were carried into the tile)
-  // symbols emitted per item: a non-zero rank flushes the run in front of it, then writes itself
-  u32 rlen[R2_ITEMS];
-  u32 sum = 0;
+  const uint4 rv = *reinterpret_cast<const uint4*>(r + p0);  // inside the 1 MiB slot; bytes past n are ignored below
+  const u32 xw[4] = {rv.x, rv.y, rv.z, rv.w};
+#define R2_RANK(j) ((xw[(j) >> 2] >> (8 * ((j) & 3))) & 255u)
+  // A non-zero rank flushes the zero run in front of it (floor(log2(L + 1)) digits for L zeros), then writes itself.
+  // Per thread: first and last non-zero position (+1, 0 if none) and the symbols of its items, but for the digits of
+  // the run in front of its first non-zero, which reaches back into earlier threads.
+  u32 fnz = 0, lnz = 0, own = 0;
 #pragma unroll
   for (int j = 0; j < R2_ITEMS; j++) {
     const u32 p = p0 + j;
-    rlen[j] = 0;
-    if (p < n && v[j] != 0) {
-      const u32 L = p - rs;
-      rlen[j] = L;
-      sum += 1 + (L ? 31 - __clz(L + 1) : 0);
-      rs = p + 1;
+    if (p < n && R2_RANK(j) != 0) {
+      if (lnz) { const u32 L = p - lnz; own += 1 + (L ? 31 - __clz(L + 1) : 0); }
+      else { own += 1; fnz = p + 1; }
+      lnz = p + 1;
     }
   }
-  u32 tot_off;
-  const u32 ex_off = block_excl_add<R2_THREADS, u32>(sum, ws, &tot_off);
+  // inside the warp: position after the last non-zero of the lanes below (0 if none)
+  const u32 inc = warp_incl_max(lnz);
+  u32 exw = __shfl_up_sync(FULL_MASK, inc, 1);
+  if (lane == 0) exw = 0;
+  // per warp: (position after its last non-zero, its first non-zero + 1, its symbols but for the digits of the run in
+  // front of its first non-zero); a warp's run comes in from the warps below, which one barrier hands over
+  {
+    const u32 s = warp_reduce_add((fnz && exw) ? own + (31 - __clz(fnz - exw)) : own);  // fnz - 1 - exw zeros in front
+    const u32 fm = __ballot_sync(FULL_MASK, fnz != 0);
+    const u32 F = __shfl_sync(FULL_MASK, fnz, fm ? __ffs(fm) - 1 : 0);
+    const u32 Lw = __shfl_sync(FULL_MASK, inc, 31);
+    if (lane == 0) wrec[w] = make_uint4(Lw, F, s, 0u);
+  }
+  __syncthreads();
+  // walk the warps' records: position after the last non-zero in front of this warp, its output offset, the tile's
+  u32 run = start - pl.y, woff = 0, tot_off = 0, wrun = 0;  // (pl.y zeros were carried into the tile)
+#pragma unroll
+  for (u32 k = 0; k < R2_THREADS / 32; k++) {
+    const uint4 rec = wrec[k];
+    if (k == w) { wrun = run; woff = tot_off; }
+    tot_off += rec.y ? rec.z + (31 - __clz(rec.y - run)) : rec.z;
+    if (rec.x) run = rec.x;
+  }
+  u32 rs = max(wrun, exw);  // position after the last non-zero in front of this thread's items
+  const u32 mine = fnz ? own + (31 - __clz(fnz - rs)) : own;
   const u32 first = pl.x & 15u;
-  u32 o = first + ex_off;  // index into `stage`
+  u32 o = first + woff + warp_incl_add(mine) - mine;  // index into `stage`
 #pragma unroll
   for (int j = 0; j < R2_ITEMS; j++) {
     const u32 p = p0 + j;
-    if (p < n && v[j] != 0) {
-      u32 L = rlen[j];
+    const u32 v = R2_RANK(j);
+    if (p < n && v != 0) {
+      u32 L = p - rs;
+      rs = p + 1;
       while (L) {  // lib/Bzip2.js:783-794 emitLastRun
         if (L & 1) { stage[o++] = 0; atomicAdd(&hist[0], 1u); L -= 1; }
         else { stage[o++] = 1; atomicAdd(&hist[1], 1u); L -= 2; }
         L >>= 1;
       }
-      const u32 sy = (u32)v[j] + 1;
+      const u32 sy = v + 1;
       if (sy == 256) {  // rank 255: a rare mask bit (a group can straddle two tiles, hence the atomic)
         const u32 og = pl.x - first + o;
         atomicOr(&hi[(size_t)seg * SEL_STRIDE + og / HUFF_GROUP], 1ull << (og % HUFF_GROUP));
@@ -429,6 +445,7 @@ k_rle2(const u8* __restrict__ R, const u32* __restrict__ seg_n, u32 tps, const u
       atomicAdd(&hist[sy], 1u);
     }
   }
+#undef R2_RANK
   __syncthreads();
   {
     const u32 last = first + tot_off;
