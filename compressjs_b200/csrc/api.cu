@@ -14,15 +14,11 @@ void bwt_inverse_sentinel_batch(Ctx& c, const u8* d_L, const u32* h_n, const u32
 size_t bwtc_bound(size_t n);
 void bwtc_compress_device(Ctx& c, const u8* d_in, size_t n, int level, u64 file_size, u8* d_out, size_t out_cap, size_t* out_n);
 u64 bwtc_parse_header(const u8* in, size_t n, size_t* pos);
-void bwtc_decompress(Ctx& c, const u8* d_in, size_t n, size_t pos, u64 fs, void* (*alloc_host)(size_t), u8** h_out, size_t* out_n);
+void bwtc_decompress(Ctx& c, const u8* d_in, size_t n, size_t pos, u64 fs, StreamOut& out);
 void dec_shard_release();
 void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* info);
 void dec_shard_export(u64* buf);
 int dec_shard_finish(Ctx& c, const u64* all, int multistream, u8* d_out, size_t out_cap, u64* res);
-int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multistream, u8* d_out, size_t out_cap, size_t* out_n,
-                     const std::vector<u64>* positions, std::vector<u64>* ends, std::vector<u64>* tab_pos, std::vector<u32>* tab_len,
-                     void* (*alloc_host)(size_t), void (*free_host)(void*), u8** h_out, StreamIn* sin = nullptr,
-                     StreamOut* sout = nullptr);
 
 static std::mutex g_mu;
 static Ctx* g_ctx = nullptr;
@@ -411,24 +407,19 @@ int b2_bwtc_decompress(const uint8_t* in, size_t n, uint8_t** out, size_t* out_n
   return guarded([&]() {
     Ctx& c = ctx_locked();
     c.reset_call();
-    size_t produced = 0;
-    u8* host = nullptr;   // pinned (size known) or malloc'ed (size unknown): b2_free releases either
-    try {
+    StreamOut dst(c.stream);
+    {
       StageScope tot(c, ST_TOTAL);
       size_t pos = 0;
       const u64 fs = bwtc_parse_header(in, n, &pos);   // before any device work
       DBuf<u8> din(c, n);
       CUDA_CHECK(cudaMemcpyAsync(din.p, in, n, cudaMemcpyHostToDevice, c.stream));
-      bwtc_decompress(c, din, n, pos, fs, pinned_alloc, &host, &produced);
-    } catch (...) {
-      if (g_pinned_live.count(host)) pinned_release(host); else free(host);
-      throw;
+      bwtc_decompress(c, din, n, pos, fs, dst);
     }
-    if (!host && !(host = (u8*)malloc(1))) throw B2Error{B2_ERR_CUDA, "out of host memory"};   // an empty stream of unknown size
     c.sync();
     c.collect();
-    c.stats.raw_bytes = produced; c.stats.comp_bytes = n;
-    *out = host; *out_n = produced;
+    c.stats.raw_bytes = dst.written; c.stats.comp_bytes = n;
+    *out_n = dst.written; *out = dst.take();
     return 0;
   });
 }
@@ -467,9 +458,9 @@ static size_t stream_window() {
   return win;
 }
 
-// ---- the callbacks of the stream entry points ----
+// ---- the host-side input and output of the host entry points ----
 StreamIn::~StreamIn() {
-  if (buf) { cudaStreamSynchronize(busy); free(buf); }
+  if (rd && buf) { cudaStreamSynchronize(busy); free(buf); }
 }
 size_t StreamIn::fill(size_t end) {
   while (base + have < end && !eof) {
@@ -497,31 +488,94 @@ size_t StreamIn::fill(size_t end) {
 void StreamIn::drop(size_t pos) {
   const size_t k = std::min(pos > base ? pos - base : 0, have);
   if (!k) return;
-  CUDA_CHECK(cudaStreamSynchronize(busy));
-  memmove(buf, buf + k, have - k);
   base += k; have -= k;
+  if (!rd) { buf += k; cap -= k; return; }  // the caller's buffer: its bytes stay where they are
+  CUDA_CHECK(cudaStreamSynchronize(busy));
+  memmove(buf, buf + k, have);
 }
-// the output buffer comes from (and goes back to) the pinned buffers b2_free recycles: a second call reuses it
+// the buffers come from (and go back to) the pinned buffers b2_free recycles: a second call reuses them
 StreamOut::~StreamOut() {
-  if (buf) pinned_release(buf);
+  if (buf) { cudaStreamSynchronize(busy); pinned_release(buf); }
 }
-void StreamOut::reserve(size_t bytes, size_t limit) {
-  if (bytes <= cap) return;
-  const size_t ncap = std::max(bytes, std::min(2 * cap, limit));
+void StreamOut::reserve(size_t bytes, bool last, size_t limit) {
+  const size_t kept = wr ? 0 : (size_t)written;
+  if (kept + bytes <= cap) return;
+  const size_t ncap = last ? kept + bytes : std::max(kept + bytes, std::min(2 * cap, wr ? limit : SIZE_MAX));
+  u8* nb = (u8*)pinned_alloc(ncap);
+  if (kept) { CUDA_CHECK(cudaStreamSynchronize(busy)); memcpy(nb, buf, kept); }
   if (buf) pinned_release(buf);
-  buf = nullptr; cap = 0;
-  buf = (u8*)pinned_alloc(ncap);
-  cap = ncap;
+  buf = nb; cap = ncap;
 }
 void StreamOut::put(const u8* p, size_t n) {
   if (!n) return;
-  int r;
-  {
-    InCallback in;
-    r = wr(user, p, n);
+  if (wr) {
+    CUDA_CHECK(cudaStreamSynchronize(busy));
+    int r;
+    {
+      InCallback in;
+      r = wr(user, p, n);
+    }
+    if (r != 0) throw B2Error{B2_ERR_STREAM, "the write callback aborted the stream"};
   }
-  if (r != 0) throw B2Error{B2_ERR_STREAM, "the write callback aborted the stream"};
   written += n;
+}
+u8* StreamOut::take() {
+  u8* p = buf ? buf : (u8*)pinned_alloc(0);
+  buf = nullptr; cap = 0;
+  return p;
+}
+
+// b2_bzip2_compress and b2_bzip2_compress_stream.  The first window sizes the buffers: an input that ends inside it is
+// one window of exactly its size.
+static int compress_host(Ctx& c, StreamIn& in, StreamOut& out, int level, bool pinned_in) {
+  size_t produced = 0;
+  try {
+    StageScope tot(c, ST_TOTAL);
+    size_t win = stream_window();
+    const size_t first = in.fill(win + 1);
+    const bool whole = in.eof && first <= win;
+    if (whole) win = first;
+    const size_t dcap = whole ? b2_bzip2_bound(first) : b2_bzip2_bound(win) + 64;
+    // a staging sink holds one window's output, a result the whole stream (its input is complete: `first` is all of it)
+    out.reserve(out.wr ? dcap : b2_bzip2_bound(first), true);
+    DBuf<u8> din(c, win ? win : 1), dout(c, dcap);
+    c.sync();  // the buffers are used from the copy streams as well
+    bzip2_compress_host(c, in, level, din, win, dout, dcap, out, &produced, pinned_in);
+  } catch (...) {
+    cudaStreamSynchronize(c.stream);  // nothing of this call may still be running when the next one starts
+    throw;
+  }
+  c.sync();
+  c.collect();
+  c.stats.raw_bytes = in.base + in.have; c.stats.comp_bytes = produced;
+  return 0;
+}
+
+// Every decode from a host input: b2_bzip2_decompress_partial and the calls built on it, and b2_bzip2_decompress_stream.
+// On a decode error (-2/-5/-7) the code is returned, not thrown, and `out` / the table rows hold what the reference has
+// written by the time it throws; any other error throws.  positions / ends: a position list (bzip2_decompress).
+static int decode_host(Ctx& c, StreamIn& in, StreamOut* out, int multistream, const std::vector<u64>* positions,
+                       std::vector<u64>* ends, std::vector<u64>* tp, std::vector<u32>* tl) {
+  size_t produced = 0;
+  int rc = 0;
+  try {
+    StageScope tot(c, ST_TOTAL);
+    try {
+      rc = bzip2_decompress(c, &in, nullptr, 0, multistream, nullptr, 0, out, &produced, positions, ends, tp, tl);
+    } catch (const B2Error& e) {
+      if (e.code != B2_ERR_NOT_BZIP_DATA && e.code != B2_ERR_DATA_ERROR && e.code != B2_ERR_OBSOLETE_INPUT) throw;
+      g_err = e.msg;
+      rc = e.code;
+    }
+    c.sync();
+  } catch (...) {
+    cudaStreamSynchronize(c.stream);
+    throw;
+  }
+  c.sync();
+  c.collect();
+  c.stats.raw_bytes = produced; c.stats.comp_bytes = in.base + in.have;
+  return rc;
 }
 
 extern "C" {
@@ -533,29 +587,8 @@ int b2_bzip2_compress_stream(b2_read_fn rd, b2_write_fn wr, void* user, int leve
     Ctx& c = ctx_locked();
     c.reset_call();
     StreamIn in(rd, user, c.h2d_stream);
-    StreamOut out(wr, user);
-    size_t produced = 0;
-    try {
-      StageScope tot(c, ST_TOTAL);
-      // the first window sizes the buffers as the input's size does in b2_bzip2_compress: an input that ends inside it
-      // is one window of exactly its size
-      size_t win = stream_window();
-      const size_t first = in.fill(win + 1);
-      const bool whole = in.eof && first <= win;
-      if (whole) win = first;
-      const size_t dcap = whole ? b2_bzip2_bound(first) : b2_bzip2_bound(win) + 64;
-      out.reserve(dcap, dcap);
-      DBuf<u8> din(c, win ? win : 1), dout(c, dcap);
-      c.sync();  // the buffers are used from the copy streams as well
-      bzip2_compress_host(c, nullptr, 0, &in, level, din, win, dout, dcap, nullptr, 0, &out, &produced, false);
-    } catch (...) {
-      cudaStreamSynchronize(c.stream);  // nothing of this call may still be running when the next one starts
-      throw;
-    }
-    c.sync();
-    c.collect();
-    c.stats.raw_bytes = in.base + in.have; c.stats.comp_bytes = produced;
-    return 0;
+    StreamOut out(wr, user, c.d2h_stream);
+    return compress_host(c, in, out, level, false);
   });
 }
 
@@ -565,28 +598,8 @@ int b2_bzip2_decompress_stream(b2_read_fn rd, b2_write_fn wr, void* user, int mu
     Ctx& c = ctx_locked();
     c.reset_call();
     StreamIn in(rd, user, c.stream);
-    StreamOut out(wr, user);
-    size_t produced = 0;
-    int rc = 0;
-    try {
-      StageScope tot(c, ST_TOTAL);
-      try {
-        rc = bzip2_decompress(c, nullptr, nullptr, 0, multistream, nullptr, 0, &produced, nullptr, nullptr, nullptr, nullptr, nullptr,
-                              nullptr, nullptr, &in, &out);
-      } catch (const B2Error& e) {
-        if (e.code != B2_ERR_NOT_BZIP_DATA && e.code != B2_ERR_DATA_ERROR && e.code != B2_ERR_OBSOLETE_INPUT) throw;
-        g_err = e.msg;
-        rc = e.code;
-      }
-      c.sync();
-    } catch (...) {
-      cudaStreamSynchronize(c.stream);
-      throw;
-    }
-    c.sync();
-    c.collect();
-    c.stats.raw_bytes = produced; c.stats.comp_bytes = in.base + in.have;
-    return rc;
+    StreamOut out(wr, user, c.stream);
+    return decode_host(c, in, &out, multistream, nullptr, nullptr, nullptr, nullptr);
   });
 }
 
@@ -611,27 +624,13 @@ int b2_bzip2_compress(const uint8_t* in, size_t n, int level, uint8_t** out, siz
     if (level < 1 || level > 9) throw B2Error{B2_ERR_BAD_LEVEL, "Invalid block size multiplier"};
     Ctx& c = ctx_locked();
     c.reset_call();
-    size_t cap = b2_bzip2_bound(n), produced = 0;
-    void* host = pinned_alloc(cap);
-    try {
-      StageScope tot(c, ST_TOTAL);
-      size_t win = stream_window();
-      if (win > n) win = n;
-      const size_t dcap = win < n ? b2_bzip2_bound(win) + 64 : cap;
-      DBuf<u8> din(c, win ? win : 1), dout(c, dcap);
-      c.sync();  // the buffers are used from the copy streams as well
-      cudaPointerAttributes pa;
-      const bool pinned_in = n && cudaPointerGetAttributes(&pa, in) == cudaSuccess && pa.type == cudaMemoryTypeHost;
-      cudaGetLastError();
-      bzip2_compress_host(c, in, n, nullptr, level, din, win, dout, dcap, (u8*)host, cap, nullptr, &produced, pinned_in);
-    } catch (...) {
-      pinned_release(host);
-      throw;
-    }
-    c.sync();
-    c.collect();
-    c.stats.raw_bytes = n; c.stats.comp_bytes = produced;
-    *out = (uint8_t*)host; *out_n = produced;
+    cudaPointerAttributes pa;
+    const bool pinned_in = n && cudaPointerGetAttributes(&pa, in) == cudaSuccess && pa.type == cudaMemoryTypeHost;
+    cudaGetLastError();
+    StreamIn src(in, n);
+    StreamOut dst(c.d2h_stream);
+    compress_host(c, src, dst, level, pinned_in);
+    *out_n = dst.written; *out = dst.take();
     return 0;
   });
 }
@@ -731,36 +730,16 @@ int b2_bzip2_encode_range_dev(const void* d_in, size_t n, int level, size_t firs
   });
 }
 
-// On a decode error (-2/-5/-7) the code is returned, not thrown, and *out / the table rows hold what the reference has
-// written by the time it throws; any other error throws and returns nothing.  positions / ends: a position list
-// (bzip2_decompress).  The input stays on the host; the decoder uploads it a window at a time.
+// The host-buffer decodes: decode_host over the caller's buffer, with the result in *out when out is given.  The input
+// stays on the host; the decoder uploads it a window at a time.
 static int decode_common(const uint8_t* in, size_t n, int multistream, const std::vector<u64>* positions, std::vector<u64>* ends,
                          uint8_t** out, size_t* out_n, std::vector<u64>* tp, std::vector<u32>* tl) {
   Ctx& c = ctx_locked();
   c.reset_call();
-  size_t produced = 0;
-  u8* host = nullptr;
-  int rc = 0;
-  try {
-    StageScope tot(c, ST_TOTAL);
-    try {
-      rc = bzip2_decompress(c, in, nullptr, n, multistream, nullptr, 0, &produced, positions, ends, tp, tl, pinned_alloc, pinned_release,
-                            out ? &host : nullptr);
-    } catch (const B2Error& e) {
-      if (e.code != B2_ERR_NOT_BZIP_DATA && e.code != B2_ERR_DATA_ERROR && e.code != B2_ERR_OBSOLETE_INPUT) throw;
-      g_err = e.msg;
-      rc = e.code;
-    }
-    if (out && !host) host = (u8*)pinned_alloc(produced);
-    c.sync();
-  } catch (...) {
-    if (host) pinned_release(host);
-    throw;
-  }
-  c.sync();
-  c.collect();
-  c.stats.raw_bytes = produced; c.stats.comp_bytes = n;
-  if (out) { *out = (uint8_t*)host; *out_n = produced; }
+  StreamIn src(in, n);
+  StreamOut dst(c.stream);
+  const int rc = decode_host(c, src, out ? &dst : nullptr, multistream, positions, ends, tp, tl);
+  if (out) { *out_n = dst.written; *out = dst.take(); }
   return rc;
 }
 
@@ -841,8 +820,8 @@ int b2_bzip2_decompress_dev(const void* d_in, size_t n, int multistream, void* d
     int rc;
     {
       StageScope tot(c, ST_TOTAL);
-      rc = bzip2_decompress(c, nullptr, (const u8*)d_in, n, multistream, (u8*)d_out, out_cap, out_n, nullptr, nullptr, nullptr, nullptr,
-                            nullptr, nullptr, nullptr);
+      rc = bzip2_decompress(c, nullptr, (const u8*)d_in, n, multistream, (u8*)d_out, out_cap, nullptr, out_n, nullptr, nullptr, nullptr,
+                            nullptr);
     }
     c.sync();
     c.collect();

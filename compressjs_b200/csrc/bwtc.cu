@@ -400,11 +400,10 @@ u64 bwtc_parse_header(const u8* in, size_t n, size_t* pos) {
 }
 
 // BWTC.decompressFile: d_in = the stream on the device, pos and fs from bwtc_parse_header.  The decoded bytes go to the
-// host, batch by batch, into *h_out (null on entry; the caller owns it afterwards, also when this throws).  Size field
-// known: one buffer from alloc_host, allocated up front.  Size unknown (fs == 0): a malloc'ed buffer that grows as the
-// batches arrive.  *out_n = the bytes decoded.  Device memory: one batch of blocks, whatever the size of the file.
-void bwtc_decompress(Ctx& c, const u8* d_in, size_t n, size_t pos, u64 fs, void* (*alloc_host)(size_t), u8** h_out, size_t* out_n) {
-  *out_n = 0;
+// host, batch by batch, into the result `out` (a sink without a write callback).  Size field known: the whole buffer is
+// reserved up front.  Size unknown (fs == 0): the buffer grows as the batches arrive.  Device memory: one batch of
+// blocks, whatever the size of the file.
+void bwtc_decompress(Ctx& c, const u8* d_in, size_t n, size_t pos, u64 fs, StreamOut& out) {
   const bool unsized = fs == 0;
   const u64 limit = unsized ? ~0ull : fs - 1;
   // the level is inside the coded stream: bound the block count for the smallest block size
@@ -419,9 +418,7 @@ void bwtc_decompress(Ctx& c, const u8* d_in, size_t n, size_t pos, u64 fs, void*
   KLAUNCH(c); KCHECK();
   std::vector<u32> hl(B), hp(B);
   // a known size gets all of its buffer now, up to what maxblocks blocks can hold (more would fail the size check)
-  size_t cap = unsized ? 0 : (size_t)std::min<u64>(limit, maxblocks * 900000u);
-  if (!unsized) *h_out = (u8*)alloc_host(cap);
-  u64 off = 0;
+  if (!unsized) out.reserve((size_t)std::min<u64>(limit, maxblocks * 900000u), true);
   for (;;) {
     {
       StageScope s(c, ST_HDEC);
@@ -437,24 +434,18 @@ void bwtc_decompress(Ctx& c, const u8* d_in, size_t n, size_t pos, u64 fs, void*
     if (h.status == BD_SIZE) throw B2Error{B2_ERR_DATA_ERROR, "outputsize does not match decoded input"};   // lib/Util.js:69-71
     u64 bytes = 0;
     for (u32 b = 0; b < h.nb; b++) bytes += hl[b];
-    if (unsized && off + bytes > cap) {
-      const size_t ncap = std::max<size_t>(off + bytes, cap * 2);
-      u8* p = (u8*)realloc(*h_out, ncap);
-      if (!p) throw B2Error{B2_ERR_CUDA, "out of host memory"};
-      *h_out = p; cap = ncap;
-    }
     if (h.nb) {
+      out.reserve((size_t)bytes);   // grows only without a size field
       {
         StageScope s(c, ST_IBWT);   // BWT.unbwtransform of every block of the batch, lib/BWTC.js:224
         bwt_inverse_sentinel_batch(c, L, hl.data(), hp.data(), h.nb, dout);
       }
-      CUDA_CHECK(cudaMemcpyAsync(*h_out + off, dout, bytes, cudaMemcpyDeviceToHost, c.stream));
-      off += bytes;
+      CUDA_CHECK(cudaMemcpyAsync(out.next(), dout, bytes, cudaMemcpyDeviceToHost, c.stream));
+      out.put(out.next(), (size_t)bytes);
       c.stats.blocks += h.nb;
     }
     if (h.status == BD_END) break;
   }
   c.sync();
-  if (!unsized && off != limit) throw B2Error{B2_ERR_DATA_ERROR, "outputsize does not match decoded input"};
-  *out_n = (size_t)off;
+  if (!unsized && out.written != limit) throw B2Error{B2_ERR_DATA_ERROR, "outputsize does not match decoded input"};
 }

@@ -1428,47 +1428,43 @@ static void scan_window(Ctx& c, const u8* in, u64 wbytes, u64 base_bit, u64 lim,
 }
 
 // ---- single-GPU decode: one rolling loop over input windows and decode batches --------------------------------------
-// The compressed input is h_in (host) or d_in (device), n bytes.  Only the window [a, a + W) of it is on the device
+// The compressed input is `sin` (host) or d_in[0, n) (device).  Only the window [a, a + W) of it is on the device
 // (W = dec_window(); a is the chain's position, rounded down to 256 bytes).  The window's magics are decoded in position
 // order, a batch at a time; after each batch the host walks the chain as far as final results allow, and the blocks that
 // walk settled are expanded, CRC-checked and delivered.  The first chain position without a final result starts the next
 // window; a window that would start where this one did is twice as long, so a block longer than W still decodes.
 // Delivery: d_out (device, absolute offsets, nothing past out_cap), or the table rows (tab_pos / tab_len: expanded only
-// for the CRCs), or else *h_out (host, grown from alloc_host / free_host; owned by the caller, also when this throws),
-// through a device staging buffer of at most max(W, one block) bytes.
+// for the CRCs), or else `sout`, through a device staging buffer of at most max(W, one block) bytes.  Each staged group's
+// events are replayed before it leaves and the group is cut at the prefix the replay allows, so nothing past the prefix
+// of b2_bzip2_decompress_partial ever reaches sout.
 // positions: decode the blocks at these bit positions, back to back in list order (ends: the end offset of every
 // position delivered in full), with the whole input on the device.
-// Stream calls (b2_bzip2_decompress_stream): the input comes from `sin` instead (h_in, d_in and n are unused), which keeps
-// the bytes from the window's start on.  Every window is read one byte past its end, so the stream's end is known exactly
-// when b2_bzip2_decompress would know it (n stays unknown until then, and no window is the last one).  The staged blocks
-// go out through `sout`, each group only as far as the replay allows, so nothing past the prefix of
-// b2_bzip2_decompress_partial is ever written.
-int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multistream, u8* d_out, size_t out_cap, size_t* out_n,
-                     const std::vector<u64>* positions, std::vector<u64>* ends, std::vector<u64>* tab_pos, std::vector<u32>* tab_len,
-                     void* (*alloc_host)(size_t), void (*free_host)(void*), u8** h_out, StreamIn* sin, StreamOut* sout) {
+// sin keeps the bytes from the window's start on, and every window is read one byte past its end, so the input's end is
+// known exactly when a complete input would show it (n stays unknown until then, and no window is the last one).
+int bzip2_decompress(Ctx& c, StreamIn* sin, const u8* d_in, size_t n, int multistream, u8* d_out, size_t out_cap, StreamOut* sout,
+                     size_t* out_n, const std::vector<u64>* positions, std::vector<u64>* ends, std::vector<u64>* tab_pos,
+                     std::vector<u32>* tab_len) {
   *out_n = 0;
-  // with neither d_out nor h_out (a table, or a device call without a buffer) the blocks are expanded only for their CRCs
+  // with neither d_out nor sout (a table, or a device call without a buffer) the blocks are expanded only for their CRCs
   const bool dev = d_out != nullptr, listed = positions != nullptr;
-  auto read_in = [&](u8* dst, u64 off, size_t len) {
+  auto read_dev = [&](u8* dst, u64 off, size_t len) {
     if (!len) return;
-    if (h_in) { memcpy(dst, h_in + off, len); return; }
     CUDA_CHECK(cudaMemcpyAsync(dst, d_in + off, len, cudaMemcpyDeviceToHost, c.stream));
     CUDA_CHECK(cudaStreamSynchronize(c.stream));
   };
   Chain ch;
-  // stream calls: the input's length, once read has returned 0
+  // the input's length, once the host input has ended
   auto learn_end = [&]() {
     if (sin->eof) ch.n = n = sin->base + sin->have;
   };
+  u8 hdr[4] = {0, 0, 0, 0};
   if (sin) {
     n = SIZE_MAX;
     const size_t end = sin->fill(5);  // the header, and whether anything follows it
-    u8 hdr[4] = {0, 0, 0, 0};
-    memcpy(hdr, sin->at(0), std::min<size_t>(end, 4));
+    std::copy_n(sin->at(0), std::min<size_t>(end, 4), hdr);
     read_level(hdr, end, &ch.cur_dbuf);
   } else {
-    u8 hdr[4] = {0, 0, 0, 0};
-    read_in(hdr, 0, std::min<size_t>(n, 4));
+    read_dev(hdr, 0, std::min<size_t>(n, 4));
     read_level(hdr, n, &ch.cur_dbuf);
   }
   ch.n = n;
@@ -1481,7 +1477,7 @@ int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multi
   DBuf<u32> tileoff;
   DBuf<CandRes> dres;
   DBuf<Cand> dcand;
-  size_t win_cap = 0, slots = 0, stage_cap = 0, h_cap = 0;
+  size_t win_cap = 0, slots = 0, stage_cap = 0;
   std::vector<Cand> cands;
   std::vector<size_t> blk;      // block candidates of the window (index into cands)
   std::vector<CandRes> hres;    // results of the batch
@@ -1501,23 +1497,9 @@ int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multi
       return avail;
     }
     const size_t avail = (size_t)std::min<u64>(4, n - bytepos);
-    read_in(h, bytepos, avail);
+    read_dev(h, bytepos, avail);
     return avail;
   };
-  // *h_out must hold the decoded bytes [0, need), of which `have` are there: it doubles, or gets the exact size when the
-  // stream is known to end there (a call of one batch: one buffer, one copy)
-  auto host_reserve = [&](u64 need, u64 have, bool final_size) {
-    if (need <= h_cap) return;
-    const size_t cap = final_size ? (size_t)need : std::max<size_t>((size_t)need, 2 * h_cap);
-    u8* p = (u8*)alloc_host(cap);
-    if (*h_out) {
-      CUDA_CHECK(cudaStreamSynchronize(c.stream));
-      memcpy(p, *h_out, (size_t)have);
-      free_host(*h_out);
-    }
-    *h_out = p; h_cap = cap;
-  };
-  u64 h_have = 0;  // bytes delivered to *h_out
   while (!ch.done && (E.ev < 0 || dev)) {
     // ---- 1. the input window ----
     const u64 a = listed ? 0 : (ch.pos >> 3) & ~(u64)255;
@@ -1533,9 +1515,9 @@ int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multi
     if (wl + 32 > win_cap) { win.alloc(c, wl + 32); win_cap = wl + 32; }
     // zero padded (aligned word reads past the end must be safe)
     CUDA_CHECK(cudaMemsetAsync(win.p + (wl & ~(u64)3), 0, 32 + (wl & 3), c.stream));
-    if (h_in || sin) {
+    if (sin) {
       StageScope s(c, ST_H2D);
-      if (wl) CUDA_CHECK(cudaMemcpyAsync(win, h_in ? h_in + a : sin->at(a), wl, cudaMemcpyHostToDevice, c.stream));
+      if (wl) CUDA_CHECK(cudaMemcpyAsync(win, sin->at(a), wl, cudaMemcpyHostToDevice, c.stream));
     } else if (wl) {
       CUDA_CHECK(cudaMemcpyAsync(win, d_in + a, wl, cudaMemcpyDeviceToDevice, c.stream));
     }
@@ -1615,7 +1597,7 @@ int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multi
       got.assign(cnt ? cnt : 1, 0);
       ob.assign(cnt ? cnt : 1, ~0ull);
       auto got_fn = [&](size_t slot) { return std::make_pair(ob[slot] != ~0ull, got[slot]); };
-      size_t er = e0;  // events replayed so far (stream calls replay group by group)
+      size_t er = e0;  // events replayed so far (a host output replays group by group)
       if (dev) {
         // straight to the caller's buffer; a block that does not fit is only counted (the needed size is returned)
         for (size_t ei : settled) { const Event& ev = ch.events[ei]; if (ev.off + ev.len <= out_cap) ob[ev.slot] = ev.off; }
@@ -1632,12 +1614,6 @@ int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multi
           if (bytes > stage_cap) { stage.alloc(c, bytes); stage_cap = bytes; }
           dec_expand(c, rle.p + (s0 << SEG_SHIFT), cls.p + (s0 << SEG_SHIFT), false, dres.p + s0, hres.data() + s0, tileoff.p + s0 * UR_TPS,
                      (u32)(s1 - s0), ob.data() + s0, stage, got.data() + s0);
-          if (h_out && bytes) {
-            host_reserve(f.off + bytes, h_have, ch.done && g1 == settled.size());
-            StageScope s(c, ST_D2H);
-            CUDA_CHECK(cudaMemcpyAsync(*h_out + f.off, stage, bytes, cudaMemcpyDeviceToHost, c.stream));
-            h_have = f.off + bytes;
-          }
           if (sout) {
             // the group's events say how much of it the reference writes before it throws
             const size_t g_end = settled[g1 - 1] + 1;
@@ -1645,13 +1621,15 @@ int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multi
             er = g_end;
             const u64 keep = E.ev < 0 ? bytes : (E.prefix > f.off ? std::min<u64>(bytes, E.prefix - f.off) : 0);
             if (keep) {
-              sout->reserve((size_t)keep, std::max<size_t>(W, (size_t)keep));
+              // no group follows the last one of a finished chain or a failure: a call of one batch makes one result
+              // buffer of exactly its size and one copy
+              sout->reserve((size_t)keep, (ch.done && g1 == settled.size()) || E.ev >= 0, W);
+              u8* dst = sout->next();
               {
                 StageScope s(c, ST_D2H);
-                CUDA_CHECK(cudaMemcpyAsync(sout->buf, stage, keep, cudaMemcpyDeviceToHost, c.stream));
+                CUDA_CHECK(cudaMemcpyAsync(dst, stage, keep, cudaMemcpyDeviceToHost, c.stream));
               }
-              CUDA_CHECK(cudaStreamSynchronize(c.stream));
-              sout->put(sout->buf, (size_t)keep);
+              sout->put(dst, (size_t)keep);
             }
             if (E.ev >= 0) break;
           }
@@ -1673,7 +1651,7 @@ int bzip2_decompress(Ctx& c, const u8* h_in, const u8* d_in, size_t n, int multi
   }
   if (E.ev >= 0) {
     // the host path hands the output in front of the error to the caller with the error (b2_bzip2_decompress_partial)
-    if (h_out || sout) *out_n = (size_t)E.prefix;
+    if (sout) *out_n = (size_t)E.prefix;
     throw B2Error{E.code, E.msg};
   }
   *out_n = (size_t)ch.total_out;

@@ -81,41 +81,53 @@ u32 crc32_device(Ctx& c, const u8* d_p, size_t n);
 void bwt_forward_batch(Ctx& c, const u8* d_T, u8* d_U, const u32* d_n, const u32* h_n, u32 nblk, u32* d_pidx, bool sentinel = false,
                        u32* d_sa_out = nullptr, u32* d_hist_out = nullptr);
 
-// ---- the callbacks of the stream entry points (b2_bzip2_*_stream; implemented in api.cu) ----
-// The input: the stream's bytes [base, base + have) in a host buffer that doubles as data arrives.  A callback that
-// aborts throws B2Error{B2_ERR_STREAM}.
+// ---- the host-side input and output of the host entry points (implemented in api.cu) ----
+// The input: the stream's bytes [base, base + have) in a host buffer.  From a read callback (b2_bzip2_*_stream) the
+// buffer doubles as data arrives; over a caller's buffer (the host-buffer calls) every byte is there from the start and
+// the buffer is only read.  A callback that aborts throws B2Error{B2_ERR_STREAM}.
 struct StreamIn {
-  b2_read_fn rd; void* user;
-  cudaStream_t busy;  // copies out of buf may be queued here: they are waited for before buf changes
+  b2_read_fn rd = nullptr; void* user = nullptr;  // null rd: buf is the caller's, borrowed for the call
+  cudaStream_t busy = nullptr;  // copies out of buf may be queued here: they are waited for before buf changes
   u8* buf = nullptr;
   size_t cap = 0, base = 0, have = 0;
   bool eof = false;   // read returned 0: the stream is base + have bytes long
   StreamIn(b2_read_fn rd_, void* user_, cudaStream_t busy_) : rd(rd_), user(user_), busy(busy_) {}
+  // never written: without rd nothing reads into buf
+  StreamIn(const u8* p, size_t n) : buf(const_cast<u8*>(p)), cap(n), have(n), eof(true) {}
   StreamIn(const StreamIn&) = delete;
   ~StreamIn();
   size_t fill(size_t end);  // read until the bytes in front of `end` are here or the input ends; returns base + have
   void drop(size_t pos);    // forget the bytes in front of pos
   const u8* at(size_t pos) const { return buf + (pos - base); }
 };
-// The output: pieces are staged in a pinned buffer (from the library's pinned pool) and handed to the write callback.
+// The output, in pinned buffers of the library's pool (a buffer still held when the sink is destroyed goes back to it).
+// With a write callback (b2_bzip2_*_stream) buf stages the pieces, and put() hands each one to the callback once the
+// copies into buf on `busy` have landed.  Without one (the host-buffer calls) buf is the result: pieces go at its end,
+// put() only counts them, and take() hands the buffer to the caller.
 struct StreamOut {
-  b2_write_fn wr; void* user;
+  b2_write_fn wr = nullptr; void* user = nullptr;
+  cudaStream_t busy;  // copies into buf are queued here
   u8* buf = nullptr;
   size_t cap = 0;
-  u64 written = 0;
-  StreamOut(b2_write_fn wr_, void* user_) : wr(wr_), user(user_) {}
+  u64 written = 0;    // bytes handed over
+  StreamOut(b2_write_fn wr_, void* user_, cudaStream_t busy_) : wr(wr_), user(user_), busy(busy_) {}
+  explicit StreamOut(cudaStream_t busy_) : busy(busy_) {}
   StreamOut(const StreamOut&) = delete;
   ~StreamOut();
-  void reserve(size_t bytes, size_t limit);  // buf holds >= bytes (doubling up to `limit`); its contents are not kept
-  void put(const u8* p, size_t n);
+  u8* next() const { return wr ? buf : buf + written; }  // where the next piece's bytes go
+  // next() has room for `bytes`.  buf doubles, or takes exactly what is needed when `last` says it will not grow again.
+  // A staging buffer drops its contents and doubles no further than `limit`; the result keeps its contents.
+  void reserve(size_t bytes, bool last = false, size_t limit = SIZE_MAX);
+  void put(const u8* p, size_t n);  // hand over the n bytes at p, which follow those handed over before
+  u8* take();                       // the result, never null (also for 0 bytes); released with b2_free
 };
 
 // ---- bzip2 encode drivers (encode.cu), one per entry point of include/b2bz.h ----
 void bzip2_compress_dev(Ctx& c, const u8* d_in, size_t n, int level, u8* d_out, size_t out_cap, size_t* out_n);
-// b2_bzip2_compress (h_in, n; output to h_out) and b2_bzip2_compress_stream (input from `sin`; output through `sout`,
-// staged in sout->buf, which holds out_cap bytes)
-void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, StreamIn* sin, int level, u8* d_in, size_t win, u8* d_out, size_t out_cap,
-                         u8* h_out, size_t h_out_cap, StreamOut* sout, size_t* out_n, bool pinned_in);
+// b2_bzip2_compress and b2_bzip2_compress_stream: the input comes from `in`, the output goes to `out`, which has room for
+// out_cap bytes at out.next()
+void bzip2_compress_host(Ctx& c, StreamIn& in, int level, u8* d_in, size_t win, u8* d_out, size_t out_cap, StreamOut& out,
+                         size_t* out_n, bool pinned_in);
 size_t bzip2_plan(Ctx& c, const u8* d_in, size_t n, int level);
 void bzip2_plan_spec(Ctx& c, const u8* d_in, size_t n, int level, int rank, int world, u64* info);
 void bzip2_share_summary(Ctx& c, const u8* d_in, size_t n, u64* out);
@@ -124,3 +136,10 @@ void bzip2_encode_range(Ctx& c, const u8* d_in, size_t n, int level, size_t firs
                         u64* out_bits, u32* block_crcs);
 void bitshift_device(Ctx& c, const void* src, u64 nbits, int phase, void* dst);
 void bzip2_release_plan();  // the plan kept for b2_bzip2_encode_range_dev
+
+// ---- bzip2 decode driver (decode.cu): every single-GPU decode entry point ----
+// The input is `sin` or the device buffer d_in[0, n); the output goes to the device buffer d_out (out_cap bytes), to
+// `sout`, or nowhere (a table).  See decode.cu.
+int bzip2_decompress(Ctx& c, StreamIn* sin, const u8* d_in, size_t n, int multistream, u8* d_out, size_t out_cap, StreamOut* sout,
+                     size_t* out_n, const std::vector<u64>* positions, std::vector<u64>* ends, std::vector<u64>* tab_pos,
+                     std::vector<u32>* tab_len);

@@ -572,23 +572,22 @@ void bzip2_plan_share(Ctx& c, const u8* d_buf, size_t n, int level, u64 st0, u64
   g_plan.put(std::move(plan), d_buf, n, level);
 }
 
-// Bzip2.compressFile with HOST buffers (b2_bzip2_compress).  With a pinned input the upload is cut into chunks
-// on a copy stream; block boundaries only depend on the bytes before them (lib/Bzip2.js:636-667 consumes its
-// input strictly forward), so every block but the last of a plan over the prefix that has arrived is final
-// and is encoded while the rest is still in flight.  Finished words of the output go back on a second copy
-// stream after every batch.  h_out must hold h_out_cap bytes (pinned).
-// Stream calls: the input comes from `sin` (h_in and n are unused) and the output goes out through `sout`.  sin keeps
-// the bytes from the window's start on and reads until it holds more than a window or the input ends, so every window
-// is the one b2_bzip2_compress would see for the whole input: the same blocks, the same stream.  Each window's output
-// is staged in sout->buf (it holds out_cap bytes, like d_out) and written after every batch.
-void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, StreamIn* sin, int level, u8* d_in, size_t win, u8* d_out, size_t out_cap,
-                         u8* h_out, size_t h_out_cap, StreamOut* sout, size_t* out_n, bool pinned_in) {
-  // d_in holds `win` bytes, d_out `out_cap` bytes (>= b2_bzip2_bound(win)).  win >= n: the whole file in one window (the
-  // usual case).  win < n: the input STREAMS through the device in windows -- every window is uploaded, planned and
+// Bzip2.compressFile from a host source into a host sink: b2_bzip2_compress (the caller's buffer, complete from the
+// start, into the result buffer) and b2_bzip2_compress_stream (read and write callbacks).  With a pinned input the
+// upload is cut into chunks on a copy stream; block boundaries only depend on the bytes before them (lib/Bzip2.js:636-667
+// consumes its input strictly forward), so every block but the last of a plan over the prefix that has arrived is final
+// and is encoded while the rest is still in flight.  Finished words of the output go back on a second copy stream after
+// every batch and are handed to `out` one batch behind, so a write callback never waits for the copy just queued.
+// `in` keeps the bytes from the window's start on and is read until it holds more than a window or the input ends, so a
+// window is the last one exactly when the input ends in it: however the input arrives, the windows, blocks and stream
+// are the same.
+void bzip2_compress_host(Ctx& c, StreamIn& in, int level, u8* d_in, size_t win, u8* d_out, size_t out_cap, StreamOut& out,
+                         size_t* out_n, bool pinned_in) {
+  // d_in holds `win` bytes, d_out `out_cap` bytes (>= b2_bzip2_bound(win)).  An input of at most win bytes is one window
+  // (the usual case).  A longer one STREAMS through the device in windows -- every window is uploaded, planned and
   // encoded like a small file whose last block is kept back (it may go on in the next window), the next window starts at
   // the first raw byte that has not been consumed, and the output window is drained and rebased in between: device
   // memory is bounded by the window, not by the file (lib/Bzip2.js:879-929 reads its input strictly forward, too).
-  if (sout) { h_out = sout->buf; h_out_cap = sout->cap; }
   size_t CH = (size_t)64 << 20;
   if (const char* e = getenv("B2_H2D_CHUNK")) {  // test hook: small chunks exercise the prefix planning on small inputs
     const long long v = atoll(e);
@@ -599,7 +598,7 @@ void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, StreamIn* sin, int le
   auto mark = [&](const char* what, size_t v) {
     if (trace_host) fprintf(stderr, "[b2 host] %8.2f ms  %s %zu\n", std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count(), what, v);
   };
-  const size_t max_ch = ((sin ? win : std::min(win, n)) + CH - 1) / CH + 1;
+  const size_t max_ch = (win + CH - 1) / CH + 1;
   std::vector<cudaEvent_t> ev(max_ch);
   struct Cleanup {
     std::vector<cudaEvent_t>& ev; Ctx& c;
@@ -612,54 +611,45 @@ void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, StreamIn* sin, int le
   c.trace.clear();
   EncSession S(c, level, d_out, out_cap, true, 0);
   mark("session ready", 0);
+  u8* h_out = nullptr;     // where the current output window's byte 0 goes on the host
+  size_t h_room = 0;       // bytes from h_out on that `out` has room for
   size_t copied = 0;       // bytes of the current output window already on their way to the host
-  size_t host_base = 0;    // offset in h_out of the window's byte 0 (stream calls: always 0)
   size_t out_base = 0;     // offset in the output of the window's byte 0
-  size_t sent = 0;         // stream calls: bytes of the current output window written
+  size_t sent = 0;         // bytes of the current output window handed to `out`
   bool d2h_started = false, h2d_started = false;
-  // stream calls: write what the copies queued so far have brought to the host
+  // hand over what the copies queued so far bring to the host
   auto drain = [&]() {
-    if (!sout || copied == sent) return;
-    CUDA_CHECK(cudaStreamSynchronize(c.d2h_stream));
-    sout->put(h_out + sent, copied - sent);
+    out.put(h_out + sent, copied - sent);
     sent = copied;
   };
   S.on_batch = [&](u64 bit_end) {
     const size_t ready = (size_t)(bit_end / 32) * 4;  // whole words below the one still being filled
     if (ready > copied) {
       drain();  // the previous batch's words: their copy has had a batch's time to land
-      if (host_base + ready > h_out_cap) throw B2Error{B2_ERR_BAD_ARG, "output buffer too small for the compressed stream"};
+      if (ready > h_room) throw B2Error{B2_ERR_BAD_ARG, "output buffer too small for the compressed stream"};
       if (!d2h_started) { c.copy_begin(c.d2h_stream, 1); d2h_started = true; }
-      CUDA_CHECK(cudaMemcpyAsync(h_out + host_base + copied, d_out + copied, ready - copied, cudaMemcpyDeviceToHost, c.d2h_stream));
+      CUDA_CHECK(cudaMemcpyAsync(h_out + copied, d_out + copied, ready - copied, cudaMemcpyDeviceToHost, c.d2h_stream));
       copied = ready;
     }
   };
   size_t file_pos = 0;  // raw bytes consumed by finished blocks
   for (bool first_window = true;; first_window = false) {
-    const u8* src;        // the window's input on the host
-    size_t wlen;
-    bool last_window;
-    if (sin) {
-      // the window and one byte more when there is one: a window that holds the rest of the input is the last one
-      sin->drop(file_pos);
-      const size_t end = sin->fill(file_pos + win + 1);
-      wlen = std::min(win, end - file_pos);
-      last_window = sin->eof && file_pos + wlen == end;
-      src = sin->at(file_pos);
-    } else {
-      wlen = std::min(win, n - file_pos);
-      last_window = file_pos + wlen == n;
-      src = h_in + file_pos;
-    }
+    // the window and one byte more when there is one: a window that holds the rest of the input is the last one
+    in.drop(file_pos);
+    const size_t end = in.fill(file_pos + win + 1);
+    const size_t wlen = std::min(win, end - file_pos);
+    const bool last_window = in.eof && file_pos + wlen == end;
+    const u8* src = in.at(file_pos);
     if (!first_window) {
       // the previous window's output is on its way: wait for it, then reuse both windows
       CUDA_CHECK(cudaStreamSynchronize(c.d2h_stream));
       drain();
       S.rebase(copied + 8);
       out_base += copied;
-      if (!sout) host_base += copied;
       copied = sent = 0;
     }
+    h_out = out.next();
+    h_room = out.cap - (size_t)(h_out - out.buf);
     const size_t nch = (pinned_in && wlen > CH) ? (wlen + CH - 1) / CH : (wlen ? 1 : 0);
     if (!h2d_started) { c.copy_begin(c.h2d_stream, 0); h2d_started = true; }
     for (size_t i = 0; i < nch; i++) {
@@ -702,9 +692,9 @@ void bzip2_compress_host(Ctx& c, const u8* h_in, size_t n, StreamIn* sin, int le
   S.finish(&total);
   *out_n = total;
   const size_t tail = *out_n - out_base;  // bytes of the last window, trailer included
-  if (host_base + tail > h_out_cap) throw B2Error{B2_ERR_BAD_ARG, "output buffer too small for the compressed stream"};
+  if (tail > h_room) throw B2Error{B2_ERR_BAD_ARG, "output buffer too small for the compressed stream"};
   if (!d2h_started) c.copy_begin(c.d2h_stream, 1);
-  CUDA_CHECK(cudaMemcpyAsync(h_out + host_base + copied, d_out + copied, tail - copied, cudaMemcpyDeviceToHost, c.d2h_stream));
+  CUDA_CHECK(cudaMemcpyAsync(h_out + copied, d_out + copied, tail - copied, cudaMemcpyDeviceToHost, c.d2h_stream));
   c.copy_end(c.d2h_stream, 1);
   mark("finished, bytes left to download", tail - copied);
   copied = tail;
