@@ -20,6 +20,7 @@ EXPORTS = [
     "b2_bzip2_decompress_partial", "b2_bzip2_decompress_block_partial", "b2_bzip2_table_partial", "b2_bzip2_decompress_blocks",
     "b2_bzip2_compress_stream", "b2_bzip2_decompress_stream",
     "b2_bwt_cyclic", "b2_bwt_cyclic_batch", "b2_suffixsort", "b2_bwt_sentinel", "b2_bwt_inverse", "b2_bwtc_compress", "b2_bwtc_compress_unsized", "b2_bwtc_decompress", "b2_crc32_bzip2",
+    "b2_bwtc_compress_stream", "b2_bwtc_decompress_stream",
     "b2_bzip2_bound", "b2_bzip2_compress_dev", "b2_bzip2_decompress_dev",
     "b2_bzip2_plan", "b2_bzip2_plan_spec", "b2_bzip2_share_summary", "b2_bzip2_plan_share", "b2_bitshift_dev", "b2_dec_shard_open", "b2_dec_shard_export", "b2_dec_shard_finish", "b2_bzip2_encode_range_dev", "b2_get_stats", "b2_last_trace",
 ]
@@ -82,6 +83,8 @@ def lib():
     L.b2_bwtc_compress.argtypes = [C.c_void_p, C.c_size_t, C.c_int, u8pp, szp]
     L.b2_bwtc_compress_unsized.argtypes = [C.c_void_p, C.c_size_t, C.c_int, u8pp, szp]
     L.b2_bwtc_decompress.argtypes = [C.c_void_p, C.c_size_t, u8pp, szp]
+    L.b2_bwtc_compress_stream.argtypes = [READ_FN, WRITE_FN, C.c_void_p, C.c_int, C.c_int64]
+    L.b2_bwtc_decompress_stream.argtypes = [READ_FN, WRITE_FN, C.c_void_p]
     L.b2_crc32_bzip2.restype = C.c_uint32
     L.b2_crc32_bzip2.argtypes = [C.c_void_p, C.c_size_t]
     L.b2_bzip2_bound.restype = C.c_size_t

@@ -13,10 +13,10 @@ The reference writes its output through a 4096-byte buffer that is flushed only 
 nothing flushes it when a decode throws (bin/compressjs:103-115): so on a decode error the output holds the bytes
 decoded before the error, cut down to a multiple of 4096.
 
-For -t bzip2 (without -b) the command line is a pipe filter, as the reference is: the input is read a chunk at a time
-and the output written as the library produces it (InStream / OutStream, the makeInStream / makeOutStream of
-bin/compressjs:60-120), so memory does not grow with the stream (include/b2bz.h gives the bound).  -b (the reference
-seeks in its input) and BWTC read the whole input first.
+Without -b the command line is a pipe filter for both compressors, as the reference is: the input is read a chunk at a
+time and the output written as the library produces it (InStream / OutStream, the makeInStream / makeOutStream of
+bin/compressjs:60-120), so memory does not grow with the stream (include/b2bz.h gives the bounds).  -b (the reference
+seeks in its input) reads the whole input first.
 
 Usage errors are found before the GPU library is loaded, so they work on a machine without a GPU.
 """
@@ -180,10 +180,15 @@ def read_input(fd):
 
 
 class InStream:
-    """makeInStream of bin/compressjs:60-98: the descriptor read a chunk at a time, straight into the caller's buffer."""
+    """makeInStream of bin/compressjs:60-98: the descriptor read a chunk at a time, straight into the caller's buffer.
+    Like there, it has a ``size`` only when fstat gives one: a regular, non-empty file.  BWTC writes it into its header,
+    and "size unknown" for a stream without one (lib/Util.js:119-124)."""
 
     def __init__(self, fd):
         self.fd = fd
+        st = os.fstat(fd)
+        if stat.S_ISREG(st.st_mode) and st.st_size > 0:
+            self.size = st.st_size
 
     def read(self, buf, bufOffset, length):
         """buf: a writable bytes-like object.  Returns the bytes read, 0 at the end of the input."""
@@ -228,14 +233,20 @@ class OutStream:
         self.f.flush()
 
 
-def stream_bzip2(decompress, level, in_fd, out):
-    """-t bzip2 without -b: Bzip2.compressFile / decompressFile from the descriptor to the binary file `out` through
-    the streams of bin/compressjs, in bounded memory.  The exit status; on an error its message is on stderr and `out`
-    has what went out before it (on a decode error: the decoded bytes cut down to a multiple of FLUSH)."""
+def stream(kind, decompress, level, in_fd, out):
+    """Without -b: compressFile / decompressFile of `kind` ('bzip2' or 'bwtc') from the descriptor to the binary file
+    `out` through the streams of bin/compressjs, in bounded memory.  The exit status; on an error its message is on
+    stderr and `out` has what went out before it (on a decode error: the decoded bytes cut down to a multiple of FLUSH)."""
+    from .bwtc import BWTC
     from .bzip2 import Bzip2
     src, dst = InStream(in_fd), OutStream(out)
     try:
-        if decompress:
+        if kind == "bwtc":
+            if decompress:
+                BWTC.decompressFile(src, dst)
+            else:
+                BWTC.compressFile(src, dst, level)   # the header's size field comes from src.size
+        elif decompress:
             Bzip2.decompressFile(src, dst)   # without multistream, as bin/compressjs:160-164 calls it
         else:
             Bzip2.compressFile(src, dst, level)
@@ -248,7 +259,8 @@ def stream_bzip2(decompress, level, in_fd, out):
 
 
 def run(kind, decompress, level, block, data, size):
-    """(output bytes, error or None).  On a decode error the bytes are those decoded before it."""
+    """The whole input at once, as -b needs it: (output bytes, error or None).  On a decode error the bytes are those
+    decoded before it."""
     from . import bwtc, bzip2
     from .bwtc import BWTC
     from .bzip2 import Bzip2
@@ -285,8 +297,8 @@ def main(argv=None):
         in_fd = os.open(args[0], os.O_RDONLY) if len(args) > 0 else sys.stdin.fileno()
         out = open(args[1], "wb") if len(args) > 1 else sys.stdout.buffer
         kind = compressor(opts["T"])
-        if kind == "bzip2" and block < 0:
-            return stream_bzip2(decompress, level, in_fd, out)
+        if block < 0:
+            return stream(kind, decompress, level, in_fd, out)
         data, size = read_input(in_fd)
         result, err = run(kind, decompress, level, block, data, size)
         if err is not None:

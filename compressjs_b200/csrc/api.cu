@@ -11,10 +11,6 @@
 
 // stages implemented in the other translation units
 void bwt_inverse_sentinel_batch(Ctx& c, const u8* d_L, const u32* h_n, const u32* h_pidx, u32 nb, u8* d_out);
-size_t bwtc_bound(size_t n);
-void bwtc_compress_device(Ctx& c, const u8* d_in, size_t n, int level, u64 file_size, u8* d_out, size_t out_cap, size_t* out_n);
-u64 bwtc_parse_header(const u8* in, size_t n, size_t* pos);
-void bwtc_decompress(Ctx& c, const u8* d_in, size_t n, size_t pos, u64 fs, StreamOut& out);
 void dec_shard_release();
 void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* info);
 void dec_shard_export(u64* buf);
@@ -373,53 +369,76 @@ int b2_bwt_inverse(const uint8_t* L, uint8_t* out, int32_t n, int32_t pidx) {
   });
 }
 
-// ---- BWTC container (experimental, see bwtc.cu) ----------------------------------------------
+}  // extern "C"
+
+// ---- BWTC container (see bwtc.cu) ----------------------------------------------------------
+// Every BWTC call is one of the two drivers of bwtc.cu between a source and a sink.
+template <typename F>
+static void bwtc_call(Ctx& c, F run) {
+  try {
+    StageScope tot(c, ST_TOTAL);
+    run();
+  } catch (...) {
+    cudaStreamSynchronize(c.stream);  // nothing of this call may still be running when the next one starts
+    throw;
+  }
+  c.sync();
+  c.collect();
+}
 // file_size: the header's size field, n or (u64)-1 for a stream without a size (lib/Util.js:118-124)
-static int bwtc_compress_common(const uint8_t* in, size_t n, int level, u64 file_size, uint8_t** out, size_t* out_n) {
+static int bwtc_compress_buffer(const uint8_t* in, size_t n, int level, u64 file_size, uint8_t** out, size_t* out_n) {
   return guarded([&]() {
     Ctx& c = ctx_locked();
     c.reset_call();
-    const size_t cap = bwtc_bound(n);
-    size_t produced = 0;
-    void* host = nullptr;
-    {
-      StageScope tot(c, ST_TOTAL);
-      DBuf<u8> din(c, n ? n : 1), dout(c, cap);
-      if (n) CUDA_CHECK(cudaMemcpyAsync(din.p, in, n, cudaMemcpyHostToDevice, c.stream));
-      bwtc_compress_device(c, din, n, level, file_size, dout, cap, &produced);
-      host = pinned_alloc(produced);
-      CUDA_CHECK(cudaMemcpyAsync(host, dout.p, produced, cudaMemcpyDeviceToHost, c.stream));
-    }
-    c.sync();
-    c.collect();
-    c.stats.raw_bytes = n; c.stats.comp_bytes = produced;
-    *out = (uint8_t*)host; *out_n = produced;
+    StreamIn src(in, n);
+    StreamOut dst(c.d2h_stream);
+    bwtc_call(c, [&]() { bwtc_compress(c, src, level, file_size, dst); });
+    *out_n = dst.written; *out = dst.take();
     return 0;
   });
 }
+
+extern "C" {
+
 int b2_bwtc_compress(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n) {
-  return bwtc_compress_common(in, n, level, n, out, out_n);
+  return bwtc_compress_buffer(in, n, level, n, out, out_n);
 }
 int b2_bwtc_compress_unsized(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n) {
-  return bwtc_compress_common(in, n, level, ~(u64)0, out, out_n);
+  return bwtc_compress_buffer(in, n, level, ~(u64)0, out, out_n);
+}
+int b2_bwtc_compress_stream(b2_read_fn rd, b2_write_fn wr, void* user, int level, int64_t size) {
+  return guarded([&]() {
+    if (!rd || !wr) throw B2Error{B2_ERR_BAD_ARG, "null callback"};
+    if (size < -1) throw B2Error{B2_ERR_BAD_ARG, "size must be >= 0, or -1 for a stream without a size"};
+    Ctx& c = ctx_locked();
+    c.reset_call();
+    StreamIn src(rd, user, c.h2d_stream);   // the uploads are from pageable memory: nothing is ever queued out of its buffer
+    StreamOut dst(wr, user, c.d2h_stream);
+    bwtc_call(c, [&]() { bwtc_compress(c, src, level, size < 0 ? ~(u64)0 : (u64)size, dst); });
+    return 0;
+  });
 }
 int b2_bwtc_decompress(const uint8_t* in, size_t n, uint8_t** out, size_t* out_n) {
   return guarded([&]() {
     Ctx& c = ctx_locked();
     c.reset_call();
+    StreamIn src(in, n);
     StreamOut dst(c.stream);
-    {
-      StageScope tot(c, ST_TOTAL);
-      size_t pos = 0;
-      const u64 fs = bwtc_parse_header(in, n, &pos);   // before any device work
-      DBuf<u8> din(c, n);
-      CUDA_CHECK(cudaMemcpyAsync(din.p, in, n, cudaMemcpyHostToDevice, c.stream));
-      bwtc_decompress(c, din, n, pos, fs, dst);
-    }
-    c.sync();
-    c.collect();
+    bwtc_call(c, [&]() { bwtc_decompress(c, src, dst); });   // on an error the result is dropped with dst
     c.stats.raw_bytes = dst.written; c.stats.comp_bytes = n;
     *out_n = dst.written; *out = dst.take();
+    return 0;
+  });
+}
+int b2_bwtc_decompress_stream(b2_read_fn rd, b2_write_fn wr, void* user) {
+  return guarded([&]() {
+    if (!rd || !wr) throw B2Error{B2_ERR_BAD_ARG, "null callback"};
+    Ctx& c = ctx_locked();
+    c.reset_call();
+    StreamIn src(rd, user, c.stream);
+    StreamOut dst(wr, user, c.stream);
+    bwtc_call(c, [&]() { bwtc_decompress(c, src, dst); });
+    c.stats.raw_bytes = dst.written; c.stats.comp_bytes = src.base + src.have;
     return 0;
   });
 }
@@ -456,6 +475,10 @@ static size_t stream_window() {
   size_t win = (size_t)8 << 30;
   if (const char* e = getenv("B2_STREAM_WINDOW")) { const long long v = atoll(e); if (v >= (1 << 20)) win = (size_t)v; }
   return win;
+}
+size_t dec_window() {
+  if (const char* e = getenv("B2_DEC_WINDOW")) { const long long v = atoll(e); if (v >= (64 << 10)) return (size_t)v; }
+  return (size_t)4 << 30;
 }
 
 // ---- the host-side input and output of the host entry points ----

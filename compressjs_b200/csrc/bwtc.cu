@@ -28,6 +28,10 @@ struct BwtcState {
   u32 pad;
 };
 
+// The coder writes each batch into an output window of its own (k_bwtc_window), from the window's byte 0.  Its output is
+// final as it is written: a carry lives in `buffer` and the `help` counter of bytes held back, never in a byte already
+// out.  The start writes nothing (the first normalisation comes with the next symbol); the finish appends the trailer to
+// the window of the last batch.
 __global__ void k_bwtc_start(BwtcState* st, u8* out, u64 cap, u32 finalByte, u32 level) {
   if (threadIdx.x || blockIdx.x) return;
   bc_enc_start(&st->rc, out, cap, finalByte);                 // lib/BWTC.js:13-14
@@ -226,6 +230,12 @@ __global__ void __launch_bounds__(32) k_bwtc_code(BwtcState* st, const u64* __re
   }
 }
 
+// the next batch's bytes go to `out`, from its byte 0 (a launch of its own: the coder's serial loop stays as it is)
+__global__ void k_bwtc_window(BwtcState* st, u8* out, u64 cap) {
+  if (threadIdx.x || blockIdx.x) return;
+  st->rc.out = out; st->rc.cap = cap; st->rc.n = 0;
+}
+
 __global__ void k_bwtc_finish(BwtcState* st) {
   if (threadIdx.x || blockIdx.x) return;
   bc_enc_code(&st->rc, bc_triple(1, 2, 3));                   // "no more blocks", lib/BWTC.js:141
@@ -234,116 +244,195 @@ __global__ void k_bwtc_finish(BwtcState* st) {
 
 size_t bwtc_bound(size_t n) { return n + n / 8 + (n / 100000 + 2) * 1024 + 64; }
 
-// BWTC.compressFile on device buffers.  file_size is the size field of the header (Util.js:118-124): n for an input of
-// known size, or (u64)-1 (a single size byte 0x80) for a stream without a size.  out_cap >= bwtc_bound(n).
-void bwtc_compress_device(Ctx& c, const u8* d_in, size_t n, int level, u64 file_size, u8* d_out, size_t out_cap, size_t* out_n) {
+// BWTC.compressFile from a host source into a host sink: b2_bwtc_compress / _unsized (the caller's buffer, complete from
+// the start, into the result buffer) and b2_bwtc_compress_stream (read and write callbacks).  file_size is the size field
+// of the header (Util.js:118-124), or (u64)-1 (a single size byte 0x80) for a stream without a size.
+//
+// Blocks are fixed cuts of the raw input (level * 100 000 bytes, lib/BWTC.js:24-44), so the input is taken a batch of
+// B blocks at a time, straight from `in` into the batch's slots: the device never holds more than one batch of input.
+// The coder writes batch k into output window k & 1, sized for the batch's coded bytes plus the `help` bytes still held
+// back when it starts.  Batch k's bytes go to the host and to `out` while batch k + 1 runs on the device, and the next
+// batch's input is read while batch k runs.  Device memory: one batch of scratch and two windows, whatever the size of
+// the input (include/b2bz.h gives the bound).
+void bwtc_compress(Ctx& c, StreamIn& in, int level, u64 file_size, StreamOut& out) {
   if (level < 1 || level > 9) level = 9;                      // lib/BWTC.js:16-19
   const u32 blockSize = (u32)level * 100000u;
   const int fast = level <= 5;                                // :22
-  if (out_cap < 32) throw B2Error{B2_ERR_BAD_ARG, "output buffer too small"};
   u8 hdr[24];
   u32 finalByte = 0;
   const u32 hlen = bc_file_header(hdr, file_size, &finalByte);
-  c.to_device(d_out, hdr, hlen);
-  DBuf<BwtcState> st(c, 1);
-  k_bwtc_start<<<1, 1, 0, c.stream>>>(st, d_out + hlen, out_cap - hlen, finalByte, (u32)level);
-  KLAUNCH(c); KCHECK();
-  const size_t nblocks = (n + blockSize - 1) / blockSize;
-  if (nblocks) {
-    const u32 B = (u32)std::min<size_t>(c.bwt_batch, nblocks);
-    const u32 tcap = 2 * (blockSize + 1) + 1024;              // every symbol can cost an escape and a literal
-    DBuf<u8> T(c, (size_t)B << SEG_SHIFT), U(c, (size_t)B << SEG_SHIFT);
-    DBuf<u8> sym_lo(c, (size_t)B << SEG_SHIFT);
-    DBuf<unsigned long long> sym_hi(c, (size_t)B * SEL_STRIDE);
-    DBuf<u32> sym_any_hi(c, B);
-    const NarrowSyms nsym{sym_lo, sym_hi, sym_any_hi};
+  // The first batch sizes the buffers: an input that ends inside it gets only the blocks it has.
+  u32 B = c.bwt_batch;
+  size_t end = in.fill((size_t)B * blockSize);
+  if (in.eof) B = (u32)std::min<size_t>(B, (end + blockSize - 1) / blockSize);
+  const u32 tcap = 2 * (blockSize + 1) + 1024;                // every symbol can cost an escape and a literal
+  DBuf<u8> T, U, sym_lo;
+  DBuf<unsigned long long> sym_hi;
+  DBuf<u32> sym_any_hi, dn, dpidx, dm, dfreq, dused, tcount;
+  DBuf<u16> sym;
+  DBuf<u64> triples;
+  if (B) {
+    T.alloc(c, (size_t)B << SEG_SHIFT); U.alloc(c, (size_t)B << SEG_SHIFT); sym_lo.alloc(c, (size_t)B << SEG_SHIFT);
+    sym_hi.alloc(c, (size_t)B * SEL_STRIDE); sym_any_hi.alloc(c, B);
     CUDA_CHECK(cudaMemsetAsync(sym_hi, 0, (size_t)B * SEL_STRIDE * 8, c.stream));
     CUDA_CHECK(cudaMemsetAsync(sym_any_hi, 0, (size_t)B * 4, c.stream));
-    DBuf<u16> sym(c, (size_t)B << SEG_SHIFT);
-    DBuf<u32> dn(c, B), dpidx(c, B), dm(c, B), dfreq(c, (size_t)B * HUFF_MAXSYM), dused(c, (size_t)B * 8), tcount(c, B);
-    DBuf<u64> triples(c, (size_t)B * tcap);
-    std::vector<u32> hn(B);
-    for (size_t k0 = 0; k0 < nblocks; k0 += B) {
-      const u32 nb = (u32)std::min<size_t>(B, nblocks - k0);
-      for (u32 b = 0; b < nb; b++) hn[b] = (u32)std::min<size_t>(blockSize, n - (k0 + b) * blockSize);
-      const u32 full = hn[nb - 1] == blockSize ? nb : nb - 1;   // only the last block of the file can be short
-      if (full)
-        CUDA_CHECK(cudaMemcpy2DAsync(T.p, SEG_SIZE, d_in + k0 * blockSize, blockSize, blockSize, full, cudaMemcpyDeviceToDevice, c.stream));
-      if (full < nb)
-        CUDA_CHECK(cudaMemcpyAsync(T.p + ((size_t)full << SEG_SHIFT), d_in + (k0 + full) * blockSize, hn[full], cudaMemcpyDeviceToDevice, c.stream));
-      c.to_device(dn, hn.data(), 4 * nb);
-      CUDA_CHECK(cudaMemsetAsync(dpidx, 0, 4 * nb, c.stream));
-      {
-        StageScope s(c, ST_BWT);
-        bwt_forward_batch(c, T, U, dn, hn.data(), nb, dpidx, true, nullptr);   // U = sentinel BWT, dpidx = pidx + 1
-      }
-      {
-        StageScope s(c, ST_MTF);
-        mtf_rle2_batch(c, T, U, dn, hn.data(), nb, nsym, dm, dfreq, dused);
-        u32 mmax = 0;   // m <= n + 1
-        for (u32 b = 0; b < nb; b++) mmax = std::max(mmax, hn[b] + 1);
-        const u32 tps = (mmax + WD_THREADS * 16 - 1) / (WD_THREADS * 16);
-        k_bwtc_widen<<<nb * tps, WD_THREADS, 0, c.stream>>>(sym_lo, sym_hi, sym_any_hi, dm, tps, sym);
-        KLAUNCH(c); KCHECK();
-      }
-      {
-        StageScope s(c, ST_HUFF);   // statistics: the model takes the slot of the Huffman stage (ms_huff) ...
-        if (fast) k_bwtc_model<<<nb, 32, 0, c.stream>>>(sym, dm, dn, dpidx, dused, blockSize, fast, triples, tcap, tcount);
-        else k_bwtc_model_fenwick<<<nb, 32, 0, c.stream>>>(sym, dm, dn, dpidx, dused, blockSize, triples, tcap, tcount);
-        KLAUNCH(c); KCHECK();
-      }
-      {
-        StageScope s(c, ST_PACK);   // ... and the serial range coder the slot of the bit packer (ms_pack)
-        k_bwtc_code<<<1, 32, 0, c.stream>>>(st, triples, tcount, nb, tcap);
-        KLAUNCH(c); KCHECK();
-      }
-      c.stats.blocks += nb;
-    }
+    sym.alloc(c, (size_t)B << SEG_SHIFT);
+    dn.alloc(c, B); dpidx.alloc(c, B); dm.alloc(c, B); dfreq.alloc(c, (size_t)B * HUFF_MAXSYM); dused.alloc(c, (size_t)B * 8); tcount.alloc(c, B);
+    triples.alloc(c, (size_t)B * tcap);
   }
+  const NarrowSyms nsym{sym_lo, sym_hi, sym_any_hi};
+  const size_t wcap = bwtc_bound((size_t)B * blockSize);     // a window grows only if `help` holds more than its slack
+  DBuf<u8> win[2];
+  size_t cap[2] = {wcap, wcap};
+  win[0].alloc(c, wcap);
+  if (B) win[1].alloc(c, wcap);
+  DBuf<BwtcState> st(c, 1);
+  k_bwtc_start<<<1, 1, 0, c.stream>>>(st, win[0], wcap, finalByte, (u32)level);
+  KLAUNCH(c); KCHECK();
+  struct Ev {
+    cudaEvent_t e = nullptr;
+    cudaStream_t d2h;
+    ~Ev() {   // no copy out of a window may outlive it, also when the call fails half way
+      cudaStreamSynchronize(d2h);
+      if (e) cudaEventDestroy(e);
+    }
+  } ev{nullptr, c.d2h_stream};
+  CUDA_CHECK(cudaEventCreateWithFlags(&ev.e, cudaEventDisableTiming));
+  // a result gets room for the whole stream at once (its input is complete: `end` is all of it)
+  out.reserve(out.wr ? hlen : hlen + bwtc_bound(end));
+  memcpy(out.next(), hdr, hlen);
+  out.put(out.next(), hlen);
+  BwtcState h;
+  // the coder's state once the launch before `ev` has finished; its bytes (window w) start on their way to `out`
+  auto fetch = [&](int w) -> size_t {
+    CUDA_CHECK(cudaEventSynchronize(ev.e));
+    CUDA_CHECK(cudaMemcpyAsync(&h, st, sizeof h, cudaMemcpyDeviceToHost, c.d2h_stream));
+    CUDA_CHECK(cudaStreamSynchronize(c.d2h_stream));
+    if (h.overflow) throw B2Error{B2_ERR_CUDA, "internal error: BWTC triple buffer overflow"};
+    if (h.rc.n > h.rc.cap) throw B2Error{B2_ERR_CUDA, "internal error: BWTC output window overflow"};
+    const size_t bytes = (size_t)h.rc.n;
+    out.reserve(bytes, false, wcap);
+    CUDA_CHECK(cudaMemcpyAsync(out.next(), win[w], bytes, cudaMemcpyDeviceToHost, c.d2h_stream));
+    return bytes;
+  };
+  std::vector<u32> hn(std::max(B, 1u));
+  size_t pos = 0;       // raw bytes taken
+  int w = 0;            // the window of the next batch
+  bool held = false;    // the previous batch's bytes are still in window w ^ 1
+  u64 help = 0;         // bytes the coder holds back when the next batch starts
+  for (;;) {
+    in.drop(pos);
+    end = in.fill(pos + (size_t)B * blockSize);
+    const size_t take = std::min(end, pos + (size_t)B * blockSize) - pos;   // < B blocks only at the end of the input
+    if (!take) break;
+    const u32 nb = (u32)((take + blockSize - 1) / blockSize);
+    for (u32 b = 0; b < nb; b++) hn[b] = (u32)std::min<size_t>(blockSize, take - (size_t)b * blockSize);
+    const u32 full = hn[nb - 1] == blockSize ? nb : nb - 1;   // only the last block of the input can be short
+    if (full)
+      CUDA_CHECK(cudaMemcpy2DAsync(T.p, SEG_SIZE, in.at(pos), blockSize, blockSize, full, cudaMemcpyHostToDevice, c.stream));
+    if (full < nb)
+      CUDA_CHECK(cudaMemcpyAsync(T.p + ((size_t)full << SEG_SHIFT), in.at(pos + (size_t)full * blockSize), hn[full], cudaMemcpyHostToDevice, c.stream));
+    c.to_device(dn, hn.data(), 4 * nb);
+    CUDA_CHECK(cudaMemsetAsync(dpidx, 0, 4 * nb, c.stream));
+    {
+      StageScope s(c, ST_BWT);
+      bwt_forward_batch(c, T, U, dn, hn.data(), nb, dpidx, true, nullptr);   // U = sentinel BWT, dpidx = pidx + 1
+    }
+    {
+      StageScope s(c, ST_MTF);
+      mtf_rle2_batch(c, T, U, dn, hn.data(), nb, nsym, dm, dfreq, dused);
+      u32 mmax = 0;   // m <= n + 1
+      for (u32 b = 0; b < nb; b++) mmax = std::max(mmax, hn[b] + 1);
+      const u32 tps = (mmax + WD_THREADS * 16 - 1) / (WD_THREADS * 16);
+      k_bwtc_widen<<<nb * tps, WD_THREADS, 0, c.stream>>>(sym_lo, sym_hi, sym_any_hi, dm, tps, sym);
+      KLAUNCH(c); KCHECK();
+    }
+    {
+      StageScope s(c, ST_HUFF);   // statistics: the model takes the slot of the Huffman stage (ms_huff) ...
+      if (fast) k_bwtc_model<<<nb, 32, 0, c.stream>>>(sym, dm, dn, dpidx, dused, blockSize, fast, triples, tcap, tcount);
+      else k_bwtc_model_fenwick<<<nb, 32, 0, c.stream>>>(sym, dm, dn, dpidx, dused, blockSize, triples, tcap, tcount);
+      KLAUNCH(c); KCHECK();
+    }
+    // the previous batch's coder has finished by now or soon: its bytes leave window w ^ 1, and its `help` sizes window w
+    size_t prev = 0;
+    if (held) {
+      prev = fetch(w ^ 1);
+      help = h.rc.help;
+    }
+    const size_t need = bwtc_bound(take) + (size_t)help + 16;   // the batch, the bytes held back, the trailer
+    if (need > cap[w]) { win[w].alloc(c, need); cap[w] = need; }
+    {
+      StageScope s(c, ST_PACK);   // ... and the serial range coder the slot of the bit packer (ms_pack)
+      k_bwtc_window<<<1, 1, 0, c.stream>>>(st, win[w], cap[w]);
+      KLAUNCH(c); KCHECK();
+      k_bwtc_code<<<1, 32, 0, c.stream>>>(st, triples, tcount, nb, tcap);
+      KLAUNCH(c); KCHECK();
+    }
+    CUDA_CHECK(cudaEventRecord(ev.e, c.stream));
+    if (held) out.put(out.next(), prev);   // while this batch runs
+    held = true;
+    w ^= 1;
+    pos += take;
+    c.stats.blocks += nb;
+  }
+  // the trailer goes behind the last batch's bytes (window w ^ 1), or into window 0 when there was no batch
   k_bwtc_finish<<<1, 1, 0, c.stream>>>(st);
   KLAUNCH(c); KCHECK();
-  BwtcState h;
-  c.to_host(&h, st, sizeof h);
-  c.sync();
-  if (h.overflow) throw B2Error{B2_ERR_CUDA, "internal error: BWTC triple buffer overflow"};
-  if (h.rc.n > h.rc.cap) throw B2Error{B2_ERR_BAD_ARG, "output buffer too small for the compressed stream"};
-  *out_n = hlen + (size_t)h.rc.n;
+  CUDA_CHECK(cudaEventRecord(ev.e, c.stream));
+  const size_t last = fetch(held ? w ^ 1 : 0);
+  out.put(out.next(), last);
+  CUDA_CHECK(cudaStreamSynchronize(c.d2h_stream));   // a result is complete when the call returns
+  c.stats.raw_bytes = pos;
+  c.stats.comp_bytes = out.written;
 }
 
 // ---- decode ---------------------------------------------------------------------------------------------------
 // The range decoder and the level are all that carries from one block to the next (the block models start afresh in
 // bc_decode_block, the length model is stateless), so the decode stops after a batch of blocks and resumes from here.
+// The coded stream reaches the device a window [a, a + wlen) at a time; rc.pos counts from the window of the last launch
+// (st->a), and a launch over another window moves it.
 #define BD_MORE 0      // more blocks may follow
 #define BD_END 1       // "no more blocks" has been read
+#define BD_NEED 2      // the next block reads past the window, which is not the end of the input: slide the window
 #define BD_CORRUPT (-1)
 #define BD_SIZE (-2)   // the blocks add up to more than the size field
+#define BC_EOF 0xFFFFFFFFu
 struct BwtcDecState {
   bc_dec rc;
+  u64 a;            // absolute position of the window of the last launch
   u64 total;        // bytes in the blocks decoded so far
   u64 limit;        // the size field's size; ~0 when the stream has no size
-  u64 maxblocks;
   u32 level;
   u32 nblocks;      // blocks decoded so far
   u32 nb;           // blocks decoded by the last launch
   int status;       // BD_*
 };
 
-__global__ void k_bwtc_dec_start(BwtcDecState* st, const u8* __restrict__ in, u64 n, u64 pos, u64 limit, u64 maxblocks) {
+// the coder's first bytes: pos = the first byte behind the header, at the window's start
+__global__ void k_bwtc_dec_start(BwtcDecState* st, const u8* __restrict__ win, u64 wlen, u64 a, u64 limit) {
   if (threadIdx.x || blockIdx.x) return;
-  bc_dec_start(&st->rc, in, n, pos);                            // lib/BWTC.js:142-143
+  bc_dec_start(&st->rc, win, wlen, 0);                          // lib/BWTC.js:142-143
   st->level = bc_dec_cul(&st->rc, 256);                         // decoder.decodeByte(), :144
   bc_dec_update(&st->rc, 1, st->level, 256);
-  st->total = 0; st->limit = limit; st->maxblocks = maxblocks;
+  st->a = a;
+  st->total = 0; st->limit = limit;
   st->nblocks = 0; st->nb = 0;
   st->status = st->level >= 1 && st->level <= 9 ? BD_MORE : BD_CORRUPT;
 }
 
-// one thread: up to B more blocks down to their L columns (inverse MTF folded in), block b of the launch at slot b << 20
-__global__ void k_bwtc_decode(BwtcDecState* st, u32 B, u8* __restrict__ L, u32* __restrict__ lengths, u32* __restrict__ pidx1) {
+// One thread: up to B more blocks down to their L columns (inverse MTF folded in), block b of the launch at slot b << 20.
+// `final`: the input ends at the window's end, so a read past it is the reference's EOF.  Otherwise a step that reads past
+// the window is undone (the decoder's state at the block's start is all that crosses a block) and the launch stops with
+// BD_NEED.  maxblocks: the most blocks the stream may hold; when `need_at_max`, it is a lower bound taken from the input
+// seen so far, and reaching it asks for more input instead of deciding.
+__global__ void k_bwtc_decode(BwtcDecState* st, u32 B, const u8* __restrict__ win, u64 wlen, u64 a, int final, u64 maxblocks,
+                              int need_at_max, u8* __restrict__ L, u32* __restrict__ lengths, u32* __restrict__ pidx1) {
   if (threadIdx.x || blockIdx.x) return;
   st->nb = 0;
-  if (st->status != BD_MORE) return;
+  if (st->status != BD_MORE && st->status != BD_NEED) return;
   bc_dec rc = st->rc;
+  rc.pos = st->a + rc.pos - a;   // a <= the next byte to read: the host never slides past it
+  rc.in = win; rc.n = wlen;
   const u32 level = st->level;
   const bool unsized = st->limit == ~0ull;
   u64 total = st->total;
@@ -351,24 +440,30 @@ __global__ void k_bwtc_decode(BwtcDecState* st, u32 B, u8* __restrict__ L, u32* 
   u32 nb = 0;
   int status = BD_MORE;
   while (nb < B) {
-    if (st->nblocks + nb >= st->maxblocks) {
-      // only "no more blocks" may follow
-      status = bc_dec_cul(&rc, 3) == 2 ? BD_END : BD_CORRUPT;
-      break;
-    }
+    const bc_dec keep = rc;
     u32 len = 0, p1 = 0;
-    const int r = bc_decode_block(&rc, &model, level * 100000u, level <= 5, L + ((size_t)nb << SEG_SHIFT), &len, &p1);
+    int r;
+    if (st->nblocks + nb >= maxblocks) {
+      if (need_at_max) { status = BD_NEED; break; }
+      r = bc_dec_cul(&rc, 3) == 2 ? 1 : -5;                     // only "no more blocks" may follow
+    } else {
+      r = bc_decode_block(&rc, &model, level * 100000u, level <= 5, L + ((size_t)nb << SEG_SHIFT), &len, &p1);
+    }
+    if (rc.buffer == BC_EOF) {   // the step has read past the window
+      if (!final) { rc = keep; status = BD_NEED; break; }
+      // Without a size, the end of the input is the only bound.  A whole stream is never read past its end (the
+      // coder's trailer is longer than the decoder's look-ahead), so a decoder that has read past it is decoding a cut
+      // stream: an error, where the reference has no check and decodes on.
+      if (unsized) { status = BD_CORRUPT; break; }
+    }
     if (r) { status = r == 1 ? BD_END : BD_CORRUPT; break; }
     if (total + len > st->limit) { status = BD_SIZE; break; }
     total += len;
     lengths[nb] = len; pidx1[nb] = p1;
     nb++;
   }
-  // Without a size, the end of the input is the only bound.  A whole stream is never read past its end (the coder's
-  // trailer is longer than the decoder's look-ahead), so a decoder that has read past it (its last byte read is EOF)
-  // is decoding a cut stream: an error, where the reference has no check and decodes on.
-  if (unsized && status >= 0 && rc.buffer == 0xFFFFFFFFu) status = BD_CORRUPT;
   st->rc = rc;
+  st->a = a;
   st->total = total;
   st->nblocks += nb;
   st->nb = nb;
@@ -383,7 +478,7 @@ static u32 bwtc_dec_batch(const Ctx& c) {
 
 // lib/Util.js:211-220 readUnsignedNumber after the magic.  Returns the size field (0 = unknown size, else size + 1) and
 // sets *pos behind it: its last byte is the range coder's first.
-u64 bwtc_parse_header(const u8* in, size_t n, size_t* pos) {
+static u64 bwtc_parse_header(const u8* in, size_t n, size_t* pos) {
   if (n < 5 || memcmp(in, "bwtc", 4)) throw B2Error{B2_ERR_BAD_MAGIC, "Bad magic"};   // lib/Util.js:151-153
   size_t p = 4;
   u64 fs = 0;
@@ -399,30 +494,53 @@ u64 bwtc_parse_header(const u8* in, size_t n, size_t* pos) {
   return fs;
 }
 
-// BWTC.decompressFile: d_in = the stream on the device, pos and fs from bwtc_parse_header.  The decoded bytes go to the
-// host, batch by batch, into the result `out` (a sink without a write callback).  Size field known: the whole buffer is
-// reserved up front.  Size unknown (fs == 0): the buffer grows as the batches arrive.  Device memory: one batch of
-// blocks, whatever the size of the file.
-void bwtc_decompress(Ctx& c, const u8* d_in, size_t n, size_t pos, u64 fs, StreamOut& out) {
+// BWTC.decompressFile from a host source: b2_bwtc_decompress (the caller's buffer into the result) and
+// b2_bwtc_decompress_stream (read and write callbacks).  The coded stream goes to the device a window of W bytes at a
+// time (dec_window()); a launch that stops with BD_NEED slides the window to the first byte the next block needs, and a
+// window that would start where the last one did is twice as long.  The decoded bytes go to `out` a batch at a time.
+// Device memory: one window and one batch of blocks, whatever the size of the file (include/b2bz.h gives the bound).
+void bwtc_decompress(Ctx& c, StreamIn& in, StreamOut& out) {
+  size_t pos = 0;
+  const u64 fs = bwtc_parse_header(in.at(0), in.fill(4 + 10), &pos);   // the longest header it accepts; before any device work
   const bool unsized = fs == 0;
   const u64 limit = unsized ? ~0ull : fs - 1;
-  // the level is inside the coded stream: bound the block count for the smallest block size
-  // (the header is not trusted: a block costs at least a few coded bytes, so n compressed bytes cannot hold more than
-  // n / 2 blocks)
-  const u64 maxblocks = unsized ? (u64)n / 2 + 2 : std::min<u64>(limit / 100000u + 2, (u64)n / 2 + 2);
+  // The header is not trusted: the level is inside the coded stream, so the size field bounds the blocks for the
+  // smallest block size, and a block costs at least a few coded bytes, so n compressed bytes cannot hold more than n / 2
+  // blocks.  n is known once the input has ended; before, the bytes seen so far give a lower bound.
+  const u64 size_blocks = unsized ? ~0ull : limit / 100000u + 2;
+  size_t W = dec_window();
+  size_t a = pos, wlen = 0;     // the window
+  bool final = false;
+  u64 maxblocks = 0;
+  int need_at_max = 0;
+  DBuf<u8> dwin;
+  size_t dcap = 0;
+  auto load = [&]() {
+    in.drop(a);
+    const size_t e = in.fill(a + W + 1);   // one byte more than the window: a window is the last one exactly when the input ends in it
+    final = in.eof && e <= a + W;
+    wlen = std::min(W, e - a);
+    const u64 from_n = (u64)e / 2 + 2;
+    maxblocks = std::min(size_blocks, from_n);
+    need_at_max = !final && from_n < size_blocks;
+    if (wlen > dcap) { dwin.alloc(c, wlen); dcap = wlen; }
+    if (wlen) CUDA_CHECK(cudaMemcpyAsync(dwin.p, in.at(a), wlen, cudaMemcpyHostToDevice, c.stream));
+  };
+  load();
   const u32 B = (u32)std::min<u64>(bwtc_dec_batch(c), maxblocks);
   DBuf<u8> L(c, (size_t)B << SEG_SHIFT), dout(c, (size_t)B * 900000u);
   DBuf<u32> lengths(c, B), pidx1(c, B);
   DBuf<BwtcDecState> st(c, 1);
-  k_bwtc_dec_start<<<1, 1, 0, c.stream>>>(st, d_in, n, pos, limit, maxblocks);
+  k_bwtc_dec_start<<<1, 1, 0, c.stream>>>(st, dwin, wlen, a, limit);
   KLAUNCH(c); KCHECK();
   std::vector<u32> hl(B), hp(B);
-  // a known size gets all of its buffer now, up to what maxblocks blocks can hold (more would fail the size check)
-  if (!unsized) out.reserve((size_t)std::min<u64>(limit, maxblocks * 900000u), true);
+  // a result with a known size gets all of its buffer now, up to what maxblocks blocks can hold (more would fail the size
+  // check); a staging buffer holds one batch
+  if (!unsized && !out.wr) out.reserve((size_t)std::min<u64>(limit, maxblocks * 900000u), true);
   for (;;) {
     {
       StageScope s(c, ST_HDEC);
-      k_bwtc_decode<<<1, 1, 0, c.stream>>>(st, B, L, lengths, pidx1);
+      k_bwtc_decode<<<1, 1, 0, c.stream>>>(st, B, dwin, wlen, a, final, maxblocks, need_at_max, L, lengths, pidx1);
       KLAUNCH(c); KCHECK();
     }
     BwtcDecState h;
@@ -430,12 +548,11 @@ void bwtc_decompress(Ctx& c, const u8* d_in, size_t n, size_t pos, u64 fs, Strea
     c.to_host(hl.data(), lengths, 4 * B);
     c.to_host(hp.data(), pidx1, 4 * B);
     c.sync();   // also ends the previous batch's copy to the host
-    if (h.status == BD_CORRUPT) throw B2Error{B2_ERR_DATA_ERROR, "Data error: BWTC stream is corrupt"};
-    if (h.status == BD_SIZE) throw B2Error{B2_ERR_DATA_ERROR, "outputsize does not match decoded input"};   // lib/Util.js:69-71
+    // the blocks decoded in full go out first, also in front of an error (lib/BWTC.js:228 writes each block as it ends)
     u64 bytes = 0;
     for (u32 b = 0; b < h.nb; b++) bytes += hl[b];
     if (h.nb) {
-      out.reserve((size_t)bytes);   // grows only without a size field
+      out.reserve((size_t)bytes, false, (size_t)B * 900000u);   // a result grows only without a size field
       {
         StageScope s(c, ST_IBWT);   // BWT.unbwtransform of every block of the batch, lib/BWTC.js:224
         bwt_inverse_sentinel_batch(c, L, hl.data(), hp.data(), h.nb, dout);
@@ -444,7 +561,15 @@ void bwtc_decompress(Ctx& c, const u8* d_in, size_t n, size_t pos, u64 fs, Strea
       out.put(out.next(), (size_t)bytes);
       c.stats.blocks += h.nb;
     }
+    if (h.status == BD_CORRUPT) throw B2Error{B2_ERR_DATA_ERROR, "Data error: BWTC stream is corrupt"};
+    if (h.status == BD_SIZE) throw B2Error{B2_ERR_DATA_ERROR, "outputsize does not match decoded input"};   // lib/Util.js:69-71
     if (h.status == BD_END) break;
+    if (h.status == BD_NEED) {
+      const size_t next = (size_t)(h.a + h.rc.pos);   // the next block's first byte still to read
+      if (next == a) W *= 2;                           // not one block fits: a longer window
+      a = next;
+      load();
+    }
   }
   c.sync();
   if (!unsized && out.written != limit) throw B2Error{B2_ERR_DATA_ERROR, "outputsize does not match decoded input"};

@@ -1137,12 +1137,6 @@ static u32 dec_keep_cls_limit() {
   if (const char* e = getenv("B2_DEC_KEEP_CLS")) { const int v = atoi(e); if (v >= 0) return (u32)v; }  // test hook
   return DEC_KEEP_CLS;
 }
-// bytes of compressed input on the device at a time, which also caps the output staged for the host ($B2_DEC_WINDOW,
-// default 4 GiB: most files are one window; down to 64 KiB as a test hook)
-static size_t dec_window() {
-  if (const char* e = getenv("B2_DEC_WINDOW")) { const long long v = atoll(e); if (v >= (64 << 10)) return (size_t)v; }
-  return (size_t)4 << 30;
-}
 
 // Scratch of one decode batch, allocated for the largest batch of a call and reused by every batch: about 20 MiB per block
 // (the radix sort's keys and values, 16 MiB, are most of it).

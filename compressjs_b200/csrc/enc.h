@@ -137,6 +137,20 @@ void bzip2_encode_range(Ctx& c, const u8* d_in, size_t n, int level, size_t firs
 void bitshift_device(Ctx& c, const void* src, u64 nbits, int phase, void* dst);
 void bzip2_release_plan();  // the plan kept for b2_bzip2_encode_range_dev
 
+// Bytes of compressed input on the device at a time in the bzip2 and BWTC decoders, which also caps the output the
+// bzip2 decoder stages for the host ($B2_DEC_WINDOW, default 4 GiB: most files are one window; down to 64 KiB as a
+// test hook).  Implemented in api.cu.
+size_t dec_window();
+
+// ---- BWTC drivers (bwtc.cu), one for each direction: the host-buffer calls run them over a complete source and a
+// result sink, the stream calls over read and write callbacks ----
+size_t bwtc_bound(size_t n);
+// BWTC.compressFile: file_size is the header's size field, or (u64)-1 for "size unknown" (lib/Util.js:118-124)
+void bwtc_compress(Ctx& c, StreamIn& in, int level, u64 file_size, StreamOut& out);
+// BWTC.decompressFile: every block goes to `out` as soon as its batch is decoded; on a data error the blocks in front of
+// the failing check have gone out when the error is thrown
+void bwtc_decompress(Ctx& c, StreamIn& in, StreamOut& out);
+
 // ---- bzip2 decode driver (decode.cu): every single-GPU decode entry point ----
 // The input is `sin` or the device buffer d_in[0, n); the output goes to the device buffer d_out (out_cap bytes), to
 // `sout`, or nowhere (a table).  See decode.cu.

@@ -148,8 +148,41 @@ int b2_bwtc_compress_unsized(const uint8_t* in, size_t n, int level, uint8_t** o
 /* BWTC.decompressFile(input, output)                  lib/BWTC.js:141-231, for streams with a size field and for
  * streams of unknown size (decoded up to the "no more blocks" marker).  Blocks are decoded a batch at a time
  * ($B2_BWTC_DEC_BATCH, default two per SM) and each batch goes to the host, so device memory is bounded by one batch
- * (about 17 MiB per block) for any file size.  A stream whose blocks exceed its size field fails as soon as they do. */
+ * (about 17 MiB per block) for any file size.  A stream whose blocks exceed its size field fails as soon as they do.
+ * On an error nothing is returned. */
 int b2_bwtc_decompress(const uint8_t* in, size_t n, uint8_t** out, size_t* out_n);
+/* ---- BWTC over read / write callbacks (b2_read_fn / b2_write_fn and their rules as for the bzip2 stream calls above) --
+ * BWTC.compressFile over a read callback (lib/BWTC.js:12-139, lib/Util.js:104-142).  size >= 0 is written as the
+ * header's size field (what the reference takes from inStream.size); size == -1 writes "size unknown"; any other size is
+ * B2_ERR_BAD_ARG before a callback runs.  The blocks are those of every byte read, as in the reference: a size that
+ * differs from the bytes read is written as given (the stream then fails the size check when decoded, as it does
+ * there).  Level outside 1..9 means 9.
+ * Everything passed to write, concatenated, is the *out of b2_bwtc_compress on everything read when size is their
+ * count, and of b2_bwtc_compress_unsized when size == -1, however the input is split into reads and whatever
+ * $B2_BWT_BATCH is; b2_get_stats reports raw_bytes, comp_bytes and blocks as those calls do. */
+int b2_bwtc_compress_stream(b2_read_fn rd, b2_write_fn wr, void* user, int level, int64_t size);
+/* BWTC.decompressFile over a read callback (lib/BWTC.js:141-231).  The return code and b2_last_error() are those of
+ * b2_bwtc_decompress on the same bytes.  On success the bytes written are its result.  On a data error (-5) they are
+ * exactly the blocks decoded in full before the failing check, in stream order, as the reference has written them when
+ * it throws (lib/BWTC.js:228): a block that passes the size field is not among them, and a size field larger than the
+ * blocks has every block written.  "Bad magic" (B2_ERR_BAD_MAGIC) and a bad header write nothing.  All of this holds
+ * however the input is split into reads, and whatever $B2_DEC_WINDOW and $B2_BWTC_DEC_BATCH are.  The input is read only
+ * as far as the decode needs (bytes behind the "no more blocks" marker may stay unread).
+ *
+ * Memory of every BWTC call (b2_stats.dev_peak_bytes for the device), whatever the size of the input:
+ *   compress, device:    B * 96 MiB + 8 MiB, B = $B2_BWT_BATCH blocks (default two per SM): per block the forward BWT
+ *                        (at most 58.5 MiB), the slots, symbols and frequency triples of the model (21 MiB at level 9)
+ *                        and two output windows of b2_bwtc_compress's bound on one batch (2 MiB).  The input is never on
+ *                        the device as a whole: it goes to the batch's slots a batch at a time.
+ *   decompress, device:  W' + B * 17 MiB + 8 MiB, B = $B2_BWTC_DEC_BATCH blocks (default two per SM): per block the L
+ *                        column, the decoded bytes and the inverse BWT (16.4 MiB).  W' is the window of coded bytes,
+ *                        W = $B2_DEC_WINDOW (default 4 GiB, at least 64 KiB), or less for a shorter input; it widens
+ *                        only for a block whose coded bytes do not fit in it, to under twice that block's coded bytes (a
+ *                        coded block is under 1.1 MB).
+ *   compress, host:      one batch of raw input (B * level * 100 000 bytes) and one pinned output buffer of at most
+ *                        b2_bwtc_compress's bound on one batch (B * 1.13 MB at level 9).
+ *   decompress, host:    the input window (W' + 1 bytes) and one pinned batch of decoded bytes (B * 900 000 bytes). */
+int b2_bwtc_decompress_stream(b2_read_fn rd, b2_write_fn wr, void* user);
 /* CRC32 helper object of lib/CRC32.js:72-103 (bzip2 polynomial, MSB first) */
 uint32_t b2_crc32_bzip2(const uint8_t* p, size_t n);
 
