@@ -1,8 +1,10 @@
 // bwtc.cu -- compressjs' BWTC container (lib/BWTC.js:12-231) on the GPU.
 //
-// STATUS: new in round 1.  The serial model / range-coder code (bwtc_core.cuh) is verified on its host build against
-// the oracle (tests/test_host_api.py::test_bwtc_core_matches_oracle); the kernels and the orchestration below are
-// checked against the oracle by tests/test_gpu_zz_bwtc.py.  Not yet measured at BASELINE config 4.
+// The serial model / range-coder code (bwtc_core.cuh) is checked on its host build against the oracle
+// (tests/test_host_api.py::test_bwtc_core_matches_oracle).  The kernels and the orchestration below are checked against
+// the oracle on whole streams (tests/test_gpu_zz_bwtc*.py) and on the designed corpus of tests/bwtc_cases.py, whose
+// inputs reach every rescale, escape, carry, reciprocal correction and batch seam (tests/test_gpu_zz_bwtc_seams.py).
+// The benchmark's `bwtc` leg measures BASELINE config 4 on a 64 MiB slice.
 //
 // Per block the container needs: sentinel BWT (lib/BWT.js:328-350), MTF over the used bytes, zero runs as
 // RUNA/RUNB digits, an adaptive model (Fenwick tree, or the deferred-sum model below level 6) that turns every
@@ -189,7 +191,7 @@ __device__ __forceinline__ void bc_enc_code_fast(bc_enc* rc, u32 sy_f, u32 lt_f,
   bc_enc_normalize(rc);
   u32 r = __umulhi(rc->range, magic);          // floor(range * floor((2^32 - 1) / tot) / 2^32) <= range / tot
   u32 rem = rc->range - r * tot_f;
-  while (rem >= tot_f) { r++; rem -= tot_f; }  // at most two steps
+  while (rem >= tot_f) { r++; rem -= tot_f; }  // at most one step: range <= 2^31 puts r within 1 of range / tot
   const u32 tmp = r * lt_f;
   rc->low += tmp;
   if (lt_f + sy_f < tot_f) rc->range = r * sy_f; else rc->range -= tmp;
@@ -242,7 +244,23 @@ __global__ void k_bwtc_finish(BwtcState* st) {
   bc_enc_finish(&st->rc);
 }
 
+// The coded size of n raw bytes as BWTC streams usually come out (random bytes grow by under 10 %): the size a result
+// buffer or a staging buffer starts with.  Both grow when a stream needs more.
 size_t bwtc_bound(size_t n) { return n + n / 8 + (n / 100000 + 2) * 1024 + 64; }
+
+// The most bytes the coder can write for nb blocks of n raw bytes in all, whatever the data: the size of an output
+// window, which cannot grow while the coder runs.  A raw byte makes at most one symbol (a zero run of length r makes
+// under log2(r + 2) digits) and a symbol at most two triples, an escape and the symbol among the unseen ones.
+// - Fenwick model (levels 6..9): a symbol is coded with sy_f >= 1 and tot_f < 0xFF00 (the tree is rescaled as soon as its
+//   total reaches 0xFF00), under 16 bits; the literal of an escape with tot_f <= 257 unseen symbols, under 8.01 bits.
+// - Deferred-sum model (levels 1..5): tot_f = 256 and sy_f >= 1, at most 8 bits, plus 8.01 bits for the literal.
+// - Range coder: r = floor(range / tot_f) with range > 2^23 and tot_f < 2^16 loses at most log2(1 / (1 - 2^-7)) < 0.0113
+//   bits per triple; its bytes out are the bits coded plus at most 8 bits of `range` over 8.
+// So a raw byte costs under 3 bytes + 0.04 bits at levels 6..9 and 2 bytes + 0.04 bits at levels 1..5: n / 64 bytes
+// cover the fractions.  A block's header (the length, the start index and the used-byte tree: under 900 bits) gets 1 KiB.
+// Random bytes come to 1.096 n at level 9, and ranks built so that every symbol is coded just after its weight was
+// halved to 1.141 n (tests/bwtc_cases.py): more than bwtc_bound gives.
+static size_t bwtc_window_bound(size_t n, size_t nb, int fast) { return (fast ? 2 : 3) * n + n / 64 + nb * 1024 + 64; }
 
 // BWTC.compressFile from a host source into a host sink: b2_bwtc_compress / _unsized (the caller's buffer, complete from
 // the start, into the result buffer) and b2_bwtc_compress_stream (read and write callbacks).  file_size is the size field
@@ -281,7 +299,7 @@ void bwtc_compress(Ctx& c, StreamIn& in, int level, u64 file_size, StreamOut& ou
     triples.alloc(c, (size_t)B * tcap);
   }
   const NarrowSyms nsym{sym_lo, sym_hi, sym_any_hi};
-  const size_t wcap = bwtc_bound((size_t)B * blockSize);     // a window grows only if `help` holds more than its slack
+  const size_t wcap = bwtc_window_bound((size_t)B * blockSize, B, fast);   // grows only if `help` holds more than its slack
   DBuf<u8> win[2];
   size_t cap[2] = {wcap, wcap};
   win[0].alloc(c, wcap);
@@ -311,7 +329,7 @@ void bwtc_compress(Ctx& c, StreamIn& in, int level, u64 file_size, StreamOut& ou
     if (h.overflow) throw B2Error{B2_ERR_CUDA, "internal error: BWTC triple buffer overflow"};
     if (h.rc.n > h.rc.cap) throw B2Error{B2_ERR_CUDA, "internal error: BWTC output window overflow"};
     const size_t bytes = (size_t)h.rc.n;
-    out.reserve(bytes, false, wcap);
+    out.reserve(bytes, false, bwtc_bound((size_t)B * blockSize));   // a staging buffer of the usual size, more if needed
     CUDA_CHECK(cudaMemcpyAsync(out.next(), win[w], bytes, cudaMemcpyDeviceToHost, c.d2h_stream));
     return bytes;
   };
@@ -359,7 +377,7 @@ void bwtc_compress(Ctx& c, StreamIn& in, int level, u64 file_size, StreamOut& ou
       prev = fetch(w ^ 1);
       help = h.rc.help;
     }
-    const size_t need = bwtc_bound(take) + (size_t)help + 16;   // the batch, the bytes held back, the trailer
+    const size_t need = bwtc_window_bound(take, nb, fast) + (size_t)help + 16;   // the batch, the bytes held back, the trailer
     if (need > cap[w]) { win[w].alloc(c, need); cap[w] = need; }
     {
       StageScope s(c, ST_PACK);   // ... and the serial range coder the slot of the bit packer (ms_pack)

@@ -172,15 +172,17 @@ int b2_bwtc_compress_stream(b2_read_fn rd, b2_write_fn wr, void* user, int level
  * Memory of every BWTC call (b2_stats.dev_peak_bytes for the device), whatever the size of the input:
  *   compress, device:    B * 96 MiB + 8 MiB, B = $B2_BWT_BATCH blocks (default two per SM): per block the forward BWT
  *                        (at most 58.5 MiB), the slots, symbols and frequency triples of the model (21 MiB at level 9)
- *                        and two output windows of b2_bwtc_compress's bound on one batch (2 MiB).  The input is never on
- *                        the device as a whole: it goes to the batch's slots a batch at a time.
+ *                        and two output windows of the coder's worst case on one batch (each 3 n, or 2 n at levels
+ *                        1..5, + n / 64 + 1 KiB for a block of n raw bytes: 5.2 MiB for both at level 9).  The input is
+ *                        never on the device as a whole: it goes to the batch's slots a batch at a time.
  *   decompress, device:  W' + B * 17 MiB + 8 MiB, B = $B2_BWTC_DEC_BATCH blocks (default two per SM): per block the L
  *                        column, the decoded bytes and the inverse BWT (16.4 MiB).  W' is the window of coded bytes,
  *                        W = $B2_DEC_WINDOW (default 4 GiB, at least 64 KiB), or less for a shorter input; it widens
  *                        only for a block whose coded bytes do not fit in it, to under twice that block's coded bytes (a
- *                        coded block is under 1.1 MB).
- *   compress, host:      one batch of raw input (B * level * 100 000 bytes) and one pinned output buffer of at most
- *                        b2_bwtc_compress's bound on one batch (B * 1.13 MB at level 9).
+ *                        coded block is under 2.72 MB; the worst one built so far, tests/bwtc_cases.py, has 1.03 MB).
+ *   compress, host:      one batch of raw input (B * level * 100 000 bytes) and one pinned output buffer, which starts at
+ *                        the usual coded size of a batch (B * 1.02 MB at level 9) and grows to a batch's coded bytes
+ *                        only when they are more (B * 2.72 MB at level 9 in the worst case).
  *   decompress, host:    the input window (W' + 1 bytes) and one pinned batch of decoded bytes (B * 900 000 bytes). */
 int b2_bwtc_decompress_stream(b2_read_fn rd, b2_write_fn wr, void* user);
 /* CRC32 helper object of lib/CRC32.js:72-103 (bzip2 polynomial, MSB first) */

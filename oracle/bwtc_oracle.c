@@ -43,6 +43,45 @@ static int get(src_t* s) { return s->pos < s->n ? s->p[s->pos++] : -1; }  /* Str
 
 static int fls32(uint32_t v) { int r = 0; while (v) { r++; v >>= 1; } return r; }  /* Util.js:301-316 */
 
+/* ---- trace (orc_bwtc_compress_trace): counters beside the reference arithmetic, which they never change ---------- */
+typedef struct {
+  uint32_t n, alpha, nsym, ntriples;      /* raw bytes, used bytes, model symbols, coded triples (header included) */
+  uint32_t rescales, rescales_esc;        /* Fenwick rescales; those triggered by the escape step of an escape */
+  uint32_t rescales_ff00, rescales_noesc; /* ... at a total of exactly 0xFF00; ... with noEscape (the escape zeroed) */
+  uint32_t escapes, last_escape;          /* symbols coded through the escape; the last escape (FenwickModel.js:68) */
+  uint32_t reescapes, esc_lane31;         /* escapes of a symbol seen before in the block; escapes at symbol k = 31 mod 32 */
+  uint32_t ds_rebuilds, ds_esc_cap;       /* deferred-sum table rebuilds; escapes not counted as update[esc] is 40 */
+  uint32_t max_tot, carries;              /* largest tot_f; carries into the buffered byte */
+  uint32_t help_carry, help_nocarry;      /* pending 0xFF bytes resolved with a carry (as 0x00) / without (as 0xFF) */
+  uint32_t corr[3];                       /* steps of r = umulhi(range, 0xFFFFFFFF / tot) up to range / tot: 0, 1, 2 */
+  uint32_t max_help;                      /* most bytes pending in the block */
+  uint32_t help_in, resolved_in;          /* bytes pending when the block starts; how they came out: 1 as 0xFF, 2 as 0x00 */
+  uint64_t help, bytes_out, bytecount;    /* the coder after the block's last triple: pending, stream bytes, bytecount */
+} orc_bwtc_block_t;
+typedef struct {
+  uint32_t nblocks, max_help;
+  uint32_t first_carry;                   /* the coder's first byte out (the size field's last group) carried */
+  uint32_t finish_carry, finish_round;    /* finish: tmp > 0xFF; the rounding rule added one */
+  uint32_t corr2;                         /* two correction steps anywhere in the file */
+  uint64_t coder_bytes, bytecount;        /* bytes the coder put out; bytecount in the trailer */
+} orc_bwtc_file_t;
+static _Thread_local orc_bwtc_block_t* TRB;   /* the block being coded, or a scratch record outside blocks */
+static _Thread_local orc_bwtc_file_t* TRF;
+static _Thread_local uint8_t TR_SEEN[260];
+#define TRC(x) do { if (TRB) { x; } } while (0)
+static void tr_put(int carry) {
+  if (!TRF) return;
+  if (TRF->coder_bytes++ == 0) TRF->first_carry = (uint32_t)carry;
+}
+static void tr_tot(uint32_t range, uint32_t tot) {
+  TRB->ntriples++;
+  if (tot > TRB->max_tot) TRB->max_tot = tot;
+  const uint32_t r0 = (uint32_t)(((uint64_t)range * (0xFFFFFFFFu / tot)) >> 32);
+  const uint32_t k = range / tot - r0;
+  TRB->corr[k < 2 ? k : 2]++;
+  if (k >= 2) TRF->corr2++;
+}
+
 /* ---- range coder (RangeCoder.js) ---------------------------------------------------------------- */
 #define TOP_VALUE 0x80000000u      /* 2^(CODE_BITS-1), :15 */
 #define SHIFT_BITS 23              /* :16 */
@@ -63,15 +102,19 @@ static void enc_start(rc_t* rc, sink_t* out, uint32_t c, uint32_t initlength) { 
 static void enc_normalize(rc_t* rc) {  /* :40-61 */
   while (rc->range <= BOTTOM_VALUE) {
     if (rc->low < (0xFFu << SHIFT_BITS)) {
+      TRC(tr_put(0); if (rc->help) TRB->help_nocarry++; if (TRB->help_in && !TRB->resolved_in) TRB->resolved_in = 1);
       put(rc->out, rc->buffer);
       for (; rc->help; rc->help--) put(rc->out, 0xFF);
       rc->buffer = (rc->low >> SHIFT_BITS) & 0xFF;
     } else if (rc->low & TOP_VALUE) {
+      TRC(tr_put(1); TRB->carries++; if (rc->help) TRB->help_carry++; if (TRB->help_in && !TRB->resolved_in) TRB->resolved_in = 2);
       put(rc->out, rc->buffer + 1);
       for (; rc->help; rc->help--) put(rc->out, 0x00);
       rc->buffer = (rc->low >> SHIFT_BITS) & 0xFF;
     } else {
       rc->help++;
+      TRC(if (rc->help > TRB->max_help) TRB->max_help = (uint32_t)rc->help;
+          if (rc->help > TRF->max_help) TRF->max_help = (uint32_t)rc->help);
     }
     rc->range <<= 8;
     rc->low = (rc->low << 8) & (TOP_VALUE - 1);
@@ -80,6 +123,7 @@ static void enc_normalize(rc_t* rc) {  /* :40-61 */
 }
 static void enc_freq(rc_t* rc, uint32_t sy_f, uint32_t lt_f, uint32_t tot_f) {  /* :81-91 */
   enc_normalize(rc);
+  TRC(tr_tot(rc->range, tot_f));
   const uint32_t r = rc->range / tot_f;
   const uint32_t tmp = r * lt_f;
   rc->low += tmp;
@@ -87,6 +131,7 @@ static void enc_freq(rc_t* rc, uint32_t sy_f, uint32_t lt_f, uint32_t tot_f) {  
 }
 static void enc_shift(rc_t* rc, uint32_t sy_f, uint32_t lt_f, uint32_t shift) {  /* :92-102 */
   enc_normalize(rc);
+  TRC(tr_tot(rc->range, 1u << shift));
   const uint32_t r = rc->range >> shift;
   const uint32_t tmp = r * lt_f;
   rc->low += tmp;
@@ -98,7 +143,8 @@ static void enc_finish(rc_t* rc) {  /* :118-144 */
   enc_normalize(rc);
   rc->bytecount += 5;
   uint32_t tmp = rc->low >> SHIFT_BITS;
-  if ((rc->low & (BOTTOM_VALUE - 1)) >= ((rc->bytecount & 0xFFFFFF) >> 1)) tmp++;
+  if ((rc->low & (BOTTOM_VALUE - 1)) >= ((rc->bytecount & 0xFFFFFF) >> 1)) { tmp++; TRC(TRF->finish_round = 1); }
+  TRC(TRF->finish_carry = tmp > 0xFF; TRF->bytecount = rc->bytecount; tr_put(tmp > 0xFF));
   if (tmp > 0xFF) {
     put(rc->out, rc->buffer + 1);
     for (; rc->help; rc->help--) put(rc->out, 0x00);
@@ -196,6 +242,7 @@ static void fen_rescale(fen_t* f) {  /* :125-154 */
     if (prob == 0) { prob = 1; noEscape = 0; }
     f->tree[f->numSyms + i] = prob;
   }
+  TRC(TRB->rescales++; TRB->rescales_noesc += noEscape);
   prob = f->tree[f->numSyms + i];
   prob = (prob & SCALE_MASK) >> 1;
   if (noEscape) prob = 0; else if (prob == 0) prob = 1u << 16;
@@ -208,10 +255,12 @@ static void fen_encode(fen_t* f, uint32_t symbol) {  /* :47-87 */
   uint32_t mask = SYM_MASK, shift = 16;
   uint32_t update = f->increment << 16;
   if ((sy_f & SYM_MASK) == 0) {                       /* not seen yet: escape first, then code it among the unseen */
+    TRC(TRB->escapes++; TRB->reescapes += TR_SEEN[symbol]; TR_SEEN[symbol] = 1; TRB->esc_lane31 += (TRB->nsym - 1) % 32 == 31);
     fen_encode(f, f->numSyms - 1);
     mask = ESC_MASK; update -= 1; shift = 0;
   } else if (symbol == f->numSyms - 1 && (f->tree[1] & ESC_MASK) == 1) {
     update = 0u - f->tree[i];                          /* the last escape: zero it out */
+    TRC(TRB->last_escape++);
   }
   uint32_t lt_f = 0;
   while (i > 1) {
@@ -226,6 +275,9 @@ static void fen_encode(fen_t* f, uint32_t symbol) {  /* :47-87 */
   lt_f = (lt_f & mask) >> shift;
   tot_f = (tot_f & mask) >> shift;
   enc_freq(f->rc, sy_f, lt_f, tot_f);
+  TRC(if (((f->tree[1] & SYM_MASK) >> 16) >= f->max_prob) {
+        TRB->rescales_esc += symbol == f->numSyms - 1;
+        TRB->rescales_ff00 += ((f->tree[1] & SYM_MASK) >> 16) == f->max_prob; });
   if (((f->tree[1] & SYM_MASK) >> 16) >= f->max_prob) fen_rescale(f);
 }
 static uint32_t fen_decode1(fen_t* f, int isEscape) {  /* :88-123 */
@@ -275,12 +327,13 @@ static void dsm_init(dsm_t* m, rc_t* rc, uint32_t size) {  /* :11-35 */
 }
 static void dsm_update(dsm_t* m, uint32_t symbol) {  /* :39-93 (the decoder's lookup tables are searched instead) */
   if (symbol == m->numSyms) {
-    if (m->update[symbol] >= DS_MAX_ESCAPE) return;
+    if (m->update[symbol] >= DS_MAX_ESCAPE) { TRC(TRB->ds_esc_cap++); return; }
     if (m->updateCount >= m->updateThresh - 1) return;   /* an escape never triggers the table rebuild */
   }
   m->update[symbol]++;
   m->updateCount++;
   if (m->updateCount < m->updateThresh) return;
+  TRC(TRB->ds_rebuilds++);
   uint32_t cumProb = 0, cumEscProb = 0, odd = 0, i;
   m->escape[0] = 0; m->prob[0] = 0;
   for (i = 0; i < m->numSyms + 1; i++) {
@@ -299,6 +352,7 @@ static void dsm_update(dsm_t* m, uint32_t symbol) {  /* :39-93 (the decoder's lo
 static void dsm_encode(dsm_t* m, uint32_t symbol) {  /* :94-111 */
   uint32_t lt_f = m->prob[symbol], sy_f = m->prob[symbol + 1] - lt_f;
   if (sy_f) { enc_shift(m->rc, sy_f, lt_f, DS_LOG_TOTAL); dsm_update(m, symbol); return; }
+  TRC(TRB->escapes++; TRB->reescapes += TR_SEEN[symbol]; TR_SEEN[symbol] = 1; TRB->esc_lane31 += (TRB->nsym - 1) % 32 == 31);
   dsm_encode(m, m->numSyms);                            /* escape, then the symbol among the escaping ones */
   lt_f = m->escape[symbol];
   sy_f = m->escape[symbol + 1] - lt_f;
@@ -328,8 +382,13 @@ static uint32_t dsm_decode(dsm_t* m) {  /* :112-131 */
 #define F_PROB_MAX 0xFF00u   /* BWTC.js:7 */
 #define F_PROB_INCR 0x0100u  /* BWTC.js:8 */
 
-/* BWTC.compressFile(input, output, level) for a buffer input of known size (Util.js:105-141: the size is written). */
-ORC_EXPORT int orc_bwtc_compress(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n) {
+/* BWTC.compressFile(input, output, level) for a buffer input of known size (Util.js:105-141: the size is written).
+ * With `blocks` (room for `cap` records) and `file`, also the trace of every block and of the file. */
+static int bwtc_compress(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n, orc_bwtc_block_t* blocks,
+                         size_t cap, orc_bwtc_file_t* file) {
+  orc_bwtc_block_t scratch;
+  memset(&scratch, 0, sizeof scratch);
+  if (file) { memset(file, 0, sizeof *file); TRF = file; TRB = &scratch; }
   if (level < 1 || level > 9) level = 9;      /* BWTC.js:16-19: anything else means 9 */
   const int fast = level <= 5;                /* :22 */
   sink_t o = {0, 0, 0, 0};
@@ -348,7 +407,7 @@ ORC_EXPORT int orc_bwtc_compress(const uint8_t* in, size_t n, int level, uint8_t
   uint8_t* U = (uint8_t*)malloc(blockSize ? blockSize : 1);
   fen_t* model = (fen_t*)malloc(sizeof(fen_t));
   dsm_t* dmodel = (dsm_t*)malloc(sizeof(dsm_t));
-  if (!U || !model || !dmodel) { free(U); free(model); free(dmodel); free(o.p); return -6; }
+  if (!U || !model || !dmodel) { TRB = NULL; TRF = NULL; free(U); free(model); free(dmodel); free(o.p); return -6; }
   logdist_t lenModel;
   logdist_init(&lenModel, blockSize);                                             /* :40-42 */
   size_t pos = 0;
@@ -358,6 +417,14 @@ ORC_EXPORT int orc_bwtc_compress(const uint8_t* in, size_t n, int level, uint8_t
     if (length == 0) break;
     const uint8_t* b = in + pos;
     pos += length;
+    if (file) {
+      TRB = file->nblocks < cap ? &blocks[file->nblocks] : &scratch;
+      memset(TRB, 0, sizeof *TRB);
+      memset(TR_SEEN, 0, sizeof TR_SEEN);
+      TRB->n = length;
+      TRB->help_in = (uint32_t)rc.help;
+      file->nblocks++;
+    }
     if (length == blockSize) enc_freq(&rc, 1, 0, 3);                               /* :50-52 */
     else { enc_freq(&rc, 1, 1, 3); logdist_encode(&lenModel, &rc, length); }       /* :54-55 */
     const uint32_t pidx = (uint32_t)orc_bwt_sentinel(b, U, (int32_t)length);       /* :58 (returns pidx + 1) */
@@ -376,6 +443,7 @@ ORC_EXPORT int orc_bwtc_compress(const uint8_t* in, size_t n, int level, uint8_t
     uint8_t M[256];
     uint32_t alphabetSize = 0;
     for (uint32_t i = 0; i < 256; i++) if (useTree[256 + i]) M[alphabetSize++] = (uint8_t)i;   /* :85-90 */
+    TRC(TRB->alpha = alphabetSize);
     for (uint32_t i = 0; i < length; i++) {                                        /* :93-107 MTF */
       const uint8_t c = U[i];
       uint32_t j = 0;
@@ -386,7 +454,7 @@ ORC_EXPORT int orc_bwtc_compress(const uint8_t* in, size_t n, int level, uint8_t
     }
     if (fast) dsm_init(dmodel, &rc, alphabetSize + 1);                             /* :111 */
     else fen_init(model, &rc, alphabetSize + 1, F_PROB_MAX, F_PROB_INCR);          /* :109-110 */
-#define MODEL_ENCODE(sym) do { if (fast) dsm_encode(dmodel, (sym)); else fen_encode(model, (sym)); } while (0)
+#define MODEL_ENCODE(sym) do { TRC(TRB->nsym++); if (fast) dsm_encode(dmodel, (sym)); else fen_encode(model, (sym)); } while (0)
     uint32_t runLength = 0;
     for (uint32_t i = 0; i <= length; i++) {                                       /* :112-137; i == length flushes */
       const uint32_t c = i < length ? U[i] : 1u;
@@ -399,13 +467,22 @@ ORC_EXPORT int orc_bwtc_compress(const uint8_t* in, size_t n, int level, uint8_t
       if (i < length) MODEL_ENCODE(c + 1);
     }
 #undef MODEL_ENCODE
+    TRC(TRB->help = rc.help; TRB->bytes_out = o.n; TRB->bytecount = rc.bytecount; TRB = &scratch);
   } while (length == blockSize);                                                   /* :139 */
   enc_freq(&rc, 1, 2, 3);                                                           /* :141 */
   enc_finish(&rc);
+  TRB = NULL; TRF = NULL;
   free(U); free(model); free(dmodel);
   if (o.oom) { free(o.p); return -6; }
   *out = o.p; *out_n = o.n;
   return 0;
+}
+ORC_EXPORT int orc_bwtc_compress(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n) {
+  return bwtc_compress(in, n, level, out, out_n, NULL, 0, NULL);
+}
+ORC_EXPORT int orc_bwtc_compress_trace(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n,
+                                       orc_bwtc_block_t* blocks, size_t cap, orc_bwtc_file_t* file) {
+  return bwtc_compress(in, n, level, out, out_n, blocks, cap, file);
 }
 
 /* BWTC.decompressFile(input) (BWTC.js:141-231).  Returns 0, -2 for a bad magic ("Bad magic", Util.js:151-153),

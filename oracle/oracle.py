@@ -28,6 +28,22 @@ class BlockTrace(C.Structure):
                 ("bit_len", C.c_uint64)]
 
 
+class BwtcBlockTrace(C.Structure):
+    """orc_bwtc_block_t (bwtc_oracle.c): counters of one block of orc_bwtc_compress_trace."""
+    _fields_ = [(f, C.c_uint32) for f in ("n", "alpha", "nsym", "ntriples", "rescales", "rescales_esc", "rescales_ff00",
+                                          "rescales_noesc", "escapes", "last_escape", "reescapes", "esc_lane31",
+                                          "ds_rebuilds", "ds_esc_cap", "max_tot", "carries", "help_carry", "help_nocarry")] + \
+        [("corr", C.c_uint32 * 3), ("max_help", C.c_uint32), ("help_in", C.c_uint32), ("resolved_in", C.c_uint32),
+         ("help", C.c_uint64), ("bytes_out", C.c_uint64),
+         ("bytecount", C.c_uint64)]
+
+
+class BwtcFileTrace(C.Structure):
+    """orc_bwtc_file_t (bwtc_oracle.c)."""
+    _fields_ = [(f, C.c_uint32) for f in ("nblocks", "max_help", "first_carry", "finish_carry", "finish_round", "corr2")] + \
+        [("coder_bytes", C.c_uint64), ("bytecount", C.c_uint64)]
+
+
 def lib():
     global _LIB
     if _LIB is None:
@@ -60,6 +76,8 @@ def lib():
         L.orc_free.argtypes = [C.c_void_p]
         L.orc_bwtc_compress.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.POINTER(u8p), szp]
         L.orc_bwtc_decompress.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(u8p), szp]
+        L.orc_bwtc_compress_trace.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.POINTER(u8p), szp, C.c_void_p, C.c_size_t,
+                                              C.POINTER(BwtcFileTrace)]
         _LIB = L
     return _LIB
 
@@ -214,14 +232,22 @@ def compress_block_stages(block, legacy_sort=False):
                 lens=lens.reshape(6, 258)[:tr.ngroups, :tr.alpha + 2].copy(), bits=bits, nbits=nbits.value)
 
 
-def bwtc_compress(data, level=9):
-    """BWTC.compressFile (lib/BWTC.js:12-139)."""
+def bwtc_compress(data, level=9, trace=False):
+    """BWTC.compressFile (lib/BWTC.js:12-139).  With `trace`: (stream, [BwtcBlockTrace per block], BwtcFileTrace)."""
     L = lib()
     a, p = _buf(data)
     out, n = C.POINTER(C.c_uint8)(), C.c_size_t()
-    rc = L.orc_bwtc_compress(p, a.size, level, C.byref(out), C.byref(n))
+    if trace:
+        bs = (level if 1 <= level <= 9 else 9) * 100000
+        cap = a.size // bs + 1
+        tr, ft = (BwtcBlockTrace * cap)(), BwtcFileTrace()
+        rc = L.orc_bwtc_compress_trace(p, a.size, level, C.byref(out), C.byref(n), tr, cap, C.byref(ft))
+    else:
+        rc = L.orc_bwtc_compress(p, a.size, level, C.byref(out), C.byref(n))
     if rc:
         raise OracleError(rc, "bwtc compress failed")
+    if trace:
+        return _take(L, out, n), [tr[i] for i in range(ft.nblocks)], ft
     return _take(L, out, n)
 
 

@@ -86,27 +86,37 @@ def zero_runs(ranks):
     return s, e - s
 
 
-def lf(L):
+def _rows(L, sentinel):
+    """The column's rows: L itself, or for the sentinel BWT (BWTC) the n + 1 rows with the sentinel, below every byte,
+    at row `sentinel` (the start index the encoder writes)."""
+    return L if sentinel is None else np.insert(np.asarray(L, np.int16), sentinel, -1)
+
+
+def lf(L, sentinel=None):
+    L = _rows(L, sentinel)
     order = np.argsort(L, kind="stable")
     out = np.empty(L.size, np.int64)
     out[order] = np.arange(L.size)
     return out
 
 
-def cycles(L):
-    n = L.size
-    g = csr_matrix((np.ones(n, np.int8), (np.arange(n), lf(L))), shape=(n, n))
+def cycles(L, sentinel=None):
+    n = L.size + (sentinel is not None)
+    g = csr_matrix((np.ones(n, np.int8), (np.arange(n), lf(L, sentinel))), shape=(n, n))
     return connected_components(g, directed=True, connection="strong")
 
 
-def merge_cycles(L, protect=None):
-    """One-cycle column close to L.  Returns (column, adjacent swaps)."""
+def merge_cycles(L, protect=None, sentinel=None):
+    """One-cycle column close to L (with the sentinel at row `sentinel`, which stays there).  Returns (column, adjacent
+    swaps)."""
     L = L.copy()
     swaps = 0
     while True:
-        k, lab = cycles(L)
+        k, lab = cycles(L, sentinel)
         if k == 1:
             return L, swaps
+        if sentinel is not None:
+            lab = np.delete(lab, sentinel)
         parent = list(range(k))
 
         def find(a):
@@ -116,6 +126,8 @@ def merge_cycles(L, protect=None):
             return a
 
         diff = (L[:-1] != L[1:]) & (lab[:-1] != lab[1:])
+        if sentinel is not None and 0 < sentinel < L.size:
+            diff[sentinel - 1] = False     # rows sentinel - 1 and sentinel + 1 are not adjacent in the full column
         did = 0
         tries = [diff & ~protect[:-1] & ~protect[1:], diff] if protect is not None else [diff]
         for cand in tries:
