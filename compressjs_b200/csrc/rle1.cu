@@ -13,10 +13,15 @@
 //   C  k_rle_blocks  : one CTA walks the blocks: a block that starts in the middle of a run
 //                      re-phases that run (fresh state), everything behind it follows W; the
 //                      end is found by a 256-ary search over W(tile) plus one in-tile scan.
-//   D  k_rle_emit    : all blocks in parallel: every raw byte computes its output position and
-//                      writes its literal (+ count byte) into the slot layout.
-//   CRC k_crc_pieces : 256-byte pieces, pure polynomial remainders shifted by x^(8*bytes after)
-//                      and XOR-combined per block (CRC is linear), then the init/final XOR.
+//   D  k_rle_emit    : one CTA per span of up to 4 tiles of one block (a per-CTA map gives the block, no
+//                      search): the span's raw bytes are staged in shared memory, a run of plain tiles is
+//                      copied out as destination-aligned 16-byte words (funnel shifts), every raw byte of
+//                      another tile computes its output position and writes its literal (+ count byte).
+//                      The same pass folds the block CRC: every thread takes the pure polynomial remainder
+//                      of 64 staged bytes (slicing by 4), shifts it by x^(8*bytes after it in the span),
+//                      the CTA XOR-reduces them and adds the span to the block's accumulators (CRC is
+//                      linear); k_crc_final applies the init/final XOR.
+//   CRC k_crc_pieces : the same remainders over 256-byte pieces of arbitrary byte ranges (decoder, b2_crc32).
 #include <algorithm>
 #include <cstdlib>
 #include "enc.h"
@@ -640,69 +645,133 @@ k_rle_blocks(const u8* __restrict__ in, u64 N, u32 BS, const u32* __restrict__ c
   if (tid == 0) *nblocks_out = k;
 }
 
-// ---- D ---------------------------------------------------------------------------------
-__global__ void __launch_bounds__(RT_THREADS)
-k_rle_emit(const u8* __restrict__ in, u64 N, const u32* __restrict__ carry, const u64* __restrict__ prefix, const u8* __restrict__ plain,
-           const BlkInfo* __restrict__ blocks, u32 first, u32 count, const u64* __restrict__ tile_base, u8* __restrict__ T) {
-  __shared__ TileScratch sc;
-  __shared__ u32 s_k;
-  __shared__ __align__(16) u8 stage[RLE_TILE + 32];
-  // which block does this CTA work for?  tile_base[k] = first CTA of block (first+k)
-  if (threadIdx.x == 0) {
-    u32 lo = 0, hi = count;
-    while (hi - lo > 1) {
-      u32 mid = (lo + hi) >> 1;
-      if (tile_base[mid] <= blockIdx.x) lo = mid; else hi = mid;
-    }
-    s_k = lo;
+// ---- CRC constants ---------------------------------------------------------------------------
+// The block CRC is linear: the pure polynomial remainder R (no init, no final XOR) of a byte string is the XOR of the
+// remainders of its pieces, each multiplied by x^(8 * bytes after the piece); leading zero bytes add nothing.
+#define CRC_POLY 0x04c11db7u
+__host__ __device__ __forceinline__ u32 gf_mulmod(u32 a, u32 b) {
+  u32 r = 0;
+  for (int i = 31; i >= 0; i--) {
+    r = (r << 1) ^ ((r & 0x80000000u) ? CRC_POLY : 0u);
+    if ((b >> i) & 1) r ^= a;
   }
-  __syncthreads();
-  const u32 kk = s_k;
-  const BlkInfo bi = blocks[first + kk];
-  const u64 t = bi.s / RLE_TILE + (blockIdx.x - tile_base[kk]);
-  const u64 tstart = t * RLE_TILE;
-  u8* Tb = T + ((size_t)kk << SEG_SHIFT);
-  const u64 Pt = prefix[t];
-  if (plain[t]) {
-    // No run reaches four bytes in or into this tile: every raw byte emits itself (w = 1), whatever the phase, so the
-    // tile's part of the block is a byte copy to output position (x - x0) + o0.  Staged in shared memory at the
-    // destination's alignment, stored 16 bytes at a time.
-    const u64 remain = N - tstart;
-    const u32 len = remain < RLE_TILE ? (u32)remain : RLE_TILE;
-    const u64 x0 = bi.s > tstart ? bi.s : tstart;                                    // first raw byte of the block in this tile
-    const u64 x1 = (bi.e < tstart + len) ? bi.e : tstart + len;
-    if (x0 >= x1) return;
-    // output position of x0 (same formulas as the general path below, with w = 1 everywhere)
-    const u64 o0 = x0 < bi.b ? (x0 - bi.s) : (u64)bi.ofs + (Pt + (x0 - tstart) - bi.Wb);
-    if (o0 >= bi.n) return;
-    const u32 cnt = (u32)min((u64)(x1 - x0), (u64)bi.n - o0);
-    const u32 fo = (u32)(o0 & 15u);
-    const u8* src = in + x0;
-    for (u32 i = threadIdx.x * 16u; i < cnt; i += RT_THREADS * 16u) {
-      if (i + 16u <= cnt && ((((size_t)src) + i) & 15u) == 0) {
-        const uint4 q = *reinterpret_cast<const uint4*>(src + i);
-        const u32 a[4] = {q.x, q.y, q.z, q.w};
+  return r;
+}
+#define EMIT_TILES 4                       // raw tiles of one block per k_rle_emit CTA
+#define EMIT_SPAN (EMIT_TILES * RLE_TILE)
+#define EMIT_SEG 64                        // raw bytes of the span whose remainder one emit thread computes
+static_assert(EMIT_SEG * RT_THREADS == EMIT_SPAN, "every emit thread takes one segment of the span");
+// x^(8 * RLE_TILE * k) for every k a block can need.  RLE1 turns at most 51 raw bytes into one output byte (a run of
+// 255 equal bytes, the costliest, emits 5), and a block's output stops at most one count byte past blockSize, so at
+// level 9 a block spans at most 51 * 899982 = 45,899,082 raw bytes, and e / RLE_TILE - s / RLE_TILE <= 11206 tile
+// edges.  rle1_materialize checks every block against the table's size.
+#define CRC_TILE_POWS 11264
+struct CrcConsts {
+  u32 slice[4][256];  // slice[0] = byte table; slice[k][i] = slice[k-1][i] after one more zero byte (slicing by 4)
+  u32 pow[48];        // pow[i] = x^(8 * 2^i) mod P
+  u32 pow_byte[EMIT_SEG + 1];            // x^(8 * r), r = 0..EMIT_SEG
+  u32 pow_seg[EMIT_SPAN / EMIT_SEG];     // x^(8 * EMIT_SEG * m)
+  u32 pow_tile[CRC_TILE_POWS];           // x^(8 * RLE_TILE * k)
+};
+static void make_crc_consts(CrcConsts& c) {
+  for (u32 i = 0; i < 256; i++) {
+    u32 v = i << 24;
+    for (int k = 0; k < 8; k++) v = (v & 0x80000000u) ? (v << 1) ^ CRC_POLY : (v << 1);
+    c.slice[0][i] = v;
+  }
+  for (int k = 1; k < 4; k++)
+    for (u32 i = 0; i < 256; i++) {
+      const u32 prev = c.slice[k - 1][i];
+      c.slice[k][i] = (prev << 8) ^ c.slice[0][prev >> 24];
+    }
+  c.pow[0] = 0x100;  // x^8
+  for (int i = 1; i < 48; i++) c.pow[i] = gf_mulmod(c.pow[i - 1], c.pow[i - 1]);
+  c.pow_byte[0] = 1u;  // bit i of a register value is the coefficient of x^i, so the polynomial 1 is 0x1
+  for (int r = 1; r <= EMIT_SEG; r++) c.pow_byte[r] = gf_mulmod(c.pow_byte[r - 1], c.pow[0]);
+  c.pow_seg[0] = 1u;
+  for (int m = 1; m < EMIT_SPAN / EMIT_SEG; m++) c.pow_seg[m] = gf_mulmod(c.pow_seg[m - 1], c.pow_byte[EMIT_SEG]);
+  const u32 xtile = c.pow[12];  // 2^12 = RLE_TILE bytes
+  c.pow_tile[0] = 1u;
+  for (int k = 1; k < CRC_TILE_POWS; k++) c.pow_tile[k] = gf_mulmod(c.pow_tile[k - 1], xtile);
+}
+static_assert(RLE_TILE == 1 << 12, "pow_tile is built from pow[12]");
+// in global memory: the tables are read at per-thread indices, which constant memory would serialise
+__device__ CrcConsts g_crc;
+static bool g_crc_ready = false;
+static void crc_setup() {
+  if (g_crc_ready) return;
+  static CrcConsts h;
+  make_crc_consts(h);
+  CUDA_CHECK(cudaMemcpyToSymbol(g_crc, &h, sizeof h));
+  g_crc_ready = true;
+}
+// x^(8*bytes) mod P
+__device__ __forceinline__ u32 crc_xpow(u64 bytes) {
+  u32 r = 1u;
+  for (int i = 0; bytes; i++, bytes >>= 1)
+    if (bytes & 1) r = gf_mulmod(r, g_crc.pow[i]);
+  return r;
+}
+// every thread of the CTA copies the four slicing tables to shared memory (blockDim.x == 256)
+__device__ __forceinline__ void crc_load_tables(u32 (*tab)[256]) {
 #pragma unroll
-        for (int j = 0; j < 16; j++) stage[fo + i + j] = (u8)(a[j >> 2] >> ((j & 3) * 8));
-      } else {
-        const u32 e = min(i + 16u, cnt);
-        for (u32 x = i; x < e; x++) stage[fo + x] = src[x];
-      }
+  for (int k = 0; k < 4; k++) tab[k][threadIdx.x] = g_crc.slice[k][threadIdx.x];
+}
+// four message bytes per dependent step: w holds them little-endian, and the stream is MSB first
+__device__ __forceinline__ u32 crc_step4(u32 crc, u32 w, const u32 (*tab)[256]) {
+  const u32 x = crc ^ __byte_perm(w, 0, 0x0123);
+  return tab[3][x >> 24] ^ tab[2][(x >> 16) & 0xff] ^ tab[1][(x >> 8) & 0xff] ^ tab[0][x & 0xff];
+}
+__device__ __forceinline__ u32 crc_step1(u32 crc, u32 byte, const u32 (*tab)[256]) { return (crc << 8) ^ tab[0][((crc >> 24) ^ byte) & 0xff]; }
+
+// ---- D ---------------------------------------------------------------------------------
+// One CTA per span of up to EMIT_TILES tiles of one block; map[CTA] = (block, span index inside the block).
+// The span's raw bytes are staged in shared memory, 16 per word: word w (span offset 16 w, w >= -8) lives at
+// stage[emit_sw(w)].  The swizzle keeps both access patterns free of bank conflicts: eight threads reading eight
+// consecutive words, and eight threads reading word j of eight consecutive EMIT_SEG-byte segments.
+#define EMIT_STAGE_WORDS (EMIT_SPAN / 16 + 16)
+__device__ __forceinline__ u32 emit_sw(int w) {
+  const u32 v = (u32)(w + 8);
+  return v ^ ((v >> 3) & 3);
+}
+__device__ __forceinline__ u32 stage_byte(const uint4* stage, u32 p) {
+  return reinterpret_cast<const u8*>(stage)[16 * emit_sw((int)(p >> 4)) + (p & 15)];
+}
+// 16 raw bytes at `off` (zero past N), with aligned 16-byte loads when the buffer allows them
+__device__ __forceinline__ uint4 load16(const u8* __restrict__ in, u64 N, u64 off) {
+  const u8* p = in + off;
+  if (off + 16 <= N && (((size_t)p) & 15) == 0) return *reinterpret_cast<const uint4*>(p);
+  u32 a[4] = {0, 0, 0, 0};
+  for (u32 j = 0; j < 16 && off + j < N; j++) a[j >> 2] |= (u32)p[j] << (8 * (j & 3));
+  return make_uint4(a[0], a[1], a[2], a[3]);
+}
+// A run of plain tiles: raw span bytes [ra, ra + cnt) go to output bytes [o0, o0 + cnt) of Tb.  Every thread builds
+// destination-aligned 16-byte words from two staged words with funnel shifts; only the two edge words go byte by byte.
+__device__ void emit_copy(const uint4* stage, u32 ra, u64 o0, u32 cnt, u8* __restrict__ Tb) {
+  const u32 fo = (u32)(o0 & 15u);
+  const int delta = (int)ra - (int)fo;  // span offset of the first byte of destination word 0
+  const int wq = delta >> 4;            // floor
+  const u32 sh = (u32)delta & 15u, q = sh >> 2, bs = 8 * (sh & 3);
+  const u32 end = fo + cnt, nw = (end + 15) >> 4;
+  u8* dst = Tb + (o0 - fo);  // 16-byte aligned
+  for (u32 k = threadIdx.x; k < nw; k += RT_THREADS) {
+    const u32 b0 = 16 * k;
+    if (b0 >= fo && b0 + 16 <= end) {
+      const uint4 lo = stage[emit_sw(wq + (int)k)], hi = stage[emit_sw(wq + (int)k + 1)];
+      const u32 a[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+      u32 b[5];
+#pragma unroll
+      for (int j = 0; j < 5; j++) b[j] = q == 0 ? a[j] : q == 1 ? a[j + 1] : q == 2 ? a[j + 2] : a[j + 3];
+      *reinterpret_cast<uint4*>(dst + b0) = make_uint4(__funnelshift_r(b[0], b[1], bs), __funnelshift_r(b[1], b[2], bs),
+                                                       __funnelshift_r(b[2], b[3], bs), __funnelshift_r(b[3], b[4], bs));
+    } else {
+      for (u32 x = max(b0, fo); x < min(b0 + 16, end); x++) dst[x] = (u8)stage_byte(stage, (u32)(delta + (int)x));
     }
-    __syncthreads();
-    const u32 last = fo + cnt;
-    u8* dst = Tb + (o0 - fo);   // 16-byte aligned
-    for (u32 c16 = threadIdx.x * 16u; c16 < last; c16 += RT_THREADS * 16u) {
-      if (c16 >= fo && c16 + 16u <= last) *reinterpret_cast<uint4*>(dst + c16) = *reinterpret_cast<const uint4*>(stage + c16);
-      else {
-        const u32 e = min(c16 + 16u, last);
-        for (u32 x = max(c16, fo); x < e; x++) dst[x] = stage[x];
-      }
-    }
-    return;
   }
-  TileView v;
-  tile_view(in, N, tstart, carry[t], sc, v);
+}
+// A tile with runs of four or more: every raw byte of the thread computes its output position and writes its literal
+// (+ count byte).
+__device__ void emit_general(const u8* __restrict__ in, const BlkInfo& bi, u64 tstart, u64 Pt, const TileView& v, u8* __restrict__ Tb) {
   u32 run = v.excl;
   for (u32 j = 0; j < v.cnt; j++) {
     const u64 x = tstart + threadIdx.x * RT_PER + j;
@@ -734,54 +803,111 @@ k_rle_emit(const u8* __restrict__ in, u64 N, const u32* __restrict__ carry, cons
     }
   }
 }
-
-// ---- CRC ---------------------------------------------------------------------------------
-#define CRC_POLY 0x04c11db7u
-__host__ __device__ __forceinline__ u32 gf_mulmod(u32 a, u32 b) {
-  u32 r = 0;
-  for (int i = 31; i >= 0; i--) {
-    r = (r << 1) ^ ((r & 0x80000000u) ? CRC_POLY : 0u);
-    if ((b >> i) & 1) r ^= a;
+// Emits the span's part [X0, X1) of the block and folds the CRC of those raw bytes (all of them, also run bytes that
+// emit nothing and bytes past the block's output length) into acc, in the layout k_crc_final reads with unit RLE_TILE.
+// 40 registers (no spills), 21 KiB of shared memory: six CTAs per SM
+__global__ void __launch_bounds__(RT_THREADS, 6)
+k_rle_emit(const u8* __restrict__ in, u64 N, const u32* __restrict__ carry, const u64* __restrict__ prefix, const u8* __restrict__ plain,
+           const BlkInfo* __restrict__ blocks, u32 first, const uint2* __restrict__ map, u8* __restrict__ T, u32* __restrict__ acc) {
+  __shared__ __align__(16) uint4 stage[EMIT_STAGE_WORDS];
+  __shared__ u32 tab[4][256];
+  __shared__ TileScratch sc;
+  __shared__ u32 red[RT_THREADS / 32 + 1];
+  const u32 tid = threadIdx.x;
+  crc_load_tables(tab);
+  const uint2 m = map[blockIdx.x];
+  const BlkInfo bi = blocks[first + m.x];
+  const u64 t0 = bi.s / RLE_TILE + (u64)m.y * EMIT_TILES;
+  const u32 ntl = (u32)min((u64)EMIT_TILES, (bi.e - 1) / RLE_TILE - t0 + 1);
+  const u64 sstart = t0 * RLE_TILE;
+  const u64 X0 = max(bi.s, sstart), X1 = min(bi.e, sstart + (u64)ntl * RLE_TILE);
+  u8* Tb = T + ((size_t)m.x << SEG_SHIFT);
+  u32 pmask = 0;
+#pragma unroll
+  for (u32 i = 0; i < EMIT_TILES; i++)
+    if (i < ntl && plain[t0 + i]) pmask |= 1u << i;
+  // 1. stage the raw bytes; tiles with long runs are emitted here, from their TileView
+  uint4 q[EMIT_TILES];
+#pragma unroll
+  for (u32 i = 0; i < EMIT_TILES; i++)
+    if ((pmask >> i) & 1) q[i] = load16(in, N, sstart + i * RLE_TILE + 16 * tid);
+#pragma unroll
+  for (u32 i = 0; i < EMIT_TILES; i++)
+    if ((pmask >> i) & 1) stage[emit_sw((int)(i * RT_THREADS + tid))] = q[i];
+  for (u32 i = 0; i < ntl; i++) {
+    if ((pmask >> i) & 1) continue;
+    const u64 t = t0 + i, tstart = t * RLE_TILE;
+    TileView v;
+    tile_view(in, N, tstart, carry[t], sc, v);
+    emit_general(in, bi, tstart, prefix[t], v, Tb);
+    u32 a[4] = {0, 0, 0, 0};
+#pragma unroll
+    for (int j = 0; j < RT_PER; j++) a[j >> 2] |= (u32)v.by[j] << (8 * (j & 3));
+    stage[emit_sw((int)(i * RT_THREADS + tid))] = make_uint4(a[0], a[1], a[2], a[3]);
   }
-  return r;
-}
-struct CrcConsts {
-  u32 table[256];
-  u32 pow[48];  // pow[i] = x^(8 * 2^i) mod P
-  u32 slice[3][256];  // slice[k][i] = table value after k+1 further zero bytes: four bytes per step (slicing by 4)
-};
-static CrcConsts make_crc_consts() {
-  CrcConsts c;
-  for (u32 i = 0; i < 256; i++) {
-    u32 v = i << 24;
-    for (int k = 0; k < 8; k++) v = (v & 0x80000000u) ? (v << 1) ^ CRC_POLY : (v << 1);
-    c.table[i] = v;
+  __syncthreads();
+  // 2. runs of plain tiles: every raw byte emits itself (w = 1) whatever the phase, so the run's part of the block is a
+  // byte copy to output position (x - x0) + o0 (o0 by the same formulas as emit_general, with w = 1 everywhere)
+  for (u32 i = 0; i < ntl;) {
+    if (!((pmask >> i) & 1)) { i++; continue; }
+    u32 j = i + 1;
+    while (j < ntl && ((pmask >> j) & 1)) j++;
+    const u64 tstart = sstart + (u64)i * RLE_TILE;
+    const u64 x0 = max(X0, tstart), x1 = min(X1, sstart + (u64)j * RLE_TILE);
+    const u64 o0 = x0 < bi.b ? (x0 - bi.s) : (u64)bi.ofs + (prefix[t0 + i] + (x0 - tstart) - bi.Wb);
+    if (o0 < bi.n) emit_copy(stage, (u32)(x0 - sstart), o0, (u32)min(x1 - x0, (u64)bi.n - o0), Tb);
+    i = j;
   }
-  for (int k = 0; k < 3; k++)
-    for (u32 i = 0; i < 256; i++) {
-      const u32 prev = k ? c.slice[k - 1][i] : c.table[i];
-      c.slice[k][i] = (prev << 8) ^ c.table[prev >> 24];
+  // 3. CRC: thread tid takes the span bytes of [64 tid, 64 tid + 64) that lie in [rx0, rx1).  Bytes before rx0 count as leading zeros;
+  // the segment that holds rx1 - 1 (segment L) stops exactly at rx1, so its remainder needs no shift.
+  const u32 rx0 = (u32)(X0 - sstart), rx1 = (u32)(X1 - sstart);
+  const u32 seg0 = tid * EMIT_SEG;
+  u32 R = 0;
+  if (seg0 < rx1 && seg0 + EMIT_SEG > rx0) {
+#pragma unroll
+    for (u32 j4 = 0; j4 < EMIT_SEG / 16; j4++) {
+      const uint4 s4 = stage[emit_sw((int)(tid * (EMIT_SEG / 16) + j4))];
+      const u32 a[4] = {s4.x, s4.y, s4.z, s4.w};
+#pragma unroll
+      for (u32 w = 0; w < 4; w++) {
+        const u32 pos = seg0 + 16 * j4 + 4 * w;
+        u32 x = a[w];
+        if (pos < rx0) x = rx0 - pos >= 4 ? 0u : x & (0xffffffffu << (8 * (rx0 - pos)));
+        if (pos + 4 <= rx1) R = crc_step4(R, x, tab);
+        else
+          for (u32 b = pos; b < rx1; b++) R = crc_step1(R, x >> (8 * (b - pos)), tab);
+      }
     }
-  c.pow[0] = 0x100;  // x^8
-  for (int i = 1; i < 48; i++) c.pow[i] = gf_mulmod(c.pow[i - 1], c.pow[i - 1]);
-  return c;
+  }
+  // segment i < L is followed by r + 64 (L - 1 - i) bytes of the span, r = rx1 - 64 L in 1..64
+  const u32 L = (rx1 - 1) / EMIT_SEG, r = rx1 - L * EMIT_SEG;
+  u32 c = tid < L ? gf_mulmod(R, g_crc.pow_seg[L - 1 - tid]) : 0u;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) c ^= __shfl_xor_sync(FULL_MASK, c, o);
+  if (lane_id() == 0) red[tid >> 5] = c;
+  if (tid == L) red[RT_THREADS / 32] = R;
+  __syncthreads();
+  if (tid == 0) {
+    u32 S = 0;
+#pragma unroll
+    for (int w = 0; w < RT_THREADS / 32; w++) S ^= red[w];
+    u32 tot = gf_mulmod(S, g_crc.pow_byte[r]) ^ red[RT_THREADS / 32];
+    if (X1 == bi.e) {
+      atomicXor(&acc[2 * m.x + 1], tot);
+    } else {
+      // X1 is a tile edge k tiles before the last tile edge at or before e
+      const u64 k = bi.e / RLE_TILE - X1 / RLE_TILE;
+      if (k) tot = gf_mulmod(tot, g_crc.pow_tile[k]);
+      atomicXor(&acc[2 * m.x], tot);
+    }
+  }
 }
-__constant__ CrcConsts c_crc;
-static bool g_crc_ready = false;
-static void crc_setup() {
-  if (g_crc_ready) return;
-  CrcConsts h = make_crc_consts();
-  CUDA_CHECK(cudaMemcpyToSymbol(c_crc, &h, sizeof h));
-  g_crc_ready = true;
-}
-// x^(8*bytes) mod P
-__device__ __forceinline__ u32 crc_xpow(u64 bytes) {
-  u32 r = 1u;  // bit i of a register value is the coefficient of x^i, so the polynomial 1 is 0x1
-  for (int i = 0; bytes; i++, bytes >>= 1)
-    if (bytes & 1) r = gf_mulmod(r, c_crc.pow[i]);
-  return r;
+__global__ void k_emit_map(const u32* __restrict__ sbase, uint2* __restrict__ map) {
+  const u32 k = blockIdx.x, b = sbase[k], n = sbase[k + 1] - b;
+  for (u32 j = threadIdx.x; j < n; j += blockDim.x) map[b + j] = make_uint2(k, j);
 }
 
+// ---- CRC of byte ranges (decoder, b2_crc32) ---------------------------------------------------
 #define CRC_PIECE 256
 // Piece j of a block is the j-th 256-byte ADDRESS-aligned window of the buffer that intersects the block's raw
 // range [s,e): every full piece is read with aligned 16-byte loads.  A piece that ends inside the block ends
@@ -794,11 +920,8 @@ __host__ __device__ __forceinline__ u64 crc_piece_count(u64 s, u64 e, u32 mis) {
 __global__ void __launch_bounds__(256)
 k_crc_pieces(const u8* __restrict__ in, const BlkInfo* __restrict__ blocks, u32 first, u32 count, const u64* __restrict__ piece_base,
              u64 total_pieces, u32* __restrict__ acc) {
-  __shared__ u32 tab[256], t1[256], t2[256], t3[256];
-  tab[threadIdx.x] = c_crc.table[threadIdx.x];
-  t1[threadIdx.x] = c_crc.slice[0][threadIdx.x];
-  t2[threadIdx.x] = c_crc.slice[1][threadIdx.x];
-  t3[threadIdx.x] = c_crc.slice[2][threadIdx.x];
+  __shared__ u32 tab[4][256];
+  crc_load_tables(tab);
   __syncthreads();
   const u64 gid = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (gid >= total_pieces) return;
@@ -819,16 +942,13 @@ k_crc_pieces(const u8* __restrict__ in, const BlkInfo* __restrict__ blocks, u32 
   if (len == CRC_PIECE) {
     for (u32 i = 0; i < CRC_PIECE; i += 16) {
       uint4 q = *reinterpret_cast<const uint4*>(p + i);
-      u32 a[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-      for (int w = 0; w < 4; w++) {
-        // four message bytes per dependent step (the stream is MSB first: byte 0 of the little-endian word comes first)
-        const u32 x = crc ^ __byte_perm(a[w], 0, 0x0123);
-        crc = t3[x >> 24] ^ t2[(x >> 16) & 0xff] ^ t1[(x >> 8) & 0xff] ^ tab[x & 0xff];
-      }
+      crc = crc_step4(crc, q.x, tab);
+      crc = crc_step4(crc, q.y, tab);
+      crc = crc_step4(crc, q.z, tab);
+      crc = crc_step4(crc, q.w, tab);
     }
   } else {
-    for (u32 i = 0; i < len; i++) crc = (crc << 8) ^ tab[((crc >> 24) ^ p[i]) & 0xff];
+    for (u32 i = 0; i < len; i++) crc = crc_step1(crc, p[i], tab);
   }
   if (pend == bi.e) {
     atomicXor(&acc[2 * lo + 1], crc);
@@ -838,14 +958,15 @@ k_crc_pieces(const u8* __restrict__ in, const BlkInfo* __restrict__ blocks, u32 
     atomicXor(&acc[2 * lo], crc);
   }
 }
-__global__ void k_crc_final(const u8* __restrict__ in, const BlkInfo* __restrict__ blocks, u32 first, u32 count, const u32* __restrict__ acc,
+// acc[2k] holds the parts of block k that end on a unit edge, shifted to the last edge at or before e' = e + mis;
+// acc[2k+1] the part that ends the block
+__global__ void k_crc_final(const BlkInfo* __restrict__ blocks, u32 first, u32 count, const u32* __restrict__ acc, u32 unit, u32 mis,
                             u32* __restrict__ crc_out) {
   u32 k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= count) return;
   const BlkInfo bi = blocks[first + k];
   const u64 len = bi.e - bi.s;
-  const u32 mis = (u32)((size_t)in & (CRC_PIECE - 1));
-  const u32 body = gf_mulmod(acc[2 * k], crc_xpow((bi.e + mis) % CRC_PIECE)) ^ acc[2 * k + 1];
+  const u32 body = gf_mulmod(acc[2 * k], crc_xpow((bi.e + mis) % unit)) ^ acc[2 * k + 1];
   crc_out[k] = ~(body ^ gf_mulmod(0xffffffffu, crc_xpow(len)));
 }
 
@@ -862,12 +983,13 @@ u32 crc32_device(Ctx& c, const u8* d_p, size_t n) {
   c.to_device(db, &bi, sizeof bi);
   c.to_device(pb, &zero, 8);
   CUDA_CHECK(cudaMemsetAsync(acc, 0, 8, c.stream));
-  const u64 pieces = crc_piece_count(0, n, (u32)((size_t)d_p & (CRC_PIECE - 1)));
+  const u32 mis = (u32)((size_t)d_p & (CRC_PIECE - 1));
+  const u64 pieces = crc_piece_count(0, n, mis);
   if (pieces) {
     k_crc_pieces<<<(unsigned)((pieces + 255) / 256), 256, 0, c.stream>>>(d_p, db, 0, 1, pb, pieces, acc);
     KLAUNCH(c); KCHECK();
   }
-  k_crc_final<<<1, 32, 0, c.stream>>>(d_p, db, 0, 1, acc, out);
+  k_crc_final<<<1, 32, 0, c.stream>>>(db, 0, 1, acc, CRC_PIECE, mis, out);
   KLAUNCH(c); KCHECK();
   u32 h = 0;
   c.to_host(&h, out, 4);
@@ -996,28 +1118,31 @@ void rle1_plan(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan) {
 }
 void rle1_materialize(Ctx& c, const u8* d_in, size_t n, const Rle1Plan& plan, size_t first, size_t count, u8* d_T, u32* d_n, u32* d_crc) {
   if (count == 0) return;
-  std::vector<u64> tbase(count + 1), pbase(count + 1);
+  crc_setup();
+  std::vector<u32> sbase(count + 1);  // first emit CTA of every block
   std::vector<u32> hn(count);
-  u64 tt = 0, pp = 0;
+  u64 ss = 0;
   for (size_t k = 0; k < count; k++) {
     const BlkInfo& bi = plan.h_blocks[first + k];
-    tbase[k] = tt; pbase[k] = pp;
-    tt += (bi.e - 1) / RLE_TILE - bi.s / RLE_TILE + 1;
-    pp += crc_piece_count(bi.s, bi.e, (u32)((size_t)d_in & (CRC_PIECE - 1)));
+    const u64 ta = bi.s / RLE_TILE, tb = (bi.e - 1) / RLE_TILE;
+    if (bi.e / RLE_TILE - ta >= CRC_TILE_POWS) throw B2Error{B2_ERR_CUDA, "internal error: RLE1 block longer than the CRC shift table"};
+    sbase[k] = (u32)ss;
+    ss += (tb - ta + EMIT_TILES) / EMIT_TILES;
     hn[k] = bi.n;
   }
-  tbase[count] = tt; pbase[count] = pp;
-  DBuf<u64> dtb(c, count + 1), dpb(c, count + 1);
+  sbase[count] = (u32)ss;
+  DBuf<u32> dsb(c, count + 1);
+  DBuf<uint2> map(c, ss);
   DBuf<u32> acc(c, 2 * count);
-  c.to_device(dtb, tbase.data(), 8 * (count + 1));
-  c.to_device(dpb, pbase.data(), 8 * (count + 1));
+  c.to_device(dsb, sbase.data(), 4 * (count + 1));
   c.to_device(d_n, hn.data(), 4 * count);
   CUDA_CHECK(cudaMemsetAsync(acc, 0, 8 * count, c.stream));
-  k_rle_emit<<<(unsigned)tt, RT_THREADS, 0, c.stream>>>(d_in, n, plan.tile_carry, plan.tile_prefix, plan.tile_plain, plan.blocks, (u32)first, (u32)count, dtb, d_T);
+  k_emit_map<<<(unsigned)count, 128, 0, c.stream>>>(dsb, map);
   KLAUNCH(c); KCHECK();
-  k_crc_pieces<<<(unsigned)((pp + 255) / 256), 256, 0, c.stream>>>(d_in, plan.blocks, (u32)first, (u32)count, dpb, pp, acc);
+  k_rle_emit<<<(unsigned)ss, RT_THREADS, 0, c.stream>>>(d_in, n, plan.tile_carry, plan.tile_prefix, plan.tile_plain, plan.blocks, (u32)first, map,
+                                                       d_T, acc);
   KLAUNCH(c); KCHECK();
-  k_crc_final<<<(unsigned)((count + 127) / 128), 128, 0, c.stream>>>(d_in, plan.blocks, (u32)first, (u32)count, acc, d_crc);
+  k_crc_final<<<(unsigned)((count + 127) / 128), 128, 0, c.stream>>>(plan.blocks, (u32)first, (u32)count, acc, RLE_TILE, 0, d_crc);
   KLAUNCH(c); KCHECK();
 }
 
@@ -1027,11 +1152,12 @@ void crc_ranges(Ctx& c, const u8* d_data, const BlkInfo* d_ranges, const std::ve
   crc_setup();
   const size_t count = h_ranges.size();
   if (count == 0) return;
+  const u32 mis = (u32)((size_t)d_data & (CRC_PIECE - 1));
   std::vector<u64> pbase(count + 1);
   u64 pp = 0;
   for (size_t k = 0; k < count; k++) {
     pbase[k] = pp;
-    pp += crc_piece_count(h_ranges[k].s, h_ranges[k].e, (u32)((size_t)d_data & (CRC_PIECE - 1)));
+    pp += crc_piece_count(h_ranges[k].s, h_ranges[k].e, mis);
   }
   pbase[count] = pp;
   DBuf<u64> dpb(c, count + 1);
@@ -1042,7 +1168,7 @@ void crc_ranges(Ctx& c, const u8* d_data, const BlkInfo* d_ranges, const std::ve
     k_crc_pieces<<<(unsigned)((pp + 255) / 256), 256, 0, c.stream>>>(d_data, d_ranges, 0, (u32)count, dpb, pp, acc);
     KLAUNCH(c); KCHECK();
   }
-  k_crc_final<<<(unsigned)((count + 127) / 128), 128, 0, c.stream>>>(d_data, d_ranges, 0, (u32)count, acc, d_crc_out);
+  k_crc_final<<<(unsigned)((count + 127) / 128), 128, 0, c.stream>>>(d_ranges, 0, (u32)count, acc, CRC_PIECE, mis, d_crc_out);
   KLAUNCH(c); KCHECK();
   c.sync();
 }
