@@ -52,6 +52,16 @@ def _level(props):
     return int(level)
 
 
+# compressFile's encoder flavors (include/b2bz.h B2_BZ2_*): the bytes of compressjs (the default) or of libbz2
+FLAVORS = {"compressjs": 0, "libbz2": 1}
+
+
+def _flavor(flavor):
+    if not isinstance(flavor, str) or flavor not in FLAVORS:
+        raise ValueError("unknown bzip2 flavor %r (expected one of %s)" % (flavor, ", ".join(sorted(FLAVORS))))
+    return FLAVORS[flavor]
+
+
 def _take(L, p, n):
     arr = np.ctypeslib.as_array(p, shape=(n.value,)).copy() if n.value else np.zeros(0, dtype=np.uint8)
     L.b2_free(p)
@@ -96,20 +106,23 @@ class Bzip2:
     Err = Err
 
     @staticmethod
-    def compressFile(input, output=None, props=None):
+    def compressFile(input, output=None, props=None, *, flavor="compressjs"):
         """lib/Bzip2.js:879-929.  props: block size multiplier 1..9 (default 9).  When input has readByte and output
-        has writeByte, the input is read and the output written as the encode goes, in bounded memory."""
+        has writeByte, the input is read and the output written as the encode goes, in bounded memory.
+        flavor: "compressjs" writes the bytes of compressjs; "libbz2" those of libbz2 (``bzip2 -N``, Python's
+        ``bz2.compress(data, N)``), whose block cut and Huffman tables differ."""
+        fl = _flavor(flavor)   # before anything is read
         if is_stream_pair(input, output):
-            level = _level(props)   # before anything is read
+            level = _level(props)
             pump = Pump(input, output)
-            rc = _native.lib().b2_bzip2_compress_stream(pump.read_fn, pump.write_fn, None, level)
+            rc = _native.lib().b2_bzip2_compress_stream_flavor(pump.read_fn, pump.write_fn, None, level, fl)
             pump.check(rc, _error)
             return output
         L = _native.lib()
         data = coerce_input(input)
         level = _level(props)
         out, n = C.POINTER(C.c_uint8)(), C.c_size_t()
-        rc = L.b2_bzip2_compress(data.ctypes.data if data.size else None, data.size, int(level), C.byref(out), C.byref(n))
+        rc = L.b2_bzip2_compress_flavor(data.ctypes.data if data.size else None, data.size, int(level), C.byref(out), C.byref(n), fl)
         if rc:
             _raise(rc)
         return deliver_output(output, _take(L, out, n))

@@ -39,6 +39,7 @@ HELP = """
     -z, --compress    Compress stdin to stdout
     -b, --block <n>   Extract a single block, starting at <n> bits.
     -t <compressor>   Select compressor type (bzip2 or bwtc)
+    --libbz2          With -z -t bzip2: write the bytes bzip2 (libbz2) writes
     -1                Fastest/largest compression
     -2
     -3
@@ -76,7 +77,7 @@ def _number(s):
 
 def parse(argv):
     """Returns a dict of the options, or raises UsageError.  --help and --version are returned as 'help'/'version'."""
-    opts = {"decompress": False, "compress": False, "block": "-1", "T": None, "levels": set(), "args": []}
+    opts = {"decompress": False, "compress": False, "block": "-1", "T": None, "levels": set(), "args": [], "libbz2": False}
     i = 0
     only_args = False
     while i < len(argv):
@@ -92,7 +93,7 @@ def parse(argv):
             name, eq, val = a[2:].partition("=")
             if name in ("help", "version"):
                 return {name: True}
-            if name in ("decompress", "compress") and not eq:
+            if name in ("decompress", "compress", "libbz2") and not eq:
                 opts[name] = True
             elif name == "block":
                 if not eq:
@@ -233,7 +234,7 @@ class OutStream:
         self.f.flush()
 
 
-def stream(kind, decompress, level, in_fd, out):
+def stream(kind, decompress, level, in_fd, out, flavor="compressjs"):
     """Without -b: compressFile / decompressFile of `kind` ('bzip2' or 'bwtc') from the descriptor to the binary file
     `out` through the streams of bin/compressjs, in bounded memory.  The exit status; on an error its message is on
     stderr and `out` has what went out before it (on a decode error: the decoded bytes cut down to a multiple of FLUSH)."""
@@ -249,7 +250,7 @@ def stream(kind, decompress, level, in_fd, out):
         elif decompress:
             Bzip2.decompressFile(src, dst)   # without multistream, as bin/compressjs:160-164 calls it
         else:
-            Bzip2.compressFile(src, dst, level)
+            Bzip2.compressFile(src, dst, level, flavor=flavor)
     except Exception as e:
         out.flush()
         sys.stderr.write("%s\n" % e)
@@ -297,8 +298,10 @@ def main(argv=None):
         in_fd = os.open(args[0], os.O_RDONLY) if len(args) > 0 else sys.stdin.fileno()
         out = open(args[1], "wb") if len(args) > 1 else sys.stdout.buffer
         kind = compressor(opts["T"])
+        if opts["libbz2"] and (decompress or kind != "bzip2"):
+            raise UsageError("--libbz2 can only be used with -z -t bzip2")
         if block < 0:
-            return stream(kind, decompress, level, in_fd, out)
+            return stream(kind, decompress, level, in_fd, out, "libbz2" if opts["libbz2"] else "compressjs")
         data, size = read_input(in_fd)
         result, err = run(kind, decompress, level, block, data, size)
         if err is not None:

@@ -603,12 +603,23 @@ static int decode_host(Ctx& c, StreamIn& in, StreamOut* out, int multistream, co
 
 extern "C" {
 
+// the encoder flavor of a compress call: checked with the other arguments, before anything is read
+static void check_flavor(int flavor) {
+  if (flavor != B2_BZ2_COMPRESSJS && flavor != B2_BZ2_LIBBZ2) throw B2Error{B2_ERR_BAD_ARG, "unknown bzip2 flavor"};
+}
+
 int b2_bzip2_compress_stream(b2_read_fn rd, b2_write_fn wr, void* user, int level) {
+  return b2_bzip2_compress_stream_flavor(rd, wr, user, level, B2_BZ2_COMPRESSJS);
+}
+
+int b2_bzip2_compress_stream_flavor(b2_read_fn rd, b2_write_fn wr, void* user, int level, int flavor) {
   return guarded([&]() {
     if (level < 1 || level > 9) throw B2Error{B2_ERR_BAD_LEVEL, "Invalid block size multiplier"};
     if (!rd || !wr) throw B2Error{B2_ERR_BAD_ARG, "null callback"};
+    check_flavor(flavor);
     Ctx& c = ctx_locked();
     c.reset_call();
+    c.bz_flavor = flavor;
     StreamIn in(rd, user, c.h2d_stream);
     StreamOut out(wr, user, c.d2h_stream);
     return compress_host(c, in, out, level, false);
@@ -627,10 +638,16 @@ int b2_bzip2_decompress_stream(b2_read_fn rd, b2_write_fn wr, void* user, int mu
 }
 
 int b2_bzip2_compress_dev(const void* d_in, size_t n, int level, void* d_out, size_t out_cap, size_t* out_n) {
+  return b2_bzip2_compress_dev_flavor(d_in, n, level, d_out, out_cap, out_n, B2_BZ2_COMPRESSJS);
+}
+
+int b2_bzip2_compress_dev_flavor(const void* d_in, size_t n, int level, void* d_out, size_t out_cap, size_t* out_n, int flavor) {
   return guarded([&]() {
     if (level < 1 || level > 9) throw B2Error{B2_ERR_BAD_LEVEL, "Invalid block size multiplier"};
+    check_flavor(flavor);
     Ctx& c = ctx_locked();
     c.reset_call();
+    c.bz_flavor = flavor;
     {
       StageScope tot(c, ST_TOTAL);
       bzip2_compress_dev(c, (const u8*)d_in, n, level, (u8*)d_out, out_cap, out_n);
@@ -643,10 +660,16 @@ int b2_bzip2_compress_dev(const void* d_in, size_t n, int level, void* d_out, si
 }
 
 int b2_bzip2_compress(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n) {
+  return b2_bzip2_compress_flavor(in, n, level, out, out_n, B2_BZ2_COMPRESSJS);
+}
+
+int b2_bzip2_compress_flavor(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n, int flavor) {
   return guarded([&]() {
     if (level < 1 || level > 9) throw B2Error{B2_ERR_BAD_LEVEL, "Invalid block size multiplier"};
+    check_flavor(flavor);
     Ctx& c = ctx_locked();
     c.reset_call();
+    c.bz_flavor = flavor;
     cudaPointerAttributes pa;
     const bool pinned_in = n && cudaPointerGetAttributes(&pa, in) == cudaSuccess && pa.type == cudaMemoryTypeHost;
     cudaGetLastError();

@@ -22,6 +22,7 @@ struct Ctx {
   std::vector<std::pair<int, size_t>> ev_tags;  // (stage id, pool index) recorded in the current call
   std::vector<b2_block_trace> trace;
   u32 bwt_batch = 264;  // bzip2 blocks processed together in one batch: 2 CTAs per SM for the per-block kernels (set from the SM count)
+  int bz_flavor = B2_BZ2_COMPRESSJS;  // bzip2 encoder flavor of the current call (block cut and Huffman table search)
   bool timing = true;
   bool bwt_msd = true;  // MSD + shared-memory bucket sort for sparse-tie batches (bwt_msd.cu); B2_BWT_MSD=0 disables it
   bool bwt_wide = false, bwt_wide_forced = false, bwt_mode_known = false;  // 8-byte initial sort for text-like batches (see bwt.cu)
@@ -80,6 +81,7 @@ struct Ctx {
     ev_used = 0;
     ev_tags.clear();
     bwt_mode_known = false;
+    bz_flavor = B2_BZ2_COMPRESSJS;
     memset(&stats, 0, sizeof stats);
   }
   void collect();  // after the final sync: fold event pairs into stats

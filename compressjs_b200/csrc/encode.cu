@@ -670,7 +670,9 @@ void bzip2_compress_host(Ctx& c, StreamIn& in, int level, u8* d_in, size_t win, 
       mark("chunks arrived", have);
       Rle1Plan plan;
       rle1_plan(c, d_in + resume, avail - resume, level, plan);
-      // only the very end of the FILE closes a short block; the last block of any other prefix may still grow
+      // only the very end of the FILE closes a short block; the last block of any other prefix may still grow (libbz2
+      // flavor: its closing piece may go on).  Every other block ends before the prefix does, and the next prefix starts
+      // on a block start, where both flavors start a fresh run state.
       const size_t nfinal = (last && last_window) ? plan.nblocks : (plan.nblocks ? plan.nblocks - 1 : 0);
       mark("planned, final blocks", nfinal);
       if (!nfinal) {

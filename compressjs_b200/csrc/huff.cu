@@ -52,6 +52,18 @@ struct HuffSmem {
   u32 misc[8];
 };
 
+// s.len of `ntab` tables -> the packed lookup s.tbl (all threads)
+template <class S>
+__device__ void pack_lengths(S& s, u32 ntab, u32 A) {
+  for (u32 i = threadIdx.x; i < A * HF_COPIES; i += HF_THREADS) {
+    const u32 sym = i / HF_COPIES;
+    u32 p = 0;
+    for (u32 t = 0; t < ntab; t++) p |= (u32)s.len[t][sym] << (5 * t);
+    s.tbl[sym][i % HF_COPIES] = p;
+  }
+  __syncthreads();
+}
+
 // build the code lengths of `ntab` tables from s.freq (all threads)
 __device__ void build_tables(HuffSmem& s, u32 ntab, u32 A) {
   const u32 tid = threadIdx.x;
@@ -77,13 +89,7 @@ __device__ void build_tables(HuffSmem& s, u32 ntab, u32 A) {
     s.len[t][s.order[t][r]] = (u8)s.work[t][r];
   }
   __syncthreads();
-  for (u32 i = tid; i < A * HF_COPIES; i += HF_THREADS) {
-    const u32 sym = i / HF_COPIES;
-    u32 p = 0;
-    for (u32 t = 0; t < ntab; t++) p |= (u32)s.len[t][sym] << (5 * t);
-    s.tbl[sym][i % HF_COPIES] = p;
-  }
-  __syncthreads();
+  pack_lengths(s, ntab, A);
 }
 
 // Tiles of 256 groups are staged through shared memory; the next tile's loads (and each thread's own
@@ -139,7 +145,8 @@ __device__ __forceinline__ void for_group(const u8* tile, u32 cnt, unsigned long
 
 // lib/Bzip2.js:671-684: every group goes to the table that codes it in the fewest bits
 // (ties -> lowest table index).  Fills s.sel / s.cost.
-__device__ __forceinline__ void assign_selectors(HuffSmem& s, const u8* nar, const unsigned long long* hmask, u32 m, u32 nsel, u32 ntab,
+template <class S>
+__device__ __forceinline__ void assign_selectors(S& s, const u8* nar, const unsigned long long* hmask, u32 m, u32 nsel, u32 ntab,
                                                  bool any_hi) {
   const u32 tid = threadIdx.x, lane = tid % HF_COPIES;
   TileRegs tr;
@@ -170,7 +177,8 @@ __device__ __forceinline__ void assign_selectors(HuffSmem& s, const u8* nar, con
   }
 }
 
-__device__ __forceinline__ void recount(HuffSmem& s, const u8* nar, const unsigned long long* hmask, u32 m, u32 nsel, u32 ntab, bool any_hi) {
+template <class S>
+__device__ __forceinline__ void recount(S& s, const u8* nar, const unsigned long long* hmask, u32 m, u32 nsel, u32 ntab, bool any_hi) {
   const u32 tid = threadIdx.x;
   for (u32 i = tid; i < ntab * (HUFF_MAXSYM + 2); i += HF_THREADS) (&s.freq[0][0])[i] = 0;
   TileRegs tr;
@@ -245,98 +253,12 @@ __device__ __forceinline__ u32 rec_full(u32 R) {  // R ++ (identity minus R): th
   return lst;
 }
 
-__global__ void __launch_bounds__(HF_THREADS, 2)
-k_huffman(const u8* __restrict__ sym_lo, const unsigned long long* __restrict__ sym_hi, const u32* __restrict__ any_hi_arr,
-          const u32* __restrict__ m_arr, const u32* __restrict__ freq0, const u32* __restrict__ used, u8* __restrict__ sel_out,
-          u8* __restrict__ selmtf_out, HuffBlk* __restrict__ hb_out, u32* __restrict__ goff_out) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  HuffSmem& s = *reinterpret_cast<HuffSmem*>(smem_raw);
-  const u32 tid = threadIdx.x;
-  const u32 blk = blockIdx.x;
-  const u32 m = m_arr[blk];
-  HuffBlk* hb = hb_out + blk;
-  if (m == 0) {
-    if (tid == 0) { hb->ngroups = 0; hb->nsel = 0; hb->alpha = 0; hb->m = 0; hb->body_bits = 0; }
-    return;
-  }
-  u32 alpha = 0;
-  for (int k = 0; k < 8; k++) alpha += __popc(used[blk * 8 + k]);
-  const u32 A = alpha + 2;                    // RUNA, RUNB, alpha-1 MTF positions, EOB
-  const u32 nsel = (m + HUFF_GROUP - 1) / HUFF_GROUP;
-  const u8* nar = sym_lo + ((size_t)blk << SEG_SHIFT);
-  const unsigned long long* hmask = sym_hi + (size_t)blk * SEL_STRIDE;
-  const bool any_hi = any_hi_arr[blk] != 0;
-  u32 target;                                 // lib/Bzip2.js:826-830
-  if (m >= 2400) target = 6; else if (m >= 1200) target = 5; else if (m >= 600) target = 4; else if (m >= 200) target = 3; else target = 2;
-  // seed tables: global frequencies, flat frequencies (lib/Bzip2.js:835-837)
-  for (u32 i = tid; i < A; i += HF_THREADS) { s.freq[0][i] = freq0[(size_t)blk * HUFF_MAXSYM + i]; s.freq[1][i] = 1; }
-  __syncthreads();  // build_tables reads the seed frequencies across threads
-  u32 ng = 2;
-  build_tables(s, ng, A);
-  while (ng < target) {
-    assign_selectors(s, nar, hmask, m, nsel, ng, any_hi);
-    // which table is used most? (first maximum, lib/Bzip2.js:699)
-    if (tid < HUFF_MAXGROUPS) s.gcount[tid] = 0;
-    for (u32 i = tid; i < 1024; i += HF_THREADS) s.chist[i] = 0;
-    __syncthreads();
-    {
-      u32 l0 = 0, l1 = 0, l2 = 0, l3 = 0, l4 = 0, l5 = 0;
-      for (u32 g = tid; g < nsel; g += HF_THREADS) {
-        const u32 v = s.sel[g];
-        l0 += v == 0; l1 += v == 1; l2 += v == 2; l3 += v == 3; l4 += v == 4; l5 += v == 5;
-      }
-      if (l0) atomicAdd(&s.gcount[0], l0);
-      if (l1) atomicAdd(&s.gcount[1], l1);
-      if (l2) atomicAdd(&s.gcount[2], l2);
-      if (l3) atomicAdd(&s.gcount[3], l3);
-      if (l4) atomicAdd(&s.gcount[4], l4);
-      if (l5) atomicAdd(&s.gcount[5], l5);
-    }
-    __syncthreads();
-    u32 which = 0;
-    for (u32 t = 1; t < ng; t++) if (s.gcount[t] > s.gcount[which]) which = t;
-    const u32 cntw = s.gcount[which];
-    // histogram of the costs of the groups coded by `which`
-    for (u32 g = tid; g < nsel; g += HF_THREADS) if (s.sel[g] == which) atomicAdd(&s.chist[s.cost[g]], 1u);
-    __syncthreads();
-    // stable sort by cost, upper half [cntw>>1, cntw) moves to the new table (lib/Bzip2.js:710-714):
-    // threshold cost cstar: below = #(cost < cstar) <= half < #(cost <= cstar)
-    if (tid == 0) {
-      const u32 half = cntw >> 1;
-      u32 cum = 0, cstar = 0;
-      for (u32 cv = 0; cv < 1024; cv++) {
-        if (cum + s.chist[cv] > half) { cstar = cv; break; }
-        cum += s.chist[cv];
-      }
-      s.misc[0] = cstar;
-      s.misc[1] = half - cum;  // how many of the groups with cost == cstar stay (the first ones in index order)
-    }
-    __syncthreads();
-    const u32 cstar = s.misc[0], keep_eq = s.misc[1];
-    {
-      // ordered prefix count of (sel == which && cost == cstar) over groups in index order
-      const u32 per = (nsel + HF_THREADS - 1) / HF_THREADS;
-      const u32 ga = tid * per, gb = min(nsel, ga + per);
-      u32 eq = 0;
-      for (u32 g = ga; g < gb; g++) eq += (s.sel[g] == which && s.cost[g] == cstar) ? 1u : 0u;
-      u32 tot;
-      u32 ex = block_excl_add<HF_THREADS, u32>(eq, s.ws, &tot);
-      for (u32 g = ga; g < gb; g++) {
-        if (s.sel[g] != which) continue;
-        const u32 cg = s.cost[g];
-        bool move;
-        if (cg > cstar) move = true;
-        else if (cg < cstar) move = false;
-        else { move = ex >= keep_eq; ex++; }
-        if (move) s.sel[g] = (u8)ng;
-      }
-    }
-    __syncthreads();
-    ng++;
-    recount(s, nar, hmask, m, nsel, ng, any_hi);
-    build_tables(s, ng, A);
-  }
-  assign_selectors(s, nar, hmask, m, nsel, ng, any_hi);  // lib/Bzip2.js:843
+// The block's results once its selectors and code lengths are final (s.sel, s.len of ng tables, s.cost = every group's
+// code bits under its table): group bit offsets, selectors, their MTF, lengths and the block's bit count.
+template <class S>
+__device__ void write_block(S& s, u32 blk, u32 m, u32 alpha, u32 nsel, u32 ng, const u32* __restrict__ used, u8* __restrict__ sel_out,
+                            u8* __restrict__ selmtf_out, HuffBlk* __restrict__ hb, u32* __restrict__ goff_out) {
+  const u32 tid = threadIdx.x, A = alpha + 2;
   // ---- results + bit accounting ----
   // bit offset of every group inside the code section: every warp scans a contiguous eighth of the groups
   // (coalesced, lane-strided), after a block scan of the eighths' sums.  A block codes at most 900001 x 20 bits.
@@ -434,12 +356,271 @@ k_huffman(const u8* __restrict__ sym_lo, const unsigned long long* __restrict__ 
   }
 }
 
+__global__ void __launch_bounds__(HF_THREADS, 2)
+k_huffman(const u8* __restrict__ sym_lo, const unsigned long long* __restrict__ sym_hi, const u32* __restrict__ any_hi_arr,
+          const u32* __restrict__ m_arr, const u32* __restrict__ freq0, const u32* __restrict__ used, u8* __restrict__ sel_out,
+          u8* __restrict__ selmtf_out, HuffBlk* __restrict__ hb_out, u32* __restrict__ goff_out) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  HuffSmem& s = *reinterpret_cast<HuffSmem*>(smem_raw);
+  const u32 tid = threadIdx.x;
+  const u32 blk = blockIdx.x;
+  const u32 m = m_arr[blk];
+  HuffBlk* hb = hb_out + blk;
+  if (m == 0) {
+    if (tid == 0) { hb->ngroups = 0; hb->nsel = 0; hb->alpha = 0; hb->m = 0; hb->body_bits = 0; }
+    return;
+  }
+  u32 alpha = 0;
+  for (int k = 0; k < 8; k++) alpha += __popc(used[blk * 8 + k]);
+  const u32 A = alpha + 2;                    // RUNA, RUNB, alpha-1 MTF positions, EOB
+  const u32 nsel = (m + HUFF_GROUP - 1) / HUFF_GROUP;
+  const u8* nar = sym_lo + ((size_t)blk << SEG_SHIFT);
+  const unsigned long long* hmask = sym_hi + (size_t)blk * SEL_STRIDE;
+  const bool any_hi = any_hi_arr[blk] != 0;
+  u32 target;                                 // lib/Bzip2.js:826-830
+  if (m >= 2400) target = 6; else if (m >= 1200) target = 5; else if (m >= 600) target = 4; else if (m >= 200) target = 3; else target = 2;
+  // seed tables: global frequencies, flat frequencies (lib/Bzip2.js:835-837)
+  for (u32 i = tid; i < A; i += HF_THREADS) { s.freq[0][i] = freq0[(size_t)blk * HUFF_MAXSYM + i]; s.freq[1][i] = 1; }
+  __syncthreads();  // build_tables reads the seed frequencies across threads
+  u32 ng = 2;
+  build_tables(s, ng, A);
+  while (ng < target) {
+    assign_selectors(s, nar, hmask, m, nsel, ng, any_hi);
+    // which table is used most? (first maximum, lib/Bzip2.js:699)
+    if (tid < HUFF_MAXGROUPS) s.gcount[tid] = 0;
+    for (u32 i = tid; i < 1024; i += HF_THREADS) s.chist[i] = 0;
+    __syncthreads();
+    {
+      u32 l0 = 0, l1 = 0, l2 = 0, l3 = 0, l4 = 0, l5 = 0;
+      for (u32 g = tid; g < nsel; g += HF_THREADS) {
+        const u32 v = s.sel[g];
+        l0 += v == 0; l1 += v == 1; l2 += v == 2; l3 += v == 3; l4 += v == 4; l5 += v == 5;
+      }
+      if (l0) atomicAdd(&s.gcount[0], l0);
+      if (l1) atomicAdd(&s.gcount[1], l1);
+      if (l2) atomicAdd(&s.gcount[2], l2);
+      if (l3) atomicAdd(&s.gcount[3], l3);
+      if (l4) atomicAdd(&s.gcount[4], l4);
+      if (l5) atomicAdd(&s.gcount[5], l5);
+    }
+    __syncthreads();
+    u32 which = 0;
+    for (u32 t = 1; t < ng; t++) if (s.gcount[t] > s.gcount[which]) which = t;
+    const u32 cntw = s.gcount[which];
+    // histogram of the costs of the groups coded by `which`
+    for (u32 g = tid; g < nsel; g += HF_THREADS) if (s.sel[g] == which) atomicAdd(&s.chist[s.cost[g]], 1u);
+    __syncthreads();
+    // stable sort by cost, upper half [cntw>>1, cntw) moves to the new table (lib/Bzip2.js:710-714):
+    // threshold cost cstar: below = #(cost < cstar) <= half < #(cost <= cstar)
+    if (tid == 0) {
+      const u32 half = cntw >> 1;
+      u32 cum = 0, cstar = 0;
+      for (u32 cv = 0; cv < 1024; cv++) {
+        if (cum + s.chist[cv] > half) { cstar = cv; break; }
+        cum += s.chist[cv];
+      }
+      s.misc[0] = cstar;
+      s.misc[1] = half - cum;  // how many of the groups with cost == cstar stay (the first ones in index order)
+    }
+    __syncthreads();
+    const u32 cstar = s.misc[0], keep_eq = s.misc[1];
+    {
+      // ordered prefix count of (sel == which && cost == cstar) over groups in index order
+      const u32 per = (nsel + HF_THREADS - 1) / HF_THREADS;
+      const u32 ga = tid * per, gb = min(nsel, ga + per);
+      u32 eq = 0;
+      for (u32 g = ga; g < gb; g++) eq += (s.sel[g] == which && s.cost[g] == cstar) ? 1u : 0u;
+      u32 tot;
+      u32 ex = block_excl_add<HF_THREADS, u32>(eq, s.ws, &tot);
+      for (u32 g = ga; g < gb; g++) {
+        if (s.sel[g] != which) continue;
+        const u32 cg = s.cost[g];
+        bool move;
+        if (cg > cstar) move = true;
+        else if (cg < cstar) move = false;
+        else { move = ex >= keep_eq; ex++; }
+        if (move) s.sel[g] = (u8)ng;
+      }
+    }
+    __syncthreads();
+    ng++;
+    recount(s, nar, hmask, m, nsel, ng, any_hi);
+    build_tables(s, ng, A);
+  }
+  assign_selectors(s, nar, hmask, m, nsel, ng, any_hi);  // lib/Bzip2.js:843
+  write_block(s, blk, m, alpha, nsel, ng, used, sel_out, selmtf_out, hb, goff_out);
+}
+
+// ---- libbz2 flavor (bzlib 1.0.3+ compress.c sendMTFValues, huffman.c BZ2_hbMakeCodeLengths) ----------------------
+// Initial tables from a partition of the symbol frequencies, then four rounds of assign + recount + rebuild; the
+// selectors of the 4th assignment and the tables built after it are written.  The assign and recount passes are those
+// of the compressjs search (lengths <= 17 and the initial 0 / 15 fit the packed 5-bit lookup); the tables of a round are
+// built side by side, one thread per table running the heap builder.
+struct LbHeap {                        // BZ2_hbMakeCodeLengths of one table (nodes 1..A leaves, A+1.. internal)
+  u32 weight[2 * HUFF_MAXSYM];         // freq << 8 | depth
+  u16 parent[2 * HUFF_MAXSYM];         // LB_ROOT: none
+  u16 heap[HUFF_MAXSYM + 2];           // 1-based min-heap of node numbers, heap[0] = sentinel node 0 (weight 0)
+};
+#define LB_ROOT 0xffffu
+#define LB_MAXLEN 17
+struct HuffSmemL {
+  u8 tile[HF_TILE_BYTES + 16];
+  u16 cost[SEL_STRIDE];
+  u8 sel[SEL_STRIDE];
+  u32 tbl[HUFF_MAXSYM][HF_COPIES];
+  u32 freq[HUFF_MAXGROUPS][HUFF_MAXSYM + 2];
+  u8 len[HUFF_MAXGROUPS][HUFF_MAXSYM + 6];
+  union {
+    LbHeap hp[HUFF_MAXGROUPS];
+    u32 chist[2 * HF_THREADS];         // write_block's selector scan, after the last build
+  };
+  u32 ws[HF_THREADS / 32 + 1];
+};
+// 114 KB with write_block's reduction: two CTAs per SM, as k_huffman
+static_assert(sizeof(HuffSmemL) + 64 <= 115 * 1024, "two libbz2 Huffman CTAs per SM");
+
+__device__ __forceinline__ void lb_up(LbHeap& h, u32 z) {
+  const u32 tmp = h.heap[z];
+  while (h.weight[tmp] < h.weight[h.heap[z >> 1]]) { h.heap[z] = h.heap[z >> 1]; z >>= 1; }
+  h.heap[z] = (u16)tmp;
+}
+__device__ __forceinline__ void lb_down(LbHeap& h, u32 z, u32 nHeap) {
+  const u32 tmp = h.heap[z];
+  for (;;) {
+    u32 y = z << 1;
+    if (y > nHeap) break;
+    if (y < nHeap && h.weight[h.heap[y + 1]] < h.weight[h.heap[y]]) y++;
+    if (h.weight[tmp] < h.weight[h.heap[y]]) break;
+    h.heap[z] = h.heap[y];
+    z = y;
+  }
+  h.heap[z] = (u16)tmp;
+}
+// code lengths of one table (one thread): Huffman by the heap above, depth in the weights' low byte as tie-break; while
+// a length exceeds 17 every frequency f becomes 1 + f / 2 and the tree is built again
+__device__ void lb_make_lengths(LbHeap& h, const u32* freq, u8* len, u32 A) {
+  for (u32 i = 0; i < A; i++) h.weight[i + 1] = (freq[i] ? freq[i] : 1u) << 8;
+  for (;;) {
+    u32 nNodes = A, nHeap = 0;
+    h.heap[0] = 0; h.weight[0] = 0;
+    for (u32 i = 1; i <= A; i++) {
+      h.parent[i] = LB_ROOT;
+      h.heap[++nHeap] = (u16)i;
+      lb_up(h, nHeap);
+    }
+    while (nHeap > 1) {
+      const u32 n1 = h.heap[1];
+      h.heap[1] = h.heap[nHeap--];
+      lb_down(h, 1, nHeap);
+      const u32 n2 = h.heap[1];
+      h.heap[1] = h.heap[nHeap--];
+      lb_down(h, 1, nHeap);
+      nNodes++;
+      h.parent[n1] = h.parent[n2] = (u16)nNodes;
+      const u32 w1 = h.weight[n1], w2 = h.weight[n2];
+      h.weight[nNodes] = ((w1 & 0xffffff00u) + (w2 & 0xffffff00u)) | (1u + max(w1 & 0xffu, w2 & 0xffu));
+      h.parent[nNodes] = LB_ROOT;
+      h.heap[++nHeap] = (u16)nNodes;
+      lb_up(h, nHeap);
+    }
+    bool too_long = false;
+    for (u32 i = 1; i <= A; i++) {
+      u32 j = 0;
+      for (u32 k = i; h.parent[k] != LB_ROOT; k = h.parent[k]) j++;
+      len[i - 1] = (u8)j;
+      too_long |= j > LB_MAXLEN;
+    }
+    if (!too_long) return;
+    for (u32 i = 1; i <= A; i++) h.weight[i] = (1u + (h.weight[i] >> 8) / 2) << 8;
+  }
+}
+
+// s.cost[g] = the bits of group g under the table it selected (the 4th assignment costed it under the tables before)
+__device__ void cost_selected(HuffSmemL& s, const u8* nar, const unsigned long long* hmask, u32 m, u32 nsel, bool any_hi) {
+  const u32 tid = threadIdx.x, lane = tid % HF_COPIES;
+  TileRegs tr;
+  tile_fetch(tr, nar, hmask, 0, nsel, any_hi);
+  for (u32 g0 = 0; g0 < nsel; g0 += HF_TILE_GROUPS) {
+    tile_store(tr, s.tile);
+    const unsigned long long hm = tr.hm;
+    __syncthreads();
+    if (g0 + HF_TILE_GROUPS < nsel) tile_fetch(tr, nar, hmask, g0 + HF_TILE_GROUPS, nsel, any_hi);
+    const u32 g = g0 + tid;
+    if (g < nsel) {
+      const u32 sh = 5 * s.sel[g];
+      u32 c = 0;
+      for_group(s.tile, min(50u, m - 50u * g), hm, [&](u32 sy) { c += (s.tbl[sy][lane] >> sh) & 31u; });
+      s.cost[g] = (u16)c;
+    }
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(HF_THREADS, 2)
+k_huffman_libbz2(const u8* __restrict__ sym_lo, const unsigned long long* __restrict__ sym_hi, const u32* __restrict__ any_hi_arr,
+                 const u32* __restrict__ m_arr, const u32* __restrict__ freq0, const u32* __restrict__ used, u8* __restrict__ sel_out,
+                 u8* __restrict__ selmtf_out, HuffBlk* __restrict__ hb_out, u32* __restrict__ goff_out) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  HuffSmemL& s = *reinterpret_cast<HuffSmemL*>(smem_raw);
+  const u32 tid = threadIdx.x;
+  const u32 blk = blockIdx.x;
+  const u32 m = m_arr[blk];
+  HuffBlk* hb = hb_out + blk;
+  if (m == 0) {
+    if (tid == 0) { hb->ngroups = 0; hb->nsel = 0; hb->alpha = 0; hb->m = 0; hb->body_bits = 0; }
+    return;
+  }
+  u32 alpha = 0;
+  for (int k = 0; k < 8; k++) alpha += __popc(used[blk * 8 + k]);
+  const u32 A = alpha + 2;
+  const u32 nsel = (m + HUFF_GROUP - 1) / HUFF_GROUP;
+  const u8* nar = sym_lo + ((size_t)blk << SEG_SHIFT);
+  const unsigned long long* hmask = sym_hi + (size_t)blk * SEL_STRIDE;
+  const bool any_hi = any_hi_arr[blk] != 0;
+  u32 ng;
+  if (m < 200) ng = 2; else if (m < 600) ng = 3; else if (m < 1200) ng = 4; else if (m < 2400) ng = 5; else ng = 6;
+  // initial tables: table nPart-1 codes the symbols gs..ge of a run of about remF / nPart of the frequency in 0 bits,
+  // everything else in 15
+  if (tid == 0) {
+    const u32* mf = freq0 + (size_t)blk * HUFF_MAXSYM;
+    u32 remF = m, gs = 0;
+    for (u32 nPart = ng; nPart > 0; nPart--) {
+      const u32 tFreq = remF / nPart;
+      int ge = (int)gs - 1;
+      u32 aFreq = 0;
+      while (aFreq < tFreq && ge < (int)A - 1) aFreq += mf[++ge];
+      if (ge > (int)gs && nPart != ng && nPart != 1 && ((ng - nPart) & 1)) aFreq -= mf[ge--];
+      for (u32 v = 0; v < A; v++) s.len[nPart - 1][v] = ((int)v >= (int)gs && (int)v <= ge) ? 0 : 15;
+      gs = (u32)(ge + 1);
+      remF -= aFreq;
+    }
+  }
+  __syncthreads();
+  pack_lengths(s, ng, A);
+  for (int it = 0; it < 4; it++) {
+    assign_selectors(s, nar, hmask, m, nsel, ng, any_hi);
+    recount(s, nar, hmask, m, nsel, ng, any_hi);
+    if (tid < ng) lb_make_lengths(s.hp[tid], s.freq[tid], s.len[tid], A);
+    __syncthreads();
+    pack_lengths(s, ng, A);
+  }
+  cost_selected(s, nar, hmask, m, nsel, any_hi);
+  write_block(s, blk, m, alpha, nsel, ng, used, sel_out, selmtf_out, hb, goff_out);
+}
+
 void huffman_batch(Ctx& c, const NarrowSyms& sym, const u32* d_m, const u32* d_freq, const u32* d_used, u32 nblk, u8* d_sel, u8* d_selmtf,
                    HuffBlk* d_hb, u32* d_goff) {
   static bool attr = false;
   if (!attr) {
     CUDA_CHECK(cudaFuncSetAttribute(k_huffman, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HuffSmem)));
+    CUDA_CHECK(cudaFuncSetAttribute(k_huffman_libbz2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HuffSmemL)));
     attr = true;
+  }
+  if (c.bz_flavor == B2_BZ2_LIBBZ2) {
+    k_huffman_libbz2<<<nblk, HF_THREADS, sizeof(HuffSmemL), c.stream>>>(sym.lo, sym.hi, sym.any_hi, d_m, d_freq, d_used, d_sel, d_selmtf, d_hb,
+                                                                        d_goff);
+    KLAUNCH(c); KCHECK();
+    return;
   }
   k_huffman<<<nblk, HF_THREADS, sizeof(HuffSmem), c.stream>>>(sym.lo, sym.hi, sym.any_hi, d_m, d_freq, d_used, d_sel, d_selmtf, d_hb, d_goff);
   KLAUNCH(c); KCHECK();

@@ -645,6 +645,97 @@ k_rle_blocks(const u8* __restrict__ in, u64 N, u32 BS, const u32* __restrict__ c
   if (tid == 0) *nblocks_out = k;
 }
 
+// ---- C (libbz2 flavor) --------------------------------------------------------------------
+// libbz2 1.0.8 (bzlib.c add_char_to_block) keeps its run state across blocks, so the pieces it reads -- stretches of
+// one byte value, at most 255 long, the 255-chunks of a maximal run -- are those of the whole input, which are exactly
+// the phases W is scanned under.  A block holds whole pieces and closes right after the first piece that brings its
+// RLE1 size to >= blockSize.  So every block starts on a piece start with W(s) known from the block before: no run is
+// re-phased (b == s, ofs == 0), and k_rle_emit writes the block unchanged.  One CTA walks the blocks: per block one
+// tile search for the byte whose W reaches W(s) + blockSize, then the end of that byte's piece.
+__global__ void __launch_bounds__(RT_THREADS)
+k_rle_blocks_libbz2(const u8* __restrict__ in, u64 N, u32 BS, const u32* __restrict__ carry, const u64* __restrict__ prefix, u64 ntiles,
+                    BlkInfo* __restrict__ blocks, u32* nblocks_out, u32 maxblocks) {
+  __shared__ BlocksShared sh;
+  const u32 tid = threadIdx.x;
+  const u64 Wtotal = prefix[ntiles];
+  u64 s = 0, Ws = prefix[0];
+  u32 k = 0;
+  while (s < N && k < maxblocks) {
+    BlkInfo bi;
+    bi.s = s; bi.b = s; bi.Wb = Ws; bi.ofs = 0;
+    const u64 V = Ws + BS;
+    u64 e, We;
+    if (V > Wtotal) {
+      e = N; We = Wtotal;
+    } else {
+      // largest tile t >= tile(s) with prefix[t] < V, as in k_rle_blocks
+      u64 lo = s / RLE_TILE, hi = ntiles;
+      {
+        const u64 plo = prefix[lo];
+        u64 tg = lo + ((V - plo) >> 12);
+        if (tg >= ntiles) tg = ntiles - 1;
+        const u64 pg = prefix[tg], pg1 = prefix[tg + 1];
+        if (pg < V && pg1 >= V) { lo = tg; hi = tg + 1; }
+        else if (pg < V) lo = tg;
+        else if (tg > lo) hi = tg;
+      }
+      while (hi - lo > 1) {
+        const u64 span = hi - lo;
+        const u64 pi = lo + 1 + (span - 1) * (u64)tid / RT_THREADS;
+        const bool valid = pi < hi && (tid == 0 || pi != lo + 1 + (span - 1) * (u64)(tid - 1) / RT_THREADS);
+        const bool pr = valid && prefix[pi] < V;
+        const u32 tr = block_max256(pr ? tid + 1 : 0, sh.sc.red);
+        const u32 fl = block_min256((valid && !pr) ? tid : 0xffffffffu, sh.sc.red);
+        u64 nlo = lo, nhi = hi;
+        if (tr) nlo = lo + 1 + (span - 1) * (u64)(tr - 1) / RT_THREADS;
+        if (fl != 0xffffffffu) nhi = lo + 1 + (span - 1) * (u64)fl / RT_THREADS;
+        lo = nlo; hi = nhi;
+      }
+      const u64 t = lo, tstart = t * RLE_TILE;
+      TileView v;
+      tile_view(in, N, tstart, carry[t], sh.sc, v);
+      // f: the smallest position whose inclusive W reaches V (it exists: prefix[t+1] >= V)
+      u32 found = 0xffffffffu;
+      {
+        u64 acc = prefix[t] + v.excl;
+        for (u32 j = 0; j < v.cnt; j++) {
+          acc += v.w[j];
+          if (acc >= V) { found = tid * RT_PER + j; break; }
+        }
+      }
+      const u32 fo = block_min256(found, sh.sc.red);
+      if (fo / RT_PER == tid) {
+        u64 acc = prefix[t] + v.excl;
+        for (u32 j = 0; j <= fo % RT_PER; j++) acc += v.w[j];
+        sh.r64 = acc;
+      }
+      // phase of f inside its maximal run: the last byte change at or before f in the tile, else the carry
+      u32 ls = 0;
+      for (u32 j = 0; j < RT_PER; j++) {
+        const u32 pos = tid * RT_PER + j;
+        if (pos >= 1 && pos <= fo && in[tstart + pos] != in[tstart + pos - 1]) ls = pos + 1;
+      }
+      ls = block_max256(ls, sh.sc.red);  // also orders the write of sh.r64 before the read below
+      const u64 Wf = sh.r64;
+      const u64 f = tstart + fo;
+      const u32 d = ls ? fo - (ls - 1) : fo + carry[t];
+      const u32 r = d % 255 + 1;  // f is byte r of its piece
+      const u32 room = 255 - r;   // bytes the piece can still take
+      const u8 ch = in[f];
+      const u64 p = f + 1 + tid;
+      const u32 stop = block_min256((tid < room && p < N && in[p] != ch) ? tid : 0xffffffffu, sh.sc.red);
+      e = min(N, f + 1 + (stop == 0xffffffffu ? room : stop));
+      const u32 L = r + (u32)(e - f - 1);  // length of the closing piece
+      We = Wf - outfresh(r) + outfresh(L);
+    }
+    bi.e = e; bi.n = (u32)(We - Ws);
+    if (tid == 0) blocks[k] = bi;
+    k++;
+    s = e; Ws = We;
+  }
+  if (tid == 0) *nblocks_out = k;
+}
+
 // ---- CRC constants ---------------------------------------------------------------------------
 // The block CRC is linear: the pure polynomial remainder R (no init, no final XOR) of a byte string is the XOR of the
 // remainders of its pieces, each multiplied by x^(8 * bytes after the piece); leading zero bytes add nothing.
@@ -1112,9 +1203,31 @@ static void cut_blocks(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& pl
 void rle1_cut_range(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan, size_t first, size_t count) {
   cut_blocks(c, d_in, n, level, plan, false, first, count);
 }
+// libbz2 flavor: every block of the buffer, walked by one CTA (see k_rle_blocks_libbz2).  A block holds at least
+// blockSize RLE1 bytes and RLE1 makes at most 5 of 4 raw bytes, so there are at most n / (4 BS / 5) + 1 blocks.
+static void cut_blocks_libbz2(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan) {
+  StageScope s(c, ST_RLE1);
+  if (n == 0) return;
+  const u32 BS = rle1_block_size(level);
+  const u64 ntiles = (n + RLE_TILE - 1) / RLE_TILE;
+  const u32 maxblocks = (u32)(n / ((u64)BS * 4 / 5) + 2);
+  plan.blocks.alloc(c, maxblocks);
+  c.stats.rle_walk_serial++;
+  DBuf<u32> dnb(c, 1);
+  k_rle_blocks_libbz2<<<1, RT_THREADS, 0, c.stream>>>(d_in, n, BS, plan.tile_carry, plan.tile_prefix, ntiles, plan.blocks, dnb, maxblocks);
+  KLAUNCH(c); KCHECK();
+  u32 nb = 0;
+  c.to_host(&nb, dnb, 4);
+  c.sync();
+  plan.nblocks = nb;
+  plan.h_blocks.resize(nb);
+  if (nb) c.to_host(plan.h_blocks.data(), plan.blocks, sizeof(BlkInfo) * nb);
+  c.sync();
+}
 void rle1_plan(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan) {
   rle1_scan_tiles(c, d_in, n, plan);
-  cut_blocks(c, d_in, n, level, plan, true, 0, 0);
+  if (c.bz_flavor == B2_BZ2_LIBBZ2) cut_blocks_libbz2(c, d_in, n, level, plan);
+  else cut_blocks(c, d_in, n, level, plan, true, 0, 0);
 }
 void rle1_materialize(Ctx& c, const u8* d_in, size_t n, const Rle1Plan& plan, size_t first, size_t count, u8* d_T, u32* d_n, u32* d_crc) {
   if (count == 0) return;

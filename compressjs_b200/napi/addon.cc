@@ -30,15 +30,16 @@ static bool buf_arg(napi_env env, napi_value v, const uint8_t** p, size_t* n) {
   return true;
 }
 
-// compressFile(buffer, level) -> Buffer            (Bzip2.compressFile, lib/Bzip2.js:879)
+// compressFile(buffer, level, flavor) -> Buffer    (Bzip2.compressFile, lib/Bzip2.js:879; flavor: B2_BZ2_*, default 0)
 static napi_value CompressFile(napi_env env, napi_callback_info info) {
-  size_t argc = 2; napi_value argv[2];
+  size_t argc = 3; napi_value argv[3];
   napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr);
-  const uint8_t* in; size_t n; int32_t level = 9;
+  const uint8_t* in; size_t n; int32_t level = 9, flavor = B2_BZ2_COMPRESSJS;
   if (!buf_arg(env, argv[0], &in, &n)) return fail(env, B2_ERR_BAD_ARG);
   napi_get_value_int32(env, argv[1], &level);
+  if (argc > 2) napi_get_value_int32(env, argv[2], &flavor);
   uint8_t* out; size_t out_n;
-  int rc = b2_bzip2_compress(in, n, level, &out, &out_n);
+  int rc = b2_bzip2_compress_flavor(in, n, level, &out, &out_n, flavor);
   if (rc) return fail(env, rc);
   napi_value buf; napi_create_external_buffer(env, out_n, out, fin, nullptr, &buf);
   return buf;

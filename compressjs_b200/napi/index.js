@@ -43,10 +43,14 @@ function decode(output, call) {
 }
 
 var Bzip2 = Object.create(null);
-Bzip2.compressFile = function(inStream, outStream, props) {
+// options.flavor: 'compressjs' (the default) or 'libbz2' (the bytes bzip2 -N writes; include/b2bz.h B2_BZ2_LIBBZ2)
+var FLAVORS = { compressjs: 0, libbz2: 1 };
+Bzip2.compressFile = function(inStream, outStream, props, options) {
+  var name = (options && options.flavor !== undefined) ? options.flavor : 'compressjs';
+  if (!Object.prototype.hasOwnProperty.call(FLAVORS, name)) { throw new Error('unknown bzip2 flavor ' + name); }
   var level = (typeof props === 'number') ? props : 9;
   if (level < 1 || level > 9) { throw new Error('Invalid block size multiplier'); }
-  return deliver(outStream, native.compressFile(drain(inStream), level));
+  return deliver(outStream, native.compressFile(drain(inStream), level, FLAVORS[name]));
 };
 Bzip2.decompressFile = function(input, output, multistream) {
   var data = drain(input);

@@ -188,6 +188,26 @@ int b2_bwtc_decompress_stream(b2_read_fn rd, b2_write_fn wr, void* user);
 /* CRC32 helper object of lib/CRC32.js:72-103 (bzip2 polynomial, MSB first) */
 uint32_t b2_crc32_bzip2(const uint8_t* p, size_t n);
 
+/* ---- encoder flavors --------------------------------------------------------------------------------------------
+ * B2_BZ2_COMPRESSJS (the default, and what every call without a flavor writes): the bytes of compressjs.
+ * B2_BZ2_LIBBZ2: the bytes of libbz2 1.0.3 and later (bzip2 -N, Python's bz2.compress(data, N)).  Two stages differ:
+ *   - block cut: libbz2 keeps its RLE1 run state across blocks, so a run never restarts at a block edge, and a block
+ *     holds whole pieces (stretches of one byte value, at most 255 long): it closes after the first piece that brings
+ *     its RLE1 size to >= 100000 N - 19, so it holds at most 100000 N - 15 RLE1 bytes.  A compressjs block can end on
+ *     four equal bytes without their count byte, which libbz2 rejects; a libbz2-flavor stream never does.
+ *   - Huffman tables: libbz2's initial partition of the symbol frequencies, four rounds of assign and rebuild, and its
+ *     heap code-length builder with a 17-bit limit.
+ * Everything else (BWT, MTF, zero-run coder, headers, CRCs) is shared, and so are memory use, b2_bzip2_bound (the output
+ * size is checked against the buffer as for the default: a stream that would not fit fails with B2_ERR_BAD_ARG),
+ * b2_last_trace and b2_get_stats.  The _flavor calls take the arguments of the call they extend plus the flavor; an
+ * unknown flavor returns B2_ERR_BAD_ARG before any callback runs.  The plan, range and share calls below
+ * (multi-GPU encode) write the compressjs flavor only. */
+#define B2_BZ2_COMPRESSJS 0
+#define B2_BZ2_LIBBZ2 1
+int b2_bzip2_compress_flavor(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n, int flavor);
+int b2_bzip2_compress_stream_flavor(b2_read_fn rd, b2_write_fn wr, void* user, int level, int flavor);
+int b2_bzip2_compress_dev_flavor(const void* d_in, size_t n, int level, void* d_out, size_t out_cap, size_t* out_n, int flavor);
+
 /* ---- device-resident entry points (buffers already in HBM) ----------------------- */
 /* Same semantics as b2_bzip2_compress, but `d_in` / `d_out` are device pointers on the
  * b2_init() device (e.g. torch tensors' data_ptr()).  out_cap must be >= b2_bzip2_bound(n).
