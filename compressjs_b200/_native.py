@@ -23,7 +23,9 @@ EXPORTS = [
     "b2_bwt_cyclic", "b2_bwt_cyclic_batch", "b2_suffixsort", "b2_bwt_sentinel", "b2_bwt_inverse", "b2_bwtc_compress", "b2_bwtc_compress_unsized", "b2_bwtc_decompress", "b2_crc32_bzip2",
     "b2_bwtc_compress_stream", "b2_bwtc_decompress_stream",
     "b2_bzip2_bound", "b2_bzip2_compress_dev", "b2_bzip2_decompress_dev",
-    "b2_bzip2_plan", "b2_bzip2_plan_spec", "b2_bzip2_share_summary", "b2_bzip2_plan_share", "b2_bitshift_dev", "b2_dec_shard_open", "b2_dec_shard_export", "b2_dec_shard_finish", "b2_bzip2_encode_range_dev", "b2_get_stats", "b2_last_trace",
+    "b2_bzip2_plan", "b2_bzip2_plan_spec", "b2_bzip2_share_summary", "b2_bzip2_plan_share",
+    "b2_bzip2_plan_flavor", "b2_bzip2_share_cut_table", "b2_bzip2_plan_share_flavor", "b2_bzip2_encode_range_dev_flavor",
+    "b2_bitshift_dev", "b2_dec_shard_open", "b2_dec_shard_export", "b2_dec_shard_finish", "b2_bzip2_encode_range_dev", "b2_get_stats", "b2_last_trace",
 ]
 
 
@@ -105,6 +107,13 @@ def lib():
     L.b2_bitshift_dev.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_void_p]
     L.b2_bzip2_encode_range_dev.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_size_t, C.c_size_t, C.c_int,
                                             C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64), C.c_void_p]
+    L.b2_bzip2_encode_range_dev_flavor.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_size_t, C.c_size_t, C.c_int,
+                                                   C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64), C.c_void_p, C.c_int]
+    L.b2_bzip2_plan_flavor.argtypes = [C.c_void_p, C.c_size_t, C.c_int, szp, C.c_int]
+    L.b2_bzip2_share_cut_table.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_uint64, C.c_uint64, C.c_size_t, C.c_uint64,
+                                           C.POINTER(C.c_uint32)]
+    L.b2_bzip2_plan_share_flavor.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_uint64, C.c_uint64, C.c_size_t, C.c_size_t,
+                                             C.c_uint64, C.c_int, C.POINTER(C.c_uint64)]
     L.b2_get_stats.argtypes = [C.POINTER(Stats)]
     L.b2_last_trace.restype = C.c_size_t
     L.b2_last_trace.argtypes = [C.c_void_p, C.c_size_t]

@@ -682,15 +682,7 @@ int b2_bzip2_compress_flavor(const uint8_t* in, size_t n, int level, uint8_t** o
 }
 
 int b2_bzip2_plan(const void* d_in, size_t n, int level, size_t* total_blocks) {
-  return guarded([&]() {
-    if (level < 1 || level > 9) throw B2Error{B2_ERR_BAD_LEVEL, "Invalid block size multiplier"};
-    Ctx& c = ctx_locked();
-    c.reset_call();
-    const size_t nb = bzip2_plan(c, (const u8*)d_in, n, level);
-    if (total_blocks) *total_blocks = nb;
-    c.sync();
-    return 0;
-  });
+  return b2_bzip2_plan_flavor(d_in, n, level, total_blocks, B2_BZ2_COMPRESSJS);
 }
 
 int b2_dec_shard_open(const void* d_in, size_t n, int rank, int world, uint64_t* info) {
@@ -759,13 +751,62 @@ int b2_bzip2_plan_share(const void* d_buf, size_t n, int level, uint64_t state_i
   });
 }
 
+int b2_bzip2_plan_flavor(const void* d_in, size_t n, int level, size_t* total_blocks, int flavor) {
+  return guarded([&]() {
+    if (level < 1 || level > 9) throw B2Error{B2_ERR_BAD_LEVEL, "Invalid block size multiplier"};
+    check_flavor(flavor);
+    Ctx& c = ctx_locked();
+    c.reset_call();
+    c.bz_flavor = flavor;
+    const size_t nb = bzip2_plan(c, (const u8*)d_in, n, level);
+    if (total_blocks) *total_blocks = nb;
+    c.sync();
+    return 0;
+  });
+}
+
+int b2_bzip2_share_cut_table(const void* d_buf, size_t n, int level, uint64_t state_in, uint64_t w_in, size_t share_len, uint64_t dmax,
+                             uint32_t* table) {
+  return guarded([&]() {
+    if (level < 1 || level > 9) throw B2Error{B2_ERR_BAD_LEVEL, "Invalid block size multiplier"};
+    if (share_len > n || !table || dmax >= ((u64)1 << 31)) throw B2Error{B2_ERR_BAD_ARG, "bad share length, drift bound or table"};
+    Ctx& c = ctx_locked();
+    c.reset_call();
+    c.bz_flavor = B2_BZ2_LIBBZ2;
+    bzip2_share_cut_table(c, (const u8*)d_buf, n, level, state_in, w_in, share_len, dmax, table);
+    c.sync();
+    return 0;
+  });
+}
+
+int b2_bzip2_plan_share_flavor(const void* d_buf, size_t n, int level, uint64_t state_in, uint64_t w_in, size_t first, size_t count,
+                               uint64_t drift, int flavor, uint64_t* info) {
+  return guarded([&]() {
+    if (level < 1 || level > 9) throw B2Error{B2_ERR_BAD_LEVEL, "Invalid block size multiplier"};
+    check_flavor(flavor);
+    Ctx& c = ctx_locked();
+    c.reset_call();
+    c.bz_flavor = flavor;
+    bzip2_plan_share_flavor(c, (const u8*)d_buf, n, level, state_in, w_in, first, count, drift, info);
+    c.sync();
+    return 0;
+  });
+}
+
 int b2_bzip2_encode_range_dev(const void* d_in, size_t n, int level, size_t first, size_t count, int bit_phase, void* d_out,
                               size_t out_cap, uint64_t* out_bits, uint32_t* block_crcs) {
+  return b2_bzip2_encode_range_dev_flavor(d_in, n, level, first, count, bit_phase, d_out, out_cap, out_bits, block_crcs, B2_BZ2_COMPRESSJS);
+}
+
+int b2_bzip2_encode_range_dev_flavor(const void* d_in, size_t n, int level, size_t first, size_t count, int bit_phase, void* d_out,
+                                     size_t out_cap, uint64_t* out_bits, uint32_t* block_crcs, int flavor) {
   return guarded([&]() {
     if (level < 1 || level > 9) throw B2Error{B2_ERR_BAD_LEVEL, "Invalid block size multiplier"};
     if (bit_phase < 0 || bit_phase > 7) throw B2Error{B2_ERR_BAD_ARG, "bit_phase must be 0..7"};
+    check_flavor(flavor);
     Ctx& c = ctx_locked();
     c.reset_call();
+    c.bz_flavor = flavor;
     {
       StageScope tot(c, ST_TOTAL);
       bzip2_encode_range(c, (const u8*)d_in, n, level, first, count, bit_phase, (u8*)d_out, out_cap, out_bits, block_crcs);

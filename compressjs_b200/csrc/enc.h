@@ -34,7 +34,16 @@ void rle1_scan_tiles(Ctx& c, const u8* d_in, size_t n, Rle1Plan& plan, u64 st0 =
 // Cut of blocks [first, first+count) of the whole input from the speculative boundary W = first * blockSize, over a
 // plan whose tiles are scanned (exact unless a run-phase slip happened earlier in the input).
 void rle1_cut_range(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan, size_t first, size_t count);
-// Tile scan and exact cut of every block of d_in[0, n).
+// libbz2 flavor over a share buffer d_buf[0, n) = share + halo entered with run state st0 and W base W0
+// (b2_bzip2_share_cut_table / b2_bzip2_plan_share_flavor): the cut table of every entry drift 0..dmax into h_table
+// (4 u32 per row), and the cut of the blocks [first, first + count) whose first block starts at W = first * blockSize +
+// drift.  The table call keeps its tile scan and piece bitmap for the cut that follows on the same buffer and entry
+// state; rle1_release_share_probe drops them.
+void rle1_share_cut_table(Ctx& c, const u8* d_buf, size_t n, int level, u64 st0, u64 W0, size_t share_len, u64 dmax, u32* h_table);
+void rle1_cut_share_libbz2(Ctx& c, const u8* d_buf, size_t n, int level, u64 st0, u64 W0, size_t first, u64 drift, size_t count,
+                           Rle1Plan& plan);
+void rle1_release_share_probe();
+// Tile scan and exact cut of every block of d_in[0, n) (the flavor of c.bz_flavor).
 void rle1_plan(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan);
 // materialise blocks [first, first+count) of the plan into the slot layout at d_T (u8[count<<20]);
 // d_n receives their lengths, d_crc their CRCs.
@@ -132,6 +141,8 @@ size_t bzip2_plan(Ctx& c, const u8* d_in, size_t n, int level);
 void bzip2_plan_spec(Ctx& c, const u8* d_in, size_t n, int level, int rank, int world, u64* info);
 void bzip2_share_summary(Ctx& c, const u8* d_in, size_t n, u64* out);
 void bzip2_plan_share(Ctx& c, const u8* d_buf, size_t n, int level, u64 st0, u64 W0, size_t first, size_t count, u64* info);
+void bzip2_share_cut_table(Ctx& c, const u8* d_buf, size_t n, int level, u64 st0, u64 W0, size_t share_len, u64 dmax, u32* table);
+void bzip2_plan_share_flavor(Ctx& c, const u8* d_buf, size_t n, int level, u64 st0, u64 W0, size_t first, size_t count, u64 drift, u64* info);
 void bzip2_encode_range(Ctx& c, const u8* d_in, size_t n, int level, size_t first, size_t count, int bit_phase, u8* d_out, size_t out_cap,
                         u64* out_bits, u32* block_crcs);
 void bitshift_device(Ctx& c, const void* src, u64 nbits, int phase, void* dst);

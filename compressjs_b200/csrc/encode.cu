@@ -474,24 +474,28 @@ struct EncSession {
 };
 
 // ---- device-resident entry points ------------------------------------------------------------------------------
-// The plan of b2_bzip2_plan, _plan_spec or _plan_share, kept for the next b2_bzip2_encode_range_dev.  That call takes
-// it if (buffer, length, level) match; the cache is empty afterwards either way.  compress_dev drops it too.
+// The plan of b2_bzip2_plan(_flavor), _plan_spec or _plan_share(_flavor), kept for the next b2_bzip2_encode_range_dev
+// (_flavor).  That call takes it if (buffer, length, level, flavor) match; the cache is empty afterwards either way.
+// compress_dev drops it too.  The two flavors cut different blocks, so a plan never serves the other flavor.
 struct PlanCache {
   std::optional<Rle1Plan> plan;
-  const u8* ptr = nullptr; size_t n = 0; int level = 0;
-  std::optional<Rle1Plan> take(const u8* p, size_t n_, int level_) {
+  const u8* ptr = nullptr; size_t n = 0; int level = 0, flavor = B2_BZ2_COMPRESSJS;
+  std::optional<Rle1Plan> take(const u8* p, size_t n_, int level_, int flavor_) {
     std::optional<Rle1Plan> r;
-    if (plan && p == ptr && n_ == n && level_ == level) r = std::move(plan);
+    if (plan && p == ptr && n_ == n && level_ == level && flavor_ == flavor) r = std::move(plan);
     plan.reset();
     return r;
   }
-  void put(Rle1Plan&& p, const u8* p_, size_t n_, int level_) { plan = std::move(p); ptr = p_; n = n_; level = level_; }
+  void put(Rle1Plan&& p, const u8* p_, size_t n_, int level_, int flavor_) {
+    plan = std::move(p); ptr = p_; n = n_; level = level_; flavor = flavor_;
+  }
 };
 static PlanCache g_plan;
-void bzip2_release_plan() { g_plan.plan.reset(); }
+void bzip2_release_plan() { g_plan.plan.reset(); rle1_release_share_probe(); }
 
 void bzip2_compress_dev(Ctx& c, const u8* d_in, size_t n, int level, u8* d_out, size_t out_cap, size_t* out_n) {
   g_plan.plan.reset();
+  rle1_release_share_probe();
   Rle1Plan plan;
   rle1_plan(c, d_in, n, level, plan);
   c.trace.clear();
@@ -506,7 +510,7 @@ size_t bzip2_plan(Ctx& c, const u8* d_in, size_t n, int level) {
   rle1_plan(c, d_in, n, level, plan);
   c.trace.clear();
   const size_t nb = plan.nblocks;
-  g_plan.put(std::move(plan), d_in, n, level);
+  g_plan.put(std::move(plan), d_in, n, level, c.bz_flavor);
   return nb;
 }
 
@@ -528,13 +532,13 @@ void bzip2_plan_spec(Ctx& c, const u8* d_in, size_t n, int level, int rank, int 
   rle1_cut_range(c, d_in, n, level, plan, first, count);
   c.trace.clear();
   range_info(plan, first, count, total, info);
-  g_plan.put(std::move(plan), d_in, n, level);
+  g_plan.put(std::move(plan), d_in, n, level, B2_BZ2_COMPRESSJS);
 }
 
 // Blocks [first, first+count) without file header and trailer, from bit `bit_phase` of d_out.
 void bzip2_encode_range(Ctx& c, const u8* d_in, size_t n, int level, size_t first, size_t count, int bit_phase, u8* d_out, size_t out_cap,
                         u64* out_bits, u32* block_crcs) {
-  std::optional<Rle1Plan> plan = g_plan.take(d_in, n, level);
+  std::optional<Rle1Plan> plan = g_plan.take(d_in, n, level, c.bz_flavor);
   if (!plan) rle1_plan(c, d_in, n, level, plan.emplace());
   c.trace.clear();
   const size_t nb_all = plan->first_index + plan->nblocks;  // exact plans: first_index == 0
@@ -569,7 +573,21 @@ void bzip2_plan_share(Ctx& c, const u8* d_buf, size_t n, int level, u64 st0, u64
   rle1_scan_tiles(c, d_buf, n, plan, st0, W0);
   rle1_cut_range(c, d_buf, n, level, plan, first, count);
   range_info(plan, first, count, plan.w_total, info);
-  g_plan.put(std::move(plan), d_buf, n, level);
+  g_plan.put(std::move(plan), d_buf, n, level, B2_BZ2_COMPRESSJS);
+}
+// libbz2 flavor: table row d = the cut of the share when its first block has drift d (see k_cut_table).
+void bzip2_share_cut_table(Ctx& c, const u8* d_buf, size_t n, int level, u64 st0, u64 W0, size_t share_len, u64 dmax, u32* table) {
+  rle1_share_cut_table(c, d_buf, n, level, st0, W0, share_len, dmax, table);
+}
+// The share plan of either flavor.  compressjs: bzip2_plan_share (drift unused).  libbz2: the blocks [first, first+count)
+// from the entry W = first * blockSize + drift that the host chained from the tables.  info as bzip2_plan_share's.
+void bzip2_plan_share_flavor(Ctx& c, const u8* d_buf, size_t n, int level, u64 st0, u64 W0, size_t first, size_t count, u64 drift, u64* info) {
+  if (c.bz_flavor != B2_BZ2_LIBBZ2) { bzip2_plan_share(c, d_buf, n, level, st0, W0, first, count, info); return; }
+  g_plan.plan.reset();
+  Rle1Plan plan;
+  rle1_cut_share_libbz2(c, d_buf, n, level, st0, W0, first, drift, count, plan);
+  range_info(plan, first, count, plan.w_total, info);
+  g_plan.put(std::move(plan), d_buf, n, level, B2_BZ2_LIBBZ2);
 }
 
 // Bzip2.compressFile from a host source into a host sink: b2_bzip2_compress (the caller's buffer, complete from the

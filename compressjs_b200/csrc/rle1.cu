@@ -24,6 +24,7 @@
 //   CRC k_crc_pieces : the same remainders over 256-byte pieces of arbitrary byte ranges (decoder, b2_crc32).
 #include <algorithm>
 #include <cstdlib>
+#include <optional>
 #include "enc.h"
 
 #define RT_THREADS 256
@@ -109,8 +110,10 @@ __device__ __forceinline__ u32 block_max256(u32 v, u32* red) {
   return r;
 }
 
-// Whole CTA (RT_THREADS threads).  carry = run length (mod 255) entering the tile.
-__device__ void tile_view(const u8* __restrict__ in, u64 N, u64 tstart, u32 carry, TileScratch& sc, TileView& v) {
+// Whole CTA (RT_THREADS threads).  carry = run length (mod 255) entering the tile.  PIECES: *pieces receives bit j for
+// every byte j of the thread that starts a piece (phase 0 mod 255 of its maximal run: a run start, or byte 255 k of it).
+template <bool PIECES = false>
+__device__ void tile_view(const u8* __restrict__ in, u64 N, u64 tstart, u32 carry, TileScratch& sc, TileView& v, u32* pieces = nullptr) {
   const u32 tid = threadIdx.x;
   const u64 remain = N - tstart;
   v.len = remain < RLE_TILE ? (u32)remain : RLE_TILE;
@@ -146,7 +149,7 @@ __device__ void tile_view(const u8* __restrict__ in, u64 N, u64 tstart, u32 carr
   }
   const u32 ex = block_excl_max256(last_local, sc.ws);  // (last start before this thread) + 1
   u32 rs = ex ? ex - 1 : 0;
-  u32 sum = 0;
+  u32 sum = 0, pm = 0;
 #pragma unroll
   for (int j = 0; j < RT_PER; j++) {
     u32 ww = 0;
@@ -155,10 +158,12 @@ __device__ void tile_view(const u8* __restrict__ in, u64 N, u64 tstart, u32 carr
       if (smask & (1u << j)) rs = pos;
       const u32 d = pos - rs + (rs == 0 ? carry : 0);
       ww = w_of_dist(d);
+      if constexpr (PIECES) pm |= (d % 255 == 0 ? 1u : 0u) << j;
     }
     v.w[j] = (u8)ww;
     sum += ww;
   }
+  if constexpr (PIECES) *pieces = pm;
   u32 total;
   v.excl = block_excl_add<RT_THREADS, u32>(sum, sc.ws, &total);
   v.total = total;
@@ -736,6 +741,128 @@ k_rle_blocks_libbz2(const u8* __restrict__ in, u64 N, u32 BS, const u32* __restr
   if (tid == 0) *nblocks_out = k;
 }
 
+// ---- E (libbz2 flavor, sharded input) ---------------------------------------------------------
+// The libbz2 cut in W space: block k + 1 starts at S(k+1) = next(S(k) + M), M = blockSize, where next(x) is the first
+// piece start at or after W position x.  A piece holds at most 5 RLE1 bytes, so next(x) - x is 0..4, and the drift
+// S(k) - k M grows by at most 4 a block.  A share that does not know the blocks in front of it walks this chain once
+// for every drift its first block can have (b2_bzip2_share_cut_table), over a bitmap of the piece starts of share +
+// halo in W space; the host then chains the shares and each walks its own entry again (b2_bzip2_plan_share_flavor).
+//
+// Probe: bit p of `bits` is set when a piece starts at W position W0 + p (W0 = the buffer's W base, prefix[0]).  One
+// CTA per tile; the tile's bits are gathered in shared memory, its interior words stored and the two edge words, which
+// it may share with its neighbours, OR-ed.  `bits` is zeroed by the caller.  *wshare = W(share_len) - W0 if
+// share_len < N (the caller presets W(N) - W0).
+#define PROBE_WORDS (RLE_TILE * 5 / 4 / 32 + 2)
+__global__ void __launch_bounds__(RT_THREADS)
+k_piece_probe(const u8* __restrict__ in, u64 N, const u32* __restrict__ carry, const u64* __restrict__ prefix, u64 share_len,
+              u32* __restrict__ bits, u64* __restrict__ wshare) {
+  __shared__ TileScratch sc;
+  __shared__ u32 sm[PROBE_WORDS];
+  const u32 tid = threadIdx.x;
+  const u64 t = blockIdx.x, tstart = t * RLE_TILE;
+  const u64 base = prefix[t] - prefix[0], end = prefix[t + 1] - prefix[0];
+  for (u32 i = tid; i < PROBE_WORDS; i += RT_THREADS) sm[i] = 0;
+  TileView v;
+  u32 pm;
+  tile_view<true>(in, N, tstart, carry[t], sc, v, &pm);  // its first barrier orders the clearing above
+  u32 a = (u32)(base & 31) + v.excl;  // bit of sm[] at the thread's first byte
+  for (u32 j = 0; j < v.cnt; j++) {
+    if ((pm >> j) & 1) atomicOr(&sm[a >> 5], 1u << (a & 31));
+    if (tstart + tid * RT_PER + j == share_len) *wshare = (base & ~(u64)31) + a;
+    a += v.w[j];
+  }
+  __syncthreads();
+  const u64 w0 = base >> 5;
+  const u32 nw = (u32)(((end + 31) >> 5) - w0);
+  for (u32 i = tid; i < nw; i += RT_THREADS) {
+    const u32 x = sm[i];
+    if (i == 0 || i == nw - 1) { if (x) atomicOr(&bits[w0 + i], x); }
+    else bits[w0 + i] = x;
+  }
+}
+
+// next(x) inside the buffer: the first piece start in [x, x + 4] (W positions relative to W0), or CUT_NONE when there
+// is none before wbuf (the piece that holds x goes on past the buffer, or x is past it).  bits has wbuf / 32 + 2 words.
+#define CUT_NONE (~0ull)
+__device__ __forceinline__ u64 next_piece(const u32* __restrict__ bits, u64 wbuf, u64 x) {
+  if (x >= wbuf) return CUT_NONE;
+  const u64 wi = x >> 5;
+  const u64 two = (u64)bits[wi] | ((u64)bits[wi + 1] << 32);
+  const u64 m = (two >> (x & 31)) & 0x1f;
+  return m ? x + (u64)(__ffsll((long long)m) - 1) : CUT_NONE;  // no piece starts at wbuf or later
+}
+__device__ __forceinline__ bool is_piece(const u32* __restrict__ bits, u64 p) { return (bits[p >> 5] >> (p & 31)) & 1; }
+
+// One thread per entry drift d in [0, dmax]: the first block at or after the share's W start w_in with drift d is
+// block k = ceil((w_in - d) / M) (0 if d >= w_in), starting at S = k M + d.  The walk counts the blocks that start in
+// the share (S - w_in < wshare) and stops at the first one that does not.  Row d = {k, blocks, drift of the block
+// after them, flags} (include/b2bz.h, B2_CUT_*).
+__global__ void k_cut_table(const u32* __restrict__ bits, u64 wbuf, u64 wshare, u64 w_in, u32 M, u64 dmax, uint4* __restrict__ table) {
+  const u64 d = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (d > dmax) return;
+  const u64 k = w_in > d ? (w_in - d + M - 1) / M : 0;
+  u64 S = k * M + d - w_in;
+  u32 flags = 0, cnt = 0;
+  if (S < wbuf && !is_piece(bits, S)) flags |= B2_CUT_NOT_PIECE;
+  while (S < wshare) {
+    cnt++;
+    const u64 nx = next_piece(bits, wbuf, S + M);
+    if (cnt == 1 && nx == S + M) flags |= B2_CUT_STEP_EXACT;
+    if (nx == CUT_NONE) { flags |= B2_CUT_BUF_END; break; }
+    S = nx;
+  }
+  const u32 exit_d = (flags & B2_CUT_BUF_END) ? 0u : (u32)(w_in + S - (k + cnt) * M);
+  table[d] = make_uint4((u32)k, cnt, exit_d, flags);
+}
+
+// The chain of one entry: starts[0] = S0, starts[i + 1] = next(starts[i] + M) for up to `count` blocks; a block whose
+// next start lies past the buffer ends at the buffer's end (wbuf), and the walk stops there.  *ncut = blocks walked.
+__global__ void k_cut_chain(const u32* __restrict__ bits, u64 wbuf, u64 S0, u32 M, u64 count, u64* __restrict__ starts, u64* __restrict__ ncut) {
+  u64 S = S0, i = 0;
+  starts[0] = S;
+  if (S < wbuf && is_piece(bits, S)) {
+    while (i < count) {
+      u64 nx = next_piece(bits, wbuf, S + M);
+      if (nx == CUT_NONE) nx = wbuf;
+      starts[++i] = nx;
+      S = nx;
+      if (S == wbuf) break;
+    }
+  }
+  *ncut = i;
+}
+
+// One CTA per W position S = W0 + starts[i]: raw[i] = the raw position of the piece that starts there (the smallest
+// position whose inclusive W exceeds S), N for S >= W(N).
+__global__ void __launch_bounds__(RT_THREADS)
+k_w_to_raw(const u8* __restrict__ in, u64 N, const u32* __restrict__ carry, const u64* __restrict__ prefix, u64 ntiles,
+           const u64* __restrict__ starts, u64* __restrict__ raw) {
+  __shared__ BlocksShared sh;
+  const u32 tid = threadIdx.x;
+  const u64 S = prefix[0] + starts[blockIdx.x];
+  if (S >= prefix[ntiles]) { if (tid == 0) raw[blockIdx.x] = N; return; }
+  if (tid == 0) {
+    u64 lo = 0, hi = ntiles;  // prefix[lo] <= S < prefix[hi]
+    while (hi - lo > 1) {
+      const u64 mid = (lo + hi) >> 1;
+      if (prefix[mid] <= S) lo = mid; else hi = mid;
+    }
+    sh.r64 = lo;
+  }
+  __syncthreads();
+  const u64 t = sh.r64;
+  TileView v;
+  tile_view(in, N, t * RLE_TILE, carry[t], sh.sc, v);
+  u32 found = 0xffffffffu;
+  u64 acc = prefix[t] + v.excl;
+  for (u32 j = 0; j < v.cnt; j++) {
+    acc += v.w[j];
+    if (acc > S) { found = tid * RT_PER + j; break; }
+  }
+  const u32 f = block_min256(found, sh.sc.red);
+  if (tid == 0) raw[blockIdx.x] = t * RLE_TILE + f;
+}
+
 // ---- CRC constants ---------------------------------------------------------------------------
 // The block CRC is linear: the pure polynomial remainder R (no init, no final XOR) of a byte string is the XOR of the
 // remainders of its pieces, each multiplied by x^(8 * bytes after the piece); leading zero bytes add nothing.
@@ -1222,6 +1349,114 @@ static void cut_blocks_libbz2(Ctx& c, const u8* d_in, size_t n, int level, Rle1P
   plan.nblocks = nb;
   plan.h_blocks.resize(nb);
   if (nb) c.to_host(plan.h_blocks.data(), plan.blocks, sizeof(BlkInfo) * nb);
+  c.sync();
+}
+// libbz2 flavor over a share buffer: the piece-start bitmap (k_piece_probe) of a scanned plan; wbuf / wshare = W of the
+// buffer's / share's end relative to the buffer's W base.
+struct PieceMap {
+  DBuf<u32> bits;
+  u64 wbuf = 0, wshare = 0;
+};
+static void piece_map(Ctx& c, const u8* d_buf, size_t n, size_t share_len, const Rle1Plan& plan, u64 W0, PieceMap& pm) {
+  StageScope s(c, ST_RLE1);
+  pm.wbuf = plan.w_total - W0;
+  pm.wshare = pm.wbuf;
+  const u64 nwords = pm.wbuf / 32 + 2;
+  pm.bits.alloc(c, nwords);
+  CUDA_CHECK(cudaMemsetAsync(pm.bits, 0, 4 * nwords, c.stream));
+  const u64 ntiles = (n + RLE_TILE - 1) / RLE_TILE;
+  DBuf<u64> dws(c, 1);
+  c.to_device(dws, &pm.wshare, 8);
+  k_piece_probe<<<(unsigned)ntiles, RT_THREADS, 0, c.stream>>>(d_buf, n, plan.tile_carry, plan.tile_prefix, share_len, pm.bits, dws);
+  KLAUNCH(c); KCHECK();
+  c.to_host(&pm.wshare, dws, 8);
+  c.sync();
+}
+// The tile scan and piece bitmap of the last b2_bzip2_share_cut_table.  The b2_bzip2_plan_share_flavor that follows on
+// the same (buffer, length, run state, W base) walks its entry over them instead of scanning and probing the share again.
+struct ShareProbe {
+  Rle1Plan plan;
+  PieceMap pm;
+  const u8* ptr = nullptr;
+  size_t n = 0;
+  u64 st0 = 0, W0 = 0;
+};
+static std::optional<ShareProbe> g_probe;
+void rle1_release_share_probe() { g_probe.reset(); }
+static void share_probe(Ctx& c, const u8* d_buf, size_t n, u64 st0, u64 W0, size_t share_len, ShareProbe& p) {
+  p.ptr = d_buf; p.n = n; p.st0 = st0; p.W0 = W0;
+  rle1_scan_tiles(c, d_buf, n, p.plan, st0, W0);
+  piece_map(c, d_buf, n, share_len, p.plan, W0, p.pm);
+}
+void rle1_share_cut_table(Ctx& c, const u8* d_buf, size_t n, int level, u64 st0, u64 W0, size_t share_len, u64 dmax, u32* h_table) {
+  g_probe.reset();
+  const u32 M = rle1_block_size(level);
+  if (n == 0) {  // nothing starts in an empty buffer: every entry passes through
+    for (u64 d = 0; d <= dmax; d++) {
+      const u64 k = W0 > d ? (W0 - d + M - 1) / M : 0;
+      u32* row = h_table + 4 * d;
+      row[0] = (u32)k; row[1] = 0; row[2] = (u32)d; row[3] = 0;
+    }
+    return;
+  }
+  ShareProbe p;
+  share_probe(c, d_buf, n, st0, W0, share_len, p);
+  StageScope s(c, ST_RLE1);
+  DBuf<uint4> dt(c, dmax + 1);
+  k_cut_table<<<(unsigned)((dmax + 128) / 128), 128, 0, c.stream>>>(p.pm.bits, p.pm.wbuf, p.pm.wshare, W0, M, dmax, dt);
+  KLAUNCH(c); KCHECK();
+  c.to_host(h_table, dt, 16 * (dmax + 1));
+  c.sync();
+  g_probe = std::move(p);
+}
+// The blocks [first, first + count) of the whole input whose first block starts at W = first * M + drift, inside the
+// share buffer d_buf[0, n) entered with run state st0 and W base W0, in the form k_rle_blocks_libbz2 writes (b == s,
+// ofs == 0).  The scan and bitmap of the table call before it are reused when they are of the same buffer and entry
+// state.  Fewer blocks are cut when the entry is not a piece start or the buffer ends first (its last block then ends at
+// the buffer's end).
+void rle1_cut_share_libbz2(Ctx& c, const u8* d_buf, size_t n, int level, u64 st0, u64 W0, size_t first, u64 drift, size_t count,
+                           Rle1Plan& plan) {
+  std::optional<ShareProbe> p;
+  if (g_probe && g_probe->ptr == d_buf && g_probe->n == n && g_probe->st0 == st0 && g_probe->W0 == W0) p = std::move(g_probe);
+  g_probe.reset();
+  const u32 M = rle1_block_size(level);
+  const u64 S0 = (u64)first * M + drift;
+  if (!p && (n == 0 || count == 0 || S0 < W0)) {  // nothing to cut: only W at the buffer's end is asked for
+    rle1_scan_tiles(c, d_buf, n, plan, st0, W0);
+  } else if (!p) {
+    p.emplace();
+    share_probe(c, d_buf, n, st0, W0, n, *p);
+  }
+  if (p) plan = std::move(p->plan);
+  plan.first_index = first;
+  plan.nblocks = 0;
+  plan.h_blocks.clear();
+  if (n == 0 || count == 0 || S0 < W0) return;
+  const PieceMap& pm = p->pm;
+  StageScope s(c, ST_RLE1);
+  const u64 ntiles = (n + RLE_TILE - 1) / RLE_TILE;
+  count = std::min<u64>(count, pm.wbuf / M + 1);  // a block holds at least M RLE1 bytes, except one that ends the buffer
+  DBuf<u64> starts(c, count + 1), raw(c, count + 1), dn(c, 1);
+  k_cut_chain<<<1, 1, 0, c.stream>>>(pm.bits, pm.wbuf, S0 - W0, M, count, starts, dn);
+  KLAUNCH(c); KCHECK();
+  u64 nb = 0;
+  c.to_host(&nb, dn, 8);
+  c.sync();
+  if (nb == 0) return;
+  k_w_to_raw<<<(unsigned)(nb + 1), RT_THREADS, 0, c.stream>>>(d_buf, n, plan.tile_carry, plan.tile_prefix, ntiles, starts, raw);
+  KLAUNCH(c); KCHECK();
+  std::vector<u64> hs(nb + 1), hr(nb + 1);
+  c.to_host(hs.data(), starts, 8 * (nb + 1));
+  c.to_host(hr.data(), raw, 8 * (nb + 1));
+  c.sync();
+  plan.h_blocks.resize(nb);
+  for (u64 i = 0; i < nb; i++) {
+    BlkInfo& bi = plan.h_blocks[i];
+    bi.s = hr[i]; bi.e = hr[i + 1]; bi.b = bi.s; bi.Wb = W0 + hs[i]; bi.ofs = 0; bi.n = (u32)(hs[i + 1] - hs[i]);
+  }
+  plan.blocks.alloc(c, nb);
+  c.to_device(plan.blocks, plan.h_blocks.data(), sizeof(BlkInfo) * nb);
+  plan.nblocks = nb;
   c.sync();
 }
 void rle1_plan(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan) {

@@ -18,7 +18,10 @@ bitstream gather (north_star: "NCCL over NVLink only for the final bitstream gat
 With a sharded INPUT (compress_shares) a rank holds only its share of the bytes plus a halo: the ranks
 exchange tiny share summaries (RLE1 run state, leading run, RLE1 output) so that every rank knows the
 run state and the RLE1 output in front of its share, cuts its blocks speculatively and checks that the
-pieces chain up (b2_bzip2_share_summary / b2_bzip2_plan_share).
+pieces chain up (b2_bzip2_share_summary / b2_bzip2_plan_share).  The libbz2 flavor's cuts drift away from
+multiples of blockSize, so there every rank cuts its share once for every drift its first block can have
+(b2_bzip2_share_cut_table), the ranks exchange these tables, and every rank chains them the same way
+(libbz2_share_chain) to find the entry of its share.
 
 The resulting stream is byte-identical to Bzip2.compressFile on one GPU (and to the oracle).
 The shifting / merging below is plain torch tensor code so that the same logic runs on CPU tensors
@@ -352,8 +355,18 @@ def compress_sharded(encode_range, nblocks, level, device, group=None):
     return place_fragments(frag, nbits, count, crcs, level, device, group)
 
 
-def _range_encoder(L, d_in, n, level):
+FLAVORS = {"compressjs": 0, "libbz2": 1}   # B2_BZ2_COMPRESSJS, B2_BZ2_LIBBZ2
+
+
+def _flavor_id(flavor):
+    if flavor not in FLAVORS:
+        raise ValueError("unknown bzip2 flavor %r (expected 'compressjs' or 'libbz2')" % (flavor,))
+    return FLAVORS[flavor]
+
+
+def _range_encoder(L, d_in, n, level, flavor="compressjs"):
     from . import _native
+    fl = _flavor_id(flavor)
 
     def encode_range(first, count):
         if count == 0:
@@ -362,25 +375,26 @@ def _range_encoder(L, d_in, n, level):
         out = torch.empty(cap, dtype=torch.uint8, device=d_in.device)
         bits = C.c_uint64()
         crcs = (C.c_uint32 * count)()
-        rc = L.b2_bzip2_encode_range_dev(d_in.data_ptr(), n, level, first, count, 0, out.data_ptr(), cap, C.byref(bits), crcs)
+        rc = L.b2_bzip2_encode_range_dev_flavor(d_in.data_ptr(), n, level, first, count, 0, out.data_ptr(), cap, C.byref(bits), crcs, fl)
         if rc:
-            raise RuntimeError("b2_bzip2_encode_range_dev: " + _native.last_error())
+            raise RuntimeError("b2_bzip2_encode_range_dev_flavor: " + _native.last_error())
         return out, int(bits.value), list(crcs)
 
     return encode_range
 
 
-def gpu_encode_range_fn(d_in, level):
+def gpu_encode_range_fn(d_in, level, flavor="compressjs"):
     """encode_range callable backed by libb2bz.so for a uint8 CUDA tensor holding the whole input
     (exact plan: every block boundary of the file is cut on this GPU)."""
     from . import _native
     L = _native.lib()
     n = d_in.numel()
+    fl = _flavor_id(flavor)
     total = C.c_size_t()
-    rc = L.b2_bzip2_plan(d_in.data_ptr(), n, level, C.byref(total))
+    rc = L.b2_bzip2_plan_flavor(d_in.data_ptr(), n, level, C.byref(total), fl)
     if rc:
-        raise RuntimeError("b2_bzip2_plan: " + _native.last_error())
-    return _range_encoder(L, d_in, n, level), int(total.value)
+        raise RuntimeError("b2_bzip2_plan_flavor: " + _native.last_error())
+    return _range_encoder(L, d_in, n, level, flavor), int(total.value)
 
 
 def spec_plan_ok(infos, n):
@@ -401,19 +415,21 @@ def spec_plan_ok(infos, n):
     return nxt == total and pos == n
 
 
-def compress_file_sharded(d_in, level=9, group=None):
+def compress_file_sharded(d_in, level=9, group=None, flavor="compressjs"):
     """Whole-file bzip2 encode of a CUDA uint8 tensor present on every rank; stream on rank 0.
 
     Block cutting: every rank cuts only ITS share of the blocks from a speculative start boundary
     (b2_bzip2_plan_spec); the ranks then check that the pieces chain exactly (end(r) == start(r+1), ...).
-    If a run-phase slip makes the speculation fail anywhere, all ranks fall back to the exact plan."""
+    If a run-phase slip makes the speculation fail anywhere, all ranks fall back to the exact plan.
+    flavor="libbz2" writes the bytes of libbz2 (bz2.compress): its cuts drift away from multiples of blockSize,
+    so every rank takes the exact plan of the whole input and encodes its range of the blocks."""
     from . import _native
     L = _native.lib()
     n = d_in.numel()
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
-    if world == 1:
-        enc, nblocks = gpu_encode_range_fn(d_in, level)
+    if world == 1 or _flavor_id(flavor) != FLAVORS["compressjs"]:
+        enc, nblocks = gpu_encode_range_fn(d_in, level, flavor)
         return compress_sharded(enc, nblocks, level, d_in.device, group)
     PHASES.clear()
     t0 = time.perf_counter()
@@ -485,6 +501,54 @@ def share_plan_inputs(summaries, level):
     return res, total, W
 
 
+CUT_NOT_PIECE, CUT_STEP_EXACT, CUT_BUF_END = 1, 2, 4   # flags of a cut-table row (include/b2bz.h B2_CUT_*)
+
+
+def share_drift_bound(w_in, level):
+    """The largest drift the first block of a share that starts at W position w_in can have: 4 per block in front."""
+    M = level * 100000 - 19
+    return 4 * ((w_in + M - 1) // M)
+
+
+def libbz2_share_chain(ins, w_total, tables, level, ends_input):
+    """Chains the libbz2 cut tables of all shares, in rank order.  ins = share_plan_inputs(...)[0]; w_total = RLE1 bytes
+    of the whole input; tables[r] = rank r's rows indexed by entry drift, (k, blocks, exit drift, flags) as
+    b2_bzip2_share_cut_table writes them (a [drifts, 4] array or a list of rows; None for an empty share); ends_input[r]: rank r's buffer ends the input.
+    Rank 0 enters at block 0 with drift 0 and every rank's row gives the next rank's entry.  Returns
+    ([(first block, drift, block count)] per rank, total blocks), or None when some rank's halo is too short for its
+    last block (or a row contradicts its entry, which a correct table never does)."""
+    M = level * 100000 - 19
+    k, d, done = 0, 0, w_total == 0
+    res = []
+    for r, row_in in enumerate(ins):
+        w_in = row_in[1]
+        w_end = ins[r + 1][1] if r + 1 < len(ins) else w_total
+        if done or k * M + d >= w_end:    # no block starts in this share: the entry passes through
+            res.append((k, d, 0))
+            continue
+        rows = tables[r]
+        if rows is None or d >= len(rows):
+            return None
+        rk, cnt, ex, fl = (int(x) for x in rows[d])
+        if rk == k and not (fl & CUT_NOT_PIECE):
+            pass
+        elif rk + 1 == k and (fl & CUT_STEP_EXACT):   # the entry is within 4 of w_in: row d less its first block
+            cnt -= 1
+        else:
+            return None
+        res.append((k, d, cnt))
+        if fl & CUT_BUF_END:
+            if not ends_input[r]:
+                return None
+            done = True
+            k += cnt
+        else:
+            k, d = k + cnt, ex
+    if not done:
+        return None
+    return res, k
+
+
 def _i64(v):
     return v - (1 << 64) if v >= (1 << 63) else v
 
@@ -493,13 +557,54 @@ def _u64(v):
     return v + (1 << 64) if v < 0 else v
 
 
-def compress_shares(d_buf, share_len, level=9, group=None, host_out=None, keep_sharded=False):
+def _all_gather_tables(rows, ends_input, world, group, dev):
+    """All-gather of every rank's cut table (an int32 array [drifts, 4]) and of whether its buffer ends the input.  The
+    tables differ in length: the ranks first exchange (rows, ends flag), then their tables padded to the longest one, so
+    each rank receives world x 16 x (rows of the longest table) bytes.  Returns ([int32 numpy array per rank], [flags])."""
+    if world == 1:
+        return [rows], [ends_input]
+    head = torch.tensor([rows.shape[0], int(ends_input)], dtype=torch.int64, device=dev)
+    heads = [torch.zeros_like(head) for _ in range(world)]
+    dist.all_gather(heads, head, group=group)
+    heads = [v.tolist() for v in heads]
+    pad = torch.zeros((max(h[0] for h in heads) or 1, 4), dtype=torch.int32, device=dev)
+    pad[: rows.shape[0]] = torch.from_numpy(rows).to(dev)
+    allp = [torch.zeros_like(pad) for _ in range(world)]
+    dist.all_gather(allp, pad, group=group)
+    return [allp[r][: heads[r][0]].cpu().numpy() for r in range(world)], [bool(h[1]) for h in heads]
+
+
+def _gpu_share_cut_table(L, d_buf, share_len, level, st_in, w_in, dmax):
+    """b2_bzip2_share_cut_table: rows (k, blocks, exit drift, flags) for the entry drifts 0..dmax, as an int32 numpy
+    array [dmax + 1, 4] (every field is below 2^31: block indices and drifts of inputs under 50 TB)."""
+    from . import _native
+    tab = (C.c_uint32 * (4 * (dmax + 1)))()
+    rc = L.b2_bzip2_share_cut_table(d_buf.data_ptr(), d_buf.numel(), level, st_in, w_in, share_len, dmax, tab)
+    if rc:
+        raise RuntimeError("b2_bzip2_share_cut_table: " + _native.last_error())
+    return np.frombuffer(tab, dtype=np.int32).reshape(-1, 4).copy()
+
+
+def _gpu_plan_share(L, d_buf, level, st_in, w_in, first, count, drift, flavor):
+    from . import _native
+    info = (C.c_uint64 * 6)()
+    rc = L.b2_bzip2_plan_share_flavor(d_buf.data_ptr(), d_buf.numel(), level, st_in, w_in, first, count, drift, _flavor_id(flavor), info)
+    if rc:
+        raise RuntimeError("b2_bzip2_plan_share_flavor: " + _native.last_error())
+    return [int(v) for v in info]
+
+
+def compress_shares(d_buf, share_len, level=9, group=None, host_out=None, keep_sharded=False, flavor="compressjs"):
     """Whole-file bzip2 encode when every rank holds only ITS share of the input: d_buf = CUDA uint8 tensor with the
     share (share_len bytes) followed by a halo (the first bytes of the next shares; empty on the last rank).  The shares
     are contiguous in rank order.  Returns the stream on rank 0 (None elsewhere); with keep_sharded a ShardedStream on
-    every rank (the output stays sharded like the input; .gather() assembles it on rank 0)."""
+    every rank (the output stays sharded like the input; .gather() assembles it on rank 0).
+    flavor="libbz2" writes the bytes of libbz2 (bz2.compress): every rank cuts its share for every drift its first
+    block can have, the tables are all-gathered (16 bytes per drift, 4 drifts per block in front of the share, every
+    table padded to the longest) and chained the same way on every rank.  A halo too short for a share's last block falls back to the whole input."""
     from . import _native
     L = _native.lib()
+    libbz2 = _flavor_id(flavor) == FLAVORS["libbz2"]
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     dev = d_buf.device
@@ -518,15 +623,27 @@ def compress_shares(d_buf, share_len, level=9, group=None, host_out=None, keep_s
     else:
         allv = [mine]
     summaries = [tuple(_u64(int(x)) for x in v.tolist()) for v in allv]
-    plan, total, _ = share_plan_inputs(summaries, level)
+    plan, total, w_total = share_plan_inputs(summaries, level)
     st_in, w_in, first, count, g0 = plan[rank]
     n_total = sum(sm[3] for sm in summaries)
     t0 = _tick("share_summaries", t0)
-    info = (C.c_uint64 * 6)()
-    rc = L.b2_bzip2_plan_share(d_buf.data_ptr(), d_buf.numel(), level, st_in, w_in, first, count, info)
-    if rc:
-        raise RuntimeError("b2_bzip2_plan_share: " + _native.last_error())
-    row = [int(v) for v in info]
+    drift, chain = 0, None
+    if libbz2:
+        # every rank's cut for every entry drift; all ranks chain the same tables to the same entries
+        if share_len:
+            rows = _gpu_share_cut_table(L, d_buf, share_len, level, st_in, w_in, share_drift_bound(w_in, level))
+        else:
+            rows = np.zeros((0, 4), dtype=np.int32)
+        t0 = _tick("cut_table", t0)
+        alltab, ends = _all_gather_tables(rows, g0 + d_buf.numel() == n_total, world, group, dev)
+        tables = [alltab[r] if summaries[r][3] else None for r in range(world)]
+        chain = libbz2_share_chain(plan, w_total, tables, level, ends)
+        t0 = _tick("cut_table_exchange", t0)
+        if chain is not None:
+            (first, drift, count), total = chain[0][rank], chain[1]
+    row = [0, 0, first, count, 0, 0]
+    if chain is not None or not libbz2:
+        row = _gpu_plan_share(L, d_buf, level, st_in, w_in, first, count, drift, flavor)
     mine = torch.tensor([row[0] + g0, row[1] + g0, row[2], row[3], row[4], total], dtype=torch.int64, device=dev)
     if world > 1:
         alli = [torch.zeros(6, dtype=torch.int64, device=dev) for _ in range(world)]
@@ -535,7 +652,7 @@ def compress_shares(d_buf, share_len, level=9, group=None, host_out=None, keep_s
         alli = [mine]
     infos = [tuple(int(x) for x in v.tolist()) for v in alli]
     _tick("plan_share+verify", t0)
-    if not spec_plan_ok(infos, n_total):
+    if (libbz2 and chain is None) or not spec_plan_ok(infos, n_total):
         # a run-phase slip or a block longer than the halo: every rank gets the whole input and the exact plan decides
         PHASES["fallback_full_input"] = 1.0
         lens = [sm[3] for sm in summaries]
@@ -550,9 +667,9 @@ def compress_shares(d_buf, share_len, level=9, group=None, host_out=None, keep_s
         else:
             full = d_buf[:share_len]
         del parts
-        return compress_file_sharded(full, level, group)
+        return compress_file_sharded(full, level, group, flavor)
     t0 = time.perf_counter()
-    enc = _range_encoder(L, d_buf, d_buf.numel(), level)
+    enc = _range_encoder(L, d_buf, d_buf.numel(), level, flavor)
     frag, nbits, crcs = enc(first, count)
     _tick("encode_range", t0)
     return place_fragments(frag, nbits, count, crcs, level, dev, group, host_out, keep_sharded)

@@ -200,8 +200,10 @@ uint32_t b2_crc32_bzip2(const uint8_t* p, size_t n);
  * Everything else (BWT, MTF, zero-run coder, headers, CRCs) is shared, and so are memory use, b2_bzip2_bound (the output
  * size is checked against the buffer as for the default: a stream that would not fit fails with B2_ERR_BAD_ARG),
  * b2_last_trace and b2_get_stats.  The _flavor calls take the arguments of the call they extend plus the flavor; an
- * unknown flavor returns B2_ERR_BAD_ARG before any callback runs.  The plan, range and share calls below
- * (multi-GPU encode) write the compressjs flavor only. */
+ * unknown flavor returns B2_ERR_BAD_ARG before any callback runs or any work is done.  The multi-GPU encode below
+ * writes both flavors: b2_bzip2_plan_flavor, b2_bzip2_plan_share_flavor and b2_bzip2_encode_range_dev_flavor take the
+ * flavor, and b2_bzip2_share_cut_table cuts the libbz2 flavor's blocks of a share.  b2_bzip2_plan_spec and the calls
+ * without a flavor write the compressjs flavor. */
 #define B2_BZ2_COMPRESSJS 0
 #define B2_BZ2_LIBBZ2 1
 int b2_bzip2_compress_flavor(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n, int flavor);
@@ -219,14 +221,18 @@ int b2_bzip2_compress_dev(const void* d_in, size_t n, int level, void* d_out, si
 int b2_bzip2_decompress_dev(const void* d_in, size_t n, int multistream, void* d_out, size_t out_cap, size_t* out_n);
 
 /* ---- block-range encode for multi-GPU sharding (SURVEY.md section 8e) ------------- */
-/* Plan cache: b2_bzip2_plan, _plan_spec and _plan_share keep their plan, replacing the one kept before.  The next
- * b2_bzip2_encode_range_dev takes it if it names the same (buffer, n, level), else plans the buffer exactly; either way
- * the cache is empty afterwards.  b2_bzip2_compress_dev empties it, no other call touches it.  The buffer must not
- * change in between. */
+/* Plan cache: b2_bzip2_plan(_flavor), _plan_spec and _plan_share(_flavor) keep their plan, replacing the one kept
+ * before.  The next b2_bzip2_encode_range_dev(_flavor) takes it if it names the same (buffer, n, level, flavor), else
+ * plans the buffer exactly in its own flavor; either way the cache is empty afterwards.  The flavors cut different
+ * blocks, so a range encode never takes a plan of the other flavor (the calls without a flavor are the compressjs
+ * flavor).  b2_bzip2_compress_dev empties it, no other call touches it.  The buffer must not change in between. */
 /* Exact plan of the whole buffer; total_blocks receives the number of blocks in the file. */
 int b2_bzip2_plan(const void* d_in, size_t n, int level, size_t* total_blocks);
+int b2_bzip2_plan_flavor(const void* d_in, size_t n, int level, size_t* total_blocks, int flavor);
 /* Speculative range plan for rank `rank` of `world`: cuts only this rank's share of the blocks, starting from
  * the boundary implied by W-space arithmetic (exact unless a run-phase slip happened earlier in the file).
+ * Compressjs flavor only: a libbz2 cut drifts away from multiples of blockSize in W; every rank holding the whole
+ * input takes b2_bzip2_plan_flavor instead.
  * info[0..5] = raw start, raw end, first block, planned count, blocks actually cut, total block guess.
  * The ranks must verify end(r) == start(r+1), start(0) == 0, end(last) == n and cut == planned on every rank
  * (compressjs_b200/sharded.py does); otherwise fall back to b2_bzip2_plan. */
@@ -241,6 +247,33 @@ int b2_bzip2_share_summary(const void* d_share, size_t n, uint64_t* summary);
  * and RLE1 output in front of it.  Speculative like b2_bzip2_plan_spec (same checks by the caller); info[0..5] = raw
  * start, raw end (offsets inside d_buf), first, planned, blocks cut, RLE1 output up to the end of the buffer. */
 int b2_bzip2_plan_share(const void* d_buf, size_t n, int level, uint64_t state_in, uint64_t w_in, size_t first, size_t count, uint64_t* info);
+/* libbz2 flavor over shares.  W is the RLE1 output position of the whole input with runs cut into pieces (one byte value,
+ * at most 255 long) as libbz2 reads them; M = 100000 level - 19.  Block k + 1 starts at the first piece start at or
+ * after S(k) + M, so the drift S(k) - k M of block k is 0..4 k.  A share does not know the drift of its first block, so
+ * it cuts itself once for every drift: row d of `table` (4 uint32 per row, rows 0..dmax) is the cut when the first block
+ * that starts at or after the share's W start w_in has drift d:
+ *   {k = that block's index = ceil((w_in - d) / M) (0 if d >= w_in), blocks that start in the share,
+ *    drift of the first block at or after the share's end (0 with B2_CUT_BUF_END), flags}.
+ * dmax = 4 ceil(w_in / M) covers every entry.  d fixes k except when k M + d is within 4 of w_in: the entry (k + 1, d)
+ * is then possible too, and it is row d without its first block when the row has B2_CUT_STEP_EXACT (otherwise it is not
+ * a piece start, and no entry).  compressjs_b200/sharded.py (libbz2_share_chain) chains the rows of all ranks.
+ * d_buf[0, n) = share (share_len bytes) + halo, state_in / w_in as for b2_bzip2_plan_share.  The table is built on the
+ * device and copied to the host array `table`.  The call keeps its tile scan and piece bitmap of the share (at most
+ * n * 5 / 32 bytes for the bitmap and 13 bytes per 4 KiB tile for the scan, in device memory) for the b2_bzip2_plan_share_flavor call that follows on the same (buffer, n,
+ * state_in, w_in), which then skips both; that call, the next table call, b2_bzip2_compress_dev and b2_shutdown drop
+ * them.  The buffer must not change in between. */
+#define B2_CUT_NOT_PIECE 1u  /* k M + d is not a piece start of the buffer: no entry */
+#define B2_CUT_STEP_EXACT 2u /* the share's first block ends exactly at k M + d + M: (k + 1, d) is this row less one block */
+#define B2_CUT_BUF_END 4u    /* the last block needs the bytes past the buffer: the halo is too short, unless the buffer
+                                ends the input, where that block ends with it */
+int b2_bzip2_share_cut_table(const void* d_buf, size_t n, int level, uint64_t state_in, uint64_t w_in, size_t share_len, uint64_t dmax,
+                             uint32_t* table);
+/* The share plan of either flavor.  B2_BZ2_COMPRESSJS: exactly b2_bzip2_plan_share (drift unused).  B2_BZ2_LIBBZ2: cuts
+ * blocks [first, first + count) whose first block starts at W = first * M + drift, the entry the host chained from the
+ * tables; a block that reaches the buffer's end ends there.  info as b2_bzip2_plan_share's: fewer blocks cut than
+ * planned means the entry was not a piece start of the buffer or the buffer was too short. */
+int b2_bzip2_plan_share_flavor(const void* d_buf, size_t n, int level, uint64_t state_in, uint64_t w_in, size_t first, size_t count,
+                               uint64_t drift, int flavor, uint64_t* info);
 /* dst := the first nbits of src moved to start at bit `phase` (0..7, MSB first), zero outside; dst must hold
  * ceil((phase+nbits)/32)*4 bytes and may not overlap src.  Used to align a fragment to its global bit offset. */
 int b2_bitshift_dev(const void* d_src, uint64_t nbits, int phase, void* d_dst);
@@ -250,6 +283,8 @@ int b2_bitshift_dev(const void* d_src, uint64_t nbits, int phase, void* d_dst);
  * block_crcs (host, one entry per block) receives the per-block CRCs so the caller can fold the stream CRC. */
 int b2_bzip2_encode_range_dev(const void* d_in, size_t n, int level, size_t first, size_t count, int bit_phase,
                               void* d_out, size_t out_cap, uint64_t* out_bits, uint32_t* block_crcs);
+int b2_bzip2_encode_range_dev_flavor(const void* d_in, size_t n, int level, size_t first, size_t count, int bit_phase,
+                                     void* d_out, size_t out_cap, uint64_t* out_bits, uint32_t* block_crcs, int flavor);
 
 /* ---- sharded decode (SURVEY.md section 8e; BASELINE config 5) ----------------------------------- */
 /* Every rank holds the compressed stream.  open: scan the magics and decode this rank's share of the
