@@ -9,10 +9,13 @@
 //   A  k_rle_summary : per 4 KiB raw tile, assuming maximal runs: first/last byte, leading /
 //                      trailing run length, sum of w behind the leading run.
 //   B  k_rle_scan    : one CTA scans the tile summaries -> per tile the run length carried in
-//                      (mod 255) and W(tile start) = total output before the tile.
+//                      (mod 255) and W(tile start) = total output before the tile.  k_rle_scan_g1..g5 do the
+//                      same in five launches for inputs of many tiles, with the same CTA scan and per-tile step.
 //   C  k_rle_blocks  : one CTA walks the blocks: a block that starts in the middle of a run
 //                      re-phases that run (fresh state), everything behind it follows W; the
-//                      end is found by a 256-ary search over W(tile) plus one in-tile scan.
+//                      end is found by the W seek (seek_W): an extrapolated guess and a 256-ary search
+//                      over W(tile), then one in-tile scan.  The libbz2 cut (k_rle_blocks_libbz2) and the
+//                      share cut (k_w_to_raw) locate their W positions with the same seek.
 //   D  k_rle_emit    : one CTA per span of up to 4 tiles of one block (a per-CTA map gives the block, no
 //                      search): the span's raw bytes are staged in shared memory, a run of plain tiles is
 //                      copied out as destination-aligned 16-byte words (funnel shifts), every raw byte of
@@ -87,28 +90,20 @@ __device__ __forceinline__ u32 block_excl_max256(u32 v, u32* ws) {
   __syncthreads();
   return exw > c ? exw : c;
 }
-__device__ __forceinline__ u32 block_min256(u32 v, u32* red) {
+template <class Op>
+__device__ __forceinline__ u32 block_reduce256(u32 v, u32* red, Op op) {
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = min(v, __shfl_xor_sync(FULL_MASK, v, o));
+  for (int o = 16; o > 0; o >>= 1) v = op(v, __shfl_xor_sync(FULL_MASK, v, o));
   if (lane_id() == 0) red[threadIdx.x >> 5] = v;
   __syncthreads();
   u32 r = red[0];
 #pragma unroll
-  for (int i = 1; i < RT_THREADS / 32; i++) r = min(r, red[i]);
+  for (int i = 1; i < RT_THREADS / 32; i++) r = op(r, red[i]);
   __syncthreads();
   return r;
 }
-__device__ __forceinline__ u32 block_max256(u32 v, u32* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = max(v, __shfl_xor_sync(FULL_MASK, v, o));
-  if (lane_id() == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  u32 r = red[0];
-#pragma unroll
-  for (int i = 1; i < RT_THREADS / 32; i++) r = max(r, red[i]);
-  __syncthreads();
-  return r;
-}
+__device__ __forceinline__ u32 block_min256(u32 v, u32* red) { return block_reduce256(v, red, [](u32 a, u32 b) { return min(a, b); }); }
+__device__ __forceinline__ u32 block_max256(u32 v, u32* red) { return block_reduce256(v, red, [](u32 a, u32 b) { return max(a, b); }); }
 
 // Whole CTA (RT_THREADS threads).  carry = run length (mod 255) entering the tile.  PIECES: *pieces receives bit j for
 // every byte j of the thread that starts a piece (phase 0 mod 255 of its maximal run: a run start, or byte 255 k of it).
@@ -259,6 +254,49 @@ __device__ __forceinline__ u64 rs_combine(u64 A, u64 B) {
   return rs_make(Aall && Ball && join, Afc, Blc, trail, (Alen + Blen) % 255);
 }
 
+struct RsCombine {
+  __device__ __forceinline__ u64 operator()(u64 a, u64 b) const { return rs_combine(a, b); }
+};
+struct Add64 {
+  __device__ __forceinline__ u64 operator()(u64 a, u64 b) const { return a + b; }
+};
+// scan state of tile t on its own
+__device__ __forceinline__ u64 tile_state(const TileSum& s, u64 t, u64 N) {
+  const u64 tl = min((u64)RLE_TILE, N - t * RLE_TILE);
+  return rs_make(s.allsame, s.fc, s.lc, s.trail % 255, (u32)(tl % 255));
+}
+// Exclusive Hillis-Steele scan of one value per thread over a CTA of NT threads.  op need not be commutative; 0 is its
+// identity.  *total = the combination of all NT values.  sa and sb (NT entries each) are free again on return.
+template <u32 NT, class Op>
+__device__ __forceinline__ u64 cta_scan_excl(u64 v, u64* sa, u64* sb, Op op, u64* total) {
+  const u32 tid = threadIdx.x;
+  sa[tid] = v;
+  __syncthreads();
+  u64* src = sa; u64* dst = sb;
+  for (u32 o = 1; o < NT; o <<= 1) {
+    u64 x = src[tid];
+    if (tid >= o) x = op(src[tid - o], x);
+    dst[tid] = x;
+    __syncthreads();
+    u64* tmp = src; src = dst; dst = tmp;
+  }
+  const u64 ex = tid ? src[tid - 1] : 0;
+  *total = src[NT - 1];
+  __syncthreads();
+  return ex;
+}
+// Tile t entered with run state st: carry[t] = the run length carried in (mod 255), prefix[t] = the tile's output size S
+// (an add scan turns the sizes into W later).  Returns S and advances st past the tile.
+__device__ __forceinline__ u64 tile_carry_step(const TileSum& s, u64 t, u64 N, u64& st, u32* carry, u64* prefix) {
+  u32 c = 0;
+  if ((st >> 63) && ((st >> 16) & 255) == s.fc) c = (st >> 8) & 255;
+  carry[t] = c;
+  const u64 S = outfresh((u64)c + s.lead) - outfresh(c) + s.rest;
+  prefix[t] = S;
+  st = rs_combine(st, tile_state(s, t, N));
+  return S;
+}
+
 #define RS_THREADS 1024
 __global__ void __launch_bounds__(RS_THREADS)
 k_rle_scan(const TileSum* __restrict__ sums, u64 ntiles, u64 N, u32* __restrict__ carry, u64* __restrict__ prefix, u64 st0, u64 W0,
@@ -269,57 +307,23 @@ k_rle_scan(const TileSum* __restrict__ sums, u64 ntiles, u64 N, u32* __restrict_
   const u64 t0 = (u64)tid * per, t1 = min(ntiles, t0 + per);
   // 1. aggregate of this thread's tiles
   u64 agg = 0;
-  for (u64 t = t0; t < t1; t++) {
-    const TileSum s = sums[t];
-    const u64 tl = min((u64)RLE_TILE, N - t * RLE_TILE);
-    agg = rs_combine(agg, rs_make(s.allsame, s.fc, s.lc, s.trail % 255, (u32)(tl % 255)));
-  }
-  // 2. exclusive scan over threads (Hillis-Steele, operator is not commutative)
-  sa[tid] = agg;
-  __syncthreads();
-  u64* src = sa; u64* dst = sb;
-  for (u32 o = 1; o < RS_THREADS; o <<= 1) {
-    u64 x = src[tid];
-    if (tid >= o) x = rs_combine(src[tid - o], x);
-    dst[tid] = x;
-    __syncthreads();
-    u64* tmp = src; src = dst; dst = tmp;
-  }
-  u64 st = rs_combine(st0, tid ? src[tid - 1] : 0);  // st0: run state entering the buffer (a share of a larger input)
-  if (tid == 0 && agg_out) *agg_out = src[RS_THREADS - 1];
-  __syncthreads();
+  for (u64 t = t0; t < t1; t++) agg = rs_combine(agg, tile_state(sums[t], t, N));
+  // 2. exclusive scan over threads; st0: run state entering the buffer (a share of a larger input)
+  u64 all;
+  u64 st = rs_combine(st0, cta_scan_excl<RS_THREADS>(agg, sa, sb, RsCombine{}, &all));
+  if (tid == 0 && agg_out) *agg_out = all;
   // 3. carries + per-tile output sums (stored in prefix[] for now)
   u64 mysum = 0;
-  for (u64 t = t0; t < t1; t++) {
-    const TileSum s = sums[t];
-    const u64 tl = min((u64)RLE_TILE, N - t * RLE_TILE);
-    u32 c = 0;
-    if ((st >> 63) && ((st >> 16) & 255) == s.fc) c = (st >> 8) & 255;
-    carry[t] = c;
-    const u64 S = outfresh((u64)c + s.lead) - outfresh(c) + s.rest;
-    prefix[t] = S;
-    mysum += S;
-    st = rs_combine(st, rs_make(s.allsame, s.fc, s.lc, s.trail % 255, (u32)(tl % 255)));
-  }
+  for (u64 t = t0; t < t1; t++) mysum += tile_carry_step(sums[t], t, N, st, carry, prefix);
   // 4. exclusive add scan of the thread sums
-  sa[tid] = mysum;
-  __syncthreads();
-  src = sa; dst = sb;
-  for (u32 o = 1; o < RS_THREADS; o <<= 1) {
-    u64 x = src[tid];
-    if (tid >= o) x += src[tid - o];
-    dst[tid] = x;
-    __syncthreads();
-    u64* tmp = src; src = dst; dst = tmp;
-  }
-  u64 run = W0 + (tid ? src[tid - 1] : 0);
-  const u64 grand = W0 + src[RS_THREADS - 1];
+  u64 grand;
+  u64 run = W0 + cta_scan_excl<RS_THREADS>(mysum, sa, sb, Add64{}, &grand);
   for (u64 t = t0; t < t1; t++) {
     const u64 S = prefix[t];
     prefix[t] = run;
     run += S;
   }
-  if (tid == 0) prefix[ntiles] = grand;
+  if (tid == 0) prefix[ntiles] = W0 + grand;
 }
 
 // Multi-CTA version of the same scan for inputs of many tiles (one CTA per RG_TILES tiles, five small launches):
@@ -329,28 +333,6 @@ k_rle_scan(const TileSum* __restrict__ sums, u64 ntiles, u64 N, u32* __restrict_
 #define RG_THREADS 256
 #define RG_PER 8
 #define RG_TILES (RG_THREADS * RG_PER)
-__device__ __forceinline__ u64 rg_tile_state(const TileSum& s, u64 t, u64 N) {
-  const u64 tl = min((u64)RLE_TILE, N - t * RLE_TILE);
-  return rs_make(s.allsame, s.fc, s.lc, s.trail % 255, (u32)(tl % 255));
-}
-// exclusive scan over the CTA's threads with the (non commutative) state operator; *total = combination of all
-__device__ __forceinline__ u64 rg_block_excl_state(u64 v, u64* sa, u64* sb, u64* total) {
-  const u32 tid = threadIdx.x;
-  sa[tid] = v;
-  __syncthreads();
-  u64* src = sa; u64* dst = sb;
-  for (u32 o = 1; o < RG_THREADS; o <<= 1) {
-    u64 x = src[tid];
-    if (tid >= o) x = rs_combine(src[tid - o], x);
-    dst[tid] = x;
-    __syncthreads();
-    u64* tmp = src; src = dst; dst = tmp;
-  }
-  const u64 ex = tid ? src[tid - 1] : 0;
-  *total = src[RG_THREADS - 1];
-  __syncthreads();
-  return ex;
-}
 __global__ void __launch_bounds__(RG_THREADS)
 k_rle_scan_g1(const TileSum* __restrict__ sums, u64 ntiles, u64 N, u64* __restrict__ group_agg) {
   __shared__ u64 sa[RG_THREADS], sb[RG_THREADS];
@@ -358,41 +340,32 @@ k_rle_scan_g1(const TileSum* __restrict__ sums, u64 ntiles, u64 N, u64* __restri
   u64 agg = 0;
   for (u32 j = 0; j < RG_PER; j++) {
     const u64 t = t0 + j;
-    if (t < ntiles) agg = rs_combine(agg, rg_tile_state(sums[t], t, N));
+    if (t < ntiles) agg = rs_combine(agg, tile_state(sums[t], t, N));
   }
   u64 total;
-  rg_block_excl_state(agg, sa, sb, &total);
+  cta_scan_excl<RG_THREADS>(agg, sa, sb, RsCombine{}, &total);
   if (threadIdx.x == 0) group_agg[blockIdx.x] = total;
 }
-// one CTA: exclusive scan of ngroups values (state operator when STATE, plain addition otherwise); out[ngroups] = total
-template <bool STATE>
+// one CTA: exclusive scan of ngroups values under Op (RsCombine for run states, Add64 for sizes); out[ngroups] = total
+template <class Op>
 __global__ void __launch_bounds__(RS_THREADS)
 k_rle_scan_groups(const u64* __restrict__ in, u32 ngroups, u64* __restrict__ out, u64 init, u64* __restrict__ agg_out) {
   __shared__ u64 sa[RS_THREADS], sb[RS_THREADS];
+  const Op op{};
   const u32 tid = threadIdx.x;
   const u32 per = (ngroups + RS_THREADS - 1) / RS_THREADS;
   const u32 g0 = tid * per, g1 = min(ngroups, g0 + per);
   u64 agg = 0;
-  for (u32 g = g0; g < g1; g++) agg = STATE ? rs_combine(agg, in[g]) : agg + in[g];
-  sa[tid] = agg;
-  __syncthreads();
-  u64* src = sa; u64* dst = sb;
-  for (u32 o = 1; o < RS_THREADS; o <<= 1) {
-    u64 x = src[tid];
-    if (tid >= o) x = STATE ? rs_combine(src[tid - o], x) : src[tid - o] + x;
-    dst[tid] = x;
-    __syncthreads();
-    u64* tmp = src; src = dst; dst = tmp;
-  }
-  u64 run = tid ? src[tid - 1] : 0;
-  run = STATE ? rs_combine(init, run) : init + run;
-  if (tid == 0 && agg_out) *agg_out = src[RS_THREADS - 1];  // combination of all groups without `init`
+  for (u32 g = g0; g < g1; g++) agg = op(agg, in[g]);
+  u64 all;
+  u64 run = op(init, cta_scan_excl<RS_THREADS>(agg, sa, sb, op, &all));
+  if (tid == 0 && agg_out) *agg_out = all;  // combination of all groups without `init`
   for (u32 g = g0; g < g1; g++) {
     const u64 v = in[g];
     out[g] = run;
-    run = STATE ? rs_combine(run, v) : run + v;
+    run = op(run, v);
   }
-  if (tid == RS_THREADS - 1) out[ngroups] = STATE ? rs_combine(init, src[RS_THREADS - 1]) : init + src[RS_THREADS - 1];
+  if (tid == RS_THREADS - 1) out[ngroups] = op(init, all);
 }
 __global__ void __launch_bounds__(RG_THREADS)
 k_rle_scan_g3(const TileSum* __restrict__ sums, u64 ntiles, u64 N, const u64* __restrict__ group_start, u32* __restrict__ carry,
@@ -405,24 +378,15 @@ k_rle_scan_g3(const TileSum* __restrict__ sums, u64 ntiles, u64 N, const u64* __
 #pragma unroll
   for (u32 j = 0; j < RG_PER; j++) {
     const u64 t = t0 + j;
-    if (t < ntiles) { ts[j] = sums[t]; agg = rs_combine(agg, rg_tile_state(ts[j], t, N)); }
+    if (t < ntiles) { ts[j] = sums[t]; agg = rs_combine(agg, tile_state(ts[j], t, N)); }
   }
   u64 total;
-  u64 st = rs_combine(group_start[blockIdx.x], rg_block_excl_state(agg, sa, sb, &total));
+  u64 st = rs_combine(group_start[blockIdx.x], cta_scan_excl<RG_THREADS>(agg, sa, sb, RsCombine{}, &total));
   u32 mysum = 0;  // <= 2048 tiles x 5120 bytes per group: fits 32 bits
 #pragma unroll
   for (u32 j = 0; j < RG_PER; j++) {
     const u64 t = t0 + j;
-    if (t < ntiles) {
-      const TileSum& s = ts[j];
-      u32 c = 0;
-      if ((st >> 63) && ((st >> 16) & 255) == s.fc) c = (st >> 8) & 255;
-      carry[t] = c;
-      const u64 S = outfresh((u64)c + s.lead) - outfresh(c) + s.rest;
-      prefix[t] = S;
-      mysum += (u32)S;
-      st = rs_combine(st, rg_tile_state(s, t, N));
-    }
+    if (t < ntiles) mysum += (u32)tile_carry_step(ts[j], t, N, st, carry, prefix);
   }
   u32 tot;
   block_excl_add<RG_THREADS, u32>(mysum, ws, &tot);
@@ -454,7 +418,6 @@ k_rle_scan_g5(u64 ntiles, const u64* __restrict__ group_base, u32 ngroups, u64* 
 struct BlocksShared {
   TileScratch sc;
   u64 r64;
-  u32 r32;
 };
 
 // W(x): RLE1 output of raw[0,x) under maximal phases.  Whole CTA.
@@ -492,6 +455,57 @@ __device__ u64 find_run_end(const u8* in, u64 s, u64 cap, BlocksShared& sh) {
   return cap;
 }
 
+// The largest tile t >= lo with prefix[t] < V.  Whole CTA; see seek_W for the precondition.  Kept out of line: inlined
+// twice into k_rle_blocks it made ptxas spill there, and a call per block costs nothing next to the probes' barriers.
+__device__ __noinline__ u64 find_tile(const u64* prefix, u64 ntiles, u64 lo, u64 V, BlocksShared& sh) {
+  const u32 tid = threadIdx.x;
+  u64 hi = ntiles;  // prefix[lo] < V <= prefix[hi]
+  {
+    // W grows by ~1 per raw byte on ordinary data: try the tile that linear extrapolation predicts
+    u64 tg = lo + ((V - prefix[lo]) >> 12);
+    if (tg >= ntiles) tg = ntiles - 1;
+    const u64 pg = prefix[tg], pg1 = prefix[tg + 1];
+    if (pg < V && pg1 >= V) { lo = tg; hi = tg + 1; }
+    else if (pg < V) lo = tg;
+    else if (tg > lo) hi = tg;
+  }
+  while (hi - lo > 1) {
+    const u64 span = hi - lo;
+    // probe points lo < p_i < hi, increasing in i
+    const u64 pi = lo + 1 + (span - 1) * (u64)tid / RT_THREADS;
+    const bool valid = pi < hi && (tid == 0 || pi != lo + 1 + (span - 1) * (u64)(tid - 1) / RT_THREADS);
+    const bool pr = valid && prefix[pi] < V;
+    // largest true probe -> new lo ; smallest false probe -> new hi
+    const u32 tr = block_max256(pr ? tid + 1 : 0, sh.sc.red);
+    const u32 fl = block_min256((valid && !pr) ? tid : 0xffffffffu, sh.sc.red);
+    u64 nlo = lo, nhi = hi;
+    if (tr) nlo = lo + 1 + (span - 1) * (u64)(tr - 1) / RT_THREADS;
+    if (fl != 0xffffffffu) nhi = lo + 1 + (span - 1) * (u64)fl / RT_THREADS;
+    lo = nlo; hi = nhi;
+  }
+  return lo;
+}
+
+// W seek: the smallest raw position f with W(f + 1) >= V, and *Wf = W(f + 1).  Whole CTA.  Requires
+// prefix[lo] < V <= prefix[ntiles]: then f lies in the tile find_tile returns, and that tile ends at W >= V.
+__device__ u64 seek_W(const u8* in, u64 N, const u32* carry, const u64* prefix, u64 ntiles, u64 lo, u64 V, BlocksShared& sh, u64* Wf) {
+  const u64 t = find_tile(prefix, ntiles, lo, V, sh);
+  TileView v;
+  tile_view(in, N, t * RLE_TILE, carry[t], sh.sc, v);
+  u32 found = 0xffffffffu;
+  u64 acc = prefix[t] + v.excl;
+  for (u32 j = 0; j < v.cnt; j++) {
+    acc += v.w[j];
+    if (acc >= V) { found = threadIdx.x * RT_PER + j; break; }
+  }
+  const u32 f = block_min256(found, sh.sc.red);
+  if (found == f) sh.r64 = acc;  // the thread that owns f
+  __syncthreads();
+  *Wf = sh.r64;
+  __syncthreads();
+  return t * RLE_TILE + f;
+}
+
 __global__ void __launch_bounds__(RT_THREADS)
 k_rle_blocks(const u8* __restrict__ in, u64 N, u32 BS, const u32* __restrict__ carry, const u64* __restrict__ prefix, u64 ntiles,
              BlkInfo* __restrict__ blocks, u32* nblocks_out, u32 maxblocks, u64 u_start, u32 range_first, u32 range_count, int open_end) {
@@ -517,41 +531,7 @@ k_rle_blocks(const u8* __restrict__ in, u64 N, u32 BS, const u32* __restrict__ c
     // speculative start (multi-GPU range plan): the first raw position x with W(x) >= u_start, i.e. where a
     // block boundary falls if no block before it was shifted by a run-phase slip (verified by the caller)
     if (u_start > Wtotal) { if (tid == 0) *nblocks_out = 0; return; }
-    u64 lo = 0, hi = ntiles;
-    while (hi - lo > 1) {
-      const u64 span = hi - lo;
-      const u64 pi = lo + 1 + (span - 1) * (u64)tid / RT_THREADS;
-      const bool valid = pi < hi && (tid == 0 || pi != lo + 1 + (span - 1) * (u64)(tid - 1) / RT_THREADS);
-      const bool pr = valid && prefix[pi] < u_start;
-      const u32 tr = block_max256(pr ? tid + 1 : 0, sh.sc.red);
-      const u32 fl = block_min256((valid && !pr) ? tid : 0xffffffffu, sh.sc.red);
-      u64 nlo = lo, nhi = hi;
-      if (tr) nlo = lo + 1 + (span - 1) * (u64)(tr - 1) / RT_THREADS;
-      if (fl != 0xffffffffu) nhi = lo + 1 + (span - 1) * (u64)fl / RT_THREADS;
-      lo = nlo; hi = nhi;
-    }
-    const u64 t = lo;
-    TileView v;
-    tile_view(in, N, t * RLE_TILE, carry[t], sh.sc, v);
-    u32 found = 0xffffffffu;
-    {
-      u64 acc = prefix[t] + v.excl;
-      for (u32 j = 0; j < v.cnt; j++) {
-        acc += v.w[j];
-        if (acc >= u_start) { found = tid * RT_PER + j; break; }
-      }
-    }
-    const u32 f = block_min256(found, sh.sc.red);
-    if (f / RT_PER == tid) {
-      u64 acc = prefix[t] + v.excl;
-      for (u32 j = 0; j <= f % RT_PER; j++) acc += v.w[j];
-      sh.r64 = acc;
-    }
-    __syncthreads();
-    Ws = sh.r64;
-    __syncthreads();
-    s = t * RLE_TILE + f + 1;
-    Ws_valid = true;
+    s = seek_W(in, N, carry, prefix, ntiles, 0, u_start, sh, &Ws) + 1;
   }
   while (s < N && k < maxblocks) {
     BlkInfo bi;
@@ -579,65 +559,8 @@ k_rle_blocks(const u8* __restrict__ in, u64 N, u32 BS, const u32* __restrict__ c
         bi.e = e; bi.b = b; bi.Wb = Wb; bi.ofs = (u32)ofs; bi.n = (u32)(ofs + (Wtotal - Wb));
         Ws_valid = false;
       } else {
-        // largest tile t >= tile(b) with prefix[t] < V
-        u64 lo = b / RLE_TILE, hi = ntiles;  // pred(lo) true, pred(hi) false
-        {
-          // W grows by ~1 per raw byte on ordinary data: try the tile that linear extrapolation predicts
-          const u64 plo = prefix[lo];
-          u64 tg = lo + ((V - plo) >> 12);
-          if (tg >= ntiles) tg = ntiles - 1;
-          const u64 pg = prefix[tg], pg1 = prefix[tg + 1];
-          if (pg < V && pg1 >= V) { lo = tg; hi = tg + 1; }
-          else if (pg < V) lo = tg;
-          else if (tg > lo) hi = tg;
-        }
-        if (hi - lo > 1) {
-          // narrow with a guess window first (typical data: about BS raw bytes per block)
-          const u64 a = ((BS - ofs) * 4 / 5) / RLE_TILE;
-          const u64 g0 = lo + (a > 1 ? a - 1 : 0);
-          if (g0 < ntiles && prefix[g0] < V) {
-            lo = g0;
-            const u64 g1 = g0 + 4 * RT_THREADS;
-            if (g1 < ntiles && !(prefix[g1] < V)) hi = g1;
-          }
-        }
-        while (hi - lo > 1) {
-          const u64 span = hi - lo;
-          // probe points lo < p_i < hi, increasing in i
-          const u64 pi = lo + 1 + (span - 1) * (u64)tid / RT_THREADS;
-          const bool valid = pi < hi && (tid == 0 || pi != lo + 1 + (span - 1) * (u64)(tid - 1) / RT_THREADS);
-          const bool pr = valid && prefix[pi] < V;
-          // largest true probe -> new lo ; smallest false probe -> new hi
-          const u32 tr = block_max256(pr ? tid + 1 : 0, sh.sc.red);
-          const u32 fl = block_min256((valid && !pr) ? tid : 0xffffffffu, sh.sc.red);
-          u64 nlo = lo, nhi = hi;
-          if (tr) nlo = lo + 1 + (span - 1) * (u64)(tr - 1) / RT_THREADS;
-          if (fl != 0xffffffffu) nhi = lo + 1 + (span - 1) * (u64)fl / RT_THREADS;
-          lo = nlo; hi = nhi;
-        }
-        const u64 t = lo;
-        TileView v;
-        tile_view(in, N, t * RLE_TILE, carry[t], sh.sc, v);
-        // smallest position whose inclusive W reaches V
-        u32 found = 0xffffffffu;
-        {
-          u64 acc = prefix[t] + v.excl;
-          for (u32 j = 0; j < v.cnt; j++) {
-            acc += v.w[j];
-            if (acc >= V) { found = tid * RT_PER + j; break; }
-          }
-        }
-        const u32 f = block_min256(found, sh.sc.red);
-        // f always exists: prefix[t+1] >= V
-        if (f / RT_PER == tid) {
-          u64 acc = prefix[t] + v.excl;
-          for (u32 j = 0; j <= f % RT_PER; j++) acc += v.w[j];
-          sh.r64 = acc;
-        }
-        __syncthreads();
-        const u64 We = sh.r64;
-        __syncthreads();
-        e = t * RLE_TILE + f + 1;
+        u64 We;
+        e = seek_W(in, N, carry, prefix, ntiles, b / RLE_TILE, V, sh, &We) + 1;
         const u64 produced = ofs + (We - Wb);
         bi.e = e; bi.b = b; bi.Wb = Wb; bi.ofs = (u32)ofs; bi.n = (u32)min(produced, (u64)BS);
         Ws = We; Ws_valid = true;
@@ -656,7 +579,7 @@ k_rle_blocks(const u8* __restrict__ in, u64 N, u32 BS, const u32* __restrict__ c
 // the phases W is scanned under.  A block holds whole pieces and closes right after the first piece that brings its
 // RLE1 size to >= blockSize.  So every block starts on a piece start with W(s) known from the block before: no run is
 // re-phased (b == s, ofs == 0), and k_rle_emit writes the block unchanged.  One CTA walks the blocks: per block one
-// tile search for the byte whose W reaches W(s) + blockSize, then the end of that byte's piece.
+// W seek for the byte whose W reaches W(s) + blockSize, then the end of that byte's piece.
 __global__ void __launch_bounds__(RT_THREADS)
 k_rle_blocks_libbz2(const u8* __restrict__ in, u64 N, u32 BS, const u32* __restrict__ carry, const u64* __restrict__ prefix, u64 ntiles,
                     BlkInfo* __restrict__ blocks, u32* nblocks_out, u32 maxblocks) {
@@ -673,56 +596,17 @@ k_rle_blocks_libbz2(const u8* __restrict__ in, u64 N, u32 BS, const u32* __restr
     if (V > Wtotal) {
       e = N; We = Wtotal;
     } else {
-      // largest tile t >= tile(s) with prefix[t] < V, as in k_rle_blocks
-      u64 lo = s / RLE_TILE, hi = ntiles;
-      {
-        const u64 plo = prefix[lo];
-        u64 tg = lo + ((V - plo) >> 12);
-        if (tg >= ntiles) tg = ntiles - 1;
-        const u64 pg = prefix[tg], pg1 = prefix[tg + 1];
-        if (pg < V && pg1 >= V) { lo = tg; hi = tg + 1; }
-        else if (pg < V) lo = tg;
-        else if (tg > lo) hi = tg;
-      }
-      while (hi - lo > 1) {
-        const u64 span = hi - lo;
-        const u64 pi = lo + 1 + (span - 1) * (u64)tid / RT_THREADS;
-        const bool valid = pi < hi && (tid == 0 || pi != lo + 1 + (span - 1) * (u64)(tid - 1) / RT_THREADS);
-        const bool pr = valid && prefix[pi] < V;
-        const u32 tr = block_max256(pr ? tid + 1 : 0, sh.sc.red);
-        const u32 fl = block_min256((valid && !pr) ? tid : 0xffffffffu, sh.sc.red);
-        u64 nlo = lo, nhi = hi;
-        if (tr) nlo = lo + 1 + (span - 1) * (u64)(tr - 1) / RT_THREADS;
-        if (fl != 0xffffffffu) nhi = lo + 1 + (span - 1) * (u64)fl / RT_THREADS;
-        lo = nlo; hi = nhi;
-      }
-      const u64 t = lo, tstart = t * RLE_TILE;
-      TileView v;
-      tile_view(in, N, tstart, carry[t], sh.sc, v);
-      // f: the smallest position whose inclusive W reaches V (it exists: prefix[t+1] >= V)
-      u32 found = 0xffffffffu;
-      {
-        u64 acc = prefix[t] + v.excl;
-        for (u32 j = 0; j < v.cnt; j++) {
-          acc += v.w[j];
-          if (acc >= V) { found = tid * RT_PER + j; break; }
-        }
-      }
-      const u32 fo = block_min256(found, sh.sc.red);
-      if (fo / RT_PER == tid) {
-        u64 acc = prefix[t] + v.excl;
-        for (u32 j = 0; j <= fo % RT_PER; j++) acc += v.w[j];
-        sh.r64 = acc;
-      }
+      u64 Wf;
+      const u64 f = seek_W(in, N, carry, prefix, ntiles, s / RLE_TILE, V, sh, &Wf);
+      const u64 t = f / RLE_TILE, tstart = t * RLE_TILE;
+      const u32 fo = (u32)(f - tstart);
       // phase of f inside its maximal run: the last byte change at or before f in the tile, else the carry
       u32 ls = 0;
       for (u32 j = 0; j < RT_PER; j++) {
         const u32 pos = tid * RT_PER + j;
         if (pos >= 1 && pos <= fo && in[tstart + pos] != in[tstart + pos - 1]) ls = pos + 1;
       }
-      ls = block_max256(ls, sh.sc.red);  // also orders the write of sh.r64 before the read below
-      const u64 Wf = sh.r64;
-      const u64 f = tstart + fo;
+      ls = block_max256(ls, sh.sc.red);
       const u32 d = ls ? fo - (ls - 1) : fo + carry[t];
       const u32 r = d % 255 + 1;  // f is byte r of its piece
       const u32 room = 255 - r;   // bytes the piece can still take
@@ -838,29 +722,10 @@ __global__ void __launch_bounds__(RT_THREADS)
 k_w_to_raw(const u8* __restrict__ in, u64 N, const u32* __restrict__ carry, const u64* __restrict__ prefix, u64 ntiles,
            const u64* __restrict__ starts, u64* __restrict__ raw) {
   __shared__ BlocksShared sh;
-  const u32 tid = threadIdx.x;
   const u64 S = prefix[0] + starts[blockIdx.x];
-  if (S >= prefix[ntiles]) { if (tid == 0) raw[blockIdx.x] = N; return; }
-  if (tid == 0) {
-    u64 lo = 0, hi = ntiles;  // prefix[lo] <= S < prefix[hi]
-    while (hi - lo > 1) {
-      const u64 mid = (lo + hi) >> 1;
-      if (prefix[mid] <= S) lo = mid; else hi = mid;
-    }
-    sh.r64 = lo;
-  }
-  __syncthreads();
-  const u64 t = sh.r64;
-  TileView v;
-  tile_view(in, N, t * RLE_TILE, carry[t], sh.sc, v);
-  u32 found = 0xffffffffu;
-  u64 acc = prefix[t] + v.excl;
-  for (u32 j = 0; j < v.cnt; j++) {
-    acc += v.w[j];
-    if (acc > S) { found = tid * RT_PER + j; break; }
-  }
-  const u32 f = block_min256(found, sh.sc.red);
-  if (tid == 0) raw[blockIdx.x] = t * RLE_TILE + f;
+  u64 f = N, Wf;
+  if (S < prefix[ntiles]) f = seek_W(in, N, carry, prefix, ntiles, 0, S + 1, sh, &Wf);
+  if (threadIdx.x == 0) raw[blockIdx.x] = f;
 }
 
 // ---- CRC constants ---------------------------------------------------------------------------
@@ -1253,11 +1118,11 @@ void rle1_scan_tiles(Ctx& c, const u8* d_in, size_t n, Rle1Plan& plan, u64 st0, 
     DBuf<u64> gagg(c, ng), gstart(c, ng + 1), gsum(c, ng), gbase(c, ng + 1);
     k_rle_scan_g1<<<ng, RG_THREADS, 0, c.stream>>>(sums, ntiles, n, gagg);
     KLAUNCH(c); KCHECK();
-    k_rle_scan_groups<true><<<1, RS_THREADS, 0, c.stream>>>(gagg, ng, gstart, st0, dagg);
+    k_rle_scan_groups<RsCombine><<<1, RS_THREADS, 0, c.stream>>>(gagg, ng, gstart, st0, dagg);
     KLAUNCH(c); KCHECK();
     k_rle_scan_g3<<<ng, RG_THREADS, 0, c.stream>>>(sums, ntiles, n, gstart, plan.tile_carry, plan.tile_prefix, gsum);
     KLAUNCH(c); KCHECK();
-    k_rle_scan_groups<false><<<1, RS_THREADS, 0, c.stream>>>(gsum, ng, gbase, W0, nullptr);
+    k_rle_scan_groups<Add64><<<1, RS_THREADS, 0, c.stream>>>(gsum, ng, gbase, W0, nullptr);
     KLAUNCH(c); KCHECK();
     k_rle_scan_g5<<<ng, RG_THREADS, 0, c.stream>>>(ntiles, gbase, ng, plan.tile_prefix);
     KLAUNCH(c); KCHECK();
@@ -1271,6 +1136,16 @@ void rle1_scan_tiles(Ctx& c, const u8* d_in, size_t n, Rle1Plan& plan, u64 st0, 
   c.sync();
 }
 
+// The blocks a single-CTA walk wrote to plan.blocks, and their count (*dnb), into plan.h_blocks and plan.nblocks.
+static void fetch_blocks(Ctx& c, Rle1Plan& plan, const u32* dnb) {
+  u32 nb = 0;
+  c.to_host(&nb, dnb, 4);
+  c.sync();
+  plan.nblocks = nb;
+  plan.h_blocks.resize(nb);
+  if (nb) c.to_host(plan.h_blocks.data(), plan.blocks, sizeof(BlkInfo) * nb);
+  c.sync();
+}
 // exact: every block of the buffer.  Otherwise blocks [first, first+count) of the whole input, walked from the
 // speculative boundary W = first * BS (see k_rle_blocks); plan.first_index records the global index of h_blocks[0].
 static void cut_blocks(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan, bool exact, size_t first, size_t count) {
@@ -1319,13 +1194,7 @@ static void cut_blocks(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& pl
   DBuf<u32> dnb(c, 1);
   k_rle_blocks<<<1, RT_THREADS, 0, c.stream>>>(d_in, n, BS, plan.tile_carry, plan.tile_prefix, ntiles, plan.blocks, dnb, maxblocks, u_start, 0, 0, 0);
   KLAUNCH(c); KCHECK();
-  u32 nb = 0;
-  c.to_host(&nb, dnb, 4);
-  c.sync();
-  plan.nblocks = nb;
-  plan.h_blocks.resize(nb);
-  if (nb) c.to_host(plan.h_blocks.data(), plan.blocks, sizeof(BlkInfo) * nb);
-  c.sync();
+  fetch_blocks(c, plan, dnb);
 }
 void rle1_cut_range(Ctx& c, const u8* d_in, size_t n, int level, Rle1Plan& plan, size_t first, size_t count) {
   cut_blocks(c, d_in, n, level, plan, false, first, count);
@@ -1343,13 +1212,7 @@ static void cut_blocks_libbz2(Ctx& c, const u8* d_in, size_t n, int level, Rle1P
   DBuf<u32> dnb(c, 1);
   k_rle_blocks_libbz2<<<1, RT_THREADS, 0, c.stream>>>(d_in, n, BS, plan.tile_carry, plan.tile_prefix, ntiles, plan.blocks, dnb, maxblocks);
   KLAUNCH(c); KCHECK();
-  u32 nb = 0;
-  c.to_host(&nb, dnb, 4);
-  c.sync();
-  plan.nblocks = nb;
-  plan.h_blocks.resize(nb);
-  if (nb) c.to_host(plan.h_blocks.data(), plan.blocks, sizeof(BlkInfo) * nb);
-  c.sync();
+  fetch_blocks(c, plan, dnb);
 }
 // libbz2 flavor over a share buffer: the piece-start bitmap (k_piece_probe) of a scanned plan; wbuf / wshare = W of the
 // buffer's / share's end relative to the buffer's W base.
