@@ -9,13 +9,6 @@
 #include <vector>
 #include "enc.h"
 
-// stages implemented in the other translation units
-void bwt_inverse_sentinel_batch(Ctx& c, const u8* d_L, const u32* h_n, const u32* h_pidx, u32 nb, u8* d_out);
-void dec_shard_release();
-void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* info);
-void dec_shard_export(u64* buf);
-int dec_shard_finish(Ctx& c, const u64* all, int multistream, u8* d_out, size_t out_cap, u64* res);
-
 static std::mutex g_mu;
 static Ctx* g_ctx = nullptr;
 static thread_local std::string g_err;
@@ -575,16 +568,16 @@ static int compress_host(Ctx& c, StreamIn& in, StreamOut& out, int level, bool p
 }
 
 // Every decode from a host input: b2_bzip2_decompress_partial and the calls built on it, and b2_bzip2_decompress_stream.
-// On a decode error (-2/-5/-7) the code is returned, not thrown, and `out` / the table rows hold what the reference has
-// written by the time it throws; any other error throws.  positions / ends: a position list (bzip2_decompress).
-static int decode_host(Ctx& c, StreamIn& in, StreamOut* out, int multistream, const std::vector<u64>* positions,
-                       std::vector<u64>* ends, std::vector<u64>* tp, std::vector<u32>* tl) {
+// run(&produced) is one of the host-input drivers of decode.cu.  On a decode error (-2/-5/-7) the code is returned, not
+// thrown, and the output / the rows hold what the reference has written by the time it throws; any other error throws.
+template <class Run>
+static int decode_host(Ctx& c, StreamIn& in, Run run) {
   size_t produced = 0;
   int rc = 0;
   try {
     StageScope tot(c, ST_TOTAL);
     try {
-      rc = bzip2_decompress(c, &in, nullptr, 0, multistream, nullptr, 0, out, &produced, positions, ends, tp, tl);
+      run(&produced);
     } catch (const B2Error& e) {
       if (e.code != B2_ERR_NOT_BZIP_DATA && e.code != B2_ERR_DATA_ERROR && e.code != B2_ERR_OBSOLETE_INPUT) throw;
       g_err = e.msg;
@@ -598,6 +591,19 @@ static int decode_host(Ctx& c, StreamIn& in, StreamOut* out, int multistream, co
   c.sync();
   c.collect();
   c.stats.raw_bytes = produced; c.stats.comp_bytes = in.base + in.have;
+  return rc;
+}
+
+// The host-buffer decodes: decode_host over the caller's buffer, run(c, src, dst, &produced), with the result dst in *out
+// when out is given.  The input stays on the host; the decoder uploads it a window at a time.
+template <class Run>
+static int decode_common(const uint8_t* in, size_t n, Run run, uint8_t** out, size_t* out_n) {
+  Ctx& c = ctx_locked();
+  c.reset_call();
+  StreamIn src(in, n);
+  StreamOut dst(c.stream);
+  const int rc = decode_host(c, src, [&](size_t* produced) { run(c, src, dst, produced); });
+  if (out) { *out_n = dst.written; *out = dst.take(); }
   return rc;
 }
 
@@ -633,7 +639,7 @@ int b2_bzip2_decompress_stream(b2_read_fn rd, b2_write_fn wr, void* user, int mu
     c.reset_call();
     StreamIn in(rd, user, c.stream);
     StreamOut out(wr, user, c.stream);
-    return decode_host(c, in, &out, multistream, nullptr, nullptr, nullptr, nullptr);
+    return decode_host(c, in, [&](size_t* produced) { bzip2_decompress_host(c, in, multistream, out, produced); });
   });
 }
 
@@ -704,8 +710,9 @@ int b2_dec_shard_export(uint64_t* buf) {
 }
 int b2_dec_shard_finish(const uint64_t* all, int multistream, void* d_out, size_t out_cap, uint64_t* res) {
   return guarded([&]() {
-    Ctx& c = ctx_locked();
-    return dec_shard_finish(c, all, multistream, (u8*)d_out, out_cap, res);
+    ctx_locked();
+    dec_shard_finish(all, multistream, (u8*)d_out, out_cap, res);
+    return 0;
   });
 }
 
@@ -817,21 +824,10 @@ int b2_bzip2_encode_range_dev_flavor(const void* d_in, size_t n, int level, size
   });
 }
 
-// The host-buffer decodes: decode_host over the caller's buffer, with the result in *out when out is given.  The input
-// stays on the host; the decoder uploads it a window at a time.
-static int decode_common(const uint8_t* in, size_t n, int multistream, const std::vector<u64>* positions, std::vector<u64>* ends,
-                         uint8_t** out, size_t* out_n, std::vector<u64>* tp, std::vector<u32>* tl) {
-  Ctx& c = ctx_locked();
-  c.reset_call();
-  StreamIn src(in, n);
-  StreamOut dst(c.stream);
-  const int rc = decode_host(c, src, out ? &dst : nullptr, multistream, positions, ends, tp, tl);
-  if (out) { *out_n = dst.written; *out = dst.take(); }
-  return rc;
-}
-
 int b2_bzip2_decompress_partial(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n) {
-  return guarded([&]() { return decode_common(in, n, multistream, nullptr, nullptr, out, out_n, nullptr, nullptr); });
+  return guarded([&]() {
+    return decode_common(in, n, [&](Ctx& c, StreamIn& s, StreamOut& d, size_t* p) { bzip2_decompress_host(c, s, multistream, d, p); }, out, out_n);
+  });
 }
 
 int b2_bzip2_decompress_blocks(const uint8_t* in, size_t n, const uint64_t* bitpos, size_t count, uint8_t** out, size_t* out_n,
@@ -841,13 +837,14 @@ int b2_bzip2_decompress_blocks(const uint8_t* in, size_t n, const uint64_t* bitp
     if (!out || !out_n || !ends || !done) throw B2Error{B2_ERR_BAD_ARG, "null output argument"};
     struct HostBuf { void* p; ~HostBuf() { free(p); } } ep{malloc(sizeof(uint64_t) * (count + 1))};
     if (!ep.p) throw B2Error{B2_ERR_CUDA, "out of host memory"};
-    std::vector<u64> pos(bitpos, bitpos + count), e;
+    const std::vector<u64> pos(bitpos, bitpos + count);
+    DecRows rows;
     int rc = 0;
     uint8_t* o = nullptr; size_t on = 0;
-    if (count) rc = decode_common(in, n, 0, &pos, &e, &o, &on, nullptr, nullptr);
+    if (count) rc = decode_common(in, n, [&](Ctx& c, StreamIn& s, StreamOut& d, size_t* p) { bzip2_decompress_list(c, s, pos, d, rows, p); }, &o, &on);
     else if (!(o = (uint8_t*)malloc(1))) throw B2Error{B2_ERR_CUDA, "out of host memory"};  // no position: nothing is read, not even the header
-    for (size_t i = 0; i < e.size(); i++) ((uint64_t*)ep.p)[i] = e[i];
-    *out = o; *out_n = on; *ends = (uint64_t*)ep.p; *done = e.size();
+    for (size_t i = 0; i < rows.ends.size(); i++) ((uint64_t*)ep.p)[i] = rows.ends[i];
+    *out = o; *out_n = on; *ends = (uint64_t*)ep.p; *done = rows.ends.size();
     ep.p = nullptr;
     return rc;
   });
@@ -863,12 +860,12 @@ int b2_bzip2_decompress_block_partial(const uint8_t* in, size_t n, uint64_t bitp
 
 int b2_bzip2_table_partial(const uint8_t* in, size_t n, int multistream, uint64_t** bitpos, uint32_t** sizes, size_t* count) {
   return guarded([&]() {
-    std::vector<u64> tp; std::vector<u32> tl;
-    const int rc = decode_common(in, n, multistream, nullptr, nullptr, nullptr, nullptr, &tp, &tl);
-    *count = tp.size();
-    *bitpos = (uint64_t*)malloc(sizeof(uint64_t) * (tp.size() + 1));
-    *sizes = (uint32_t*)malloc(sizeof(uint32_t) * (tp.size() + 1));
-    for (size_t i = 0; i < tp.size(); i++) { (*bitpos)[i] = tp[i]; (*sizes)[i] = tl[i]; }
+    DecRows rows;
+    const int rc = decode_common(in, n, [&](Ctx& c, StreamIn& s, StreamOut&, size_t* p) { bzip2_table(c, s, multistream, rows, p); }, nullptr, nullptr);
+    *count = rows.pos.size();
+    *bitpos = (uint64_t*)malloc(sizeof(uint64_t) * (rows.pos.size() + 1));
+    *sizes = (uint32_t*)malloc(sizeof(uint32_t) * (rows.pos.size() + 1));
+    for (size_t i = 0; i < rows.pos.size(); i++) { (*bitpos)[i] = rows.pos[i]; (*sizes)[i] = rows.len[i]; }
     return rc;
   });
 }
@@ -904,16 +901,15 @@ int b2_bzip2_decompress_dev(const void* d_in, size_t n, int multistream, void* d
   return guarded([&]() {
     Ctx& c = ctx_locked();
     c.reset_call();
-    int rc;
     {
       StageScope tot(c, ST_TOTAL);
-      rc = bzip2_decompress(c, nullptr, (const u8*)d_in, n, multistream, (u8*)d_out, out_cap, nullptr, out_n, nullptr, nullptr, nullptr,
-                            nullptr);
+      if (d_out) bzip2_decompress_dev(c, (const u8*)d_in, n, multistream, (u8*)d_out, out_cap, out_n);
+      else bzip2_decompress_size(c, (const u8*)d_in, n, multistream, out_n);
     }
     c.sync();
     c.collect();
     c.stats.raw_bytes = *out_n; c.stats.comp_bytes = n;
-    return rc;
+    return 0;
   });
 }
 

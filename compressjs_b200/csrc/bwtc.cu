@@ -22,8 +22,6 @@
 #include "enc.h"
 #include "bwtc_core.cuh"
 
-void bwt_inverse_sentinel_batch(Ctx& c, const u8* d_L, const u32* h_n, const u32* h_pidx, u32 nb, u8* d_out);
-
 struct BwtcState {
   bc_enc rc;
   u32 overflow;  // a block's triples did not fit its buffer

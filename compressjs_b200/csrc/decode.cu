@@ -27,12 +27,15 @@
 //                    synchronisation points (8 bytes per thread, decided in registers), output
 //                    offsets from tile sums + one warp scan per block, tiles expanded in shared
 //                    memory, CRC32 per block
-//   host           : one rolling loop over windows of the compressed input and batches of blocks
-//                    (bzip2_decompress): walks the block chain (a block must start exactly where the previous
-//                    one ended) after every batch, folds/validates CRCs, delivers the settled blocks and
-//                    raises the reference's errors in stream order; a position list is taken in list order
-//                    instead, without a chain.
+//   host           : one driver per kind of decode (enc.h).  A chain decode is one rolling loop over windows of
+//                    the compressed input (DecIn: a host source or a device buffer) and batches of blocks: it walks
+//                    the block chain (a block must start exactly where the previous one ended) after every batch,
+//                    folds/validates CRCs, delivers the settled blocks (to a device buffer, a host sink, or only
+//                    for their CRCs) and raises the reference's errors in stream order.  A position list uploads
+//                    the whole input once and walks its blocks in list order, without a chain.  The sharded decode
+//                    runs the same batch, walk and device delivery over the whole file.
 #include <algorithm>
+#include <memory>
 #include <vector>
 #include "enc.h"
 #include "radix.cuh"
@@ -833,6 +836,21 @@ __global__ void k_ibwt_tail(const u32* __restrict__ P, const CandRes* __restrict
 
 static void dec_attr_once();
 
+// The four walk launches of the inverse BWT over cnt blocks, from their vectors P (P[row] = successor << 8 | byte, slot
+// layout): the sampled-row walks, recording into slotA / slotB (4 MiB per block each), their chain, the placement of what
+// they recorded and the walks behind the records.  Each block goes back to front into its slot at out.
+static void ibwt_walks(Ctx& c, const u32* P, const CandRes* res, u32 cnt, Seg* segs, u32* capr, Visit* visits, u32* nvis, u32* tails,
+                       u32* ntails, u8* slotA, u8* slotB, u8* out) {
+  k_ibwt_walk1<<<(cnt * IB_SEGS + 127) / 128, 128, 0, c.stream>>>(P, res, cnt, segs, capr, slotA, slotB);
+  KLAUNCH(c); KCHECK();
+  k_ibwt_chain<<<cnt, 128, sizeof(Seg) * IB_SEGS, c.stream>>>(P, res, cnt, segs, visits, nvis, tails, ntails);
+  KLAUNCH(c); KCHECK();
+  k_ibwt_place<<<cnt * IB_PLACE_CTAS, IB_PLACE_THREADS, 0, c.stream>>>(P, res, cnt, visits, nvis, slotA, slotB, out);
+  KLAUNCH(c); KCHECK();
+  k_ibwt_tail<<<(cnt * IB_VCAP + 127) / 128, 128, 0, c.stream>>>(P, res, cnt, visits, nvis, tails, ntails, capr, out);
+  KLAUNCH(c); KCHECK();
+}
+
 // ---- BWT.unbwtransform (lib/BWT.js:352-363): inverse of the sentinel BWT ------------------------------
 // Reference walk: t = 0; for i = n-1..0: U[i] = T[t]; t = LF[t] + C[T[t]]; t += (t < pidx).  LF[t] + C[T[t]] is
 // the rank x of position t in the stable order by byte, i.e. the inverse of the sorted-position vector that one
@@ -871,8 +889,6 @@ static void dec_attr_once() {
   CUDA_CHECK(cudaFuncSetAttribute(k_ibwt_chain, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(Seg) * IB_SEGS)));
   attr = true;
 }
-// nb blocks at once: block b is the L column in slot b of d_L (d_L + (b << SEG_SHIFT)), h_n[b] bytes (1 <= n <= 2^20 - 2)
-// with primary index h_pidx[b] (0 <= pidx <= n).  The decoded blocks go to d_out back to back, in block order.
 // Scratch: about 14 MiB per block.
 void bwt_inverse_sentinel_batch(Ctx& c, const u8* d_L, const u32* h_n, const u32* h_pidx, u32 nb, u8* d_out) {
   if (!nb) return;
@@ -904,16 +920,7 @@ void bwt_inverse_sentinel_batch(Ctx& c, const u8* d_L, const u32* h_n, const u32
   KLAUNCH(c); KCHECK();
   // the walks record into slotA (4 MiB per block); the start row's slot goes to the head of the block's 4 MiB of the
   // sorted positions, which k_unbwt_pack has consumed
-  u8* sA = reinterpret_cast<u8*>(slotA.p);
-  u8* sB = reinterpret_cast<u8*>(vin);
-  k_ibwt_walk1<<<(nb * IB_SEGS + 127) / 128, 128, 0, c.stream>>>(P, res, nb, segs, capr, sA, sB);
-  KLAUNCH(c); KCHECK();
-  k_ibwt_chain<<<nb, 128, sizeof(Seg) * IB_SEGS, c.stream>>>(P, res, nb, segs, visits, nvis, tails, ntails);
-  KLAUNCH(c); KCHECK();
-  k_ibwt_place<<<nb * IB_PLACE_CTAS, IB_PLACE_THREADS, 0, c.stream>>>(P, res, nb, visits, nvis, sA, sB, tmp);
-  KLAUNCH(c); KCHECK();
-  k_ibwt_tail<<<(nb * IB_VCAP + 127) / 128, 128, 0, c.stream>>>(P, res, nb, visits, nvis, tails, ntails, capr, tmp);
-  KLAUNCH(c); KCHECK();
+  ibwt_walks(c, P, res, nb, segs, capr, visits, nvis, tails, ntails, reinterpret_cast<u8*>(slotA.p), reinterpret_cast<u8*>(vin), tmp);
   k_reverse_blocks<<<grid, 256, 0, c.stream>>>(tmp, dn, doff, d_out);
   KLAUNCH(c); KCHECK();
 }
@@ -1214,16 +1221,8 @@ static void dec_batch(Ctx& c, DecScratch& B, const u8* in, u64 wbytes, u64 base_
     // all blocks of the batch walk together: the launch lasts as long as its longest segment walk, so fewer,
     // bigger launches win over keeping the packed T-vectors L2 resident (measured: 75 ms -> 36 ms per GiB).
     // The walks record into the free key / value buffers of the sort (4 MiB per block each).
-    u8* slotA = reinterpret_cast<u8*>(B.keyA.p);
-    u8* slotB = reinterpret_cast<u8*>(B.valA.p);
-    k_ibwt_walk1<<<(cnt * IB_SEGS + 127) / 128, 128, 0, c.stream>>>(Pp, rb, cnt, B.segs, B.capr, slotA, slotB);
-    KLAUNCH(c); KCHECK();
-    k_ibwt_chain<<<cnt, 128, sizeof(Seg) * IB_SEGS, c.stream>>>(Pp, rb, cnt, B.segs, B.visits, B.nvis, B.tails, B.ntails);
-    KLAUNCH(c); KCHECK();
-    k_ibwt_place<<<cnt * IB_PLACE_CTAS, IB_PLACE_THREADS, 0, c.stream>>>(Pp, rb, cnt, B.visits, B.nvis, slotA, slotB, rle);
-    KLAUNCH(c); KCHECK();
-    k_ibwt_tail<<<(cnt * IB_VCAP + 127) / 128, 128, 0, c.stream>>>(Pp, rb, cnt, B.visits, B.nvis, B.tails, B.ntails, B.capr, rle);
-    KLAUNCH(c); KCHECK();
+    ibwt_walks(c, Pp, rb, cnt, B.segs, B.capr, B.visits, B.nvis, B.tails, B.ntails, reinterpret_cast<u8*>(B.keyA.p),
+               reinterpret_cast<u8*>(B.valA.p), rle);
   }
   if (nmax) {
     StageScope ss(c, ST_UNRLE);
@@ -1240,36 +1239,53 @@ static void dec_batch(Ctx& c, DecScratch& B, const u8* in, u64 wbytes, u64 base_
   c.stats.blocks += cnt;
 }
 
-// Expand the results [0, cnt) whose ob[i] is not ~0 (RLE1 decode of their slots at rle) to dout + ob[i], and CRC each
-// into got[i].  classify: the count-byte classes were not kept; find them again, into cls.
-static void dec_expand(Ctx& c, const u8* rle, u8* cls, bool classify, const CandRes* d_res, const CandRes* h_res, const u32* tileoff, u32 cnt,
-                       const u64* ob, u8* dout, u32* got) {
-  if (!cnt) return;
-  StageScope ss(c, ST_UNRLE);
-  DBuf<u64> dob(c, cnt);
-  CUDA_CHECK(cudaMemcpyAsync(dob, ob, 8 * (size_t)cnt, cudaMemcpyHostToDevice, c.stream));
-  if (classify) {
-    k_unrle_classify<<<(unsigned)((((size_t)cnt << SEG_SHIFT) / 8 + 255) / 256), 256, 0, c.stream>>>(rle, d_res, cnt, cls);
-    KLAUNCH(c); KCHECK();
+// ---- the compressed input ----
+// A host stream (StreamIn, whose length is known once it has ended) or a device buffer [0, n).  The drivers read the
+// input through these calls only.
+struct DecIn {
+  StreamIn* s = nullptr;
+  const u8* d = nullptr;
+  size_t n = 0;
+  explicit DecIn(StreamIn& in) : s(&in) {}
+  DecIn(const u8* d_in, size_t n_) : d(d_in), n(n_) {}
+  size_t length() const { return s ? (s->eof ? s->base + s->have : SIZE_MAX) : n; }  // a stream's once it has ended
+  u64 end() const { return s ? s->base + s->have : n; }  // the end of the bytes there are so far
+  // Up to 4 bytes at bytepos (a member header) into h; returns how many there are.  The header may lie past the window:
+  // a stream reads one byte more, which tells whether the input ends behind it.
+  size_t head(Ctx& c, u64 bytepos, u8* h) {
+    if (s) s->fill(bytepos + 5);
+    const size_t avail = (size_t)std::min<u64>(4, end() - bytepos);
+    if (s) {
+      memcpy(h, s->at(bytepos), avail);
+    } else {
+      CUDA_CHECK(cudaMemcpyAsync(h, d + bytepos, avail, cudaMemcpyDeviceToHost, c.stream));
+      CUDA_CHECK(cudaStreamSynchronize(c.stream));
+    }
+    return avail;
   }
-  k_unrle_emit<<<(unsigned)((size_t)cnt * UR_TPS), UR_THREADS, 0, c.stream>>>(rle, cls, d_res, UR_TPS, tileoff, dob, dout);
-  KLAUNCH(c); KCHECK();
-  std::vector<BlkInfo> ranges(cnt);
-  for (u32 i = 0; i < cnt; i++) {
-    memset(&ranges[i], 0, sizeof(BlkInfo));
-    if (ob[i] != ~0ull) { ranges[i].s = ob[i]; ranges[i].e = ob[i] + h_res[i].rawlen; }
+  // As much of [a, a + len) as the input has into the device buffer win, zero padded (aligned word reads past the end
+  // must be safe); returns its length.  A stream keeps its bytes from a on and reads one byte past a + len, so its end is
+  // known exactly when a complete input would show it (until then no window is the last one).
+  u64 window(Ctx& c, DBuf<u8>& win, u64 a, u64 want) {
+    if (s) {
+      s->drop(a);
+      s->fill(a + want + 1);
+    }
+    const u64 len = std::min<u64>(want, end() - a);
+    if (len + 32 > win.n) win.alloc(c, len + 32);
+    CUDA_CHECK(cudaMemsetAsync(win.p + (len & ~(u64)3), 0, 32 + (len & 3), c.stream));
+    if (s) {
+      StageScope st(c, ST_H2D);
+      if (len) CUDA_CHECK(cudaMemcpyAsync(win, s->at(a), len, cudaMemcpyHostToDevice, c.stream));
+    } else if (len) {
+      CUDA_CHECK(cudaMemcpyAsync(win, d + a, len, cudaMemcpyDeviceToDevice, c.stream));
+    }
+    return len;
   }
-  DBuf<BlkInfo> dr(c, cnt);
-  DBuf<u32> dcrc(c, cnt);
-  CUDA_CHECK(cudaMemcpyAsync(dr, ranges.data(), sizeof(BlkInfo) * cnt, cudaMemcpyHostToDevice, c.stream));
-  crc_ranges(c, dout, dr, ranges, dcrc);
-  CUDA_CHECK(cudaMemcpyAsync(got, dcrc, 4 * (size_t)cnt, cudaMemcpyDeviceToHost, c.stream));
-  CUDA_CHECK(cudaStreamSynchronize(c.stream));
-}
+};
 
 // ---- the block chain (lib/Bzip2.js:454-481 / 508-548) ----
 struct Chain {
-  size_t n = 0;             // bytes of the file
   int multistream = 0;
   u32 cur_dbuf = 0;         // dbufSize of the member the walk is in (lib/Bzip2.js:121)
   u64 pos = 32;             // bit position of the next magic
@@ -1302,32 +1318,175 @@ static bool block_event(Chain& ch, const Cand& cd, const CandRes& r, size_t slot
   return true;
 }
 
-// What the caller knows of the magic at a bit position.  kind: -1 nothing final yet (walk on later), 0 no magic,
-// 1 block (cd, its results r in slot), 2 end of stream (cd).
-struct At { int kind; const Cand* cd; const CandRes* r; size_t slot; };
+// The first failure in stream order: event index, code, message, and the bytes the reference has written when it throws
+// (a block's own bytes go out before its CRC check).
+struct DecErr { long ev = -1; int code = 0; std::string msg; u64 prefix = 0; };
 
-// Walk the chain from ch.pos as far as look() has final results.  head(bytepos, h) reads up to 4 bytes of the file at
-// bytepos for a member header and returns how many there are.
-template <class Look, class Head>
-static void chain_walk(Chain& ch, Look look, Head head) {
+// ---- one decode ----
+// Its input, the device window [a, a + wl) of it (last: the window ends the input), the magics found there, the decode
+// batch, the chain, and what its replay found.
+struct Decode {
+  Ctx& c;
+  DecIn in;
+  const size_t W = dec_window();
+  const u32 DB;
+  DBuf<u8> win, stage;
+  u64 a = 0, wl = 0;
+  bool last = false;
+  std::vector<Cand> cands;  // the window's magics: sorted by position, or a position list's in list order
+  std::vector<size_t> blk;  // the block candidates among them (indices into cands, in order)
+  DecScratch B;
+  DBuf<Cand> dcand;
+  // the decoded blocks waiting for their expansion, one slot each: the L column, the count-byte classes, the tile
+  // offsets and the device results.  A sharded share of more than DEC_KEEP_CLS blocks keeps no classes: cls holds one
+  // batch's, found again on expansion.
+  DBuf<u8> rle, cls;
+  DBuf<u32> tileoff;
+  DBuf<CandRes> dres;
+  bool keep_cls = true;
+  std::vector<CandRes> hres;
+  size_t kb = 0;  // the batch: block candidates [kb, kb + cnt), in slots [0, cnt)
+  u32 cnt = 0;
+  std::vector<u64> ob;   // per slot of a delivery: its output offset (~0: not expanded)
+  std::vector<u32> got;  // and the CRC of what it expanded to
+  Chain ch;
+  DecErr E;
+  DecRows rows;
+  // reads the first header (lib/Bzip2.js:105-124 _start_bunzip)
+  Decode(Ctx& c_, const DecIn& in_) : c(c_), in(in_), DB(dec_batch_blocks(c_)) {
+    u8 hdr[4] = {0, 0, 0, 0};
+    if (in.head(c, 0, hdr) < 4 || hdr[0] != 'B' || hdr[1] != 'Z' || hdr[2] != 'h') throw B2Error{DEC_NOT_BZIP, "Not bzip data: bad magic"};
+    const int level = hdr[3] - 0x30;
+    if (level < 1 || level > 9) throw B2Error{DEC_NOT_BZIP, "Not bzip data: level out of range"};
+    ch.cur_dbuf = 100000u * (u32)level;
+  }
+  void load(u64 a_, u64 len) {
+    a = a_;
+    wl = in.window(c, win, a, len);
+    last = a + wl == in.length();
+  }
+  // Every magic of the window below window bit lim, sorted by position, and the block candidates among them.
+  void scan(u64 lim) {
+    StageScope ss(c, ST_SCAN);
+    // Highly repetitive input compresses to a few dozen bytes per block (and multistream files may hold thousands of
+    // tiny members), so the number of magics is not bounded by the usual ~100 KB per block: when the first guess is too
+    // small the scan counts them all and runs once more with exactly that capacity.
+    u32 cap = (u32)(wl / 8000 + 1024);
+    DBuf<Cand> dc(c, cap);
+    DBuf<u32> dcount(c, 1);
+    u32 cnt = 0;
+    for (int attempt = 0; attempt < 2; attempt++) {
+      CUDA_CHECK(cudaMemsetAsync(dcount, 0, 4, c.stream));
+      k_scan_magic<<<(unsigned)(((wl + 3) / 4 + 255) / 256), 256, 0, c.stream>>>(win, wl, a * 8, lim, dc, dcount, cap);
+      KLAUNCH(c); KCHECK();
+      CUDA_CHECK(cudaMemcpyAsync(&cnt, dcount, 4, cudaMemcpyDeviceToHost, c.stream));
+      CUDA_CHECK(cudaStreamSynchronize(c.stream));
+      if (cnt <= cap) break;
+      cap = cnt;
+      dc.alloc(c, cap);
+    }
+    if (cnt > cap) throw B2Error{B2_ERR_CUDA, "magic scan did not settle"};
+    cands.resize(cnt);
+    if (cnt) CUDA_CHECK(cudaMemcpyAsync(cands.data(), dc, sizeof(Cand) * cnt, cudaMemcpyDeviceToHost, c.stream));
+    CUDA_CHECK(cudaStreamSynchronize(c.stream));
+    std::sort(cands.begin(), cands.end(), [](const Cand& x, const Cand& y) { return x.pos < y.pos; });
+    blk.clear();
+    for (size_t i = 0; i < cands.size(); i++) if (cands[i].type == 1) blk.push_back(i);
+  }
+  // the first block candidate at or behind bit position pos (an index into blk)
+  size_t blk_from(u64 pos) const {
+    return (size_t)(std::lower_bound(blk.begin(), blk.end(), pos, [&](size_t ci, u64 p) { return cands[ci].pos < p; }) - blk.begin());
+  }
+  // slots for nb blocks, the classes of ncls
+  void alloc(size_t nb, size_t ncls) {
+    rle.alloc(c, nb << SEG_SHIFT); cls.alloc(c, ncls << SEG_SHIFT); tileoff.alloc(c, nb * UR_TPS); dres.alloc(c, nb);
+  }
+  // slots for the largest batch of the window, kept for the largest of the call
+  void reserve() {
+    const size_t nbm = std::min<size_t>(DB, blk.size());
+    if (nbm > dres.n) { alloc(nbm, nbm); dcand.alloc(c, nbm); }
+  }
+  // decode block candidates [j0, j0 + n) into slots [s0, s0 + n), their results into h
+  void decode(size_t j0, u32 n, size_t s0, CandRes* h) {
+    std::vector<Cand> bc(n);
+    for (u32 i = 0; i < n; i++) bc[i] = cands[blk[j0 + i]];
+    CUDA_CHECK(cudaMemcpyAsync(dcand, bc.data(), sizeof(Cand) * n, cudaMemcpyHostToDevice, c.stream));
+    dec_batch(c, B, win, wl, a * 8, last, dcand, n, dres.p + s0, h, rle.p + (s0 << SEG_SHIFT), cls.p + (keep_cls ? s0 << SEG_SHIFT : 0),
+              tileoff.p + s0 * UR_TPS);
+  }
+  // Expand the slots of [s0, s1) whose ob is not ~0 (RLE1 decode) to dout + ob, and CRC each into got; hres, ob and got
+  // are indexed by slot.  Without the classes, DB slots at a time are classified again first.
+  void expand(size_t s0, size_t s1, const CandRes* h, const u64* ob, u8* dout, u32* got) {
+    const size_t step = keep_cls ? s1 - s0 : DB;
+    for (size_t k0 = s0; k0 < s1; k0 += step) {
+      const u32 m = (u32)std::min<size_t>(step, s1 - k0);
+      StageScope ss(c, ST_UNRLE);
+      u8* kcls = cls.p + (keep_cls ? k0 << SEG_SHIFT : 0);
+      DBuf<u64> dob(c, m);
+      CUDA_CHECK(cudaMemcpyAsync(dob, ob + k0, 8 * (size_t)m, cudaMemcpyHostToDevice, c.stream));
+      if (!keep_cls) {
+        k_unrle_classify<<<(unsigned)((((size_t)m << SEG_SHIFT) / 8 + 255) / 256), 256, 0, c.stream>>>(rle.p + (k0 << SEG_SHIFT), dres.p + k0, m, kcls);
+        KLAUNCH(c); KCHECK();
+      }
+      k_unrle_emit<<<(unsigned)((size_t)m * UR_TPS), UR_THREADS, 0, c.stream>>>(rle.p + (k0 << SEG_SHIFT), kcls, dres.p + k0, UR_TPS,
+                                                                                   tileoff.p + k0 * UR_TPS, dob, dout);
+      KLAUNCH(c); KCHECK();
+      std::vector<BlkInfo> ranges(m);
+      for (u32 i = 0; i < m; i++) {
+        memset(&ranges[i], 0, sizeof(BlkInfo));
+        if (ob[k0 + i] != ~0ull) { ranges[i].s = ob[k0 + i]; ranges[i].e = ob[k0 + i] + h[k0 + i].rawlen; }
+      }
+      DBuf<BlkInfo> dr(c, m);
+      DBuf<u32> dcrc(c, m);
+      CUDA_CHECK(cudaMemcpyAsync(dr, ranges.data(), sizeof(BlkInfo) * m, cudaMemcpyHostToDevice, c.stream));
+      crc_ranges(c, dout, dr, ranges, dcrc);
+      CUDA_CHECK(cudaMemcpyAsync(got + k0, dcrc, 4 * (size_t)m, cudaMemcpyDeviceToHost, c.stream));
+      CUDA_CHECK(cudaStreamSynchronize(c.stream));
+    }
+  }
+  // the batch from block candidate kb on
+  void batch() {
+    cnt = (u32)std::min<size_t>(DB, blk.size() - kb);
+    if (!cnt) return;
+    hres.resize(cnt);
+    decode(kb, cnt, 0, hres.data());
+  }
+  // the call's end: *out_n = the decoded size, or on a failure `failed` and the failure is thrown
+  void finish(size_t* out_n, u64 failed) const {
+    *out_n = (size_t)(E.ev >= 0 ? failed : ch.total_out);
+    if (E.ev >= 0) throw B2Error{E.code, E.msg};
+  }
+};
+
+// Walk R's chain from ch.pos over the sorted magics as far as the batch has final results (block candidate j of the batch
+// is in slot j - kb).  Returns true when the walk stopped for input behind the device window: a magic the window's end
+// (bit end_bit) may cut off, or a block whose decode reached that end.
+static bool chain_walk(Decode& R, u64 end_bit) {
+  Chain& ch = R.ch;
   while (!ch.done) {
-    if ((ch.pos + 7) / 8 >= ch.n) { ch.done = true; break; }  // 'eof' in inputStream && inputStream.eof() (lib/Bzip2.js:462)
-    const At at = look(ch.pos);
-    if (at.kind < 0) return;
-    if (at.kind == 0) { ch.events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data", ch.total_out, 0, 0}); ch.done = true; break; }
-    if (at.kind == 1) {
-      ch.stream_crc = at.cd->next32 ^ ((ch.stream_crc << 1) | (ch.stream_crc >> 31));  // lib/Bzip2.js:138-139
-      if (!block_event(ch, *at.cd, *at.r, at.slot)) { ch.done = true; break; }
-      ch.pos = at.r->endbit;
+    if ((ch.pos + 7) / 8 >= R.in.length()) { ch.done = true; break; }  // 'eof' in inputStream && inputStream.eof() (lib/Bzip2.js:462)
+    const auto it = std::lower_bound(R.cands.begin(), R.cands.end(), ch.pos, [](const Cand& x, u64 p) { return x.pos < p; });
+    if (it == R.cands.end() || it->pos != ch.pos) {
+      if (ch.pos + 80 > end_bit) return true;
+      ch.events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data", ch.total_out, 0, 0}); ch.done = true; break;
+    }
+    if (it->type == 1) {
+      const size_t j = R.blk_from(ch.pos);
+      if (j >= R.kb + R.cnt) return false;  // in a later batch
+      const CandRes& r = R.hres[j - R.kb];
+      if (r.open) return true;
+      ch.stream_crc = it->next32 ^ ((ch.stream_crc << 1) | (ch.stream_crc >> 31));  // lib/Bzip2.js:138-139
+      if (!block_event(ch, *it, r, j - R.kb)) { ch.done = true; break; }
+      ch.pos = r.endbit;
       continue;
     }
-    ch.events.push_back({1, 0, ch.stream_crc, at.cd->next32, 0, "", ch.total_out, 0, 0});
+    ch.events.push_back({1, 0, ch.stream_crc, it->next32, 0, "", ch.total_out, 0, 0});
     ch.pos += 80;
     const u64 bytepos = (ch.pos + 7) / 8;
-    if (!ch.multistream || bytepos >= ch.n) { ch.done = true; break; }
+    if (!ch.multistream || bytepos >= R.in.length()) { ch.done = true; break; }
     // _start_bunzip on the byte stream (resyncs to the next byte)
     u8 h2[4] = {0, 0, 0, 0};
-    const size_t avail = head(bytepos, h2);
+    const size_t avail = R.in.head(R.c, bytepos, h2);
     if (avail != 4 || h2[0] != 'B' || h2[1] != 'Z' || h2[2] != 'h') {
       ch.events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data: bad magic", ch.total_out, 0, 0}); ch.done = true; break;
     }
@@ -1337,495 +1496,341 @@ static void chain_walk(Chain& ch, Look look, Head head) {
     ch.stream_crc = 0;
     ch.pos = (bytepos + 4) * 8;
   }
+  return false;
 }
 
 // The same for a position list (lib/Bzip2.js:482-503 once per position), in list order: cands[i] is the magic at the
-// i-th position (type 0: none).  look(i, &r, &slot) gives a block's results, or false when they are not decoded yet.
-template <class Look>
-static void list_walk(Chain& ch, const std::vector<Cand>& cands, Look look) {
+// i-th position (type 0: none).
+static void list_walk(Decode& R) {
+  Chain& ch = R.ch;
   while (!ch.done) {
-    if (ch.li >= cands.size()) { ch.done = true; break; }
-    const Cand& cd = cands[ch.li];
+    if (ch.li >= R.cands.size()) { ch.done = true; break; }
+    const Cand& cd = R.cands[ch.li];
     if (cd.type == 0) { ch.events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data", ch.total_out, 0, 0}); ch.done = true; break; }
     if (cd.type == 2) { ch.events.push_back({3, 0, 0, 0, 0, "", ch.total_out, 0, 0}); ch.li++; continue; }
-    const CandRes* r = nullptr; size_t slot = 0;
-    if (!look(ch.li, &r, &slot)) return;
-    if (!block_event(ch, cd, *r, slot)) { ch.done = true; break; }
+    const size_t j = (size_t)(std::lower_bound(R.blk.begin(), R.blk.end(), ch.li) - R.blk.begin());
+    if (j >= R.kb + R.cnt) return;  // in a later batch
+    if (!block_event(ch, cd, R.hres[j - R.kb], j - R.kb)) { ch.done = true; break; }
     ch.li++;
   }
 }
 
-// The first failure in stream order: event index, code, message, and the bytes the reference has written when it throws
-// (a block's own bytes go out before its CRC check).
-struct DecErr { long ev = -1; int code = 0; std::string msg; u64 prefix = 0; };
-
-// Replay events [e0, e1) up to the first failure, which goes to E: block CRCs against got(slot) = {known, crc} (a block
-// whose CRC is not known here passes: another rank checks it), stream CRCs unless for a table; the table rows and list
-// ends of everything in front of the failure.
-template <class Got>
-static void replay(const Chain& ch, size_t e0, size_t e1, Got got, std::vector<u64>* tab_pos, std::vector<u32>* tab_len,
-                   std::vector<u64>* ends, DecErr& E) {
+// Replay events [e0, e1) up to the first failure, which goes to R.E: block CRCs against R.got for the slots s whose offset
+// R.ob[s - lo] is set (any other block passes: it was not expanded here, and in a sharded decode its owner checks it),
+// stream CRCs unless for a table (Bzip2.table does not check them).  The rows and ends of everything in front of the
+// failure go to R.rows.
+static void replay(Decode& R, size_t e0, size_t e1, size_t lo, bool table) {
+  DecErr& E = R.E;
   for (size_t ei = e0; ei < e1 && E.ev < 0; ei++) {
-    const Event& ev = ch.events[ei];
+    const Event& ev = R.ch.events[ei];
     if (ev.kind == 0) {
-      const std::pair<bool, u32> g = got(ev.slot);
-      if (g.first && g.second != ev.a) {
-        E.ev = (long)ei; E.code = DEC_DATA_ERROR; E.msg = "Data error: Bad block CRC (got " + hexs(g.second) + " expected " + hexs(ev.a) + ")";
+      const size_t s = ev.slot - lo;
+      if (ev.slot >= lo && s < R.ob.size() && R.ob[s] != ~0ull && R.got[s] != ev.a) {
+        E.ev = (long)ei; E.code = DEC_DATA_ERROR; E.msg = "Data error: Bad block CRC (got " + hexs(R.got[s]) + " expected " + hexs(ev.a) + ")";
         E.prefix = ev.off + ev.len;
       }
-      if (E.ev < 0 && tab_pos) { tab_pos->push_back(ev.pos); tab_len->push_back(ev.len); }
+      if (E.ev < 0) { R.rows.pos.push_back(ev.pos); R.rows.len.push_back(ev.len); }
     } else if (ev.kind == 1) {
-      if (!tab_pos && ev.a != ev.b) {
+      if (!table && ev.a != ev.b) {
         E.ev = (long)ei; E.code = DEC_DATA_ERROR; E.msg = "Data error: Bad stream CRC (got " + hexs(ev.a) + " expected " + hexs(ev.b) + ")";
         E.prefix = ev.off;
       }
     } else if (ev.kind == 2) {
       E.ev = (long)ei; E.code = ev.code; E.msg = ev.msg; E.prefix = ev.off;
     }
-    if (ends && E.ev < 0) ends->push_back(ev.kind == 0 ? ev.off + ev.len : ev.off);
+    if (E.ev < 0) R.rows.ends.push_back(ev.kind == 0 ? ev.off + ev.len : ev.off);
   }
 }
 
-static void read_level(const u8* hdr, size_t n, u32* dbuf_size) {
-  // lib/Bzip2.js:105-124 _start_bunzip
-  if (n < 4 || hdr[0] != 'B' || hdr[1] != 'Z' || hdr[2] != 'h') throw B2Error{DEC_NOT_BZIP, "Not bzip data: bad magic"};
-  const int level = hdr[3] - 0x30;
-  if (level < 1 || level > 9) throw B2Error{DEC_NOT_BZIP, "Not bzip data: level out of range"};
-  *dbuf_size = 100000u * (u32)level;
+// ---- deliveries: expand, CRC-check and replay the block events of [e0, e1), which a walk settled ----
+// Device delivery: each block event whose slot s lies in [lo, lo + cnt) goes to dout + off - base from slot s - lo, if it
+// fits below cap (one that does not is only counted: the caller reports the size needed).
+static void deliver_dev(Decode& R, size_t e0, size_t e1, size_t lo, size_t cnt, u64 base, u8* dout, u64 cap) {
+  R.ob.assign(cnt ? cnt : 1, ~0ull);
+  R.got.assign(cnt ? cnt : 1, 0);
+  for (size_t ei = e0; ei < e1; ei++) {
+    const Event& ev = R.ch.events[ei];
+    if (ev.kind == 0 && ev.slot >= lo && ev.slot < lo + cnt && ev.off - base + ev.len <= cap) R.ob[ev.slot - lo] = ev.off - base;
+  }
+  R.expand(0, cnt, R.hres.data() + lo, R.ob.data(), dout, R.got.data());
+  replay(R, e0, e1, lo, false);
 }
 
-// Every magic of the window `in` (wbytes bytes from bit base_bit of the file) below window bit lim, sorted by position.
-static void scan_window(Ctx& c, const u8* in, u64 wbytes, u64 base_bit, u64 lim, std::vector<Cand>& cands) {
-  StageScope ss(c, ST_SCAN);
-  // Highly repetitive input compresses to a few dozen bytes per block (and multistream files may hold thousands of
-  // tiny members), so the number of magics is not bounded by the usual ~100 KB per block: when the first guess is too
-  // small the scan counts them all and runs once more with exactly that capacity.
-  u32 cap = (u32)(wbytes / 8000 + 1024);
-  DBuf<Cand> dc(c, cap);
-  DBuf<u32> dcount(c, 1);
-  u32 cnt = 0;
-  for (int attempt = 0; attempt < 2; attempt++) {
-    CUDA_CHECK(cudaMemsetAsync(dcount, 0, 4, c.stream));
-    k_scan_magic<<<(unsigned)(((wbytes + 3) / 4 + 255) / 256), 256, 0, c.stream>>>(in, wbytes, base_bit, lim, dc, dcount, cap);
-    KLAUNCH(c); KCHECK();
-    CUDA_CHECK(cudaMemcpyAsync(&cnt, dcount, 4, cudaMemcpyDeviceToHost, c.stream));
-    CUDA_CHECK(cudaStreamSynchronize(c.stream));
-    if (cnt <= cap) break;
-    cap = cnt;
-    dc.alloc(c, cap);
+// The staged deliveries: the blocks go through a device staging buffer in groups of consecutive blocks of at most
+// max(W, one block) bytes.  group(bytes, off, g_end, last_group) sees each group there (off: its offset in the decoded
+// stream, g_end: the end of its events) and ends the delivery by returning false.
+template <class Group>
+static void stage_groups(Decode& R, size_t e0, size_t e1, Group group) {
+  std::vector<size_t> settled;
+  for (size_t ei = e0; ei < e1; ei++) if (R.ch.events[ei].kind == 0) settled.push_back(ei);
+  R.ob.assign(R.cnt ? R.cnt : 1, ~0ull);
+  R.got.assign(R.cnt ? R.cnt : 1, 0);
+  for (size_t g0 = 0; g0 < settled.size();) {
+    const Event& f = R.ch.events[settled[g0]];
+    u64 bytes = f.len;
+    size_t g1 = g0 + 1;
+    while (g1 < settled.size() && bytes + R.ch.events[settled[g1]].len <= R.W) bytes += R.ch.events[settled[g1++]].len;
+    const size_t s0 = f.slot, s1 = R.ch.events[settled[g1 - 1]].slot + 1;
+    for (size_t g = g0; g < g1; g++) { const Event& ev = R.ch.events[settled[g]]; R.ob[ev.slot] = ev.off - f.off; }
+    if (bytes > R.stage.n) R.stage.alloc(R.c, bytes);
+    R.expand(s0, s1, R.hres.data(), R.ob.data(), R.stage, R.got.data());
+    if (!group(bytes, f.off, settled[g1 - 1] + 1, g1 == settled.size())) return;
+    g0 = g1;
   }
-  if (cnt > cap) throw B2Error{B2_ERR_CUDA, "magic scan did not settle"};
-  cands.resize(cnt);
-  if (cnt) CUDA_CHECK(cudaMemcpyAsync(cands.data(), dc, sizeof(Cand) * cnt, cudaMemcpyDeviceToHost, c.stream));
-  CUDA_CHECK(cudaStreamSynchronize(c.stream));
-  std::sort(cands.begin(), cands.end(), [](const Cand& a, const Cand& b) { return a.pos < b.pos; });
 }
 
-// ---- single-GPU decode: one rolling loop over input windows and decode batches --------------------------------------
-// The compressed input is `sin` (host) or d_in[0, n) (device).  Only the window [a, a + W) of it is on the device
-// (W = dec_window(); a is the chain's position, rounded down to 256 bytes).  The window's magics are decoded in position
-// order, a batch at a time; after each batch the host walks the chain as far as final results allow, and the blocks that
-// walk settled are expanded, CRC-checked and delivered.  The first chain position without a final result starts the next
-// window; a window that would start where this one did is twice as long, so a block longer than W still decodes.
-// Delivery: d_out (device, absolute offsets, nothing past out_cap), or the table rows (tab_pos / tab_len: expanded only
-// for the CRCs), or else `sout`, through a device staging buffer of at most max(W, one block) bytes.  Each staged group's
-// events are replayed before it leaves and the group is cut at the prefix the replay allows, so nothing past the prefix
-// of b2_bzip2_decompress_partial ever reaches sout.
-// positions: decode the blocks at these bit positions, back to back in list order (ends: the end offset of every
-// position delivered in full), with the whole input on the device.
-// sin keeps the bytes from the window's start on, and every window is read one byte past its end, so the input's end is
-// known exactly when a complete input would show it (n stays unknown until then, and no window is the last one).
-int bzip2_decompress(Ctx& c, StreamIn* sin, const u8* d_in, size_t n, int multistream, u8* d_out, size_t out_cap, StreamOut* sout,
-                     size_t* out_n, const std::vector<u64>* positions, std::vector<u64>* ends, std::vector<u64>* tab_pos,
-                     std::vector<u32>* tab_len) {
-  *out_n = 0;
-  // with neither d_out nor sout (a table, or a device call without a buffer) the blocks are expanded only for their CRCs
-  const bool dev = d_out != nullptr, listed = positions != nullptr;
-  auto read_dev = [&](u8* dst, u64 off, size_t len) {
-    if (!len) return;
-    CUDA_CHECK(cudaMemcpyAsync(dst, d_in + off, len, cudaMemcpyDeviceToHost, c.stream));
-    CUDA_CHECK(cudaStreamSynchronize(c.stream));
-  };
-  Chain ch;
-  // the input's length, once the host input has ended
-  auto learn_end = [&]() {
-    if (sin->eof) ch.n = n = sin->base + sin->have;
-  };
-  u8 hdr[4] = {0, 0, 0, 0};
-  if (sin) {
-    n = SIZE_MAX;
-    const size_t end = sin->fill(5);  // the header, and whether anything follows it
-    std::copy_n(sin->at(0), std::min<size_t>(end, 4), hdr);
-    read_level(hdr, end, &ch.cur_dbuf);
-  } else {
-    read_dev(hdr, 0, std::min<size_t>(n, 4));
-    read_level(hdr, n, &ch.cur_dbuf);
-  }
-  ch.n = n;
-  if (sin) learn_end();
-  ch.multistream = listed ? 0 : multistream;
-  const size_t W = dec_window();
-  const u32 DB = dec_batch_blocks(c);
-  DecScratch B;
-  DBuf<u8> win, rle, cls, stage;
-  DBuf<u32> tileoff;
-  DBuf<CandRes> dres;
-  DBuf<Cand> dcand;
-  size_t win_cap = 0, slots = 0, stage_cap = 0;
-  std::vector<Cand> cands;
-  std::vector<size_t> blk;      // block candidates of the window (index into cands)
-  std::vector<CandRes> hres;    // results of the batch
-  std::vector<u32> got;
-  std::vector<u64> ob;
-  std::vector<size_t> settled;  // block events of the batch
-  DecErr E;
+// Host delivery: each group's events are replayed before it leaves and the group is cut at the prefix the replay allows,
+// so nothing past the prefix of b2_bzip2_decompress_partial ever reaches `out`.
+static void deliver_host(Decode& R, size_t e0, size_t e1, StreamOut& out) {
+  size_t er = e0;  // events replayed so far
+  stage_groups(R, e0, e1, [&](u64 bytes, u64 off, size_t g_end, bool last_group) {
+    replay(R, er, g_end, 0, false);
+    er = g_end;
+    const u64 keep = R.E.ev < 0 ? bytes : (R.E.prefix > off ? std::min<u64>(bytes, R.E.prefix - off) : 0);
+    if (keep) {
+      // no group follows the last one of a finished chain or a failure: a call of one batch makes one result buffer of
+      // exactly its size and one copy
+      out.reserve((size_t)keep, (R.ch.done && last_group) || R.E.ev >= 0, R.W);
+      u8* dst = out.next();
+      {
+        StageScope s(R.c, ST_D2H);
+        CUDA_CHECK(cudaMemcpyAsync(dst, R.stage, keep, cudaMemcpyDeviceToHost, R.c.stream));
+      }
+      out.put(dst, (size_t)keep);
+    }
+    return R.E.ev < 0;
+  });
+  replay(R, er, e1, 0, false);
+}
+
+// CRC-only delivery (a table, or a device decode without an output buffer): the blocks are expanded for their CRCs only.
+static void deliver_crc(Decode& R, size_t e0, size_t e1, bool table) {
+  stage_groups(R, e0, e1, [](u64, u64, size_t, bool) { return true; });
+  replay(R, e0, e1, 0, table);
+}
+
+// ---- single-GPU drivers ----
+// A chain decode: one rolling loop over input windows and decode batches.  Only the window [a, a + W) of the input is on
+// the device (W = dec_window(); a is the chain's position, rounded down to 256 bytes).  The window's magics are decoded in
+// position order, a batch at a time; after each batch the host walks the chain as far as final results allow, and
+// deliver(e0, e1) delivers the blocks that walk settled.  The first chain position without a final result starts the
+// next window; a window that would start where this one did is twice as long, so a block longer than W still decodes.
+// The first failure in stream order ends the walk, unless past_error (the device delivery walks on for the needed size).
+template <class Deliver>
+static void chain_decode(Decode& R, int multistream, bool past_error, Deliver deliver) {
+  Chain& ch = R.ch;
+  ch.multistream = multistream;
   u64 prev_a = ~0ull;
-  size_t wcur = W;
-  auto head = [&](u64 bytepos, u8* h) -> size_t {
-    if (sin) {
-      // the header may lie past the window; one byte more tells whether the file ends behind it
-      const size_t end = sin->fill(bytepos + 5);
-      learn_end();
-      const size_t avail = (size_t)std::min<u64>(4, end - bytepos);
-      memcpy(h, sin->at(bytepos), avail);
-      return avail;
-    }
-    const size_t avail = (size_t)std::min<u64>(4, n - bytepos);
-    read_dev(h, bytepos, avail);
-    return avail;
-  };
-  while (!ch.done && (E.ev < 0 || dev)) {
-    // ---- 1. the input window ----
-    const u64 a = listed ? 0 : (ch.pos >> 3) & ~(u64)255;
-    wcur = a == prev_a ? wcur * 2 : W;
+  size_t wcur = R.W;
+  while (!ch.done && (R.E.ev < 0 || past_error)) {
+    const u64 a = (ch.pos >> 3) & ~(u64)255;
+    wcur = a == prev_a ? wcur * 2 : R.W;
     prev_a = a;
-    if (sin) {
-      sin->drop(a);
-      sin->fill(a + wcur + 1);
-      learn_end();
-    }
-    const u64 wl = listed ? n : std::min<u64>(wcur, (sin ? sin->base + sin->have : n) - a);
-    const bool last = a + wl == n;
-    if (wl + 32 > win_cap) { win.alloc(c, wl + 32); win_cap = wl + 32; }
-    // zero padded (aligned word reads past the end must be safe)
-    CUDA_CHECK(cudaMemsetAsync(win.p + (wl & ~(u64)3), 0, 32 + (wl & 3), c.stream));
-    if (sin) {
-      StageScope s(c, ST_H2D);
-      if (wl) CUDA_CHECK(cudaMemcpyAsync(win, sin->at(a), wl, cudaMemcpyHostToDevice, c.stream));
-    } else if (wl) {
-      CUDA_CHECK(cudaMemcpyAsync(win, d_in + a, wl, cudaMemcpyDeviceToDevice, c.stream));
-    }
-    cands.clear(); blk.clear();
-    if (listed) {
-      // only the given positions are tested; the first one without a magic raises "Not bzip data", so nothing behind it
-      // is decoded
-      StageScope ss(c, ST_SCAN);
-      const size_t np = positions->size();
-      DBuf<u64> dpos(c, np ? np : 1);
-      DBuf<Cand> dc(c, np ? np : 1);
-      cands.resize(np);
-      if (np) {
-        CUDA_CHECK(cudaMemcpyAsync(dpos, positions->data(), 8 * np, cudaMemcpyHostToDevice, c.stream));
-        k_magic_at<<<(unsigned)((np + 255) / 256), 256, 0, c.stream>>>(win, n, dpos, np, dc);
-        KLAUNCH(c); KCHECK();
-        CUDA_CHECK(cudaMemcpyAsync(cands.data(), dc, sizeof(Cand) * np, cudaMemcpyDeviceToHost, c.stream));
-      }
-      CUDA_CHECK(cudaStreamSynchronize(c.stream));
-      for (size_t i = 0; i < np; i++) if (cands[i].type == 0) { cands.resize(i + 1); break; }
-    } else {
-      // a magic whose 80 bits (magic + CRC) run past the window's end belongs to the next window
-      const u64 lim = last ? wl * 8 : (wl * 8 >= 80 ? wl * 8 - 79 : 0);
-      scan_window(c, win, wl, a * 8, lim, cands);
-    }
-    for (size_t i = 0; i < cands.size(); i++) if (cands[i].type == 1) blk.push_back(i);
-    const size_t nbm = std::min<size_t>(DB, blk.size());
-    if (nbm > slots) {
-      // per-batch state, kept for the largest batch of the call
-      rle.alloc(c, nbm << SEG_SHIFT); cls.alloc(c, nbm << SEG_SHIFT); tileoff.alloc(c, nbm * UR_TPS);
-      dres.alloc(c, nbm); dcand.alloc(c, nbm);
-      slots = nbm;
-    }
-    auto first_blk_from = [&](u64 pos) {
-      return (size_t)(std::lower_bound(blk.begin(), blk.end(), pos, [&](size_t ci, u64 p) { return cands[ci].pos < p; }) - blk.begin());
-    };
-    size_t kb = listed ? 0 : first_blk_from(ch.pos);
-    // ---- 2. batches ----
+    R.load(a, wcur);
+    // a magic whose 80 bits (magic + CRC) run past the window's end belongs to the next window
+    const u64 bits = R.wl * 8;
+    R.scan(R.last ? bits : (bits >= 80 ? bits - 79 : 0));
+    R.reserve();
+    R.kb = R.blk_from(ch.pos);
     for (;;) {
-      const u32 cnt = (u32)std::min<size_t>(DB, blk.size() - kb);
-      if (cnt) {
-        std::vector<Cand> bc(cnt);
-        for (u32 i = 0; i < cnt; i++) bc[i] = cands[blk[kb + i]];
-        CUDA_CHECK(cudaMemcpyAsync(dcand, bc.data(), sizeof(Cand) * cnt, cudaMemcpyHostToDevice, c.stream));
-        hres.resize(cnt);
-        dec_batch(c, B, win, wl, a * 8, last, dcand, cnt, dres, hres.data(), rle, cls, tileoff);
-      }
-      // ---- 3. walk ----
-      bool need_window = false;
+      R.batch();
       const size_t e0 = ch.events.size();
-      if (listed) {
-        list_walk(ch, cands, [&](size_t li, const CandRes** r, size_t* slot) {
-          const size_t j = (size_t)(std::lower_bound(blk.begin(), blk.end(), li) - blk.begin());
-          if (j >= kb + cnt) return false;
-          *r = &hres[j - kb]; *slot = j - kb;
-          return true;
-        });
-      } else {
-        chain_walk(ch, [&](u64 pos) -> At {
-          const auto it = std::lower_bound(cands.begin(), cands.end(), pos, [](const Cand& x, u64 p) { return x.pos < p; });
-          if (it == cands.end() || it->pos != pos) {
-            if (!last && pos + 80 > (a + wl) * 8) { need_window = true; return {-1, nullptr, nullptr, 0}; }
-            return {0, nullptr, nullptr, 0};
-          }
-          if (it->type == 2) return {2, &*it, nullptr, 0};
-          const size_t j = first_blk_from(pos);
-          if (j >= kb + cnt) return {-1, nullptr, nullptr, 0};  // in a later batch of this window
-          const CandRes& r = hres[j - kb];
-          if (r.open) { need_window = true; return {-1, nullptr, nullptr, 0}; }
-          return {1, &*it, &r, j - kb};
-        }, head);
-      }
-      const size_t e1 = ch.events.size();
-      // ---- 4. expand and deliver the blocks this walk settled ----
-      settled.clear();
-      for (size_t ei = e0; ei < e1; ei++) if (ch.events[ei].kind == 0) settled.push_back(ei);
-      got.assign(cnt ? cnt : 1, 0);
-      ob.assign(cnt ? cnt : 1, ~0ull);
-      auto got_fn = [&](size_t slot) { return std::make_pair(ob[slot] != ~0ull, got[slot]); };
-      size_t er = e0;  // events replayed so far (a host output replays group by group)
-      if (dev) {
-        // straight to the caller's buffer; a block that does not fit is only counted (the needed size is returned)
-        for (size_t ei : settled) { const Event& ev = ch.events[ei]; if (ev.off + ev.len <= out_cap) ob[ev.slot] = ev.off; }
-        if (!settled.empty()) dec_expand(c, rle, cls, false, dres, hres.data(), tileoff, cnt, ob.data(), d_out, got.data());
-      } else {
-        // through the staging buffer, groups of consecutive blocks of at most max(W, one block) bytes
-        for (size_t g0 = 0; g0 < settled.size();) {
-          const Event& f = ch.events[settled[g0]];
-          u64 bytes = f.len;
-          size_t g1 = g0 + 1;
-          while (g1 < settled.size() && bytes + ch.events[settled[g1]].len <= W) bytes += ch.events[settled[g1++]].len;
-          const size_t s0 = f.slot, s1 = ch.events[settled[g1 - 1]].slot + 1;
-          for (size_t g = g0; g < g1; g++) { const Event& ev = ch.events[settled[g]]; ob[ev.slot] = ev.off - f.off; }
-          if (bytes > stage_cap) { stage.alloc(c, bytes); stage_cap = bytes; }
-          dec_expand(c, rle.p + (s0 << SEG_SHIFT), cls.p + (s0 << SEG_SHIFT), false, dres.p + s0, hres.data() + s0, tileoff.p + s0 * UR_TPS,
-                     (u32)(s1 - s0), ob.data() + s0, stage, got.data() + s0);
-          if (sout) {
-            // the group's events say how much of it the reference writes before it throws
-            const size_t g_end = settled[g1 - 1] + 1;
-            replay(ch, er, g_end, got_fn, tab_pos, tab_len, ends, E);
-            er = g_end;
-            const u64 keep = E.ev < 0 ? bytes : (E.prefix > f.off ? std::min<u64>(bytes, E.prefix - f.off) : 0);
-            if (keep) {
-              // no group follows the last one of a finished chain or a failure: a call of one batch makes one result
-              // buffer of exactly its size and one copy
-              sout->reserve((size_t)keep, (ch.done && g1 == settled.size()) || E.ev >= 0, W);
-              u8* dst = sout->next();
-              {
-                StageScope s(c, ST_D2H);
-                CUDA_CHECK(cudaMemcpyAsync(dst, stage, keep, cudaMemcpyDeviceToHost, c.stream));
-              }
-              sout->put(dst, (size_t)keep);
-            }
-            if (E.ev >= 0) break;
-          }
-          g0 = g1;
-        }
-      }
-      // ---- replay: the first failure in stream order ends the call (the device path walks on for the needed size) ----
-      if (E.ev < 0) replay(ch, er, e1, got_fn, tab_pos, tab_len, ends, E);
-      if (ch.done || (E.ev >= 0 && !dev) || need_window) break;
-      const size_t nk = listed ? kb + cnt : first_blk_from(ch.pos);
-      if (nk <= kb) throw B2Error{B2_ERR_CUDA, "bzip2 decode: the chain walk made no progress"};
-      kb = nk;
+      const bool need_window = chain_walk(R, R.last ? ~0ull : (R.a + R.wl) * 8);
+      deliver(e0, ch.events.size());
+      if (ch.done || (R.E.ev >= 0 && !past_error) || need_window) break;
+      const size_t nk = R.blk_from(ch.pos);
+      if (nk <= R.kb) throw B2Error{B2_ERR_CUDA, "bzip2 decode: the chain walk made no progress"};
+      R.kb = nk;
     }
   }
-  CUDA_CHECK(cudaStreamSynchronize(c.stream));
-  if (dev && ch.total_out > out_cap) {
-    *out_n = (size_t)ch.total_out;
+  CUDA_CHECK(cudaStreamSynchronize(R.c.stream));
+}
+
+void bzip2_decompress_dev(Ctx& c, const u8* d_in, size_t n, int multistream, u8* d_out, size_t out_cap, size_t* out_n) {
+  *out_n = 0;
+  Decode R(c, DecIn(d_in, n));
+  chain_decode(R, multistream, true, [&](size_t e0, size_t e1) {
+    // a walk that settled no block expands nothing
+    const auto& ev = R.ch.events;
+    const bool any = std::any_of(ev.begin() + (long)e0, ev.begin() + (long)e1, [](const Event& x) { return x.kind == 0; });
+    deliver_dev(R, e0, e1, 0, any ? R.cnt : 0, 0, d_out, out_cap);
+  });
+  if (R.ch.total_out > out_cap) {
+    *out_n = (size_t)R.ch.total_out;
     throw B2Error{B2_ERR_BAD_ARG, "output buffer too small"};
   }
-  if (E.ev >= 0) {
-    // the host path hands the output in front of the error to the caller with the error (b2_bzip2_decompress_partial)
-    if (sout) *out_n = (size_t)E.prefix;
-    throw B2Error{E.code, E.msg};
+  R.finish(out_n, 0);
+}
+
+void bzip2_decompress_size(Ctx& c, const u8* d_in, size_t n, int multistream, size_t* out_n) {
+  *out_n = 0;
+  Decode R(c, DecIn(d_in, n));
+  chain_decode(R, multistream, false, [&](size_t e0, size_t e1) { deliver_crc(R, e0, e1, false); });
+  R.finish(out_n, 0);
+}
+
+void bzip2_decompress_host(Ctx& c, StreamIn& in, int multistream, StreamOut& out, size_t* out_n) {
+  *out_n = 0;
+  Decode R(c, DecIn(in));
+  chain_decode(R, multistream, false, [&](size_t e0, size_t e1) { deliver_host(R, e0, e1, out); });
+  R.finish(out_n, R.E.prefix);
+}
+
+void bzip2_table(Ctx& c, StreamIn& in, int multistream, DecRows& rows, size_t* out_n) {
+  *out_n = 0;
+  Decode R(c, DecIn(in));
+  chain_decode(R, multistream, false, [&](size_t e0, size_t e1) { deliver_crc(R, e0, e1, true); });
+  rows = std::move(R.rows);
+  R.finish(out_n, 0);
+}
+
+// A position list: the whole input on the device, only the given positions tested for a magic, the blocks decoded a
+// batch at a time in list order.  The first position without a magic raises "Not bzip data", so nothing behind it is
+// decoded.
+void bzip2_decompress_list(Ctx& c, StreamIn& in, const std::vector<u64>& positions, StreamOut& out, DecRows& rows, size_t* out_n) {
+  *out_n = 0;
+  Decode R(c, DecIn(in));
+  const size_t n = R.in.length();  // the input is complete
+  R.load(0, n);
+  {
+    StageScope ss(c, ST_SCAN);
+    const size_t np = positions.size();
+    DBuf<u64> dpos(c, np);
+    DBuf<Cand> dc(c, np);
+    R.cands.resize(np);
+    CUDA_CHECK(cudaMemcpyAsync(dpos, positions.data(), 8 * np, cudaMemcpyHostToDevice, c.stream));
+    k_magic_at<<<(unsigned)((np + 255) / 256), 256, 0, c.stream>>>(R.win, n, dpos, np, dc);
+    KLAUNCH(c); KCHECK();
+    CUDA_CHECK(cudaMemcpyAsync(R.cands.data(), dc, sizeof(Cand) * np, cudaMemcpyDeviceToHost, c.stream));
+    CUDA_CHECK(cudaStreamSynchronize(c.stream));
   }
-  *out_n = (size_t)ch.total_out;
-  return 0;
+  for (size_t i = 0; i < R.cands.size(); i++) {
+    if (R.cands[i].type == 0) { R.cands.resize(i + 1); break; }
+    if (R.cands[i].type == 1) R.blk.push_back(i);
+  }
+  R.reserve();
+  for (;;) {
+    R.batch();
+    const size_t e0 = R.ch.events.size();
+    list_walk(R);
+    deliver_host(R, e0, R.ch.events.size(), out);
+    if (R.ch.done || R.E.ev >= 0) break;
+    if (!R.cnt) throw B2Error{B2_ERR_CUDA, "bzip2 decode: the chain walk made no progress"};
+    R.kb += R.cnt;
+  }
+  CUDA_CHECK(cudaStreamSynchronize(c.stream));
+  rows = std::move(R.rows);
+  R.finish(out_n, R.E.prefix);
 }
 
 // ---- sharded decode (SURVEY.md section 8e): open on every rank, exchange results, finish ------------
-// open() parses the header, finds every block candidate of the whole file and decodes the share [lo, hi) of them;
-// finish() walks the chain over ALL candidates' results (imported from the other ranks), expands + CRC-checks the blocks
-// of the own share and raises the reference's errors in stream order.  A rank keeps its share's results until the
-// all-gather, so its device memory grows with its share of the file.
+// The open session decodes the share [lo, hi) of the whole input's block candidates (one window: the whole input, zero
+// padded); finish walks the chain over ALL candidates' results (imported from the other ranks), expands + CRC-checks
+// the blocks of the own share and raises the reference's errors in stream order.  A rank keeps its share's results
+// until the all-gather, so its device memory grows with its share of the file.
 struct DecSession {
-  size_t n = 0;
-  u32 dbuf_size = 0;
-  DBuf<u8> din;                    // the whole file, zero padded
-  std::vector<Cand> cands;         // every magic found, sorted by position
-  std::vector<size_t> blk_idx;     // block candidates (index into cands)
-  std::vector<CandRes> hres;       // per block candidate (valid for [lo,hi) after open, for all after import)
-  size_t lo = 0, hi = 0;           // own share of the block candidates
-  DBuf<Cand> dcand;
-  DBuf<CandRes> dres;              // own share only
-  DBuf<u8> rle, cls;               // cls (count-byte classes) is kept for the whole share only while that is cheap (keep_cls)
-  bool keep_cls = true;
-  DBuf<u32> tileoff;
+  Decode R;  // hres: one entry per block candidate (the own share's after open, all after the import)
+  size_t lo = 0, hi = 0;
+
+  DecSession(Ctx& c, const u8* d_in, size_t n, int rank, int world) : R(c, DecIn(d_in, n)) {
+    R.load(0, n);
+    R.in = DecIn(R.win.p, n);  // later headers are read from the session's copy: the caller's buffer may be gone by then
+    R.scan(n * 8);
+    const size_t nb_all = R.blk.size();
+    R.hres.assign(nb_all, CandRes());
+    for (auto& r : R.hres) { memset(&r, 0, sizeof r); r.status = DEC_DATA_ERROR; }
+    lo = (size_t)rank * nb_all / (size_t)world;
+    hi = (size_t)(rank + 1) * nb_all / (size_t)world;
+    const size_t nb = hi - lo;
+    {
+      // every block of the own share keeps 2 MiB (L column + count-byte classes; 1 MiB beyond DEC_KEEP_CLS blocks) until
+      // the stream is assembled, and a batch of up to 2048 blocks needs ~20 MiB of scratch per block: say so instead of
+      // failing inside an allocation
+      const size_t need = nb * ((size_t)(nb <= dec_keep_cls_limit() ? 2 : 1) << 20) + std::min<size_t>(nb, R.DB) * ((size_t)20 << 20) + n;
+      // memory the stream-ordered pool holds but does not use is available too: when that covers the call (every call
+      // after the first of a kind) the driver is not asked at all -- cudaMemGetInfo takes milliseconds on a busy context
+      uint64_t reserved = 0, used = 0;
+      cudaMemPool_t pool;
+      if (cudaDeviceGetDefaultMemPool(&pool, c.device) == cudaSuccess) {
+        cudaMemPoolGetAttribute(pool, cudaMemPoolAttrReservedMemCurrent, &reserved);
+        cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemCurrent, &used);
+      }
+      cudaGetLastError();
+      const size_t spare = (size_t)(reserved > used ? reserved - used : 0);
+      size_t free_b = 0, total_b = 0;
+      if (need > spare) {
+        if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess) {
+          if (need > free_b + spare) {
+            char msg[256];
+            snprintf(msg, sizeof msg, "stream of %zu blocks needs about %zu MiB of device memory for one sharded call (%zu MiB free): decode it "
+                                      "on more GPUs, or on one (decompressFile), whose device memory does not grow with the file", nb, need >> 20, free_b >> 20);
+            throw B2Error{B2_ERR_CUDA, msg};
+          }
+        } else cudaGetLastError();
+      }
+    }
+    // The count-byte classes of a block are needed twice (length scan here, expansion in finish).  Up to DEC_KEEP_CLS
+    // blocks they stay on the device in between; a share of more blocks (tens of GB of level-1 data) keeps only the L
+    // columns (1 MiB per block) and classifies a second time, batch by batch, when it expands them.
+    R.keep_cls = nb <= dec_keep_cls_limit();
+    R.alloc(nb ? nb : 1, R.keep_cls ? (nb ? nb : 1) : std::min<size_t>(nb, R.DB));
+    R.dcand.alloc(c, std::max<size_t>(std::min<size_t>(nb, R.DB), 1));
+    for (size_t k0 = 0; k0 < nb; k0 += R.DB) R.decode(lo + k0, (u32)std::min<size_t>(R.DB, nb - k0), k0, R.hres.data() + lo + k0);
+    CUDA_CHECK(cudaStreamSynchronize(c.stream));
+    R.B = DecScratch();  // the batch scratch is not kept until finish
+  }
+
+  // Walks the chain over every rank's results, expands the own blocks into d_out (or a buffer of its own), and fills
+  // info.  Throws the first failure in stream order; info[3] tells the ranks which failure is the earliest.
+  void finish(int multistream, u8* d_out, size_t out_cap, u64* info) {
+    Chain& ch = R.ch;
+    ch.multistream = multistream;
+    R.kb = 0;  // the batch the walk sees: every block candidate
+    R.cnt = (u32)R.hres.size();
+    chain_walk(R, ~0ull);
+    // own output window: [my_off, my_off + my_len) of the decoded stream, from the first to the last own block
+    auto mine = [&](const Event& ev) { return ev.kind == 0 && ev.slot >= lo && ev.slot < hi; };
+    const auto f = std::find_if(ch.events.begin(), ch.events.end(), mine);
+    const auto l = std::find_if(ch.events.rbegin(), ch.events.rend(), mine);
+    const u64 my_off = f == ch.events.end() ? 0 : f->off, my_len = f == ch.events.end() ? 0 : l->off + l->len - my_off;
+    DBuf<u8> own;
+    if (!d_out) {
+      own.alloc(R.c, my_len ? my_len : 1);
+      d_out = own.p;
+      out_cap = my_len;
+    } else if (my_len > out_cap) {
+      throw B2Error{B2_ERR_BAD_ARG, "output buffer too small"};
+    }
+    deliver_dev(R, 0, ch.events.size(), lo, hi - lo, my_off, d_out, out_cap);
+    info[0] = my_off; info[1] = my_len; info[2] = ch.total_out; info[3] = (u64)(long long)R.E.ev; info[4] = (u64)(long long)R.E.code;
+    // the caller compares info[3] across ranks and keeps the earliest
+    if (R.E.ev >= 0) throw B2Error{R.E.code, R.E.msg};
+  }
 };
 
-static void dec_open(Ctx& c, DecSession& S, const u8* d_in_user, size_t n, int rank, int world) {
-  S.n = n;
-  // padded private copy of the input (aligned word reads past the end must be safe)
-  S.din.alloc(c, n + 32);
-  CUDA_CHECK(cudaMemsetAsync(S.din.p + (n & ~(size_t)3), 0, (n + 32) - (n & ~(size_t)3), c.stream));
-  if (n) CUDA_CHECK(cudaMemcpyAsync(S.din, d_in_user, n, cudaMemcpyDeviceToDevice, c.stream));
-  u8 hdr[4] = {0, 0, 0, 0};
-  if (n >= 4) CUDA_CHECK(cudaMemcpyAsync(hdr, S.din, 4, cudaMemcpyDeviceToHost, c.stream));
-  CUDA_CHECK(cudaStreamSynchronize(c.stream));
-  read_level(hdr, n, &S.dbuf_size);
-  scan_window(c, S.din, n, 0, n * 8, S.cands);
-  for (size_t i = 0; i < S.cands.size(); i++) if (S.cands[i].type == 1) S.blk_idx.push_back(i);
-  const size_t nb_all = S.blk_idx.size();
-  std::vector<Cand> bc(nb_all);
-  for (size_t i = 0; i < nb_all; i++) bc[i] = S.cands[S.blk_idx[i]];
-  S.hres.assign(nb_all, CandRes());
-  for (auto& r : S.hres) { memset(&r, 0, sizeof r); r.status = DEC_DATA_ERROR; }
-  S.lo = (size_t)rank * nb_all / (size_t)world;
-  S.hi = (size_t)(rank + 1) * nb_all / (size_t)world;
-  const size_t nb = S.hi - S.lo;
-  const u32 DB = dec_batch_blocks(c);
-  {
-    // every block of the own share keeps 2 MiB (L column + count-byte classes; 1 MiB beyond DEC_KEEP_CLS blocks) until the
-    // stream is assembled, and a batch of up to 2048 blocks needs ~20 MiB of scratch per block: say so instead of failing
-    // inside an allocation
-    const size_t need = nb * ((size_t)(nb <= dec_keep_cls_limit() ? 2 : 1) << 20) + std::min<size_t>(nb, DB) * ((size_t)20 << 20) + n;
-    // memory the stream-ordered pool holds but does not use is available too: when that covers the call (every call
-    // after the first of a kind) the driver is not asked at all -- cudaMemGetInfo takes milliseconds on a busy context
-    uint64_t reserved = 0, used = 0;
-    cudaMemPool_t pool;
-    if (cudaDeviceGetDefaultMemPool(&pool, c.device) == cudaSuccess) {
-      cudaMemPoolGetAttribute(pool, cudaMemPoolAttrReservedMemCurrent, &reserved);
-      cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemCurrent, &used);
-    }
-    cudaGetLastError();
-    const size_t spare = (size_t)(reserved > used ? reserved - used : 0);
-    size_t free_b = 0, total_b = 0;
-    if (need > spare) {
-      if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess) {
-        if (need > free_b + spare) {
-          char msg[256];
-          snprintf(msg, sizeof msg, "stream of %zu blocks needs about %zu MiB of device memory for one sharded call (%zu MiB free): decode it "
-                                    "on more GPUs, or on one (decompressFile), whose device memory does not grow with the file", nb, need >> 20, free_b >> 20);
-          throw B2Error{B2_ERR_CUDA, msg};
-        }
-      } else cudaGetLastError();
-    }
-  }
-  S.dcand.alloc(c, nb_all ? nb_all : 1);
-  S.dres.alloc(c, nb ? nb : 1);
-  S.rle.alloc(c, (nb ? nb : 1) << SEG_SHIFT);
-  // The count-byte classes of a block are needed twice (length scan here, expansion in dec_finish).  Up to DEC_KEEP_CLS
-  // blocks they stay on the device in between; a share of more blocks (tens of GB of level-1 data) keeps only the L
-  // columns (1 MiB per block) and classifies a second time, batch by batch, when it expands them.
-  S.keep_cls = nb <= dec_keep_cls_limit();
-  S.cls.alloc(c, (size_t)(S.keep_cls ? (nb ? nb : 1) : std::min<size_t>(nb, DB)) << SEG_SHIFT);
-  S.tileoff.alloc(c, (nb ? nb : 1) * (size_t)UR_TPS);
-  if (nb_all) CUDA_CHECK(cudaMemcpyAsync(S.dcand, bc.data(), sizeof(Cand) * nb_all, cudaMemcpyHostToDevice, c.stream));
-  DecScratch B;
-  for (size_t k0 = 0; k0 < nb; k0 += DB) {
-    const u32 cnt = (u32)std::min<size_t>(DB, nb - k0);
-    dec_batch(c, B, S.din, n, 0, true, S.dcand.p + S.lo + k0, cnt, S.dres.p + k0, S.hres.data() + S.lo + k0, S.rle.p + (k0 << SEG_SHIFT),
-              S.cls.p + (S.keep_cls ? (k0 << SEG_SHIFT) : 0), S.tileoff.p + k0 * UR_TPS);
-  }
-  CUDA_CHECK(cudaStreamSynchronize(c.stream));
-}
-
-// Walks the chain over every rank's results, expands the own blocks into d_out, and fills shard_info.  Throws the first
-// failure in stream order; shard_info[3] tells the ranks which failure is the earliest.
-static int dec_finish(Ctx& c, DecSession& S, int multistream, u8* d_out, size_t out_cap, u64* shard_info) {
-  const std::vector<Cand>& cands = S.cands;
-  Chain ch;
-  ch.n = S.n; ch.multistream = multistream; ch.cur_dbuf = S.dbuf_size;
-  std::vector<long> cand_to_blk(cands.size(), -1);
-  for (size_t i = 0; i < S.blk_idx.size(); i++) cand_to_blk[S.blk_idx[i]] = (long)i;
-  chain_walk(ch, [&](u64 pos) -> At {
-    const auto it = std::lower_bound(cands.begin(), cands.end(), pos, [](const Cand& x, u64 p) { return x.pos < p; });
-    if (it == cands.end() || it->pos != pos) return {0, nullptr, nullptr, 0};
-    if (it->type == 2) return {2, &*it, nullptr, 0};
-    const size_t bi = (size_t)cand_to_blk[it - cands.begin()];
-    return {1, &*it, &S.hres[bi], bi};
-  }, [&](u64 bytepos, u8* h) -> size_t {
-    const size_t avail = (size_t)std::min<u64>(4, S.n - bytepos);
-    CUDA_CHECK(cudaMemcpyAsync(h, S.din.p + bytepos, avail, cudaMemcpyDeviceToHost, c.stream));
-    CUDA_CHECK(cudaStreamSynchronize(c.stream));
-    return avail;
-  });
-  // own output window: [my_off, my_off + my_len) of the decoded stream
-  const size_t nb = S.hi - S.lo;
-  std::vector<u64> ob(nb ? nb : 1, ~0ull);
-  u64 my_off = 0, my_len = 0;
-  bool first = true;
-  for (const Event& ev : ch.events)
-    if (ev.kind == 0 && ev.slot >= S.lo && ev.slot < S.hi) {
-      if (first) { my_off = ev.off; first = false; }
-      ob[ev.slot - S.lo] = ev.off - my_off;
-      my_len = ev.off + ev.len - my_off;
-    }
-  u8* dout = d_out;
-  DBuf<u8> own;
-  if (!d_out) {
-    own.alloc(c, my_len ? my_len : 1);
-    dout = own.p;
-  } else if (my_len > out_cap) {
-    throw B2Error{B2_ERR_BAD_ARG, "output buffer too small"};
-  }
-  std::vector<u32> got(nb ? nb : 1, 0);
-  if (S.keep_cls) {
-    dec_expand(c, S.rle, S.cls, false, S.dres, S.hres.data() + S.lo, S.tileoff, (u32)nb, ob.data(), dout, got.data());
-  } else {
-    const size_t DBc = dec_batch_blocks(c);
-    for (size_t k0 = 0; k0 < nb; k0 += DBc) {
-      const u32 cnt = (u32)std::min<size_t>(DBc, nb - k0);
-      dec_expand(c, S.rle.p + (k0 << SEG_SHIFT), S.cls, true, S.dres.p + k0, S.hres.data() + S.lo + k0, S.tileoff.p + k0 * UR_TPS, cnt,
-                 ob.data() + k0, dout, got.data() + k0);
-    }
-  }
-  DecErr E;
-  replay(ch, 0, ch.events.size(), [&](size_t slot) {
-    // CRCs of foreign blocks are checked by their owners
-    return slot >= S.lo && slot < S.hi ? std::make_pair(true, got[slot - S.lo]) : std::make_pair(false, 0u);
-  }, nullptr, nullptr, nullptr, E);
-  shard_info[0] = my_off; shard_info[1] = my_len; shard_info[2] = ch.total_out; shard_info[3] = (u64)(long long)E.ev; shard_info[4] = (u64)(long long)E.code;
-  // the caller compares shard_info[3] across ranks and keeps the earliest
-  if (E.ev >= 0) throw B2Error{E.code, E.msg};
-  return 0;
-}
-
-static DecSession* g_shard = nullptr;
-// frees an open sharded decode (b2_shutdown, while the context its buffers belong to is alive)
-void dec_shard_release() { delete g_shard; g_shard = nullptr; }
+static std::unique_ptr<DecSession> g_shard;
+void dec_shard_release() { g_shard.reset(); }
 void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* info) {
-  delete g_shard;
-  g_shard = new DecSession();
-  dec_open(c, *g_shard, d_in, n, rank, world);
-  info[0] = g_shard->blk_idx.size(); info[1] = g_shard->lo; info[2] = g_shard->hi;
+  g_shard.reset();
+  g_shard = std::make_unique<DecSession>(c, d_in, n, rank, world);
+  info[0] = g_shard->R.blk.size(); info[1] = g_shard->lo; info[2] = g_shard->hi;
 }
 void dec_shard_export(u64* buf) {
   if (!g_shard) throw B2Error{B2_ERR_BAD_ARG, "no sharded decode in flight"};
   for (size_t i = g_shard->lo; i < g_shard->hi; i++) {
-    const CandRes& r = g_shard->hres[i];
+    const CandRes& r = g_shard->R.hres[i];
     u64* o = buf + (i - g_shard->lo) * 6;
     o[0] = (u64)(long long)r.status; o[1] = r.detail; o[2] = r.endbit; o[3] = r.n; o[4] = r.rawlen; o[5] = r.orig;
   }
 }
-int dec_shard_finish(Ctx& c, const u64* all, int multistream, u8* d_out, size_t out_cap, u64* res) {
+void dec_shard_finish(const u64* all, int multistream, u8* d_out, size_t out_cap, u64* res) {
   if (!g_shard) throw B2Error{B2_ERR_BAD_ARG, "no sharded decode in flight"};
-  DecSession& S = *g_shard;
-  for (size_t i = 0; i < S.hres.size(); i++) {
-    if (i >= S.lo && i < S.hi) continue;
+  const std::unique_ptr<DecSession> S = std::move(g_shard);  // the session ends with this call
+  for (size_t i = 0; i < S->R.hres.size(); i++) {
+    if (i >= S->lo && i < S->hi) continue;
     const u64* o = all + i * 6;
-    CandRes& r = S.hres[i];
+    CandRes& r = S->R.hres[i];
     r.status = (int)(long long)o[0]; r.detail = (u32)o[1]; r.endbit = o[2]; r.n = (u32)o[3]; r.rawlen = (u32)o[4]; r.orig = (u32)o[5];
   }
-  struct Closer { ~Closer() { delete g_shard; g_shard = nullptr; } } closer;
-  return dec_finish(c, S, multistream, d_out, out_cap, res);
+  S->finish(multistream, d_out, out_cap, res);
 }

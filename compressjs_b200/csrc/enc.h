@@ -162,9 +162,30 @@ void bwtc_compress(Ctx& c, StreamIn& in, int level, u64 file_size, StreamOut& ou
 // the failing check have gone out when the error is thrown
 void bwtc_decompress(Ctx& c, StreamIn& in, StreamOut& out);
 
-// ---- bzip2 decode driver (decode.cu): every single-GPU decode entry point ----
-// The input is `sin` or the device buffer d_in[0, n); the output goes to the device buffer d_out (out_cap bytes), to
-// `sout`, or nowhere (a table).  See decode.cu.
-int bzip2_decompress(Ctx& c, StreamIn* sin, const u8* d_in, size_t n, int multistream, u8* d_out, size_t out_cap, StreamOut* sout,
-                     size_t* out_n, const std::vector<u64>* positions, std::vector<u64>* ends, std::vector<u64>* tab_pos,
-                     std::vector<u32>* tab_len);
+// ---- bzip2 decode drivers (decode.cu), one per kind of decode ----
+// Each throws the reference's first error in stream order.  *out_n: the decoded size, or what the call says on an error.
+// b2_bzip2_decompress_dev: d_in[0, n) into d_out, each block at its offset in the decoded stream.  A block that does not
+// fit is only counted and the walk goes on past a data error, so a buffer too small throws with *out_n = the size needed.
+void bzip2_decompress_dev(Ctx& c, const u8* d_in, size_t n, int multistream, u8* d_out, size_t out_cap, size_t* out_n);
+// b2_bzip2_decompress_dev without an output buffer: the blocks are expanded only for their CRCs.
+void bzip2_decompress_size(Ctx& c, const u8* d_in, size_t n, int multistream, size_t* out_n);
+// b2_bzip2_decompress_partial and b2_bzip2_decompress_stream: into `out`, which never receives a byte past the prefix the
+// reference writes before an error (*out_n on an error).
+void bzip2_decompress_host(Ctx& c, StreamIn& in, int multistream, StreamOut& out, size_t* out_n);
+// What the replay of a table or a position list records in front of the first failure: per block its bit position and
+// decoded length (the table rows), and per position the end of its bytes in the output (the list ends).
+struct DecRows { std::vector<u64> pos, ends; std::vector<u32> len; };
+// b2_bzip2_table_partial: the rows of the blocks in front of the first failure (stream CRCs are not checked).
+void bzip2_table(Ctx& c, StreamIn& in, int multistream, DecRows& rows, size_t* out_n);
+// b2_bzip2_decompress_blocks: the blocks at a non-empty list of bit positions, back to back in list order, from a complete
+// input; rows.ends, and *out_n on an error, as bzip2_decompress_host's.
+void bzip2_decompress_list(Ctx& c, StreamIn& in, const std::vector<u64>& positions, StreamOut& out, DecRows& rows, size_t* out_n);
+// The sharded decode (b2_dec_shard_open / _export / _finish): one session at a time, ended by finish or released by
+// b2_shutdown.
+void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* info);
+void dec_shard_export(u64* buf);
+void dec_shard_finish(const u64* all, int multistream, u8* d_out, size_t out_cap, u64* res);
+void dec_shard_release();
+// BWT.unbwtransform of nb blocks at once (BWTC decode, b2_bwt_inverse): block b is the L column in slot b of d_L, h_n[b]
+// bytes (1 <= n <= 2^20 - 2) with primary index h_pidx[b] (0 <= pidx <= n); the blocks go to d_out back to back.
+void bwt_inverse_sentinel_batch(Ctx& c, const u8* d_L, const u32* h_n, const u32* h_pidx, u32 nb, u8* d_out);
