@@ -18,7 +18,7 @@ EXPORTS = [
     "b2_init", "b2_shutdown", "b2_last_error", "b2_free",
     "b2_bzip2_compress", "b2_bzip2_decompress", "b2_bzip2_decompress_block", "b2_bzip2_table",
     "b2_bzip2_decompress_partial", "b2_bzip2_decompress_block_partial", "b2_bzip2_table_partial", "b2_bzip2_decompress_blocks",
-    "b2_bzip2_compress_stream", "b2_bzip2_decompress_stream",
+    "b2_bzip2_compress_stream", "b2_bzip2_decompress_stream", "b2_bzip2_recover", "b2_bzip2_recover_stream",
     "b2_bzip2_compress_flavor", "b2_bzip2_compress_stream_flavor", "b2_bzip2_compress_dev_flavor",
     "b2_bwt_cyclic", "b2_bwt_cyclic_batch", "b2_suffixsort", "b2_bwt_sentinel", "b2_bwt_inverse", "b2_bwtc_compress", "b2_bwtc_compress_unsized", "b2_bwtc_decompress", "b2_crc32_bzip2",
     "b2_bwtc_compress_stream", "b2_bwtc_decompress_stream",
@@ -44,6 +44,12 @@ class Stats(C.Structure):
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+class RecoveredBlock(C.Structure):
+    """b2_recovered_block: one row of b2_bzip2_recover."""
+    _fields_ = [("bitpos", C.c_uint64), ("endbit", C.c_uint64), ("out_off", C.c_uint64), ("size", C.c_uint32),
+                ("crc", C.c_uint32), ("got", C.c_uint32), ("status", C.c_int32)]
 
 
 class BlockTrace(C.Structure):
@@ -79,6 +85,9 @@ def lib():
                                              C.POINTER(C.POINTER(C.c_uint64)), szp]
     L.b2_bzip2_compress_stream.argtypes = [READ_FN, WRITE_FN, C.c_void_p, C.c_int]
     L.b2_bzip2_decompress_stream.argtypes = [READ_FN, WRITE_FN, C.c_void_p, C.c_int]
+    recp = C.POINTER(C.POINTER(RecoveredBlock))
+    L.b2_bzip2_recover.argtypes = [C.c_void_p, C.c_size_t, C.c_int, u8pp, szp, recp, szp]
+    L.b2_bzip2_recover_stream.argtypes = [READ_FN, WRITE_FN, C.c_void_p, C.c_int, recp, szp]
     L.b2_bwt_cyclic.restype = C.c_int32
     L.b2_bwt_cyclic.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
     L.b2_bwt_cyclic_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]

@@ -1,6 +1,7 @@
 """compressjs.Bzip2 on the GPU: same four entry points as lib/Bzip2.js:879-933, and decompressBlocks (decompressBlock at
 many positions in one pass)."""
 import ctypes as C
+from collections import namedtuple
 
 import numpy as np
 
@@ -94,6 +95,18 @@ def _block(input, pos):
         data.ctypes.data if data.size else None, data.size, int(pos), out, n))
 
 
+# Bzip2.recover's rows (include/b2bz.h b2_recovered_block), with the status as a string
+RecoveredBlock = namedtuple("RecoveredBlock", "bitpos endbit out_off size crc got status")
+REC_STATUS = ("INTACT", "BAD_CRC", "DATA_ERROR", "OBSOLETE", "INSIDE")
+
+
+def _rows(L, rows, count):
+    out = [RecoveredBlock(r.bitpos, r.endbit, r.out_off, r.size, r.crc, r.got, REC_STATUS[r.status])
+           for r in (rows[i] for i in range(count.value))]
+    L.b2_free(rows)
+    return out
+
+
 def _deliver(output, data, err):
     """On a decode error `output` gets the bytes decoded before it first, then the error is raised."""
     if err is not None:
@@ -174,6 +187,32 @@ class Bzip2:
         if output is not None:
             return output
         return [buf[s:e].tobytes() for s, e in zip([0] + stops[:-1], stops)]
+
+    @staticmethod
+    def recover(input, output=None, *, repair=False):
+        """GPU extension: recover the intact blocks of a damaged bzip2 file.  Every block magic of the input is a
+        candidate, decoded as decompressBlock decodes a block of a BZh9 file and walked in position order
+        (include/b2bz.h b2_bzip2_recover gives the rules).  Returns (output, blocks): output receives the intact blocks'
+        decoded bytes, or with `repair` one bzip2 stream made of their bits, and blocks has one RecoveredBlock per
+        candidate, whose status is "INTACT", "BAD_CRC", "DATA_ERROR", "OBSOLETE" or "INSIDE" (it starts inside an intact
+        block).  Damage is a result, not an error.  When input has readByte and output has writeByte, the input is read
+        and the output written as the recovery goes, in bounded memory."""
+        L = _native.lib()
+        mode = 1 if repair else 0
+        rows, count = C.POINTER(_native.RecoveredBlock)(), C.c_size_t()
+        if is_stream_pair(input, output):
+            pump = Pump(input, output)
+            rc = L.b2_bzip2_recover_stream(pump.read_fn, pump.write_fn, None, mode, C.byref(rows), C.byref(count))
+            pump.check(rc, _error)
+            return output, _rows(L, rows, count)
+        data = coerce_input(input)
+        out, n = C.POINTER(C.c_uint8)(), C.c_size_t()
+        rc = L.b2_bzip2_recover(data.ctypes.data if data.size else None, data.size, mode, C.byref(out), C.byref(n),
+                                C.byref(rows), C.byref(count))
+        if rc:
+            _raise(rc)
+        blocks = _rows(L, rows, count)
+        return deliver_output(output, _take(L, out, n)), blocks
 
     @staticmethod
     def table(input, callback, multistream=False):

@@ -18,6 +18,10 @@ time and the output written as the library produces it (InStream / OutStream, th
 bin/compressjs:60-120), so memory does not grow with the stream (include/b2bz.h gives the bounds).  -b (the reference
 seeks in its input) reads the whole input first.
 
+``-d -t bzip2 --recover`` writes the decoded bytes of every intact block of a damaged file, and ``-d -t bzip2 --repair``
+one bzip2 stream made of those blocks (Bzip2.recover).  Both are pipe filters; stderr gets one line per lost block and
+a count, and the exit status is 1 when a block was lost.  The output is complete either way.
+
 Usage errors are found before the GPU library is loaded, so they work on a machine without a GPU.
 """
 import math
@@ -40,6 +44,8 @@ HELP = """
     -b, --block <n>   Extract a single block, starting at <n> bits.
     -t <compressor>   Select compressor type (bzip2 or bwtc)
     --libbz2          With -z -t bzip2: write the bytes bzip2 (libbz2) writes
+    --recover         With -d -t bzip2: write the bytes of every intact block of a damaged file
+    --repair          With -d -t bzip2: write one bzip2 stream of every intact block of a damaged file
     -1                Fastest/largest compression
     -2
     -3
@@ -77,7 +83,8 @@ def _number(s):
 
 def parse(argv):
     """Returns a dict of the options, or raises UsageError.  --help and --version are returned as 'help'/'version'."""
-    opts = {"decompress": False, "compress": False, "block": "-1", "T": None, "levels": set(), "args": [], "libbz2": False}
+    opts = {"decompress": False, "compress": False, "block": "-1", "T": None, "levels": set(), "args": [], "libbz2": False,
+            "recover": False, "repair": False}
     i = 0
     only_args = False
     while i < len(argv):
@@ -93,7 +100,7 @@ def parse(argv):
             name, eq, val = a[2:].partition("=")
             if name in ("help", "version"):
                 return {name: True}
-            if name in ("decompress", "compress", "libbz2") and not eq:
+            if name in ("decompress", "compress", "libbz2", "recover", "repair") and not eq:
                 opts[name] = True
             elif name == "block":
                 if not eq:
@@ -152,6 +159,56 @@ def check(opts):
     if level and decompress:
         raise UsageError("Compression level has no effect when decompressing.")
     return decompress, level or 7, block
+
+
+def check_recover(opts):
+    """--recover / --repair: None without them, else "recover" or "repair"; UsageError when the other options do not
+    allow them (they take -d -t bzip2 and nothing else)."""
+    rec, rep = opts["recover"], opts["repair"]
+    if not (rec or rep):
+        return None
+    if rec and rep:
+        raise UsageError("--recover and --repair cannot be used together")
+    flag = "--recover" if rec else "--repair"
+    if not opts["decompress"] or opts["compress"]:
+        raise UsageError("%s can only be used with -d -t bzip2" % flag)
+    if compressor(opts["T"]) != "bzip2":
+        raise UsageError("%s can only be used with -d -t bzip2" % flag)
+    if _number(opts["block"]) >= 0:
+        raise UsageError("%s cannot be used with --block" % flag)
+    if opts["levels"]:
+        raise UsageError("%s cannot be used with a compression level" % flag)
+    if opts["libbz2"]:
+        raise UsageError("%s cannot be used with --libbz2" % flag)
+    return "repair" if rep else "recover"
+
+
+# the reference's messages of the decode failures a lost block has
+REC_MESSAGES = {"DATA_ERROR": "Data error", "OBSOLETE": "Obsolete (pre 0.9.5) bzip format not supported."}
+
+
+def recover(in_fd, out, repair):
+    """--recover / --repair: Bzip2.recover from the descriptor to the binary file `out` through the streams of
+    bin/compressjs.  stderr gets "block at bit <p>: <message>" for every candidate that was walked and is not intact, and
+    "<k> of <m> blocks intact"; the exit status is 0 when every walked candidate is intact, else 1."""
+    from .bzip2 import Bzip2
+    src, dst = InStream(in_fd), OutStream(out)
+    try:
+        _, blocks = Bzip2.recover(src, dst, repair=repair)
+    except Exception as e:
+        out.flush()
+        sys.stderr.write("%s\n" % e)
+        return 1
+    dst.flush()
+    walked = [b for b in blocks if b.status != "INSIDE"]
+    intact = sum(b.status == "INTACT" for b in walked)
+    for b in walked:
+        if b.status == "BAD_CRC":
+            sys.stderr.write("block at bit %d: Data error: Bad block CRC (got %x expected %x)\n" % (b.bitpos, b.got, b.crc))
+        elif b.status != "INTACT":
+            sys.stderr.write("block at bit %d: %s\n" % (b.bitpos, REC_MESSAGES[b.status]))
+    sys.stderr.write("%d of %d blocks intact\n" % (intact, len(walked)))
+    return 0 if intact == len(walked) else 1
 
 
 def compressor(name):
@@ -293,6 +350,7 @@ def main(argv=None):
         if opts.get("version"):
             sys.stdout.write(VERSION + "\n")
             return 0
+        rec = check_recover(opts)
         decompress, level, block = check(opts)
         args = opts["args"]
         in_fd = os.open(args[0], os.O_RDONLY) if len(args) > 0 else sys.stdin.fileno()
@@ -300,6 +358,8 @@ def main(argv=None):
         kind = compressor(opts["T"])
         if opts["libbz2"] and (decompress or kind != "bzip2"):
             raise UsageError("--libbz2 can only be used with -z -t bzip2")
+        if rec:
+            return recover(in_fd, out, rec == "repair")
         if block < 0:
             return stream(kind, decompress, level, in_fd, out, "libbz2" if opts["libbz2"] else "compressjs")
         data, size = read_input(in_fd)

@@ -607,7 +607,57 @@ static int decode_common(const uint8_t* in, size_t n, Run run, uint8_t** out, si
   return rc;
 }
 
+// b2_bzip2_recover and b2_bzip2_recover_stream: the recovery from `in` to `out`, its rows in *rows / *count
+static int recover_host(Ctx& c, StreamIn& in, StreamOut& out, int mode, b2_recovered_block** rows, size_t* count) {
+  std::vector<b2_recovered_block> r;
+  try {
+    StageScope tot(c, ST_TOTAL);
+    bzip2_recover(c, in, mode == B2_RECOVER_BZ2, out, r);
+  } catch (...) {
+    cudaStreamSynchronize(c.stream);
+    throw;
+  }
+  c.sync();
+  c.collect();
+  c.stats.raw_bytes = out.written; c.stats.comp_bytes = in.base + in.have;
+  b2_recovered_block* p = (b2_recovered_block*)malloc(sizeof(b2_recovered_block) * (r.size() + 1));
+  if (!p) throw B2Error{B2_ERR_CUDA, "out of host memory"};
+  if (!r.empty()) memcpy(p, r.data(), sizeof(b2_recovered_block) * r.size());
+  *rows = p; *count = r.size();
+  return 0;
+}
+static void check_recover(int mode, b2_recovered_block** rows, size_t* count) {
+  if (mode != B2_RECOVER_BYTES && mode != B2_RECOVER_BZ2) throw B2Error{B2_ERR_BAD_ARG, "unknown recovery mode"};
+  if (!rows || !count) throw B2Error{B2_ERR_BAD_ARG, "null output argument"};
+}
+
 extern "C" {
+
+int b2_bzip2_recover(const uint8_t* in, size_t n, int mode, uint8_t** out, size_t* out_n, b2_recovered_block** rows, size_t* count) {
+  return guarded([&]() {
+    check_recover(mode, rows, count);
+    if (!out || !out_n || (n && !in)) throw B2Error{B2_ERR_BAD_ARG, "null output argument or input"};
+    Ctx& c = ctx_locked();
+    c.reset_call();
+    StreamIn src(in, n);
+    StreamOut dst(c.stream);
+    recover_host(c, src, dst, mode, rows, count);
+    *out_n = dst.written; *out = dst.take();
+    return 0;
+  });
+}
+
+int b2_bzip2_recover_stream(b2_read_fn rd, b2_write_fn wr, void* user, int mode, b2_recovered_block** rows, size_t* count) {
+  return guarded([&]() {
+    if (!rd || !wr) throw B2Error{B2_ERR_BAD_ARG, "null callback"};
+    check_recover(mode, rows, count);
+    Ctx& c = ctx_locked();
+    c.reset_call();
+    StreamIn src(rd, user, c.stream);
+    StreamOut dst(wr, user, c.stream);
+    return recover_host(c, src, dst, mode, rows, count);
+  });
+}
 
 // the encoder flavor of a compress call: checked with the other arguments, before anything is read
 static void check_flavor(int flavor) {

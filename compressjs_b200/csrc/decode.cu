@@ -33,7 +33,8 @@
 //                    folds/validates CRCs, delivers the settled blocks (to a device buffer, a host sink, or only
 //                    for their CRCs) and raises the reference's errors in stream order.  A position list uploads
 //                    the whole input once and walks its blocks in list order, without a chain.  The sharded decode
-//                    runs the same batch, walk and device delivery over the whole file.
+//                    runs the same batch, walk and device delivery over the whole file.  Block recovery walks every
+//                    candidate by intactness instead of by the chain and splices the intact blocks' bits (k_splice).
 #include <algorithm>
 #include <memory>
 #include <vector>
@@ -1352,6 +1353,9 @@ struct Decode {
   Chain ch;
   DecErr E;
   DecRows rows;
+  // reads no header: every block is held to the largest dbufSize (the recovery decodes blocks wherever they are)
+  struct NoHeader {};
+  Decode(Ctx& c_, const DecIn& in_, NoHeader) : c(c_), in(in_), DB(dec_batch_blocks(c_)) { ch.cur_dbuf = 900000u; }
   // reads the first header (lib/Bzip2.js:105-124 _start_bunzip)
   Decode(Ctx& c_, const DecIn& in_) : c(c_), in(in_), DB(dec_batch_blocks(c_)) {
     u8 hdr[4] = {0, 0, 0, 0};
@@ -1721,6 +1725,207 @@ void bzip2_decompress_list(Ctx& c, StreamIn& in, const std::vector<u64>& positio
   CUDA_CHECK(cudaStreamSynchronize(c.stream));
   rows = std::move(R.rows);
   R.finish(out_n, R.E.prefix);
+}
+
+// ---- block recovery ----------------------------------------------------------------------------
+// Bit splice: range k copies bits [src, src + nbits) of the source to bits [dst, dst + nbits) of the destination (MSB
+// first, any phase to any phase).  One CTA per range; each thread builds whole 32-bit destination words from two source
+// words.  A word the range covers entirely is stored; the first and last words of a range may be shared with its
+// neighbours and are ORed in, so the destination is zeroed first.  The source is read up to 8 bytes past its last range
+// (the decode window is zero padded), the destination written up to the word that holds its last bit.
+struct SpliceRange { u64 src, dst, nbits; };
+__global__ void __launch_bounds__(256) k_splice(const u8* __restrict__ src, const SpliceRange* __restrict__ ranges, u8* __restrict__ dst) {
+  const SpliceRange s = ranges[blockIdx.x];
+  if (!s.nbits) return;
+  const u32* sw = reinterpret_cast<const u32*>(src);
+  u32* dw = reinterpret_cast<u32*>(dst);
+  const u64 w0 = s.dst >> 5, w1 = (s.dst + s.nbits - 1) >> 5, e = s.dst + s.nbits;
+  const long long off = (long long)s.src - (long long)s.dst;
+  for (u64 w = w0 + threadIdx.x; w <= w1; w += blockDim.x) {
+    const long long sb = (long long)(w * 32) + off;  // source bit of the word's first bit: >= -31
+    const long long q = sb >> 5;
+    const u32 hi = q >= 0 ? __byte_perm(sw[q], 0, 0x0123) : 0u, lo = __byte_perm(sw[q + 1], 0, 0x0123);
+    const u32 v = __funnelshift_l(lo, hi, (u32)(sb & 31));
+    const u64 b0 = w * 32;
+    const u32 from = s.dst > b0 ? (u32)(s.dst - b0) : 0u, to = e < b0 + 32 ? (u32)(e - b0) : 32u;
+    if (from == 0 && to == 32) {
+      dw[w] = __byte_perm(v, 0, 0x0123);
+    } else {
+      const u32 m = (0xffffffffu >> from) & (to == 32 ? 0xffffffffu : ~(0xffffffffu >> to));
+      atomicOr(dw + w, __byte_perm(v & m, 0, 0x0123));
+    }
+  }
+}
+
+// The walk's state and the output of a recovery.
+struct Recover {
+  Decode& R;
+  bool repair;
+  StreamOut& out;
+  std::vector<b2_recovered_block>& rows;
+  u64 end = 0;         // the bit behind the last intact block's end-of-block code
+  u64 total = 0;       // recovered bytes so far
+  u32 scrc = 0;        // combined CRC of the intact blocks (lib/Bzip2.js:138-139)
+  u8 carry = 0;        // the repaired stream's last partial byte (carry_bits bits, MSB first)
+  u32 carry_bits = 0;
+  DBuf<u8> sbuf;       // one delivery group of the repaired stream
+};
+
+// n bytes at p (host) to the sink
+static void rec_put_host(Recover& V, const u8* p, size_t n) {
+  V.out.reserve(n, false, V.R.W);
+  u8* d = V.out.next();
+  memcpy(d, p, n);
+  V.out.put(d, n);
+}
+// n bytes at d (device) to the sink
+static void rec_put_dev(Recover& V, const u8* d, size_t n) {
+  V.out.reserve(n, false, V.R.W);
+  u8* h = V.out.next();
+  {
+    StageScope s(V.R.c, ST_D2H);
+    CUDA_CHECK(cudaMemcpyAsync(h, d, n, cudaMemcpyDeviceToHost, V.R.c.stream));
+  }
+  V.out.put(h, n);
+}
+
+// The repaired stream's bits of one delivery group: the ranges (window bits) go back to back behind the carried partial
+// byte, in one launch; the whole bytes go to the sink and the partial last byte is carried to the next group.
+static void rec_splice(Recover& V, std::vector<SpliceRange>& sp) {
+  if (sp.empty()) return;
+  Ctx& c = V.R.c;
+  u64 bits = V.carry_bits;
+  for (auto& x : sp) { x.dst = bits; bits += x.nbits; }
+  const size_t cap = ((bits + 31) / 32) * 4;
+  if (cap > V.sbuf.n) V.sbuf.alloc(c, cap);
+  CUDA_CHECK(cudaMemsetAsync(V.sbuf, 0, cap, c.stream));
+  if (V.carry_bits) CUDA_CHECK(cudaMemcpyAsync(V.sbuf, &V.carry, 1, cudaMemcpyHostToDevice, c.stream));
+  DBuf<SpliceRange> dsp(c, sp.size());
+  CUDA_CHECK(cudaMemcpyAsync(dsp, sp.data(), sizeof(SpliceRange) * sp.size(), cudaMemcpyHostToDevice, c.stream));
+  k_splice<<<(unsigned)sp.size(), 256, 0, c.stream>>>(V.R.win, dsp, V.sbuf);
+  KLAUNCH(c); KCHECK();
+  const size_t whole = (size_t)(bits / 8);
+  V.carry_bits = (u32)(bits & 7);
+  if (whole) rec_put_dev(V, V.sbuf, whole);
+  V.carry = 0;
+  if (V.carry_bits) CUDA_CHECK(cudaMemcpyAsync(&V.carry, V.sbuf.p + whole, 1, cudaMemcpyDeviceToHost, c.stream));
+  CUDA_CHECK(cudaStreamSynchronize(c.stream));
+}
+
+// Settle the batch's candidates in position order, one staging group at a time: every candidate that decoded is
+// expanded for its CRC, then the walk gives each its row, and the group's intact blocks go out (bytes: runs of
+// consecutive blocks from staging; repair: their bit ranges spliced from the window).  Returns false when a candidate
+// that starts at or behind the walk's end has no final result (its decode reached the end of a window that does not end
+// the input): *next is then its position, and nothing from it on is settled.
+static bool recover_batch(Recover& V, u64* next) {
+  Decode& R = V.R;
+  const u32 cnt = R.cnt;
+  auto decoded = [&](u32 s) { return R.hres[s].status == 0 && !R.hres[s].open; };
+  R.ob.assign(cnt, ~0ull);
+  R.got.assign(cnt, 0);
+  for (u32 g0 = 0; g0 < cnt;) {
+    u64 bytes = 0;
+    u32 g1 = g0;
+    for (; g1 < cnt; g1++) {
+      if (!decoded(g1)) continue;
+      if (bytes && bytes + R.hres[g1].rawlen > R.W) break;
+      R.ob[g1] = bytes;
+      bytes += R.hres[g1].rawlen;
+    }
+    if (bytes) {
+      if (bytes > R.stage.n) R.stage.alloc(R.c, bytes);
+      R.expand(g0, g1, R.hres.data(), R.ob.data(), R.stage, R.got.data());
+    }
+    std::vector<SpliceRange> sp;
+    u64 run0 = ~0ull, run1 = 0;  // staging bytes of the current run of intact blocks
+    auto deliver = [&]() {
+      if (run0 != ~0ull) rec_put_dev(V, R.stage.p + run0, run1 - run0);
+      run0 = ~0ull;
+      rec_splice(V, sp);
+    };
+    for (u32 s = g0; s < g1; s++) {
+      const Cand& cd = R.cands[R.blk[R.kb + s]];
+      const CandRes& r = R.hres[s];
+      b2_recovered_block row = {cd.pos, 0, V.total, 0, cd.next32, 0, B2_REC_INSIDE};
+      if (cd.pos >= V.end) {
+        if (r.open) { deliver(); *next = cd.pos; return false; }
+        if (r.status != 0) {
+          row.status = r.status == DEC_OBSOLETE ? B2_REC_OBSOLETE : B2_REC_DATA_ERROR;
+        } else {
+          row.endbit = r.endbit; row.size = r.rawlen; row.got = R.got[s];
+          row.status = row.got == cd.next32 ? B2_REC_INTACT : B2_REC_BAD_CRC;
+        }
+      }
+      if (row.status == B2_REC_INTACT) {
+        V.end = r.endbit;
+        V.total += r.rawlen;
+        V.scrc = cd.next32 ^ ((V.scrc << 1) | (V.scrc >> 31));
+        if (V.repair) {
+          sp.push_back({cd.pos - R.a * 8, 0, r.endbit - cd.pos});
+        } else if (run0 != ~0ull && R.ob[s] == run1) {
+          run1 += r.rawlen;
+        } else {
+          if (run0 != ~0ull) rec_put_dev(V, R.stage.p + run0, run1 - run0);
+          run0 = R.ob[s]; run1 = run0 + r.rawlen;
+        }
+      }
+      V.rows.push_back(row);
+    }
+    deliver();
+    g0 = g1;
+  }
+  return true;
+}
+
+// Block recovery: every block magic of the input is a candidate, decoded as Bzip2.decompressBlock decodes a block of a
+// BZh9 file, and walked in position order: a candidate that starts inside the last intact block is INSIDE, any other
+// is INTACT when it decodes and its CRC matches (the walk's end moves behind it), else it gets the status its decode
+// failed with.  The loop has the chain decode's shape: windows [a, a + W) of the input (no magic whose 80 bits cross a
+// window's end is taken from it), batches of B candidates, and the next window starts at the first candidate without a
+// final result, twice as long when it would start where this one did.  No header is read: any input is walked to its
+// end.  The output is the intact blocks' bytes, or (repair) one BZh9 stream of their bits followed by the end-of-stream
+// magic and the combined CRC.
+void bzip2_recover(Ctx& c, StreamIn& in, bool repair, StreamOut& out, std::vector<b2_recovered_block>& rows) {
+  Decode R(c, DecIn(in), Decode::NoHeader{});
+  Recover V{R, repair, out, rows};
+  if (repair) rec_put_host(V, reinterpret_cast<const u8*>("BZh9"), 4);
+  u64 next = 0, prev_a = ~0ull;  // next: the first candidate position without a row
+  size_t wcur = R.W;
+  for (;;) {
+    const u64 a = (next >> 3) & ~(u64)255;
+    wcur = a == prev_a ? wcur * 2 : R.W;
+    prev_a = a;
+    R.load(a, wcur);
+    const u64 bits = R.wl * 8, lim = R.last ? bits : (bits >= 80 ? bits - 79 : 0);
+    if (R.wl) {
+      R.scan(lim);
+    } else {
+      R.cands.clear(); R.blk.clear();
+    }
+    R.reserve();
+    bool settled = true;
+    for (R.kb = R.blk_from(next); R.kb < R.blk.size(); R.kb += R.cnt) {
+      R.batch();
+      if (!(settled = recover_batch(V, &next))) break;
+    }
+    if (settled) {
+      if (R.last) break;
+      next = std::max(next, R.a * 8 + lim);
+    }
+  }
+  if (repair) {
+    // the end-of-stream magic, the combined CRC and zero bits to the next byte, behind the carried bits
+    u8 t[12] = {0};
+    const u64 tail[2] = {SQRTPI, V.scrc};
+    const u32 tlen[2] = {48, 32};
+    u32 nb = V.carry_bits;
+    t[0] = V.carry;
+    for (int k = 0; k < 2; k++)
+      for (int i = (int)tlen[k] - 1; i >= 0; i--, nb++)
+        if ((tail[k] >> i) & 1) t[nb >> 3] |= (u8)(0x80u >> (nb & 7));
+    rec_put_host(V, t, (nb + 7) / 8);
+  }
+  CUDA_CHECK(cudaStreamSynchronize(c.stream));
 }
 
 // ---- sharded decode (SURVEY.md section 8e): open on every rank, exchange results, finish ------------

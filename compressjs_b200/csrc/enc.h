@@ -180,6 +180,10 @@ void bzip2_table(Ctx& c, StreamIn& in, int multistream, DecRows& rows, size_t* o
 // b2_bzip2_decompress_blocks: the blocks at a non-empty list of bit positions, back to back in list order, from a complete
 // input; rows.ends, and *out_n on an error, as bzip2_decompress_host's.
 void bzip2_decompress_list(Ctx& c, StreamIn& in, const std::vector<u64>& positions, StreamOut& out, DecRows& rows, size_t* out_n);
+// b2_bzip2_recover and b2_bzip2_recover_stream: one row per block magic of `in`, in position order, and into `out` the
+// intact blocks' bytes or (repair) the repaired stream.  Damage is a result, not an error: only a CUDA failure or a
+// callback abort throws.
+void bzip2_recover(Ctx& c, StreamIn& in, bool repair, StreamOut& out, std::vector<b2_recovered_block>& rows);
 // The sharded decode (b2_dec_shard_open / _export / _finish): one session at a time, ended by finish or released by
 // b2_shutdown.
 void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* info);

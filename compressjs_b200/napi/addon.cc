@@ -136,6 +136,34 @@ static napi_value Table(napi_env env, napi_callback_info info) {
   if (rc) return fail(env, rc, "rows", arr);
   return arr;
 }
+// recover(buffer, repair) -> [Buffer, [[bitpos, endbit, out_off, size, crc, got, status], ...]]   (b2_bzip2_recover:
+// the intact blocks' bytes, or with repair the repaired stream, and one row per block magic; status is B2_REC_*)
+static napi_value Recover(napi_env env, napi_callback_info info) {
+  size_t argc = 2; napi_value argv[2];
+  napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr);
+  const uint8_t* in; size_t n; bool repair = false;
+  if (!buf_arg(env, argv[0], &in, &n)) return fail(env, B2_ERR_BAD_ARG);
+  if (argc > 1) napi_get_value_bool(env, argv[1], &repair);
+  uint8_t* out = nullptr; size_t out_n = 0; b2_recovered_block* rows = nullptr; size_t cnt = 0;
+  int rc = b2_bzip2_recover(in, n, repair ? B2_RECOVER_BZ2 : B2_RECOVER_BYTES, &out, &out_n, &rows, &cnt);
+  if (rc) return fail(env, rc);
+  napi_value buf, arr;
+  napi_create_external_buffer(env, out_n, out, fin, nullptr, &buf);
+  napi_create_array_with_length(env, cnt, &arr);
+  for (size_t i = 0; i < cnt; i++) {
+    const b2_recovered_block& r = rows[i];
+    const double f[7] = {(double)r.bitpos, (double)r.endbit, (double)r.out_off, (double)r.size, (double)r.crc, (double)r.got,
+                         (double)r.status};
+    napi_value o;
+    napi_create_array_with_length(env, 7, &o);
+    for (uint32_t k = 0; k < 7; k++) { napi_value v; napi_create_double(env, f[k], &v); napi_set_element(env, o, k, v); }
+    napi_set_element(env, arr, (uint32_t)i, o);
+  }
+  b2_free(rows);
+  napi_value res; napi_create_array_with_length(env, 2, &res);
+  napi_set_element(env, res, 0, buf); napi_set_element(env, res, 1, arr);
+  return res;
+}
 // bwtransform2(T, U, n) -> pidx                     (BWT.bwtransform2, lib/BWT.js:372)
 static napi_value Bwtransform2(napi_env env, napi_callback_info info) {
   size_t argc = 3; napi_value argv[3];
@@ -220,6 +248,7 @@ static napi_value Init(napi_env env, napi_value exports) {
       {"decompressFile", nullptr, DecompressFile, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"decompressBlock", nullptr, DecompressBlock, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"decompressBlocks", nullptr, DecompressBlocks, nullptr, nullptr, nullptr, napi_default, nullptr},
+      {"recover", nullptr, Recover, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"table", nullptr, Table, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"bwtransform2", nullptr, Bwtransform2, nullptr, nullptr, nullptr, napi_default, nullptr},
       {"suffixsort", nullptr, Suffixsort, nullptr, nullptr, nullptr, napi_default, nullptr},

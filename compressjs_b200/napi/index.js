@@ -78,6 +78,17 @@ Bzip2.decompressBlocks = function(input, positions, output) {
   r[1].forEach(function(e) { blocks.push(new Uint8Array(r[0].subarray(s, e))); s = e; });
   return blocks;
 };
+// GPU extension: the intact blocks of a damaged file (include/b2bz.h b2_bzip2_recover).  Returns [output, blocks]:
+// output gets the intact blocks' bytes, or with opts.repair one bzip2 stream of them; blocks has one row per block magic,
+// its status a string.
+var REC_STATUS = ['INTACT', 'BAD_CRC', 'DATA_ERROR', 'OBSOLETE', 'INSIDE'];
+Bzip2.recover = function(input, output, opts) {
+  var r = native.recover(drain(input), !!(opts && opts.repair));
+  var blocks = r[1].map(function(b) {
+    return {bitpos: b[0], endbit: b[1], out_off: b[2], size: b[3], crc: b[4], got: b[5], status: REC_STATUS[b[6]]};
+  });
+  return [deliver(output, r[0]), blocks];
+};
 Bzip2.table = function(input, callback, multistream) {
   var rows;
   try { rows = native.table(drain(input), !!multistream); } catch (e) {

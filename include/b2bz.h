@@ -121,6 +121,51 @@ int b2_bzip2_compress_stream(b2_read_fn rd, b2_write_fn wr, void* user, int leve
  * under 2 MiB). */
 int b2_bzip2_decompress_stream(b2_read_fn rd, b2_write_fn wr, void* user, int multistream);
 
+/* ---- recovery of a damaged bzip2 file (GPU extension; what bzip2recover + bzip2 -t do, without losing a block whose
+ * neighbour's magic is damaged) ----
+ * Candidates are the 48-bit block magics 0x314159265359 at every bit position of the input, in position order; headers,
+ * end-of-stream magics and stream CRCs play no part.  Decoding the candidate at bit p is Bzip2.decompressBlock(B, p + 32)
+ * with B = "BZh9" + input (lib/Bzip2.js:482-503 with dbufSize 900 000, whatever the file's headers say, and the block CRC
+ * check).  The walk keeps `end`, starting at 0; a candidate with p < end starts inside an intact block and is INSIDE;
+ * any other is decoded: INTACT when that raises nothing (end becomes the bit behind its end-of-block code), else BAD_CRC
+ * ("Bad block CRC"), OBSOLETE (-7) or DATA_ERROR (anything else: reading past the input, origPtr out of bounds, more than
+ * 900 000 symbols or bytes, ...).
+ *   B2_RECOVER_BYTES: *out = the decoded bytes of the INTACT candidates, in position order.
+ *   B2_RECOVER_BZ2:   *out = one bzip2 stream: "BZh9", the bits [p, endbit) of every intact block copied unchanged and
+ *                     back to back, the end-of-stream magic, the combined CRC (crc = rotl1(crc) ^ stored block CRC over
+ *                     the intact blocks, lib/Bzip2.js:138-139) and zero bits to the next byte: the 14-byte empty stream
+ *                     when nothing is intact.  It decodes to the B2_RECOVER_BYTES output with b2_bzip2_decompress.
+ * *rows: one row per candidate, in position order (*count of them), released with b2_free().
+ * Returns B2_OK whenever the input was read to its end: damage, no intact block and input that is not bzip2 at all are
+ * results, not errors.  B2_ERR_BAD_ARG for an unknown mode or a NULL output pointer, B2_ERR_STREAM for a callback abort,
+ * B2_ERR_CUDA for a CUDA failure; on an error nothing is returned.
+ * Memory: the input passes through the device in the windows and batches of b2_bzip2_decompress ($B2_DEC_WINDOW,
+ * $B2_DEC_BATCH): the same device bound, plus, for B2_RECOVER_BZ2, one window's bytes for the repaired stream's staging:
+ *     2 * max(W, 48 MiB) + B * 24 MiB + 16 bytes per magic in a window (+ W + 8 for B2_RECOVER_BZ2).
+ * A damaged candidate reads up to ~2.3 MB before it fails (900 000 symbols of at most 20 bits): a window widens past W
+ * only for such a candidate or a block longer than W.  The stream call holds the host memory of b2_bzip2_decompress_stream
+ * (the input window plus 5 bytes, and max(W, 48 MiB) of output: under 3 max(W, 48 MiB) in all), plus 40 bytes per row. */
+typedef struct b2_recovered_block {
+  uint64_t bitpos;   /* bit position of the block magic in the input */
+  uint64_t endbit;   /* bit behind its end-of-block code: INTACT and BAD_CRC rows, else 0 */
+  uint64_t out_off;  /* offset of its bytes in the recovered bytes: INTACT rows, else the offset it would have had */
+  uint32_t size;     /* decoded bytes: INTACT and BAD_CRC rows, else 0 */
+  uint32_t crc;      /* stored block CRC (the 32 bits behind the magic) */
+  uint32_t got;      /* CRC of the decoded bytes: INTACT and BAD_CRC rows, else 0 */
+  int32_t status;    /* B2_REC_* */
+} b2_recovered_block;
+#define B2_REC_INTACT 0
+#define B2_REC_BAD_CRC 1
+#define B2_REC_DATA_ERROR 2
+#define B2_REC_OBSOLETE 3
+#define B2_REC_INSIDE 4
+#define B2_RECOVER_BYTES 0  /* output: the recovered bytes */
+#define B2_RECOVER_BZ2   1  /* output: the repaired stream */
+int b2_bzip2_recover(const uint8_t* in, size_t n, int mode, uint8_t** out, size_t* out_n, b2_recovered_block** rows, size_t* count);
+/* The same over read / write callbacks (b2_read_fn / b2_write_fn and their rules as above): everything passed to write,
+ * concatenated, is the *out of b2_bzip2_recover on everything read, however the input is split into reads. */
+int b2_bzip2_recover_stream(b2_read_fn rd, b2_write_fn wr, void* user, int mode, b2_recovered_block** rows, size_t* count);
+
 /* ---- compressjs.BWT (lib/BWT.js) ------------------------------------------------- */
 /* BWT.bwtransform2(T, U, n, 256) -> pidx  (cyclic)    lib/BWT.js:372-417
  * n is limited to 900 000 (the largest bzip2 block; the reference has no limit): longer strings return B2_ERR_BAD_ARG. */
