@@ -138,10 +138,17 @@ def check_table_case(data, level, corner):
 
 
 def golden_corpus():
-    """(key, data, level) of tests/golden/libbz2.json: every cut and table case, and the compressjs samples at 1..9."""
+    """(key, data, level) of tests/golden/libbz2.json: every cut and table case, the compressjs samples at 1..9, the
+    designed table-search blocks of tests/libbz2_table_cases.py (table2_, and all of them as one file) and every case of tests/mtfhuff_cases.py at
+    its levels (mtfhuff_; building those needs the oracle)."""
+    from tests import libbz2_table_cases as TC
+    from tests import mtfhuff_cases as MC
     from tests.util import fixture
     out = [("%s_-%d" % (name, lv), d, lv) for name, d, lv, _ in cut_cases() + table_cases()]
     for i in range(6):
         d = fixture("sample%d.ref" % i)
         out += [("sample%d_-%d" % (i, lv), d, lv) for lv in range(1, 10)]
+    out += [("table2_%s_-%d" % (name, lv), d, lv) for name, d, lv in TC.corpus()]
+    out.append(("table2_whole_-9", TC.whole(), 9))
+    out += [("mtfhuff_%s_-%d" % (c.name, lv), MC.info(c.name).raw, lv) for c in MC.cases() for lv in c.levels]
     return out

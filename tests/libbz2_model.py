@@ -108,7 +108,8 @@ def n_groups(nmtf):
 
 
 def make_lengths(freq, max_len=17, stats=None):
-    """BZ2_hbMakeCodeLengths.  stats (a dict, optional) counts the 17-bit rescales in 'rescales'."""
+    """BZ2_hbMakeCodeLengths.  stats (a dict, optional) counts the 17-bit rescales in 'rescales' and sets 'heap_tie'
+    when two equal weights (frequency and depth byte) met at a comparison of the heap."""
     a = len(freq)
     weight, parent, heap = [0] * (2 * a + 2), [0] * (2 * a + 2), [0] * (a + 3)
     for i in range(a):
@@ -118,11 +119,17 @@ def make_lengths(freq, max_len=17, stats=None):
         heap[0] = 0
         weight[0] = 0
 
+        def tie(a, b):
+            if stats is not None and weight[a] == weight[b]:
+                stats["heap_tie"] = True
+
         def up(z):
             tmp = heap[z]
+            tie(tmp, heap[z >> 1])
             while weight[tmp] < weight[heap[z >> 1]]:
                 heap[z] = heap[z >> 1]
                 z >>= 1
+                tie(tmp, heap[z >> 1])
             heap[z] = tmp
 
         def down(z):
@@ -131,8 +138,11 @@ def make_lengths(freq, max_len=17, stats=None):
                 y = z << 1
                 if y > n_heap:
                     break
-                if y < n_heap and weight[heap[y + 1]] < weight[heap[y]]:
-                    y += 1
+                if y < n_heap:
+                    tie(heap[y + 1], heap[y])
+                    if weight[heap[y + 1]] < weight[heap[y]]:
+                        y += 1
+                tie(tmp, heap[y])
                 if weight[tmp] < weight[heap[y]]:
                     break
                 heap[z] = heap[y]
@@ -170,71 +180,114 @@ def make_lengths(freq, max_len=17, stats=None):
             weight[i] = (1 + (weight[i] >> 8) // 2) << 8
 
 
-def initial_tables(freq, nmtf, ng):
-    """sendMTFValues' initial tables: lists of 0 / 15 lengths; also returns whether the odd-nPart step moved a bound."""
+def initial_tables(freq, nmtf, ng, report=None):
+    """sendMTFValues' initial tables: lists of 0 / 15 lengths; also returns whether the odd-nPart step moved a bound.
+
+    report (a dict, optional) gets 'odd_moved' and 'odd_single': the nPart values at which the odd step moved a bound,
+    and at which it was due but skipped because the range was a single symbol; 'exhausted': whether the alphabet ran
+    out before nPart reached 1 (the later tables are all 15s); 'ranges': per table the (gs, ge, tFreq) of its part."""
     a = len(freq)
     lens = [[15] * a for _ in range(ng)]
     n_part, rem_f, gs, adjusted = ng, nmtf, 0, False
+    moved, single, ranges = [], [], [None] * ng
     while n_part > 0:
         t_freq = rem_f // n_part
         ge, a_freq = gs - 1, 0
         while a_freq < t_freq and ge < a - 1:
             ge += 1
             a_freq += freq[ge]
-        if ge > gs and n_part != ng and n_part != 1 and (ng - n_part) % 2 == 1:
+        odd = n_part != ng and n_part != 1 and (ng - n_part) % 2 == 1
+        if ge > gs and odd:
             a_freq -= freq[ge]
             ge -= 1
             adjusted = True
+            moved.append(n_part)
+        elif ge == gs and odd:
+            single.append(n_part)
+        ranges[n_part - 1] = (gs, ge, t_freq)
         for v in range(a):
             lens[n_part - 1][v] = 0 if gs <= v <= ge else 15
         n_part -= 1
         gs = ge + 1
         rem_f -= a_freq
+    if report is not None:
+        report.update(odd_moved=moved, odd_single=single, ranges=ranges,
+                      exhausted=any(r[0] > r[1] for r in ranges))
     return lens, adjusted
 
 
-def tables(syms, alpha_size, stats=None):
-    """(selectors, code lengths of every table) after the four rounds of sendMTFValues."""
+def tables(syms, alpha_size, stats=None, report=None):
+    """(selectors, code lengths of every table) after the four rounds of sendMTFValues.
+
+    report (a dict, optional) gets 'init' (initial_tables' report) and 'rounds': per round a dict of 'ties' (groups
+    whose least cost two or more tables share; the first of them is selected), 'max_cost' (the largest cost of a group
+    under any table) and 'tables', per table of the round a dict of 'selected' (groups that selected it), 'rescales'
+    (17-bit rescales of its build), 'heap_tie', 'max_len' (its longest code) and 'equal_used' (the most used symbols
+    that share one frequency in it) and 'zeros' (its symbols of frequency 0, weight 1 in the build).  The tables of round 4 are written."""
     nmtf = len(syms)
-    freq = [0] * alpha_size
-    for s in syms:
-        freq[s] += 1
+    sy = np.asarray(syms, np.int64)
+    freq = np.bincount(sy, minlength=alpha_size).tolist()
     ng = n_groups(nmtf)
-    lens, adjusted = initial_tables(freq, nmtf, ng)
+    init = {}
+    lens, adjusted = initial_tables(freq, nmtf, ng, init)
     if stats is not None:
         stats["odd_adjust"] = stats.get("odd_adjust", False) or adjusted
+    nsel = (nmtf + 49) // 50
+    G = np.zeros((nsel, alpha_size), np.int64)           # symbol counts of every group
+    np.add.at(G, (np.arange(nmtf) // 50, sy), 1)
+    rounds = []
     for _ in range(4):
-        rf = [[0] * alpha_size for _ in range(ng)]
-        sel = []
-        for g0 in range(0, nmtf, 50):
-            grp = syms[g0:g0 + 50]
-            costs = [sum(lens[t][s] for s in grp) for t in range(ng)]
-            bt = costs.index(min(costs))
-            sel.append(bt)
-            for s in grp:
-                rf[bt][s] += 1
-        lens = [make_lengths(rf[t], 17, stats) for t in range(ng)]
-    return sel, lens
+        cost = G @ np.array(lens, np.int64).T
+        best = cost.min(1)
+        sel = np.argmin(cost, axis=1)                    # the first least cost, as the scan of sendMTFValues
+        rf = np.zeros((ng, alpha_size), np.int64)
+        np.add.at(rf, sel, G)
+        built = [{} for _ in range(ng)]
+        lens = [make_lengths(rf[t].tolist(), 17, built[t]) for t in range(ng)]
+        counts = np.bincount(sel, minlength=ng)
+        for t in range(ng):
+            f = rf[t][rf[t] > 0]
+            if stats is not None:
+                stats["rescales"] = stats.get("rescales", 0) + built[t].get("rescales", 0)
+            built[t] = dict(selected=int(counts[t]), rescales=built[t].get("rescales", 0),
+                            heap_tie=built[t].get("heap_tie", False), max_len=max(lens[t]),
+                            equal_used=int(np.bincount(f).max()) if f.size else 0, zeros=int((rf[t] == 0).sum()))
+        rounds.append(dict(ties=int(((cost == best[:, None]).sum(1) > 1).sum()), max_cost=int(cost.max()), tables=built))
+    if report is not None:
+        report.update(init=init, rounds=rounds)
+    return sel.tolist(), lens
 
 
 class _Bits:
     def __init__(self):
-        self.bits = []
+        self.parts, self.n = [], 0
 
     def w(self, n, v):
-        for i in range(n - 1, -1, -1):
-            self.bits.append((v >> i) & 1)
+        self.parts.append(format(v, "0%db" % n))
+        self.n += n
 
     def out(self):
-        b = self.bits + [0] * (-len(self.bits) % 8)
-        return np.packbits(np.array(b, dtype=np.uint8)).tobytes() if b else b""
+        b = "".join(self.parts)
+        b += "0" * (-len(b) % 8)
+        return int(b, 2).to_bytes(len(b) // 8, "big") if b else b""
+
+
+def _crc_table():
+    t = []
+    for i in range(256):
+        c = i << 24
+        for _ in range(8):
+            c = ((c << 1) ^ 0x04C11DB7) & 0xFFFFFFFF if c & 0x80000000 else (c << 1) & 0xFFFFFFFF
+        t.append(c)
+    return t
+
+
+_CRC = _crc_table()
 
 
 def crc32(data, c=0xFFFFFFFF):
     for x in data:
-        c ^= x << 24
-        for _ in range(8):
-            c = ((c << 1) ^ 0x04C11DB7) & 0xFFFFFFFF if c & 0x80000000 else (c << 1) & 0xFFFFFFFF
+        c = ((c << 8) & 0xFFFFFFFF) ^ _CRC[(c >> 24) ^ x]
     return c ^ 0xFFFFFFFF
 
 
@@ -250,14 +303,22 @@ def block_facts(data, level, stats=None):
     return facts
 
 
-def compress(data, level):
-    """The whole model: the bytes of bz2.compress(data, level)."""
+TRACE_FIELDS = ("n", "pidx", "m", "alpha", "ngroups", "nsel", "crc", "bit_len")
+
+
+def encode(data, level):
+    """The whole model: (the bytes of bz2.compress(data, level), per block a dict of the TRACE_FIELDS of b2_last_trace
+    -- bit_len counts the bits from the block magic to the end of the block's symbols -- together with raw_start,
+    raw_len, the zero-run coder's symbols 'syms', the selectors 'sel', the written code lengths 'lens' and the table
+    search's 'report' (see tables))."""
     bw = _Bits()
     for ch in b"BZh":
         bw.w(8, ch)
     bw.w(8, ord("0") + level)
     scrc = 0
+    blocks = []
     for start, length, blk in cut(data, level):
+        b0 = bw.n
         c = crc32(data[start:start + length])
         scrc = (((scrc << 1) | (scrc >> 31)) & 0xFFFFFFFF) ^ c
         bw.w(24, 0x314159); bw.w(24, 0x265359); bw.w(32, c); bw.w(1, 0)
@@ -272,7 +333,8 @@ def compress(data, level):
                 for j in range(16):
                     bw.w(1, int((i * 16 + j) in uset))
         a = len(used) + 2
-        sel, lens = tables(syms, a)
+        report = {}
+        sel, lens = tables(syms, a, report=report)
         ng = len(lens)
         bw.w(3, ng); bw.w(15, len(sel))
         mt = list(range(ng))
@@ -299,8 +361,21 @@ def compress(data, level):
                 vec <<= 1
             codes.append(code)
         for gi, g0 in enumerate(range(0, len(syms), 50)):
-            t = sel[gi]
+            ln, cd = lens[sel[gi]], codes[sel[gi]]
             for s in syms[g0:g0 + 50]:
-                bw.w(lens[t][s], codes[t][s])
+                bw.w(ln[s], cd[s])
+        blocks.append(dict(n=len(blk), pidx=pidx, m=len(syms), alpha=len(used), ngroups=ng, nsel=len(sel), crc=c,
+                           bit_len=bw.n - b0, raw_start=start, raw_len=length, syms=syms, sel=sel, lens=lens,
+                           report=report))
     bw.w(24, 0x177245); bw.w(24, 0x385090); bw.w(32, scrc)
-    return bw.out()
+    return bw.out(), blocks
+
+
+def compress(data, level):
+    """The bytes of bz2.compress(data, level)."""
+    return encode(data, level)[0]
+
+
+def trace(data, level):
+    """Per block the fields of b2_last_trace (TRACE_FIELDS), as the GPU encoder reports them for the libbz2 flavor."""
+    return [tuple(b[f] for f in TRACE_FIELDS) for b in encode(data, level)[1]]
