@@ -55,7 +55,8 @@ k_msd_prep(const u32* __restrict__ hist, u32* __restrict__ bstart, u32* __restri
 struct MsdScatterSmem {
   __align__(16) u8 raw[16 + MSD_TILE + 16];  // raw[15] = byte before the tile, raw[16..] the tile, then 4 bytes of look-ahead
   __align__(16) u8 rk[MSD_TILE + 16];        // dense symbol ranks of raw[16..]
-  __align__(16) u64 rec[MSD_TILE];
+  u32 key[MSD_TILE];  // the staged records as two 32-bit planes: a warp's stores in digit order meet fewer bank conflicts
+  u32 low[MSD_TILE];  // than 64-bit stores
   u32 cnt[256];
   int gdst[256];
   u8 lut[256];
@@ -100,20 +101,42 @@ k_msd_scatter(const u8* __restrict__ T, const u32* __restrict__ seg_n, u32 tps, 
   if (tid == 32) s.raw[15] = edge;
   if (tid < 4) s.raw[16 + count + tid] = edge;
   __syncthreads();
-  // ---- dense ranks of the own 16 bytes ----
+  const u32 a = mb.a, a2 = mb.a2, S_lo = (u32)mb.S, S_hi = (u32)(mb.S >> 32);
+  // the rest twice: full tiles (all but the last of a block) carry no per-record bounds checks
+  auto body = [&](auto full_c) {
+  constexpr bool full = decltype(full_c)::value;
+  // ---- dense ranks of the own 16 bytes, and their slots among the tile's records of the same digit (the digit is
+  // the byte itself, so the tile's digit counts are known before any key is computed) ----
   const uint4 rv = *reinterpret_cast<const uint4*>(s.raw + 16 + tid * 16);
+  const u32 rw[4] = {rv.x, rv.y, rv.z, rv.w};
+  u32 slot[MSD_ITEMS / 2];
   {
     uint4 kv;
     kv.x = lut4(s.lut, rv.x); kv.y = lut4(s.lut, rv.y); kv.z = lut4(s.lut, rv.z); kv.w = lut4(s.lut, rv.w);
     *reinterpret_cast<uint4*>(s.rk + tid * 16) = kv;
     if (tid < 4) s.rk[count + tid] = s.lut[s.raw[16 + count + tid]];  // look-ahead ranks (same value as the owner's store, if any)
+#pragma unroll
+    for (int j = 0; j < MSD_ITEMS; j++) {
+      const u32 d = (rw[j >> 2] >> (8 * (j & 3))) & 0xffu;
+      u32 sl = 0;
+      if (full || tid * MSD_ITEMS + j < count) sl = atomicAdd(&s.cnt[d], 1u);
+      if (j & 1) slot[j >> 1] |= sl << 16; else slot[j >> 1] = sl;
+    }
   }
   __syncthreads();
-  const u32 a = mb.a, a2 = mb.a2, S_lo = (u32)mb.S, S_hi = (u32)(mb.S >> 32);
-  // the rest twice: full tiles (all but the last of a block) carry no per-record bounds checks
-  auto body = [&](auto full_c) {
-  constexpr bool full = decltype(full_c)::value;
-  u32 key[MSD_ITEMS], slot[MSD_ITEMS / 2];
+  // ---- per digit: space in the block's bucket (any order: the bucket is sorted afterwards).  The global atomic is
+  // issued here and its result is first needed after the keys are computed and staged. ----
+  u32 g, ex;
+  {
+    const u32 c = s.cnt[tid];
+    u32 tot;
+    ex = block_excl_add<MSD_THREADS, u32>(c, s.ws, &tot);
+    g = c ? atomicAdd(&cursor[b * 256 + tid], c) : 0u;
+    s.cnt[tid] = ex;
+  }
+  __syncthreads();
+  // ---- keys, staged in digit order as two 32-bit planes (key, low word); the low word carries (byte before, digit,
+  // position inside the tile) for now ----
   {
     const uint4 k0 = *reinterpret_cast<const uint4*>(s.rk + tid * 16);
     const u32 k1 = *reinterpret_cast<const u32*>(s.rk + tid * 16 + 16);
@@ -124,39 +147,16 @@ k_msd_scatter(const u8* __restrict__ T, const u32* __restrict__ seg_n, u32 tps, 
     u32 v2[19];  // two symbols starting at j
 #pragma unroll
     for (int j = 1; j < 19; j++) v2[j] = rr[j] * a + rr[j + 1];
-    const u32 rw[4] = {rv.x, rv.y, rv.z, rv.w};
-#pragma unroll
-    for (int j = 0; j < MSD_ITEMS; j++) {
-      const u32 k = v2[j + 1] * a2 + v2[j + 3];          // symbols j+1 .. j+4 as a base-a number
-      key[j] = k * S_hi + __umulhi(k, S_lo);             // spread over 32 bits (order preserving, injective)
-      const u32 d = (rw[j >> 2] >> (8 * (j & 3))) & 0xffu;
-      u32 sl = 0;
-      if (full || tid * MSD_ITEMS + j < count) sl = atomicAdd(&s.cnt[d], 1u);
-      if (j & 1) slot[j >> 1] |= sl << 16; else slot[j >> 1] = sl;
-    }
-  }
-  __syncthreads();
-  // ---- per digit: space in the block's bucket (any order: the bucket is sorted afterwards).  The global atomic is
-  // issued here and its result is first needed after the staging step.
-  u32 g, ex;
-  {
-    const u32 c = s.cnt[tid];
-    u32 tot;
-    ex = block_excl_add<MSD_THREADS, u32>(c, s.ws, &tot);
-    g = c ? atomicAdd(&cursor[b * 256 + tid], c) : 0u;
-    s.cnt[tid] = ex;
-  }
-  __syncthreads();
-  // ---- stage the tile in digit order; the low word carries (byte before, digit, position inside the tile) for now ----
-  {
-    const u32 rw[4] = {rv.x, rv.y, rv.z, rv.w};
     u32 prev = s.raw[15 + tid * 16];
 #pragma unroll
     for (int j = 0; j < MSD_ITEMS; j++) {
       const u32 d = (rw[j >> 2] >> (8 * (j & 3))) & 0xffu;
       if (full || tid * MSD_ITEMS + j < count) {
+        const u32 k = v2[j + 1] * a2 + v2[j + 3];          // symbols j+1 .. j+4 as a base-a number
         const u32 sl = (j & 1) ? (slot[j >> 1] >> 16) : (slot[j >> 1] & 0xffffu);
-        s.rec[s.cnt[d] + sl] = ((u64)key[j] << 32) | (u64)((prev << SEG_SHIFT) | (d << 12) | (tid * MSD_ITEMS + j));
+        const u32 at = s.cnt[d] + sl;
+        s.key[at] = k * S_hi + __umulhi(k, S_lo);           // spread over 32 bits (order preserving, injective)
+        s.low[at] = (prev << SEG_SHIFT) | (d << 12) | (tid * MSD_ITEMS + j);
       }
       prev = d;
     }
@@ -168,10 +168,9 @@ k_msd_scatter(const u8* __restrict__ T, const u32* __restrict__ seg_n, u32 tps, 
   for (int k = 0; k < MSD_ITEMS; k++) {
     const u32 p = k * MSD_THREADS + tid;
     if (full || p < count) {
-      const u64 rvv = s.rec[p];
-      const u32 lw = (u32)rvv;
+      const u32 lw = s.low[p];
       const u32 low = (lw & 0x0ff00000u) | (start + (lw & 0xfffu));
-      out[(int)p + s.gdst[(lw >> 12) & 0xffu]] = (rvv & 0xffffffff00000000ull) | low;
+      out[(int)p + s.gdst[(lw >> 12) & 0xffu]] = ((u64)s.key[p] << 32) | low;
     }
   }
   };
@@ -179,6 +178,26 @@ k_msd_scatter(const u8* __restrict__ T, const u32* __restrict__ seg_n, u32 tps, 
 }
 
 // ---------------------------------------------------------------------------------------
+// Phase probe of k_msd_bucket, off by default (tools/msd_phases.py builds the library with -DB2_MSD_PROBE and prints
+// it): thread 0 of every CTA adds the clock64() cycles from one phase boundary to the next over all of its buckets,
+// and at the end adds its sums and its bucket count to g_msd_probe.  A boundary is where thread 0 leaves a barrier, so a
+// phase's cycles are those of the CTA's slowest warp in it.  The sums live in shared memory, not in registers, so the
+// probe build keeps the default build's registers and does not spill.
+#define MB_PHASES 6  // wait for the bucket, histogram, scan + queue, scatter, ordering, write-out
+#ifdef B2_MSD_PROBE
+__device__ unsigned long long g_msd_probe[MB_PHASES + 1];
+#define MB_STAMP(k) do { if (tid == 0) { const long long t_ = clock64(); s.ph[k] += t_ - s.ph[MB_PHASES + 1]; s.ph[MB_PHASES + 1] = t_; } } while (0)
+extern "C" __attribute__((visibility("default"))) int b2_msd_probe(unsigned long long* out) {
+  // out: MB_PHASES cycle sums and the number of buckets, summed over every launch since the last call; resets them
+  unsigned long long zero[MB_PHASES + 1] = {};
+  if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(out, g_msd_probe, sizeof(zero)) != cudaSuccess ||
+      cudaMemcpyToSymbol(g_msd_probe, zero, sizeof(zero)) != cudaSuccess) return -1;
+  return MB_PHASES;
+}
+#else
+#define MB_STAMP(k) do { } while (0)
+#endif
+
 struct MsdBucketSmem {
   __align__(16) u64 buf[2][MB_BUF];
   __align__(16) u32 cnt[MB_CELLS / 2];  // two 16-bit cell counters per word
@@ -188,9 +207,13 @@ struct MsdBucketSmem {
   __align__(8) u64 bar[2];
   u32 w[2], M[2], off[2], st[2];
   u32 nl[4];  // queued cells of 2, 3, 4 records / of more
+#ifdef B2_MSD_PROBE
+  long long ph[MB_PHASES + 2];  // phase sums, buckets, clock64() at the last boundary
+#endif
 };
 
 static_assert(sizeof(MsdBucketSmem) <= 227 * 1024, "bucket sort state must fit the 227 KiB of shared memory a CTA can have");
+
 
 __device__ __forceinline__ u32 cell_of(u32 key) { return key >> (32 - MB_CELL_BITS); }
 
@@ -327,6 +350,12 @@ k_msd_bucket(const u64* __restrict__ rec, const uint4* __restrict__ work, u8* __
   };
   clear_cells();
   __syncthreads();
+#ifdef B2_MSD_PROBE
+  if (tid == 0) {
+    for (int k = 0; k <= MB_PHASES; k++) s.ph[k] = 0;
+    s.ph[MB_PHASES + 1] = clock64();
+  }
+#endif
   for (u32 it = 0;; it++) {
     const u32 i = it & 1u;
     if (s.M[i] == 0) break;
@@ -345,6 +374,7 @@ k_msd_bucket(const u64* __restrict__ rec, const uint4* __restrict__ work, u8* __
       const u32 p = tid + k * MB_THREADS;
       r[k] = p < M ? buf[off + p] : 0ull;
     }
+    MB_STAMP(0);
     // ---- cell histogram (the counters were cleared behind the barrier that ended the last round) ----
 #pragma unroll
     for (int k = 0; k < MB_ITEMS; k++) {
@@ -355,6 +385,7 @@ k_msd_bucket(const u64* __restrict__ rec, const uint4* __restrict__ work, u8* __
       }
     }
     __syncthreads();
+    MB_STAMP(1);
     // ---- exclusive scan of the cell counts (each thread owns 8 words = 16 cells, two 16-bit counts per word, handled
     // two at a time without branches: counts are < 2^14, so "count >= k" is bit 15 of count + (0x8000 - k) in both halves
     // at once).  Cells of one record are flagged (bit 15 of their start): their record is final when it is scattered.
@@ -413,6 +444,7 @@ k_msd_bucket(const u64* __restrict__ rec, const uint4* __restrict__ work, u8* __
       }
     }
     __syncthreads();
+    MB_STAMP(2);
     // ---- scatter (every record of the bucket sits in a register by now).  A record alone in its cell is final: its
     // byte goes straight to the column slice; the others are stored in cell order for the ordering passes. ----
 #pragma unroll
@@ -433,6 +465,7 @@ k_msd_bucket(const u64* __restrict__ rec, const uint4* __restrict__ work, u8* __
       }
     }
     __syncthreads();
+    MB_STAMP(3);
     // ---- ordering passes.  Cells of 2, 3 and 4 records: one thread per cell, a fixed compare-exchange network in
     // registers (the rarer sizes go to the high thread numbers so that no warp collects all the long jobs); larger cells
     // (a handful per bucket on uniform data, the rule on skewed data): one WARP per cell, every lane ranks its records
@@ -452,6 +485,7 @@ k_msd_bucket(const u64* __restrict__ rec, const uint4* __restrict__ work, u8* __
       for (u32 j = tid; j < n2; j += MB_THREADS) small_cell<2>(buf, s.multi[j] & 0xffffu, ob, base, urow, pidx, tie_head, tie_idx, ctl);
     }
     __syncthreads();
+    MB_STAMP(4);
     // ---- the column slice goes out in 16-byte pieces ----
     {
       const u32 first = ust & 15u, last = first + M;
@@ -468,7 +502,15 @@ k_msd_bucket(const u64* __restrict__ rec, const uint4* __restrict__ work, u8* __
     clear_cells();       // the ordering passes are done with their scratch in the counters
     fence_async_smem();  // the generic-proxy writes to this buffer are ordered before the bulk copy that refills it
     __syncthreads();
+    MB_STAMP(5);
+#ifdef B2_MSD_PROBE
+    if (tid == 0) s.ph[MB_PHASES]++;
+#endif
   }
+#ifdef B2_MSD_PROBE
+  if (tid == 0)
+    for (int k = 0; k <= MB_PHASES; k++) atomicAdd(&g_msd_probe[k], (unsigned long long)s.ph[k]);
+#endif
 }
 
 // ---------------------------------------------------------------------------------------
