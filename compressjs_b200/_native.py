@@ -20,6 +20,7 @@ EXPORTS = [
     "b2_bzip2_decompress_partial", "b2_bzip2_decompress_block_partial", "b2_bzip2_table_partial", "b2_bzip2_decompress_blocks",
     "b2_bzip2_compress_stream", "b2_bzip2_decompress_stream", "b2_bzip2_recover", "b2_bzip2_recover_stream",
     "b2_bzip2_compress_flavor", "b2_bzip2_compress_stream_flavor", "b2_bzip2_compress_dev_flavor",
+    "b2_bzip2_decompress_flavor", "b2_bzip2_decompress_partial_flavor", "b2_bzip2_decompress_stream_flavor",
     "b2_bwt_cyclic", "b2_bwt_cyclic_batch", "b2_suffixsort", "b2_bwt_sentinel", "b2_bwt_inverse", "b2_bwtc_compress", "b2_bwtc_compress_unsized", "b2_bwtc_decompress", "b2_crc32_bzip2",
     "b2_bwtc_compress_stream", "b2_bwtc_decompress_stream",
     "b2_bzip2_bound", "b2_bzip2_compress_dev", "b2_bzip2_decompress_dev",
@@ -78,6 +79,7 @@ def lib():
     L.b2_bzip2_compress_dev_flavor.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t, szp, C.c_int]
     for sfx in ("", "_partial"):
         getattr(L, "b2_bzip2_decompress" + sfx).argtypes = [C.c_void_p, C.c_size_t, C.c_int, u8pp, szp]
+        getattr(L, "b2_bzip2_decompress" + sfx + "_flavor").argtypes = [C.c_void_p, C.c_size_t, C.c_int, u8pp, szp, C.c_int]
         getattr(L, "b2_bzip2_decompress_block" + sfx).argtypes = [C.c_void_p, C.c_size_t, C.c_uint64, u8pp, szp]
         getattr(L, "b2_bzip2_table" + sfx).argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.POINTER(C.POINTER(C.c_uint64)),
                                                       C.POINTER(C.POINTER(C.c_uint32)), szp]
@@ -85,6 +87,7 @@ def lib():
                                              C.POINTER(C.POINTER(C.c_uint64)), szp]
     L.b2_bzip2_compress_stream.argtypes = [READ_FN, WRITE_FN, C.c_void_p, C.c_int]
     L.b2_bzip2_decompress_stream.argtypes = [READ_FN, WRITE_FN, C.c_void_p, C.c_int]
+    L.b2_bzip2_decompress_stream_flavor.argtypes = [READ_FN, WRITE_FN, C.c_void_p, C.c_int, C.c_int]
     recp = C.POINTER(C.POINTER(RecoveredBlock))
     L.b2_bzip2_recover.argtypes = [C.c_void_p, C.c_size_t, C.c_int, u8pp, szp, recp, szp]
     L.b2_bzip2_recover_stream.argtypes = [READ_FN, WRITE_FN, C.c_void_p, C.c_int, recp, szp]

@@ -34,7 +34,7 @@ def _error(rc):
     msg = _native.last_error()
     if rc == -100:
         return ValueError(msg or "Invalid block size multiplier")  # `new Error(...)` lib/Bzip2.js:888-890
-    if rc in (Err.NOT_BZIP_DATA, Err.DATA_ERROR, Err.OBSOLETE_INPUT):
+    if rc in (Err.NOT_BZIP_DATA, Err.UNEXPECTED_INPUT_EOF, Err.DATA_ERROR, Err.OBSOLETE_INPUT):
         return Bzip2Error(rc, msg)
     return RuntimeError("libb2bz: %s (code %d)" % (msg, rc))
 
@@ -53,7 +53,8 @@ def _level(props):
     return int(level)
 
 
-# compressFile's encoder flavors (include/b2bz.h B2_BZ2_*): the bytes of compressjs (the default) or of libbz2
+# The flavors (include/b2bz.h B2_BZ2_*): compressFile writes the bytes of compressjs (the default) or of libbz2, and
+# decompressFile reads as compressjs (the default) or as bzip2 -d reads
 FLAVORS = {"compressjs": 0, "libbz2": 1}
 
 
@@ -81,11 +82,11 @@ def _partial(call):
     return _take(L, out, n), err
 
 
-def _file(input, multistream=False):
+def _file(input, multistream=False, flavor=0):
     L = _native.lib()
     data = coerce_input(input)
-    return _partial(lambda out, n: L.b2_bzip2_decompress_partial(
-        data.ctypes.data if data.size else None, data.size, int(bool(multistream)), out, n))
+    return _partial(lambda out, n: L.b2_bzip2_decompress_partial_flavor(
+        data.ctypes.data if data.size else None, data.size, int(bool(multistream)), out, n, flavor))
 
 
 def _block(input, pos):
@@ -141,16 +142,20 @@ class Bzip2:
         return deliver_output(output, _take(L, out, n))
 
     @staticmethod
-    def decompressFile(input, output=None, multistream=False):
+    def decompressFile(input, output=None, multistream=False, *, flavor="compressjs"):
         """lib/Bzip2.js:454-481 (Bunzip.decode).  On a decode error the output receives the bytes decoded before it.
         When input has readByte and output has writeByte, the input is read and the output written as the decode goes,
-        in bounded memory."""
+        in bounded memory.
+        flavor: "compressjs" decodes as compressjs does; "libbz2" as ``bzip2 -d`` does: it decodes randomised blocks,
+        raises errorCode -3 (Err.UNEXPECTED_INPUT_EOF) for a file cut off where a magic is due, ignores trailing
+        garbage behind a member, and rejects two streams compressjs accepts (include/b2bz.h states the rules)."""
+        fl = _flavor(flavor)   # before anything is read
         if is_stream_pair(input, output):
             pump = Pump(input, output)
-            rc = _native.lib().b2_bzip2_decompress_stream(pump.read_fn, pump.write_fn, None, int(bool(multistream)))
+            rc = _native.lib().b2_bzip2_decompress_stream_flavor(pump.read_fn, pump.write_fn, None, int(bool(multistream)), fl)
             pump.check(rc, _error)
             return output
-        return _deliver(output, *_file(input, multistream))
+        return _deliver(output, *_file(input, multistream, fl))
 
     @staticmethod
     def decompressBlock(input, pos, output=None):

@@ -22,6 +22,9 @@ seeks in its input) reads the whole input first.
 one bzip2 stream made of those blocks (Bzip2.recover).  Both are pipe filters; stderr gets one line per lost block and
 a count, and the exit status is 1 when a block was lost.  The output is complete either way.
 
+``-d -t bzip2 --libbz2-decode`` reads .bz2 files as ``bzip2 -d`` does (Bzip2.decompressFile with flavor="libbz2"): every
+member, randomised blocks, trailing garbage ignored, and "Unexpected input EOF" for a truncated file.
+
 Usage errors are found before the GPU library is loaded, so they work on a machine without a GPU.
 """
 import math
@@ -46,6 +49,7 @@ HELP = """
     --libbz2          With -z -t bzip2: write the bytes bzip2 (libbz2) writes
     --recover         With -d -t bzip2: write the bytes of every intact block of a damaged file
     --repair          With -d -t bzip2: write one bzip2 stream of every intact block of a damaged file
+    --libbz2-decode   With -d -t bzip2: read every member as bzip2 -d (libbz2) reads it
     -1                Fastest/largest compression
     -2
     -3
@@ -84,7 +88,7 @@ def _number(s):
 def parse(argv):
     """Returns a dict of the options, or raises UsageError.  --help and --version are returned as 'help'/'version'."""
     opts = {"decompress": False, "compress": False, "block": "-1", "T": None, "levels": set(), "args": [], "libbz2": False,
-            "recover": False, "repair": False}
+            "recover": False, "repair": False, "libbz2-decode": False}
     i = 0
     only_args = False
     while i < len(argv):
@@ -100,7 +104,7 @@ def parse(argv):
             name, eq, val = a[2:].partition("=")
             if name in ("help", "version"):
                 return {name: True}
-            if name in ("decompress", "compress", "libbz2", "recover", "repair") and not eq:
+            if name in ("decompress", "compress", "libbz2", "recover", "repair", "libbz2-decode") and not eq:
                 opts[name] = True
             elif name == "block":
                 if not eq:
@@ -181,6 +185,22 @@ def check_recover(opts):
     if opts["libbz2"]:
         raise UsageError("%s cannot be used with --libbz2" % flag)
     return "repair" if rep else "recover"
+
+
+def check_libbz2_decode(opts):
+    """--libbz2-decode: whether it is given; UsageError when the other options do not allow it (it takes -d -t bzip2
+    and nothing else)."""
+    if not opts["libbz2-decode"]:
+        return False
+    if not opts["decompress"] or opts["compress"] or compressor(opts["T"]) != "bzip2":
+        raise UsageError("--libbz2-decode can only be used with -d -t bzip2")
+    if _number(opts["block"]) >= 0:
+        raise UsageError("--libbz2-decode cannot be used with --block")
+    if opts["recover"] or opts["repair"]:
+        raise UsageError("--libbz2-decode cannot be used with --recover or --repair")
+    if opts["libbz2"]:
+        raise UsageError("--libbz2-decode cannot be used with --libbz2")
+    return True
 
 
 # the reference's messages of the decode failures a lost block has
@@ -294,7 +314,8 @@ class OutStream:
 def stream(kind, decompress, level, in_fd, out, flavor="compressjs"):
     """Without -b: compressFile / decompressFile of `kind` ('bzip2' or 'bwtc') from the descriptor to the binary file
     `out` through the streams of bin/compressjs, in bounded memory.  The exit status; on an error its message is on
-    stderr and `out` has what went out before it (on a decode error: the decoded bytes cut down to a multiple of FLUSH)."""
+    stderr and `out` has what went out before it (on a decode error: the decoded bytes cut down to a multiple of FLUSH).
+    A bzip2 decode of the libbz2 flavor reads every member, as bzip2 -d does."""
     from .bwtc import BWTC
     from .bzip2 import Bzip2
     src, dst = InStream(in_fd), OutStream(out)
@@ -304,6 +325,8 @@ def stream(kind, decompress, level, in_fd, out, flavor="compressjs"):
                 BWTC.decompressFile(src, dst)
             else:
                 BWTC.compressFile(src, dst, level)   # the header's size field comes from src.size
+        elif decompress and flavor == "libbz2":
+            Bzip2.decompressFile(src, dst, True, flavor=flavor)
         elif decompress:
             Bzip2.decompressFile(src, dst)   # without multistream, as bin/compressjs:160-164 calls it
         else:
@@ -350,6 +373,7 @@ def main(argv=None):
         if opts.get("version"):
             sys.stdout.write(VERSION + "\n")
             return 0
+        lb_dec = check_libbz2_decode(opts)
         rec = check_recover(opts)
         decompress, level, block = check(opts)
         args = opts["args"]
@@ -361,7 +385,7 @@ def main(argv=None):
         if rec:
             return recover(in_fd, out, rec == "repair")
         if block < 0:
-            return stream(kind, decompress, level, in_fd, out, "libbz2" if opts["libbz2"] else "compressjs")
+            return stream(kind, decompress, level, in_fd, out, "libbz2" if opts["libbz2"] or lb_dec else "compressjs")
         data, size = read_input(in_fd)
         result, err = run(kind, decompress, level, block, data, size)
         if err is not None:

@@ -579,7 +579,9 @@ static int decode_host(Ctx& c, StreamIn& in, Run run) {
     try {
       run(&produced);
     } catch (const B2Error& e) {
-      if (e.code != B2_ERR_NOT_BZIP_DATA && e.code != B2_ERR_DATA_ERROR && e.code != B2_ERR_OBSOLETE_INPUT) throw;
+      if (e.code != B2_ERR_NOT_BZIP_DATA && e.code != B2_ERR_UNEXPECTED_INPUT_EOF && e.code != B2_ERR_DATA_ERROR &&
+          e.code != B2_ERR_OBSOLETE_INPUT)
+        throw;
       g_err = e.msg;
       rc = e.code;
     }
@@ -683,13 +685,18 @@ int b2_bzip2_compress_stream_flavor(b2_read_fn rd, b2_write_fn wr, void* user, i
 }
 
 int b2_bzip2_decompress_stream(b2_read_fn rd, b2_write_fn wr, void* user, int multistream) {
+  return b2_bzip2_decompress_stream_flavor(rd, wr, user, multistream, B2_BZ2_COMPRESSJS);
+}
+
+int b2_bzip2_decompress_stream_flavor(b2_read_fn rd, b2_write_fn wr, void* user, int multistream, int flavor) {
   return guarded([&]() {
     if (!rd || !wr) throw B2Error{B2_ERR_BAD_ARG, "null callback"};
+    check_flavor(flavor);
     Ctx& c = ctx_locked();
     c.reset_call();
     StreamIn in(rd, user, c.stream);
     StreamOut out(wr, user, c.stream);
-    return decode_host(c, in, [&](size_t* produced) { bzip2_decompress_host(c, in, multistream, out, produced); });
+    return decode_host(c, in, [&](size_t* produced) { bzip2_decompress_host(c, in, multistream, flavor, out, produced); });
   });
 }
 
@@ -875,8 +882,14 @@ int b2_bzip2_encode_range_dev_flavor(const void* d_in, size_t n, int level, size
 }
 
 int b2_bzip2_decompress_partial(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n) {
+  return b2_bzip2_decompress_partial_flavor(in, n, multistream, out, out_n, B2_BZ2_COMPRESSJS);
+}
+
+int b2_bzip2_decompress_partial_flavor(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n, int flavor) {
   return guarded([&]() {
-    return decode_common(in, n, [&](Ctx& c, StreamIn& s, StreamOut& d, size_t* p) { bzip2_decompress_host(c, s, multistream, d, p); }, out, out_n);
+    check_flavor(flavor);
+    return decode_common(in, n, [&](Ctx& c, StreamIn& s, StreamOut& d, size_t* p) { bzip2_decompress_host(c, s, multistream, flavor, d, p); },
+                         out, out_n);
   });
 }
 
@@ -928,8 +941,12 @@ static int drop_on_error(int rc, uint8_t* p, size_t pn, uint8_t** out, size_t* o
 }
 
 int b2_bzip2_decompress(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n) {
+  return b2_bzip2_decompress_flavor(in, n, multistream, out, out_n, B2_BZ2_COMPRESSJS);
+}
+
+int b2_bzip2_decompress_flavor(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n, int flavor) {
   uint8_t* p = nullptr; size_t pn = 0;
-  const int rc = b2_bzip2_decompress_partial(in, n, multistream, &p, &pn);
+  const int rc = b2_bzip2_decompress_partial_flavor(in, n, multistream, &p, &pn, flavor);
   return drop_on_error(rc, p, pn, out, out_n);
 }
 

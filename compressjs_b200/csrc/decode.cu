@@ -23,6 +23,7 @@
 //                    is assembled by copies (only what lies behind a walk's 512-byte record is
 //                    walked again)
 //   bwt_inverse_sentinel_batch: BWT.unbwtransform (lib/BWT.js:352-363) of a batch of blocks on the same walk kernels
+//   k_derand       : libbz2 flavor only: the flipped bytes of randomised blocks, XORed in place before RLE1 decode
 //   k_unrle_*      : RLE1 decode (lib/Bzip2.js:424-436): count bytes are identified from local
 //                    synchronisation points (8 bytes per thread, decided in registers), output
 //                    offsets from tile sums + one warp scan per block, tiles expanded in shared
@@ -47,6 +48,7 @@
 #define SEL_CAP 32768
 #define DEC_OK 0
 #define DEC_NOT_BZIP (-2)
+#define DEC_EOF (-3)
 #define DEC_DATA_ERROR (-5)
 #define DEC_OBSOLETE (-7)
 
@@ -65,6 +67,8 @@ struct CandRes {
   u32 n;           // block length after un-MTF (filled later)
   u32 rawlen;      // bytes after RLE1 decode (filled later)
   u32 open;        // 1 = decoding it read up to the end of an input window that is not the end of the file: not final
+  u32 rand;        // libbz2 flavor only: the randomised bit is set (the compressjs flavor fails the block instead)
+  u32 run4;        // the pre-RLE1 bytes end on the fourth byte of a run, without its count byte (k_unrle_tileoff)
   u64 endbit;      // bit position just behind the EOB code
   u8 sym_to_byte[256];
 };
@@ -207,7 +211,10 @@ __device__ __noinline__ u32 hdec_slow(const HdecWarp& s, u32 g, u32 bits20, int 
 // The input is a window of nbytes bytes that starts at bit base_bit of the file (a multiple of 32) and is zero padded
 // behind; candidate positions and endbit are bits of the file.  A result that depends on no bit at or past the window's
 // end is what the whole file gives; any other is marked open unless the window ends where the file does (`last`).
-template <int HD_T>
+// LB (the libbz2 flavor) decodes a randomised block (its bytes are derandomised after the inverse BWT: k_derand) and
+// rejects a selector MTF code of groupCount ones, as libbz2 does; without it this is the reference's decoder, which
+// leaves `rand` unset.  A template argument, so that the compressjs flavor's kernel is compiled as before.
+template <int HD_T, bool LB>
 __global__ void __launch_bounds__(HD_T, HD_T == 128 ? 10 : 1152 / HD_T)
 k_hdec(const u8* __restrict__ in, u64 nbytes, u64 base_bit, u32 last, const Cand* __restrict__ cands, u32 count, u32 dbuf_size,
        u8* __restrict__ sel_buf, u16* __restrict__ sym_out, CandRes* __restrict__ res) {
@@ -227,7 +234,8 @@ k_hdec(const u8* __restrict__ in, u64 nbytes, u64 base_bit, u32 last, const Cand
     r->detail = 0; r->m = 0; r->n = 0; r->rawlen = 0; r->endbit = 0;
     br.init(in, nbytes, cd.pos - base_bit + 48 + 32);
     do {
-      if (br.get(1)) { s.status = DEC_OBSOLETE; break; }           // lib/Bzip2.js:143
+      if (LB) r->rand = br.get(1);
+      else if (br.get(1)) { s.status = DEC_OBSOLETE; break; }           // lib/Bzip2.js:143
       const u32 orig = br.get(24);
       r->orig = orig;
       if (orig > dbuf_size) { s.status = DEC_DATA_ERROR; r->detail = 1; break; }  // :146
@@ -246,9 +254,10 @@ k_hdec(const u8* __restrict__ in, u64 nbytes, u64 base_bit, u32 last, const Cand
       u8 mtf[HUFF_MAXGROUPS + 2];  // the reference's list is a zero-filled 256-entry buffer: slot gc reads as 0
       for (u32 i = 0; i < HUFF_MAXGROUPS + 2; i++) mtf[i] = (u8)(i < gc ? i : 0);
       bool bad = false;
+      const u32 jmax = LB ? gc - 1 : gc;  // the most ones a selector's MTF code may have
       for (u32 i = 0; i < ns && !bad; i++) {
         u32 j = 0;
-        while (br.get(1)) { if (j >= gc) { bad = true; break; } j++; }   // :184-185
+        while (br.get(1)) { if (j >= jmax) { bad = true; break; } j++; }   // :184-185
         if (bad) break;
         const u8 v = mtf[j];
         for (u32 k = j; k > 0; k--) mtf[k] = mtf[k - 1];
@@ -873,7 +882,7 @@ __global__ void k_unbwt_setup(CandRes* res, const u32* __restrict__ d_n, u32 nb)
   if (b >= nb) return;
   CandRes* r = res + b;
   const u32 n = d_n[b];
-  r->status = 0; r->detail = 0; r->m = 0; r->orig = SEG_SIZE - 1; r->sym_total = 0; r->n = n; r->rawlen = n; r->open = 0; r->endbit = 0;
+  r->status = 0; r->detail = 0; r->m = 0; r->orig = SEG_SIZE - 1; r->sym_total = 0; r->n = n; r->rawlen = n; r->open = 0; r->rand = 0; r->run4 = 0; r->endbit = 0;
 }
 // the walks write each block back to front into its slot; the blocks go out front to back and back to back
 __global__ void k_reverse_blocks(const u8* __restrict__ in, const u32* __restrict__ d_n, const u64* __restrict__ d_off, u8* __restrict__ out) {
@@ -884,9 +893,8 @@ __global__ void k_reverse_blocks(const u8* __restrict__ in, const u32* __restric
 static void dec_attr_once() {
   static bool attr = false;
   if (attr) return;
-  CUDA_CHECK(cudaFuncSetAttribute(k_hdec<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HdecWarp)));
-  CUDA_CHECK(cudaFuncSetAttribute(k_hdec<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HdecWarp)));
-  CUDA_CHECK(cudaFuncSetAttribute(k_hdec<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HdecWarp)));
+  for (auto k : {k_hdec<128, false>, k_hdec<256, false>, k_hdec<512, false>, k_hdec<128, true>, k_hdec<256, true>, k_hdec<512, true>})
+    CUDA_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HdecWarp)));
   CUDA_CHECK(cudaFuncSetAttribute(k_ibwt_chain, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(Seg) * IB_SEGS)));
   attr = true;
 }
@@ -938,7 +946,7 @@ __device__ __forceinline__ bool unrle_sync(const u8* b, u32 i) {
   if (i >= 4 && b[i - 1] == b[i - 2] && b[i - 2] == b[i - 3] && b[i - 3] == b[i - 4]) return false;
   return true;
 }
-// the reference's loop (lib/Bzip2.js:424-436) from a synchronisation point i to the next one: cls[j] = 1 for repeat counts
+// the reference's loop (lib/Bzip2.js:424-436) from a synchronisation point i to the next one: cls[j] = 1 for repeat counts.
 __device__ __noinline__ void unrle_walk(const u8* __restrict__ b, u8* __restrict__ c, u32 i, u32 n) {
   u32 j = i, run = 0;
   int prev = -1;
@@ -1009,6 +1017,65 @@ __global__ void __launch_bounds__(256) k_unrle_classify(const u8* __restrict__ r
   }
 }
 
+// ---- derandomise (libbz2 flavor) ----------------------------------------------------------------
+// libbz2's BZ2_rNums: the gaps between the flipped bytes of a randomised block (bzip2 0.9.0 and older wrote them).
+static const int RNUMS[512] = {
+    619, 720, 127, 481, 931, 816, 813, 233, 566, 247, 985, 724, 205, 454, 863, 491, 741, 242, 949, 214, 733, 859, 335, 708,
+    621, 574, 73,  654, 730, 472, 419, 436, 278, 496, 867, 210, 399, 680, 480, 51,  878, 465, 811, 169, 869, 675, 611, 697,
+    867, 561, 862, 687, 507, 283, 482, 129, 807, 591, 733, 623, 150, 238, 59,  379, 684, 877, 625, 169, 643, 105, 170, 607,
+    520, 932, 727, 476, 693, 425, 174, 647, 73,  122, 335, 530, 442, 853, 695, 249, 445, 515, 909, 545, 703, 919, 874, 474,
+    882, 500, 594, 612, 641, 801, 220, 162, 819, 984, 589, 513, 495, 799, 161, 604, 958, 533, 221, 400, 386, 867, 600, 782,
+    382, 596, 414, 171, 516, 375, 682, 485, 911, 276, 98,  553, 163, 354, 666, 933, 424, 341, 533, 870, 227, 730, 475, 186,
+    263, 647, 537, 686, 600, 224, 469, 68,  770, 919, 190, 373, 294, 822, 808, 206, 184, 943, 795, 384, 383, 461, 404, 758,
+    839, 887, 715, 67,  618, 276, 204, 918, 873, 777, 604, 560, 951, 160, 578, 722, 79,  804, 96,  409, 713, 940, 652, 934,
+    970, 447, 318, 353, 859, 672, 112, 785, 645, 863, 803, 350, 139, 93,  354, 99,  820, 908, 609, 772, 154, 274, 580, 184,
+    79,  626, 630, 742, 653, 282, 762, 623, 680, 81,  927, 626, 789, 125, 411, 521, 938, 300, 821, 78,  343, 175, 128, 250,
+    170, 774, 972, 275, 999, 639, 495, 78,  352, 126, 857, 956, 358, 619, 580, 124, 737, 594, 701, 612, 669, 112, 134, 694,
+    363, 992, 809, 743, 168, 974, 944, 375, 748, 52,  600, 747, 642, 182, 862, 81,  344, 805, 988, 739, 511, 655, 814, 334,
+    249, 515, 897, 955, 664, 981, 649, 113, 974, 459, 893, 228, 433, 837, 553, 268, 926, 240, 102, 654, 459, 51,  686, 754,
+    806, 760, 493, 403, 415, 394, 687, 700, 946, 670, 656, 610, 738, 392, 760, 799, 887, 653, 978, 321, 576, 617, 626, 502,
+    894, 679, 243, 440, 680, 879, 194, 572, 640, 724, 926, 56,  204, 700, 707, 151, 457, 449, 797, 195, 791, 558, 945, 679,
+    297, 59,  87,  824, 713, 663, 412, 693, 342, 606, 134, 108, 571, 364, 631, 212, 174, 643, 304, 329, 343, 97,  430, 751,
+    497, 314, 983, 374, 822, 928, 140, 206, 73,  263, 980, 736, 876, 478, 430, 305, 170, 514, 364, 692, 829, 82,  855, 953,
+    676, 246, 369, 970, 294, 750, 807, 827, 150, 790, 288, 923, 804, 378, 215, 828, 592, 281, 565, 555, 710, 82,  896, 831,
+    547, 261, 524, 462, 293, 465, 502, 56,  661, 821, 976, 991, 658, 869, 905, 758, 745, 193, 768, 550, 608, 933, 378, 286,
+    215, 979, 792, 961, 61,  688, 793, 644, 986, 403, 106, 366, 905, 644, 372, 567, 466, 434, 645, 210, 389, 550, 919, 135,
+    780, 773, 635, 389, 707, 100, 626, 958, 165, 504, 920, 176, 193, 713, 857, 265, 203, 50,  668, 108, 645, 990, 626, 197,
+    510, 357, 358, 850, 858, 364, 936, 638};
+#define DR_FLIPS 1655  // flipped bytes below 900 000 (the largest block)
+__constant__ u32 c_flips[DR_FLIPS];
+
+// The positions libbz2 XORs with 1 in a randomised block's pre-RLE1 bytes: togo counts down from rNums[t], t cycling
+// through the table, and the byte where togo reaches 1 is flipped.  __constant__ memory belongs to a device's context,
+// so the table is uploaded once per device (b2_init may bind another device after b2_shutdown; the library never
+// resets a device, so a device's copy stays valid).
+static void derand_table_once(int device) {
+  static std::vector<bool> done;
+  if (device < (int)done.size() && done[device]) return;
+  std::vector<u32> f;
+  int togo = 0, t = 0;
+  for (u32 i = 0; i < 900000u; i++) {
+    if (togo == 0) { togo = RNUMS[t]; t = (t + 1) & 511; }
+    if (--togo == 1) f.push_back(i);
+  }
+  if (f.size() != DR_FLIPS) throw B2Error{B2_ERR_CUDA, "derandomise table has the wrong length"};
+  CUDA_CHECK(cudaMemcpyToSymbol(c_flips, f.data(), sizeof(u32) * DR_FLIPS));
+  if (device >= (int)done.size()) done.resize(device + 1, false);
+  done[device] = true;
+}
+
+// One thread per (block, flip): the flipped bytes of every randomised block are XORed in place in its slot, before the
+// count bytes are classified, so that everything behind (classes, lengths, expansion, CRC) sees derandomised bytes.
+__global__ void k_derand(u8* __restrict__ rle, const CandRes* __restrict__ res, u32 ncand) {
+  const u32 g = blockIdx.x * blockDim.x + threadIdx.x;
+  const u32 ci = g / DR_FLIPS, f = g % DR_FLIPS;
+  if (ci >= ncand) return;
+  const CandRes* r = res + ci;
+  if (r->status != 0 || !r->rand) return;
+  const u32 p = c_flips[f];
+  if (p < r->n) rle[((size_t)ci << SEG_SHIFT) + p] ^= 1u;
+}
+
 // expanded size of every tile (no chain between tiles: the per-block scan below is a separate, tiny kernel)
 __global__ void __launch_bounds__(UR_THREADS)
 k_unrle_tilesum(const u8* __restrict__ rle, const u8* __restrict__ cls, const CandRes* __restrict__ res, u32 tps, u32* __restrict__ tilesum) {
@@ -1040,9 +1107,12 @@ k_unrle_tilesum(const u8* __restrict__ rle, const u8* __restrict__ cls, const Ca
     if (tid == 0) tilesum[(size_t)ci * tps + lt] = v;
   }
 }
-// one warp per block: output offset of every tile, decoded size of the block
+// one warp per block: output offset of every tile, decoded size of the block, and run4: the last four bytes are equal
+// and none is a count byte.  The serial loop's run then counts four at the end (the byte in front of them is another
+// value or a count byte: five equal literals cannot occur), and libbz2 wants the count byte behind them.
 __global__ void __launch_bounds__(32)
-k_unrle_tileoff(CandRes* __restrict__ res, u32 tps, const u32* __restrict__ tilesum, u32* __restrict__ tileoff) {
+k_unrle_tileoff(const u8* __restrict__ rle, const u8* __restrict__ cls, CandRes* __restrict__ res, u32 tps, const u32* __restrict__ tilesum,
+                u32* __restrict__ tileoff) {
   const u32 ci = blockIdx.x, lane = threadIdx.x;
   CandRes* r = res + ci;
   if (r->status != 0) return;
@@ -1056,7 +1126,16 @@ k_unrle_tileoff(CandRes* __restrict__ res, u32 tps, const u32* __restrict__ tile
     if (t < nt) tileoff[(size_t)ci * tps + t] = run + inc - v;
     run += __shfl_sync(FULL_MASK, inc, 31);
   }
-  if (lane == 0) r->rawlen = run;
+  if (lane == 0) {
+    r->rawlen = run;
+    u32 run4 = 0;
+    if (n >= 4) {
+      const u8* b = rle + ((size_t)ci << SEG_SHIFT) + (n - 4);
+      const u8* c = cls + ((size_t)ci << SEG_SHIFT) + (n - 4);
+      run4 = b[0] == b[1] && b[1] == b[2] && b[2] == b[3] && !(c[0] | c[1] | c[2] | c[3]);
+    }
+    r->run4 = run4;
+  }
 }
 
 __global__ void __launch_bounds__(UR_THREADS)
@@ -1177,7 +1256,7 @@ struct DecScratch {
 // file; `last`: the window ends with the file) through the Huffman stage, un-MTF, the inverse BWT (into the slots at rle)
 // and the RLE1 length scan (count-byte classes into the slots at cls, tile offsets into tileoff).  Results in rb on the
 // device and in hres on the host.
-static void dec_batch(Ctx& c, DecScratch& B, const u8* in, u64 wbytes, u64 base_bit, bool last, const Cand* dcand, u32 cnt,
+static void dec_batch(Ctx& c, DecScratch& B, const u8* in, u64 wbytes, u64 base_bit, bool last, const Cand* dcand, u32 cnt, int flavor,
                       CandRes* rb, CandRes* hres, u8* rle, u8* cls, u32* tileoff) {
   // The kernels decode every candidate under the largest block size: the members of a multistream file may have
   // different levels (lib/Bzip2.js:105-124 re-reads the level per member), and which member a candidate belongs to is
@@ -1191,9 +1270,11 @@ static void dec_batch(Ctx& c, DecScratch& B, const u8* in, u64 wbytes, u64 base_
     StageScope ss(c, ST_HDEC);
     static int sms = 0;
     if (!sms) CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c.device));
-    if (cnt <= 2u * (u32)sms) k_hdec<512><<<cnt, 512, sizeof(HdecWarp), c.stream>>>(in, wbytes, base_bit, last, dcand, cnt, dbuf_size, B.selbuf, B.sym, rb);
-    else if (cnt <= 4u * (u32)sms) k_hdec<256><<<cnt, 256, sizeof(HdecWarp), c.stream>>>(in, wbytes, base_bit, last, dcand, cnt, dbuf_size, B.selbuf, B.sym, rb);
-    else k_hdec<HD_THREADS><<<cnt, HD_THREADS, sizeof(HdecWarp), c.stream>>>(in, wbytes, base_bit, last, dcand, cnt, dbuf_size, B.selbuf, B.sym, rb);
+    const bool lb = flavor == B2_BZ2_LIBBZ2;
+    const u32 t = cnt <= 2u * (u32)sms ? 512 : cnt <= 4u * (u32)sms ? 256 : HD_THREADS;
+    auto k = t == 512 ? (lb ? k_hdec<512, true> : k_hdec<512, false>)
+           : t == 256 ? (lb ? k_hdec<256, true> : k_hdec<256, false>) : (lb ? k_hdec<HD_THREADS, true> : k_hdec<HD_THREADS, false>);
+    k<<<cnt, t, sizeof(HdecWarp), c.stream>>>(in, wbytes, base_bit, last, dcand, cnt, dbuf_size, B.selbuf, B.sym, rb);
     KLAUNCH(c); KCHECK();
   }
   {
@@ -1228,11 +1309,16 @@ static void dec_batch(Ctx& c, DecScratch& B, const u8* in, u64 wbytes, u64 base_
   if (nmax) {
     StageScope ss(c, ST_UNRLE);
     const u32 nslots = cnt << SEG_SHIFT;
+    if (flavor == B2_BZ2_LIBBZ2 && std::any_of(hres, hres + cnt, [](const CandRes& r) { return r.status == 0 && r.rand; })) {
+      derand_table_once(c.device);
+      k_derand<<<(cnt * DR_FLIPS + 255) / 256, 256, 0, c.stream>>>(rle, rb, cnt);
+      KLAUNCH(c); KCHECK();
+    }
     k_unrle_classify<<<(nslots / 8 + 255) / 256, 256, 0, c.stream>>>(rle, rb, cnt, cls);
     KLAUNCH(c); KCHECK();
     k_unrle_tilesum<<<cnt * ur_tps, UR_THREADS, 0, c.stream>>>(rle, cls, rb, ur_tps, B.tilesum);
     KLAUNCH(c); KCHECK();
-    k_unrle_tileoff<<<cnt, 32, 0, c.stream>>>(rb, ur_tps, B.tilesum, tileoff);
+    k_unrle_tileoff<<<cnt, 32, 0, c.stream>>>(rle, cls, rb, ur_tps, B.tilesum, tileoff);
     KLAUNCH(c); KCHECK();
     CUDA_CHECK(cudaMemcpyAsync(hres, rb, sizeof(CandRes) * cnt, cudaMemcpyDeviceToHost, c.stream));
   }
@@ -1251,11 +1337,11 @@ struct DecIn {
   DecIn(const u8* d_in, size_t n_) : d(d_in), n(n_) {}
   size_t length() const { return s ? (s->eof ? s->base + s->have : SIZE_MAX) : n; }  // a stream's once it has ended
   u64 end() const { return s ? s->base + s->have : n; }  // the end of the bytes there are so far
-  // Up to 4 bytes at bytepos (a member header) into h; returns how many there are.  The header may lie past the window:
-  // a stream reads one byte more, which tells whether the input ends behind it.
-  size_t head(Ctx& c, u64 bytepos, u8* h) {
-    if (s) s->fill(bytepos + 5);
-    const size_t avail = (size_t)std::min<u64>(4, end() - bytepos);
+  // Up to k bytes at bytepos (a member header, or a magic the input may cut off) into h; returns how many there are.  They
+  // may lie past the window: a stream reads one byte more, which tells whether the input ends behind them.
+  size_t head(Ctx& c, u64 bytepos, u8* h, size_t k = 4) {
+    if (s) s->fill(bytepos + k + 1);
+    const size_t avail = (size_t)std::min<u64>(k, end() - bytepos);
     if (s) {
       memcpy(h, s->at(bytepos), avail);
     } else {
@@ -1288,6 +1374,7 @@ struct DecIn {
 // ---- the block chain (lib/Bzip2.js:454-481 / 508-548) ----
 struct Chain {
   int multistream = 0;
+  int flavor = B2_BZ2_COMPRESSJS;  // B2_BZ2_LIBBZ2: the rules of include/b2bz.h's b2_bzip2_decompress_flavor
   u32 cur_dbuf = 0;         // dbufSize of the member the walk is in (lib/Bzip2.js:121)
   u64 pos = 32;             // bit position of the next magic
   u32 stream_crc = 0;
@@ -1311,6 +1398,10 @@ static bool block_event(Chain& ch, const Cand& cd, const CandRes& r, size_t slot
     return false;
   }
   if (r.n > ch.cur_dbuf) {  // dbufCount would have run over dbufSize (lib/Bzip2.js:338,354)
+    ch.events.push_back({2, slot, 0, 0, DEC_DATA_ERROR, "Data error", ch.total_out, 0, 0});
+    return false;
+  }
+  if (ch.flavor == B2_BZ2_LIBBZ2 && r.run4) {  // libbz2 wants the count byte of the last run of four
     ch.events.push_back({2, slot, 0, 0, DEC_DATA_ERROR, "Data error", ch.total_out, 0, 0});
     return false;
   }
@@ -1415,7 +1506,7 @@ struct Decode {
     std::vector<Cand> bc(n);
     for (u32 i = 0; i < n; i++) bc[i] = cands[blk[j0 + i]];
     CUDA_CHECK(cudaMemcpyAsync(dcand, bc.data(), sizeof(Cand) * n, cudaMemcpyHostToDevice, c.stream));
-    dec_batch(c, B, win, wl, a * 8, last, dcand, n, dres.p + s0, h, rle.p + (s0 << SEG_SHIFT), cls.p + (keep_cls ? s0 << SEG_SHIFT : 0),
+    dec_batch(c, B, win, wl, a * 8, last, dcand, n, ch.flavor, dres.p + s0, h, rle.p + (s0 << SEG_SHIFT), cls.p + (keep_cls ? s0 << SEG_SHIFT : 0),
               tileoff.p + s0 * UR_TPS);
   }
   // Expand the slots of [s0, s1) whose ob is not ~0 (RLE1 decode) to dout + ob, and CRC each into got; hres, ob and got
@@ -1462,12 +1553,39 @@ struct Decode {
   }
 };
 
+// libbz2 flavor: does the input end before the 80 bits (magic + CRC) at bit pos, with every whole byte from pos on agreeing
+// with the start of a block or end-of-stream magic?  libbz2 reads a magic a byte at a time, so a part byte never differs.
+// Only an input whose length is known can be cut off there; a stream that has not ended yet has at least 80 more bits
+// once a window is found to hold pos + 80.
+static bool cut_magic(Decode& R, u64 pos) {
+  const u64 len = R.in.length();
+  if (len == SIZE_MAX || pos + 80 <= len * 8) return false;
+  const u64 bits = len * 8 > pos ? len * 8 - pos : 0;
+  const u32 groups = (u32)std::min<u64>(bits / 8, 6);  // whole bytes of the magic (the CRC behind it always agrees)
+  if (!groups) return true;
+  u8 h[7] = {0};
+  const size_t got = R.in.head(R.c, pos >> 3, h, 7);
+  const u32 sh = (u32)(pos & 7);
+  bool blk = true, eos = true;
+  for (u32 k = 0; k < groups; k++) {
+    const u32 hi = k < got ? h[k] : 0, lo = k + 1 < got ? h[k + 1] : 0;
+    const u8 v = (u8)(((hi << 8 | lo) << sh) >> 8);
+    blk = blk && v == (u8)(WHOLEPI >> (40 - 8 * k));
+    eos = eos && v == (u8)(SQRTPI >> (40 - 8 * k));
+  }
+  return blk || eos;
+}
+
 // Walk R's chain from ch.pos over the sorted magics as far as the batch has final results (block candidate j of the batch
 // is in slot j - kb).  Returns true when the walk stopped for input behind the device window: a magic the window's end
 // (bit end_bit) may cut off, or a block whose decode reached that end.
 static bool chain_walk(Decode& R, u64 end_bit) {
   Chain& ch = R.ch;
+  const bool lb = ch.flavor == B2_BZ2_LIBBZ2;
   while (!ch.done) {
+    if (lb && cut_magic(R, ch.pos)) {
+      ch.events.push_back({2, 0, 0, 0, DEC_EOF, "Unexpected input EOF", ch.total_out, 0, 0}); ch.done = true; break;
+    }
     if ((ch.pos + 7) / 8 >= R.in.length()) { ch.done = true; break; }  // 'eof' in inputStream && inputStream.eof() (lib/Bzip2.js:462)
     const auto it = std::lower_bound(R.cands.begin(), R.cands.end(), ch.pos, [](const Cand& x, u64 p) { return x.pos < p; });
     if (it == R.cands.end() || it->pos != ch.pos) {
@@ -1491,6 +1609,14 @@ static bool chain_walk(Decode& R, u64 end_bit) {
     // _start_bunzip on the byte stream (resyncs to the next byte)
     u8 h2[4] = {0, 0, 0, 0};
     const size_t avail = R.in.head(R.c, bytepos, h2);
+    if (lb) {
+      // bzip2 -d: a tail that is not the start of "BZh1".."BZh9" is ignored; a cut-off header is a truncated file
+      const char want[3] = {'B', 'Z', 'h'};
+      bool match = true;
+      for (size_t k = 0; k < avail; k++) match = match && (k < 3 ? h2[k] == (u8)want[k] : h2[k] >= '1' && h2[k] <= '9');
+      if (!match) { ch.done = true; break; }
+      if (avail < 4) { ch.events.push_back({2, 0, 0, 0, DEC_EOF, "Unexpected input EOF", ch.total_out, 0, 0}); ch.done = true; break; }
+    }
     if (avail != 4 || h2[0] != 'B' || h2[1] != 'Z' || h2[2] != 'h') {
       ch.events.push_back({2, 0, 0, 0, DEC_NOT_BZIP, "Not bzip data: bad magic", ch.total_out, 0, 0}); ch.done = true; break;
     }
@@ -1673,9 +1799,10 @@ void bzip2_decompress_size(Ctx& c, const u8* d_in, size_t n, int multistream, si
   R.finish(out_n, 0);
 }
 
-void bzip2_decompress_host(Ctx& c, StreamIn& in, int multistream, StreamOut& out, size_t* out_n) {
+void bzip2_decompress_host(Ctx& c, StreamIn& in, int multistream, int flavor, StreamOut& out, size_t* out_n) {
   *out_n = 0;
   Decode R(c, DecIn(in));
+  R.ch.flavor = flavor;
   chain_decode(R, multistream, false, [&](size_t e0, size_t e1) { deliver_host(R, e0, e1, out); });
   R.finish(out_n, R.E.prefix);
 }

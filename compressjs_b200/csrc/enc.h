@@ -170,8 +170,8 @@ void bzip2_decompress_dev(Ctx& c, const u8* d_in, size_t n, int multistream, u8*
 // b2_bzip2_decompress_dev without an output buffer: the blocks are expanded only for their CRCs.
 void bzip2_decompress_size(Ctx& c, const u8* d_in, size_t n, int multistream, size_t* out_n);
 // b2_bzip2_decompress_partial and b2_bzip2_decompress_stream: into `out`, which never receives a byte past the prefix the
-// reference writes before an error (*out_n on an error).
-void bzip2_decompress_host(Ctx& c, StreamIn& in, int multistream, StreamOut& out, size_t* out_n);
+// reference writes before an error (*out_n on an error).  flavor B2_BZ2_LIBBZ2 reads as libbz2 reads (b2_bzip2_decompress_flavor).
+void bzip2_decompress_host(Ctx& c, StreamIn& in, int multistream, int flavor, StreamOut& out, size_t* out_n);
 // What the replay of a table or a position list records in front of the first failure: per block its bit position and
 // decoded length (the table rows), and per position the end of its bytes in the output (the list ends).
 struct DecRows { std::vector<u64> pos, ends; std::vector<u32> len; };

@@ -51,15 +51,16 @@ static napi_value decoded(napi_env env, int rc, uint8_t* out, size_t out_n) {
   if (rc) return fail(env, rc, "partial", buf);
   return buf;
 }
-// decompressFile(buffer, multistream) -> Buffer    (Bunzip.decode, lib/Bzip2.js:454)
+// decompressFile(buffer, multistream, flavor) -> Buffer    (Bunzip.decode, lib/Bzip2.js:454; flavor: B2_BZ2_*, default 0)
 static napi_value DecompressFile(napi_env env, napi_callback_info info) {
-  size_t argc = 2; napi_value argv[2];
+  size_t argc = 3; napi_value argv[3];
   napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr);
-  const uint8_t* in; size_t n; bool ms = false;
+  const uint8_t* in; size_t n; bool ms = false; int32_t flavor = B2_BZ2_COMPRESSJS;
   if (!buf_arg(env, argv[0], &in, &n)) return fail(env, B2_ERR_BAD_ARG);
   if (argc > 1) napi_get_value_bool(env, argv[1], &ms);
+  if (argc > 2) napi_get_value_int32(env, argv[2], &flavor);
   uint8_t* out = nullptr; size_t out_n = 0;
-  int rc = b2_bzip2_decompress_partial(in, n, ms ? 1 : 0, &out, &out_n);
+  int rc = b2_bzip2_decompress_partial_flavor(in, n, ms ? 1 : 0, &out, &out_n, flavor);
   return decoded(env, rc, out, out_n);
 }
 // decompressBlock(buffer, bitpos) -> Buffer        (Bunzip.decodeBlock, lib/Bzip2.js:482)

@@ -43,18 +43,24 @@ function decode(output, call) {
 }
 
 var Bzip2 = Object.create(null);
-// options.flavor: 'compressjs' (the default) or 'libbz2' (the bytes bzip2 -N writes; include/b2bz.h B2_BZ2_LIBBZ2)
+// options.flavor: 'compressjs' (the default) or 'libbz2': compressFile writes the bytes bzip2 -N writes, decompressFile
+// reads as bzip2 -d reads (include/b2bz.h B2_BZ2_LIBBZ2)
 var FLAVORS = { compressjs: 0, libbz2: 1 };
-Bzip2.compressFile = function(inStream, outStream, props, options) {
+function flavor(options) {
   var name = (options && options.flavor !== undefined) ? options.flavor : 'compressjs';
   if (!Object.prototype.hasOwnProperty.call(FLAVORS, name)) { throw new Error('unknown bzip2 flavor ' + name); }
+  return FLAVORS[name];
+}
+Bzip2.compressFile = function(inStream, outStream, props, options) {
+  var fl = flavor(options);
   var level = (typeof props === 'number') ? props : 9;
   if (level < 1 || level > 9) { throw new Error('Invalid block size multiplier'); }
-  return deliver(outStream, native.compressFile(drain(inStream), level, FLAVORS[name]));
+  return deliver(outStream, native.compressFile(drain(inStream), level, fl));
 };
-Bzip2.decompressFile = function(input, output, multistream) {
+Bzip2.decompressFile = function(input, output, multistream, options) {
+  var fl = flavor(options);   // before anything is read
   var data = drain(input);
-  return decode(output, function() { return native.decompressFile(data, !!multistream); });
+  return decode(output, function() { return native.decompressFile(data, !!multistream, fl); });
 };
 Bzip2.decompressBlock = function(input, pos, output) {
   var data = drain(input);

@@ -8,7 +8,7 @@
  *
  * Conventions
  *   - return value 0 = OK; negative = the reference's Bunzip.Err code
- *     (lib/Bzip2.js:62-72: -2 NOT_BZIP_DATA, -5 DATA_ERROR, -7 OBSOLETE_INPUT) or
+ *     (lib/Bzip2.js:62-72: -2 NOT_BZIP_DATA, -3 UNEXPECTED_INPUT_EOF, -5 DATA_ERROR, -7 OBSOLETE_INPUT) or
  *     B2_ERR_* below.  b2_last_error() returns the reference's message text.
  *   - inputs are borrowed for the duration of the call; outputs are allocated by the
  *     library in pinned host memory and released with b2_free().
@@ -29,6 +29,7 @@ extern "C" {
 
 #define B2_OK 0
 #define B2_ERR_NOT_BZIP_DATA (-2) /* lib/Bzip2.js:66 */
+#define B2_ERR_UNEXPECTED_INPUT_EOF (-3) /* lib/Bzip2.js:66,76; only the libbz2 decoder flavor returns it */
 #define B2_ERR_DATA_ERROR (-5)    /* lib/Bzip2.js:69 */
 #define B2_ERR_OBSOLETE_INPUT (-7) /* lib/Bzip2.js:71 */
 #define B2_ERR_BAD_LEVEL (-100)   /* lib/Bzip2.js:888-890 "Invalid block size multiplier" */
@@ -254,6 +255,36 @@ uint32_t b2_crc32_bzip2(const uint8_t* p, size_t n);
 int b2_bzip2_compress_flavor(const uint8_t* in, size_t n, int level, uint8_t** out, size_t* out_n, int flavor);
 int b2_bzip2_compress_stream_flavor(b2_read_fn rd, b2_write_fn wr, void* user, int level, int flavor);
 int b2_bzip2_compress_dev_flavor(const void* d_in, size_t n, int level, void* d_out, size_t out_cap, size_t* out_n, int flavor);
+
+/* ---- decoder flavors --------------------------------------------------------------------------------------------
+ * B2_BZ2_COMPRESSJS is the decoder of every call without a flavor: compressjs' Bunzip.decode.  B2_BZ2_LIBBZ2 reads
+ * .bz2 files as bzip2 -d (libbz2 1.0.x) reads them.  It is the same decoder with these rules and nothing else changed:
+ * every other check, code, message and partial-output prefix is the compressjs flavor's, and where both reject an
+ * input they reject it with the same code and message.
+ *   R1  A block with the randomised bit set (bzip2 0.9.0 and older wrote them) is decoded instead of failing with -7.
+ *       Its bytes before RLE1 decoding (the inverse BWT's output, count bytes included, index i from 0 in each block)
+ *       are XORed with libbz2's mask: togo = 0, t = 0; for each i: if togo == 0 { togo = BZ2_rNums[t]; t = (t+1) % 512 };
+ *       togo -= 1; byte[i] ^= (togo == 1).  The block CRC is checked on the derandomised bytes.
+ *   R2  A selector MTF code of groupCount ones is -5 "Data error" (the compressjs flavor first rejects groupCount + 1).
+ *   R3  A block whose bytes before RLE1 decoding (after R1) end on the fourth equal byte of a run, without the count byte
+ *       behind it (a count byte restarts the run), is -5 "Data error", and none of its bytes are delivered.
+ *   R4  Where the chain expects a block magic or an end-of-stream magic, an input that ends before the 80 bits of magic
+ *       and CRC are complete, with every whole byte from there on agreeing with the start of either 48-bit magic, is
+ *       -3 "Unexpected input EOF".  This covers an input that ends right there (a file cut behind a block, a bare
+ *       "BZh9") and a cut inside a magic or the stream CRC.  libbz2 reads magics a byte at a time, so bits short of a
+ *       byte never disagree.  Truncation inside a block stays -5.
+ *   R5  With multistream, behind a complete member: the remaining bytes, up to four, are compared with "BZh" and a
+ *       level digit 1-9.  Nothing left: done.  All four match: the next member.  Fewer than four left, all matching: -3.
+ *       Any byte differs (zero padding, "BZh0", a signature, ...): the rest is ignored and the decode succeeds.  Without
+ *       multistream the rest is ignored, as in the compressjs flavor.  The first header of the file keeps the -2 rules.
+ * The prefix delivered on an error is that of b2_bzip2_decompress_partial: for -3, every block in front (they all passed
+ * their CRCs).  Device and host memory bounds are those of the calls without a flavor.  The _flavor calls take the
+ * arguments of the call they extend plus the flavor; an unknown flavor returns B2_ERR_BAD_ARG before any callback runs or
+ * any work is done.  decompress_block[s], table, b2_bzip2_decompress_dev, the sharded decode and recovery read the
+ * compressjs flavor only. */
+int b2_bzip2_decompress_flavor(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n, int flavor);
+int b2_bzip2_decompress_partial_flavor(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n, int flavor);
+int b2_bzip2_decompress_stream_flavor(b2_read_fn rd, b2_write_fn wr, void* user, int multistream, int flavor);
 
 /* ---- device-resident entry points (buffers already in HBM) ----------------------- */
 /* Same semantics as b2_bzip2_compress, but `d_in` / `d_out` are device pointers on the
