@@ -773,6 +773,32 @@ int b2_dec_shard_finish(const uint64_t* all, int multistream, void* d_out, size_
   });
 }
 
+int b2_dec_share_open(const void* d_buf, size_t hold, uint64_t g0, size_t share_len, size_t total, uint64_t* info) {
+  return guarded([&]() {
+    if (share_len > hold || g0 > total || hold > total - g0) throw B2Error{B2_ERR_BAD_ARG, "the buffer is not a share of the stream"};
+    if (g0 + hold < total && hold - share_len < B2_SHARE_HALO_MIN) throw B2Error{B2_ERR_BAD_ARG, "halo shorter than 14 bytes"};
+    Ctx& c = ctx_locked();
+    c.reset_call();
+    {
+      StageScope tot(c, ST_TOTAL);
+      dec_share_open(c, (const u8*)d_buf, hold, g0, share_len, total, info);
+    }
+    c.sync();
+    c.collect();
+    return 0;
+  });
+}
+int b2_dec_share_export(uint64_t* buf) {
+  return guarded([&]() { dec_share_export(buf); return 0; });
+}
+int b2_dec_share_finish(const uint64_t* all, size_t count, int multistream, void* d_out, size_t out_cap, uint64_t* res) {
+  return guarded([&]() {
+    ctx_locked();
+    dec_share_finish(all, count, multistream, (u8*)d_out, out_cap, res);
+    return 0;
+  });
+}
+
 int b2_bitshift_dev(const void* d_src, uint64_t nbits, int phase, void* d_dst) {
   return guarded([&]() {
     if (phase < 0 || phase > 7 || (((size_t)d_src | (size_t)d_dst) & 3)) throw B2Error{B2_ERR_BAD_ARG, "bad phase or unaligned buffers"};

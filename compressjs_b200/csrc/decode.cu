@@ -33,8 +33,8 @@
 //                    the block chain (a block must start exactly where the previous one ended) after every batch,
 //                    folds/validates CRCs, delivers the settled blocks (to a device buffer, a host sink, or only
 //                    for their CRCs) and raises the reference's errors in stream order.  A position list uploads
-//                    the whole input once and walks its blocks in list order, without a chain.  The sharded decode
-//                    runs the same batch, walk and device delivery over the whole file.  Block recovery walks every
+//                    the whole input once and walks its blocks in list order, without a chain.  The sharded decodes
+//                    run the same batch, walk and device delivery over the whole file or a rank's share.  Block recovery walks every
 //                    candidate by intactness instead of by the chain and splices the intact blocks' bits (k_splice).
 #include <algorithm>
 #include <memory>
@@ -1327,16 +1327,20 @@ static void dec_batch(Ctx& c, DecScratch& B, const u8* in, u64 wbytes, u64 base_
 }
 
 // ---- the compressed input ----
-// A host stream (StreamIn, whose length is known once it has ended) or a device buffer [0, n).  The drivers read the
-// input through these calls only.
+// A host stream (StreamIn, whose length is known once it has ended) or a device buffer holding bytes [off, off + n) of
+// an input of `total` bytes (a share of a sharded stream; the whole input when off = 0 and total = n).  The drivers
+// read the input through these calls only, at stream offsets.
 struct DecIn {
   StreamIn* s = nullptr;
   const u8* d = nullptr;
   size_t n = 0;
+  u64 off = 0;
+  size_t total = 0;
   explicit DecIn(StreamIn& in) : s(&in) {}
-  DecIn(const u8* d_in, size_t n_) : d(d_in), n(n_) {}
-  size_t length() const { return s ? (s->eof ? s->base + s->have : SIZE_MAX) : n; }  // a stream's once it has ended
-  u64 end() const { return s ? s->base + s->have : n; }  // the end of the bytes there are so far
+  DecIn(const u8* d_in, size_t n_) : d(d_in), n(n_), total(n_) {}
+  DecIn(const u8* d_in, size_t n_, u64 off_, size_t total_) : d(d_in), n(n_), off(off_), total(total_) {}
+  size_t length() const { return s ? (s->eof ? s->base + s->have : SIZE_MAX) : total; }  // a stream's once it has ended
+  u64 end() const { return s ? s->base + s->have : off + n; }  // the end of the bytes there are so far
   // Up to k bytes at bytepos (a member header, or a magic the input may cut off) into h; returns how many there are.  They
   // may lie past the window: a stream reads one byte more, which tells whether the input ends behind them.
   size_t head(Ctx& c, u64 bytepos, u8* h, size_t k = 4) {
@@ -1345,14 +1349,15 @@ struct DecIn {
     if (s) {
       memcpy(h, s->at(bytepos), avail);
     } else {
-      CUDA_CHECK(cudaMemcpyAsync(h, d + bytepos, avail, cudaMemcpyDeviceToHost, c.stream));
+      CUDA_CHECK(cudaMemcpyAsync(h, d + (bytepos - off), avail, cudaMemcpyDeviceToHost, c.stream));
       CUDA_CHECK(cudaStreamSynchronize(c.stream));
     }
     return avail;
   }
   // As much of [a, a + len) as the input has into the device buffer win, zero padded (aligned word reads past the end
   // must be safe); returns its length.  A stream keeps its bytes from a on and reads one byte past a + len, so its end is
-  // known exactly when a complete input would show it (until then no window is the last one).
+  // known exactly when a complete input would show it (until then no window is the last one).  A device buffer that
+  // starts behind a (a share, whose window starts at a word boundary) reads zeros in front of off.
   u64 window(Ctx& c, DBuf<u8>& win, u64 a, u64 want) {
     if (s) {
       s->drop(a);
@@ -1365,7 +1370,9 @@ struct DecIn {
       StageScope st(c, ST_H2D);
       if (len) CUDA_CHECK(cudaMemcpyAsync(win, s->at(a), len, cudaMemcpyHostToDevice, c.stream));
     } else if (len) {
-      CUDA_CHECK(cudaMemcpyAsync(win, d + a, len, cudaMemcpyDeviceToDevice, c.stream));
+      const u64 lead = std::min<u64>(off > a ? off - a : 0, len);
+      if (lead) CUDA_CHECK(cudaMemsetAsync(win, 0, lead, c.stream));
+      if (len > lead) CUDA_CHECK(cudaMemcpyAsync(win.p + lead, d + (a + lead - off), len - lead, cudaMemcpyDeviceToDevice, c.stream));
     }
     return len;
   }
@@ -1444,13 +1451,26 @@ struct Decode {
   Chain ch;
   DecErr E;
   DecRows rows;
+  // A share session's imported candidates (parallel to cands): the bytes behind an end-of-stream magic, which only its
+  // owner's buffer holds (byte k at bits 8k, their count at bits 32 and up).  Empty: the walk reads the input.
+  std::vector<u64> tails;
+  // up to 4 bytes at bytepos, behind end-of-stream candidate ci, into h; returns how many there are
+  size_t eos_head(size_t ci, u64 bytepos, u8* h) {
+    if (tails.empty()) return in.head(c, bytepos, h);
+    for (int k = 0; k < 4; k++) h[k] = (u8)(tails[ci] >> (8 * k));
+    return (size_t)(tails[ci] >> 32);
+  }
   // reads no header: every block is held to the largest dbufSize (the recovery decodes blocks wherever they are)
   struct NoHeader {};
   Decode(Ctx& c_, const DecIn& in_, NoHeader) : c(c_), in(in_), DB(dec_batch_blocks(c_)) { ch.cur_dbuf = 900000u; }
   // reads the first header (lib/Bzip2.js:105-124 _start_bunzip)
   Decode(Ctx& c_, const DecIn& in_) : c(c_), in(in_), DB(dec_batch_blocks(c_)) {
     u8 hdr[4] = {0, 0, 0, 0};
-    if (in.head(c, 0, hdr) < 4 || hdr[0] != 'B' || hdr[1] != 'Z' || hdr[2] != 'h') throw B2Error{DEC_NOT_BZIP, "Not bzip data: bad magic"};
+    first_header(hdr, in.head(c, 0, hdr));
+  }
+  // the stream's first `avail` (up to 4) bytes set the first member's dbufSize, or throw
+  void first_header(const u8* hdr, size_t avail) {
+    if (avail < 4 || hdr[0] != 'B' || hdr[1] != 'Z' || hdr[2] != 'h') throw B2Error{DEC_NOT_BZIP, "Not bzip data: bad magic"};
     const int level = hdr[3] - 0x30;
     if (level < 1 || level > 9) throw B2Error{DEC_NOT_BZIP, "Not bzip data: level out of range"};
     ch.cur_dbuf = 100000u * (u32)level;
@@ -1608,7 +1628,7 @@ static bool chain_walk(Decode& R, u64 end_bit) {
     if (!ch.multistream || bytepos >= R.in.length()) { ch.done = true; break; }
     // _start_bunzip on the byte stream (resyncs to the next byte)
     u8 h2[4] = {0, 0, 0, 0};
-    const size_t avail = R.in.head(R.c, bytepos, h2);
+    const size_t avail = R.eos_head((size_t)(it - R.cands.begin()), bytepos, h2);
     if (lb) {
       // bzip2 -d: a tail that is not the start of "BZh1".."BZh9" is ignored; a cut-off header is a truncated file
       const char want[3] = {'B', 'Z', 'h'};
@@ -2056,13 +2076,23 @@ void bzip2_recover(Ctx& c, StreamIn& in, bool repair, StreamOut& out, std::vecto
 }
 
 // ---- sharded decode (SURVEY.md section 8e): open on every rank, exchange results, finish ------------
-// The open session decodes the share [lo, hi) of the whole input's block candidates (one window: the whole input, zero
-// padded); finish walks the chain over ALL candidates' results (imported from the other ranks), expands + CRC-checks
-// the blocks of the own share and raises the reference's errors in stream order.  A rank keeps its share's results
-// until the all-gather, so its device memory grows with its share of the file.
+// Two kinds of session, one slot, which differ only in their input, the candidates a rank owns and the rows it imports:
+//  - the whole input (b2_dec_shard_*): every rank holds the stream, scans all of it (one window: the whole input, zero
+//    padded) and decodes the share [lo, hi) of its block candidates; the rows are the block results, in candidate order.
+//  - shares (b2_dec_share_*): a rank holds bytes [g0, g0 + hold) of the stream and owns the magics at bit positions
+//    [8 g0, 8 (g0 + share_len)); it scans and decodes those only (one window over its buffer), and its rows carry the
+//    candidates themselves, the bytes behind its end-of-stream magics and the stream's first bytes (include/b2bz.h).
+// finish walks the chain over ALL candidates' results (imported from the other ranks), expands + CRC-checks the blocks
+// of the own share and raises the reference's errors in stream order.  A rank keeps its share's results until the
+// all-gather, so its device memory grows with its share of the file.
 struct DecSession {
   Decode R;  // hres: one entry per block candidate (the own share's after open, all after the import)
   size_t lo = 0, hi = 0;
+  // shares: the owned bit range, and the stream's first bytes from the rows (read by the rank that owns bit 0)
+  bool share = false;
+  u64 own0 = 0, own1 = 0;
+  u8 hdr[4] = {0, 0, 0, 0};
+  size_t hdr_n = 0;
 
   DecSession(Ctx& c, const u8* d_in, size_t n, int rank, int world) : R(c, DecIn(d_in, n)) {
     R.load(0, n);
@@ -2073,12 +2103,47 @@ struct DecSession {
     for (auto& r : R.hres) { memset(&r, 0, sizeof r); r.status = DEC_DATA_ERROR; }
     lo = (size_t)rank * nb_all / (size_t)world;
     hi = (size_t)(rank + 1) * nb_all / (size_t)world;
+    decode_own(n);
+  }
+
+  DecSession(Ctx& c, const u8* d_buf, size_t hold, u64 g0, size_t share_len, size_t total)
+      : R(c, DecIn(d_buf, hold, g0, total), Decode::NoHeader{}), share(true), own0(8 * g0), own1(8 * (g0 + share_len)) {
+    if (g0 == 0 && share_len) hdr_n = R.in.head(c, 0, hdr);
+    if (share_len) {
+      // One window over the buffer from the word that holds byte g0: k_scan_magic and k_hdec take a window that starts
+      // at a multiple of 32 bits, and the bytes in front of g0 read as zeros.  The scan stops at the owned range's end
+      // (the halo holds the 80 bits of a magic that starts in front of it); a magic in front of g0 is the rank before's.
+      const u64 a = g0 & ~(u64)3;
+      R.load(a, g0 + hold - a);
+      R.scan(own1 - a * 8);
+      R.cands.erase(R.cands.begin(), std::lower_bound(R.cands.begin(), R.cands.end(), own0, [](const Cand& x, u64 p) { return x.pos < p; }));
+      // the bytes a multistream walk reads behind each end-of-stream magic (the next member's header)
+      R.tails.assign(R.cands.size(), 0);
+      R.blk.clear();
+      for (size_t i = 0; i < R.cands.size(); i++) {
+        if (R.cands[i].type == 1) { R.blk.push_back(i); continue; }
+        const u64 bytepos = (R.cands[i].pos + 80 + 7) / 8;
+        if (bytepos >= total) continue;
+        u8 h[4] = {0, 0, 0, 0};
+        const u64 k = R.in.head(c, bytepos, h);
+        R.tails[i] = k << 32 | (u64)h[0] | (u64)h[1] << 8 | (u64)h[2] << 16 | (u64)h[3] << 24;
+      }
+    }
+    hi = R.blk.size();
+    R.hres.assign(hi, CandRes());
+    decode_own(hold);
+    R.win = DBuf<u8>();  // finish reads nothing of the input
+  }
+
+  // Decodes the own block candidates [lo, hi) into slots [0, hi - lo); in_bytes: the input the session holds.
+  void decode_own(size_t in_bytes) {
+    Ctx& c = R.c;
     const size_t nb = hi - lo;
     {
       // every block of the own share keeps 2 MiB (L column + count-byte classes; 1 MiB beyond DEC_KEEP_CLS blocks) until
       // the stream is assembled, and a batch of up to 2048 blocks needs ~20 MiB of scratch per block: say so instead of
       // failing inside an allocation
-      const size_t need = nb * ((size_t)(nb <= dec_keep_cls_limit() ? 2 : 1) << 20) + std::min<size_t>(nb, R.DB) * ((size_t)20 << 20) + n;
+      const size_t need = nb * ((size_t)(nb <= dec_keep_cls_limit() ? 2 : 1) << 20) + std::min<size_t>(nb, R.DB) * ((size_t)20 << 20) + in_bytes;
       // memory the stream-ordered pool holds but does not use is available too: when that covers the call (every call
       // after the first of a kind) the driver is not asked at all -- cudaMemGetInfo takes milliseconds on a busy context
       uint64_t reserved = 0, used = 0;
@@ -2112,14 +2177,83 @@ struct DecSession {
     R.B = DecScratch();  // the batch scratch is not kept until finish
   }
 
-  // Walks the chain over every rank's results, expands the own blocks into d_out (or a buffer of its own), and fills
-  // info.  Throws the first failure in stream order; info[3] tells the ranks which failure is the earliest.
-  void finish(int multistream, u8* d_out, size_t out_cap, u64* info) {
+  // The rows of b2_dec_share_export, B2_SHARE_ROW words each: the stream's first bytes (on the rank that owns bit 0),
+  // then every owned candidate in position order.
+  size_t share_rows() const { return (size_t)(own0 == 0 && own1 > 0) + R.cands.size(); }
+  void share_export(u64* buf) const {
+    u64* o = buf;
+    if (own0 == 0 && own1 > 0) {
+      memset(o, 0, 8 * B2_SHARE_ROW);
+      o[10] = (u64)hdr_n << 32 | (u64)hdr[0] | (u64)hdr[1] << 8 | (u64)hdr[2] << 16 | (u64)hdr[3] << 24;
+      o += B2_SHARE_ROW;
+    }
+    size_t j = 0;
+    for (size_t i = 0; i < R.cands.size(); i++, o += B2_SHARE_ROW) {
+      const Cand& cd = R.cands[i];
+      memset(o, 0, 8 * B2_SHARE_ROW);
+      o[0] = cd.pos; o[1] = cd.type; o[2] = cd.next32; o[10] = R.tails[i];
+      if (cd.type != 1) continue;
+      const CandRes& r = R.hres[j++];
+      // an obsolete block's decode stops before its origPtr, which the walk does not read then
+      o[3] = (u64)(long long)r.status; o[4] = r.detail; o[5] = r.endbit; o[6] = r.n; o[7] = r.rawlen;
+      o[8] = r.status == DEC_OBSOLETE ? 0 : r.orig; o[9] = r.open;
+    }
+  }
+  // Every rank's rows, in rank order, become the candidates and results the walk sees; the own ones keep the results
+  // of this session's decode.
+  void share_import(const u64* all, size_t count) {
+    std::vector<Cand> cands;
+    std::vector<u64> tails;
+    std::vector<CandRes> hres;
+    bool head = false;
+    size_t own_c = 0, own_b = 0;
+    for (size_t i = 0; i < count; i++) {
+      const u64* o = all + i * B2_SHARE_ROW;
+      if (o[1] > 2 || (o[1] && !cands.empty() && o[0] <= cands.back().pos)) throw B2Error{B2_ERR_BAD_ARG, "share rows out of order or of an unknown kind"};
+      if (o[1] == 0) {
+        if (!head) for (int k = 0; k < 4; k++) hdr[k] = (u8)(o[10] >> (8 * k));
+        if (!head) hdr_n = (size_t)std::min<u64>(o[10] >> 32, 4);
+        head = true;
+        continue;
+      }
+      const bool mine = o[0] >= own0 && o[0] < own1;
+      own_c += mine;
+      cands.push_back(Cand{o[0], (u32)o[1], (u32)o[2]});
+      tails.push_back(o[10]);
+      if (o[1] != 1) continue;
+      if (mine) {
+        if (own_b >= R.hres.size()) throw B2Error{B2_ERR_BAD_ARG, "the share rows do not hold this rank's candidates"};
+        if (own_b == 0) lo = hres.size();
+        hres.push_back(R.hres[own_b++]);
+        continue;
+      }
+      CandRes r;
+      memset(&r, 0, sizeof r);
+      r.status = (int)(long long)o[3]; r.detail = (u32)o[4]; r.endbit = o[5]; r.n = (u32)o[6]; r.rawlen = (u32)o[7]; r.orig = (u32)o[8];
+      r.open = (u32)o[9];
+      hres.push_back(r);
+    }
+    if (own_c != R.cands.size() || own_b != R.hres.size()) throw B2Error{B2_ERR_BAD_ARG, "the share rows do not hold this rank's candidates"};
+    if (!own_b) lo = 0;
+    hi = lo + own_b;
+    if (!head) hdr_n = 0;
+    R.cands = std::move(cands);
+    R.tails = std::move(tails);
+    R.hres = std::move(hres);
+    R.blk.clear();
+    for (size_t i = 0; i < R.cands.size(); i++) if (R.cands[i].type == 1) R.blk.push_back(i);
+  }
+
+  // Walks the chain over every rank's results, expands the own blocks into d_out (or a buffer of its own), fills info
+  // and returns true.  Throws the first failure in stream order; info[3] tells the ranks which failure is the earliest.
+  // Returns false, having delivered nothing, when the walk reaches a block that decoded past the end of its owner's
+  // buffer: only a share session has such blocks (a whole-input session's one window ends the input).
+  bool finish(int multistream, u8* d_out, size_t out_cap, u64* info) {
     Chain& ch = R.ch;
     ch.multistream = multistream;
     R.kb = 0;  // the batch the walk sees: every block candidate
     R.cnt = (u32)R.hres.size();
-    chain_walk(R, ~0ull);
+    if (chain_walk(R, ~0ull)) return false;
     // own output window: [my_off, my_off + my_len) of the decoded stream, from the first to the last own block
     auto mine = [&](const Event& ev) { return ev.kind == 0 && ev.slot >= lo && ev.slot < hi; };
     const auto f = std::find_if(ch.events.begin(), ch.events.end(), mine);
@@ -2137,6 +2271,7 @@ struct DecSession {
     info[0] = my_off; info[1] = my_len; info[2] = ch.total_out; info[3] = (u64)(long long)R.E.ev; info[4] = (u64)(long long)R.E.code;
     // the caller compares info[3] across ranks and keeps the earliest
     if (R.E.ev >= 0) throw B2Error{R.E.code, R.E.msg};
+    return true;
   }
 };
 
@@ -2147,16 +2282,20 @@ void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* 
   g_shard = std::make_unique<DecSession>(c, d_in, n, rank, world);
   info[0] = g_shard->R.blk.size(); info[1] = g_shard->lo; info[2] = g_shard->hi;
 }
+static DecSession& session(bool share) {
+  if (!g_shard || g_shard->share != share) throw B2Error{B2_ERR_BAD_ARG, share ? "no share decode in flight" : "no sharded decode in flight"};
+  return *g_shard;
+}
 void dec_shard_export(u64* buf) {
-  if (!g_shard) throw B2Error{B2_ERR_BAD_ARG, "no sharded decode in flight"};
-  for (size_t i = g_shard->lo; i < g_shard->hi; i++) {
-    const CandRes& r = g_shard->R.hres[i];
-    u64* o = buf + (i - g_shard->lo) * 6;
+  const DecSession& S = session(false);
+  for (size_t i = S.lo; i < S.hi; i++) {
+    const CandRes& r = S.R.hres[i];
+    u64* o = buf + (i - S.lo) * 6;
     o[0] = (u64)(long long)r.status; o[1] = r.detail; o[2] = r.endbit; o[3] = r.n; o[4] = r.rawlen; o[5] = r.orig;
   }
 }
 void dec_shard_finish(const u64* all, int multistream, u8* d_out, size_t out_cap, u64* res) {
-  if (!g_shard) throw B2Error{B2_ERR_BAD_ARG, "no sharded decode in flight"};
+  session(false);
   const std::unique_ptr<DecSession> S = std::move(g_shard);  // the session ends with this call
   for (size_t i = 0; i < S->R.hres.size(); i++) {
     if (i >= S->lo && i < S->hi) continue;
@@ -2165,4 +2304,25 @@ void dec_shard_finish(const u64* all, int multistream, u8* d_out, size_t out_cap
     r.status = (int)(long long)o[0]; r.detail = (u32)o[1]; r.endbit = o[2]; r.n = (u32)o[3]; r.rawlen = (u32)o[4]; r.orig = (u32)o[5];
   }
   S->finish(multistream, d_out, out_cap, res);
+}
+
+void dec_share_open(Ctx& c, const u8* d_buf, size_t hold, u64 g0, size_t share_len, size_t total, u64* info) {
+  g_shard.reset();
+  g_shard = std::make_unique<DecSession>(c, d_buf, hold, g0, share_len, total);
+  info[0] = g_shard->share_rows(); info[1] = g_shard->R.cands.size(); info[2] = g_shard->R.blk.size();
+}
+void dec_share_export(u64* buf) { session(true).share_export(buf); }
+void dec_share_finish(const u64* all, size_t count, int multistream, u8* d_out, size_t out_cap, u64* res) {
+  session(true);
+  const std::unique_ptr<DecSession> S = std::move(g_shard);  // the session ends with this call
+  for (int k = 0; k < 6; k++) res[k] = 0;
+  res[3] = ~0ull;
+  S->share_import(all, count);
+  try {
+    S->R.first_header(S->hdr, S->hdr_n);  // lib/Bzip2.js:105-124 _start_bunzip: the stream's first failure
+  } catch (const B2Error& e) {
+    res[3] = 0; res[4] = (u64)(long long)e.code;
+    throw;
+  }
+  res[5] = S->finish(multistream, d_out, out_cap, res) ? 0 : 1;
 }

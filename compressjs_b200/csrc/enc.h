@@ -184,11 +184,14 @@ void bzip2_decompress_list(Ctx& c, StreamIn& in, const std::vector<u64>& positio
 // intact blocks' bytes or (repair) the repaired stream.  Damage is a result, not an error: only a CUDA failure or a
 // callback abort throws.
 void bzip2_recover(Ctx& c, StreamIn& in, bool repair, StreamOut& out, std::vector<b2_recovered_block>& rows);
-// The sharded decode (b2_dec_shard_open / _export / _finish): one session at a time, ended by finish or released by
-// b2_shutdown.
+// The sharded decodes (b2_dec_shard_open / _export / _finish over the whole input, b2_dec_share_open / _export / _finish
+// over shares): one session of either kind at a time, ended by finish or by the next open, or released by b2_shutdown.
 void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* info);
 void dec_shard_export(u64* buf);
 void dec_shard_finish(const u64* all, int multistream, u8* d_out, size_t out_cap, u64* res);
+void dec_share_open(Ctx& c, const u8* d_buf, size_t hold, u64 g0, size_t share_len, size_t total, u64* info);
+void dec_share_export(u64* buf);
+void dec_share_finish(const u64* all, size_t count, int multistream, u8* d_out, size_t out_cap, u64* res);
 void dec_shard_release();
 // BWT.unbwtransform of nb blocks at once (BWTC decode, b2_bwt_inverse): block b is the L column in slot b of d_L, h_n[b]
 // bytes (1 <= n <= 2^20 - 2) with primary index h_pidx[b] (0 <= pidx <= n); the blocks go to d_out back to back.

@@ -30,6 +30,7 @@ is injected.
 """
 import ctypes as C
 import time
+from collections import namedtuple
 
 import numpy as np
 
@@ -720,10 +721,10 @@ def decode_shard_finish(L, all_rows, multistream, device):
                                                       err_code=err_code if rc else 0, msg=msg)
 
 
-def decompress_file_sharded(d_in, multistream=False, group=None):
-    """Decode a .bz2 stream held on every rank; the decoded bytes are gathered on rank 0 (uint8 tensor)."""
+def _decode_whole_input(d_in, multistream=False, group=None):
+    """The sharded decode of a stream held on every rank, up to the error exchange: (own output tensor or None, res) on
+    every rank, as decode_shard_finish returns them."""
     from . import _native
-    from .bzip2 import Bzip2Error
     L = _native.lib()
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
@@ -749,8 +750,16 @@ def decompress_file_sharded(d_in, multistream=False, group=None):
         all_rows = torch.cat(parts) if parts else rows
     else:
         all_rows = rows
-    out, res = decode_shard_finish(L, all_rows, multistream, device)
-    # earliest failing event over all ranks wins (every rank sees the same event list)
+    return decode_shard_finish(L, all_rows, multistream, device)
+
+
+def _settle(res, device, group=None):
+    """The earliest failing event over all ranks wins (every rank sees the same event list): every rank raises its code,
+    with the message on the rank that found it and "Data error" elsewhere.  Otherwise returns every rank's (offset,
+    length) of its output in the decoded stream, and the stream's length."""
+    from .bzip2 import Bzip2Error
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    rank = dist.get_rank(group) if dist.is_initialized() else 0
     mine = torch.tensor([res["err_idx"] if res["err_idx"] >= 0 else 2 ** 62, res["err_code"], res["off"], res["len"], res["total"]],
                         dtype=torch.int64, device=device)
     if world > 1:
@@ -762,16 +771,21 @@ def decompress_file_sharded(d_in, multistream=False, group=None):
     if errs:
         idx, code, who = min(errs)
         raise Bzip2Error(code, res["msg"] if who == rank else "Data error")
-    if world == 1:
-        return out
-    # the shards travel to rank 0 straight into their place in the decoded stream (send/recv into offset views)
+    return [(int(v[2]), int(v[3])) for v in allv], int(allv[0][4])
+
+
+def _place(out, spans, total, device, group=None):
+    """Every rank's decoded piece travels to rank 0 straight into its place in the decoded stream (send/recv into offset
+    views).  Returns the stream on rank 0, None elsewhere."""
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    rank = dist.get_rank(group) if dist.is_initialized() else 0
     ops, full = [], None
     if rank == 0:
-        full = torch.empty(int(allv[0][4]), dtype=torch.uint8, device=device)
-        o0, l0 = int(allv[0][2]), int(allv[0][3])
+        full = torch.empty(total, dtype=torch.uint8, device=device)
+        o0, l0 = spans[0]
         full[o0: o0 + l0] = out[:l0]
         for r in range(1, world):
-            o, ln = int(allv[r][2]), int(allv[r][3])
+            o, ln = spans[r]
             if ln:
                 ops.append(dist.P2POp(dist.irecv, full[o: o + ln], r, group))
     elif out.numel():
@@ -780,3 +794,160 @@ def decompress_file_sharded(d_in, multistream=False, group=None):
         for req in dist.batch_isend_irecv(ops):
             req.wait()
     return full
+
+
+def decompress_file_sharded(d_in, multistream=False, group=None):
+    """Decode a .bz2 stream held on every rank; the decoded bytes are gathered on rank 0 (uint8 tensor)."""
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    out, res = _decode_whole_input(d_in, multistream, group)
+    spans, total = _settle(res, d_in.device, group)
+    if world == 1:
+        return out
+    return _place(out, spans, total, d_in.device, group)
+
+
+# ---- sharded decode from sharded input ------------------------------------------------------------------------------
+# A block that decodes to at most 900 000 bytes has at most 900 001 codes of at most 20 bits, at most 32 767 selectors
+# and 6 code length tables: with code lengths reached by direct delta paths, about 2.3 MB.  So a block that starts in a
+# share ends inside a halo of 4 MiB, the halo compress_shares takes, unless it is corrupt or a table takes a
+# pathological delta path; decompress_shares falls back to the whole input then.
+DEC_HALO = 4 << 20
+DEC_HALO_MIN = 14   # B2_SHARE_HALO_MIN: a magic and its CRC (10 bytes), and the member header behind an end-of-stream magic
+SHARE_ROW = 11      # B2_SHARE_ROW: uint64 per exported row (include/b2bz.h)
+
+DecodedShare = namedtuple("DecodedShare", "piece offset total")
+DecodedShare.__doc__ = """A rank's piece of the decoded stream: its bytes `piece` are bytes [offset, offset + len(piece)) of
+the decoded stream of `total` bytes.  The pieces of all ranks tile the stream."""
+
+
+def share_layout(sizes):
+    """sizes[r] = (share_len, hold) of rank r, in rank order.  Returns (the first byte of every rank's share, the stream's
+    length).  Raises ValueError for the first rank whose buffer is not a share of the stream or whose halo is shorter
+    than DEC_HALO_MIN bytes and does not reach the stream's end."""
+    total = sum(s for s, _ in sizes)
+    g0s, g = [], 0
+    for r, (share_len, hold) in enumerate(sizes):
+        if share_len < 0 or hold < share_len or g + hold > total:
+            raise ValueError("decompress_shares: rank %d holds %d bytes from byte %d of a %d-byte stream for a share of %d bytes"
+                             % (r, hold, g, total, share_len))
+        if g + hold < total and hold - share_len < DEC_HALO_MIN:
+            raise ValueError("decompress_shares: rank %d has a halo of %d bytes; a halo must hold at least %d bytes unless it "
+                             "reaches the end of the stream" % (r, hold - share_len, DEC_HALO_MIN))
+        g0s.append(g)
+        g += share_len
+    return g0s, total
+
+
+def _share_open(d_buf, share_len, g0, total):
+    """Stage 1 on one rank (b2_dec_share_open + export): (rows, 0, "") with rows an int64 CPU tensor [k, SHARE_ROW], or
+    (no rows, error code, message) when the open failed, which the caller reports after the exchange."""
+    from . import _native
+    L = _native.lib()
+    if d_buf.is_cuda:
+        torch.cuda.current_stream().synchronize()   # the library works on its own stream: the input must have landed
+    none = torch.zeros((0, SHARE_ROW), dtype=torch.int64)
+    info = (C.c_uint64 * 3)()
+    rc = L.b2_dec_share_open(d_buf.data_ptr(), d_buf.numel(), g0, share_len, total, info)
+    if rc:
+        return none, rc, "b2_dec_share_open: " + _native.last_error()
+    k = int(info[0])
+    buf = (C.c_uint64 * (SHARE_ROW * max(k, 1)))()
+    rc = L.b2_dec_share_export(buf)
+    if rc:
+        return none, rc, "b2_dec_share_export: " + _native.last_error()
+    rows = np.frombuffer(buf, dtype=np.int64, count=SHARE_ROW * k).reshape(k, SHARE_ROW)
+    return torch.from_numpy(rows.copy()), 0, ""
+
+
+def _share_finish(all_rows, own_rows, multistream, device):
+    """Stage 2 on one rank (b2_dec_share_finish): all_rows = every rank's rows in rank order, own_rows = this rank's.
+    Returns (own output tensor, or None on an error, res) with res as decode_shard_finish's plus `unsettled`."""
+    from . import _native
+    L = _native.lib()
+    flat = np.ascontiguousarray(all_rows.numpy(), dtype=np.int64)
+    own = own_rows.numpy()
+    need = int(own[(own[:, 1] == 1) & (own[:, 3] == 0), 7].sum())   # upper bound: every owned block that decoded
+    out = torch.empty(max(need, 1), dtype=torch.uint8, device=device)
+    res = (C.c_uint64 * 6)()
+    rc = L.b2_dec_share_finish(flat.ctypes.data, flat.shape[0], int(bool(multistream)), out.data_ptr(), out.numel(), res)
+    vals = [_i64(int(v)) for v in res]
+    msg = _native.last_error() if rc else ""
+    err_idx = (vals[3] if vals[3] >= 0 else 0) if rc else -1   # a failure that is no event of the stream fails every rank
+    return out[: vals[1]] if rc == 0 else None, dict(off=vals[0], len=vals[1], total=vals[2], err_idx=err_idx,
+                                                      err_code=(vals[4] or rc) if rc else 0, msg=msg, unsettled=rc == 0 and vals[5] != 0)
+
+
+def _gather_shares(d_buf, share_len, lens, group=None):
+    """The whole stream on every rank, from every rank's share (lens[r]: rank r's share length)."""
+    world = len(lens)
+    if world == 1:
+        return d_buf[:share_len]
+    pad = torch.zeros(max(lens + [1]), dtype=torch.uint8, device=d_buf.device)
+    pad[:share_len] = d_buf[:share_len]
+    gl = [torch.empty_like(pad) for _ in range(world)]
+    dist.all_gather(gl, pad, group=group)
+    return torch.cat([gl[r][: lens[r]] for r in range(world)])
+
+
+def decompress_shares(d_buf, share_len, multistream=False, group=None, keep_sharded=False):
+    """Decode a .bz2 stream that no rank holds whole: the decode counterpart of compress_shares.  d_buf = uint8 tensor
+    with the rank's share of the stream (share_len bytes) followed by a halo, the first bytes of the next shares (at least
+    DEC_HALO_MIN bytes unless it reaches the end of the stream; DEC_HALO is enough for any intact block).  The shares are
+    contiguous in rank order.  Every rank scans and decodes only the blocks that start in its share; the ranks exchange
+    the results, and every rank walks the block chain over all of them.  When the rows cannot settle the stream (a block
+    that runs past its owner's halo), every rank gathers the shares and decodes the whole input (decompress_file_sharded's
+    path) instead.  The decoded bytes, or the error, are exactly those of Bzip2.decompressFile(stream, multistream=...)
+    on one GPU; nothing is delivered on an error.  Returns the decoded stream on rank 0 (None elsewhere); with
+    keep_sharded a DecodedShare on every rank (with one rank: the whole stream)."""
+    return _decompress_shares(d_buf, share_len, multistream, group, keep_sharded, _share_open, _share_finish, _decode_whole_input)
+
+
+def _decompress_shares(d_buf, share_len, multistream, group, keep_sharded, open_stage, finish_stage, whole_stage):
+    """decompress_shares with its library stages passed in: open_stage(d_buf, share_len, g0, total) -> (rows, code,
+    message); finish_stage(all rows, own rows, multistream, device) -> (own output, res); whole_stage(stream,
+    multistream, group) -> (own output, res) from the whole input on every rank."""
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    rank = dist.get_rank(group) if dist.is_initialized() else 0
+    dev = d_buf.device
+    PHASES.clear()
+    # 1. every rank's (share length, bytes held): where the shares start, the stream's length, every rank's halo
+    mine = torch.tensor([share_len, d_buf.numel()], dtype=torch.int64, device=dev)
+    if world > 1:
+        alls = [torch.zeros_like(mine) for _ in range(world)]
+        dist.all_gather(alls, mine, group=group)
+    else:
+        alls = [mine]
+    sizes = [(int(v[0]), int(v[1])) for v in alls]
+    g0s, total = share_layout(sizes)
+    # 2. open and export; a failed open travels with the row counts, so that every rank raises after the exchange
+    rows, rc, msg = open_stage(d_buf, share_len, g0s[rank], total)
+    head = torch.tensor([rows.shape[0], rc], dtype=torch.int64, device=dev)
+    if world > 1:
+        heads = [torch.zeros_like(head) for _ in range(world)]
+        dist.all_gather(heads, head, group=group)
+    else:
+        heads = [head]
+    heads = [(int(v[0]), int(v[1])) for v in heads]
+    failed = [r for r, (_, code) in enumerate(heads) if code]
+    if failed:
+        raise RuntimeError(msg if rc else "decompress_shares: rank %d could not open its share (code %d)" % (failed[0], heads[failed[0]][1]))
+    # 3. every rank's rows, padded to the longest
+    if world > 1:
+        pad = torch.zeros((max(k for k, _ in heads) or 1, SHARE_ROW), dtype=torch.int64, device=dev)
+        pad[: rows.shape[0]] = rows.to(dev)
+        allp = [torch.zeros_like(pad) for _ in range(world)]
+        dist.all_gather(allp, pad, group=group)
+        all_rows = torch.cat([allp[r][: heads[r][0]].cpu() for r in range(world)])
+    else:
+        all_rows = rows
+    # 4. the walk: every rank sees the same rows, so every rank settles the stream or falls back with the others
+    out, res = finish_stage(all_rows, rows, multistream, dev)
+    if res["unsettled"]:
+        PHASES["fallback_full_input"] = 1.0
+        out, res = whole_stage(_gather_shares(d_buf, share_len, [s for s, _ in sizes], group), multistream, group)
+    spans, n_out = _settle(res, dev, group)
+    if keep_sharded:
+        return DecodedShare(out, spans[rank][0], n_out)
+    if world == 1:
+        return out
+    return _place(out, spans, n_out, dev, group)

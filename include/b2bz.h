@@ -373,6 +373,47 @@ int b2_dec_shard_open(const void* d_in, size_t n, int rank, int world, uint64_t*
 int b2_dec_shard_export(uint64_t* buf);
 int b2_dec_shard_finish(const uint64_t* all, int multistream, void* d_out, size_t out_cap, uint64_t* res);
 
+/* ---- sharded decode from sharded input ---------------------------------------------------------------------------
+ * No rank holds the whole stream.  Rank r holds d_buf = bytes [g0, g0 + hold) of a stream of `total` bytes: its share,
+ * the first share_len bytes, followed by a halo (the first bytes of the following shares).  The shares are contiguous
+ * in rank order, as for b2_bzip2_share_summary, so g0 is the sum of the shares in front and total the sum of all.
+ * A rank owns the magics that start at bit positions [8 g0, 8 (g0 + share_len)): the last rank's share ends the stream,
+ * so every magic has one owner.  It scans its own buffer only (the 80 bits of magic and CRC may reach into the halo) and
+ * decodes only the block candidates it owns: the ranks split the work by compressed bytes.
+ * The halo must hold at least B2_SHARE_HALO_MIN = 14 bytes unless the buffer ends the stream (g0 + hold = total): the 10
+ * bytes of a magic and its CRC, and the 4 bytes of the member header behind an end-of-stream magic.  A shorter halo, or a
+ * buffer that is not a share (share_len > hold, g0 + hold > total), is B2_ERR_BAD_ARG.  A block that decodes past the end
+ * of its owner's buffer is `open`: its result is not final.
+ * open: scans and decodes; info = {rows to export, owned candidates, owned block candidates}.  A failure of open (device
+ * memory: the session needs about 2 MiB per owned block, 20 MiB per block of a decode batch and `hold` bytes) is the
+ * caller's to report after the exchange, so that no rank stops while the others wait in a collective.
+ * export: B2_SHARE_ROW uint64 per row.  The rank with g0 = 0 and share_len > 0 starts with a row of kind 0, the stream's
+ * first bytes; every owned candidate follows, in position order:
+ *   [0] bit position of the magic (0 for kind 0)
+ *   [1] kind: 0 the stream's first bytes, 1 block, 2 end of stream
+ *   [2] the 32 bits behind the magic (block CRC, stream CRC)
+ *   [3] block status: 0, or the reference's (negative) error code      [4] detail: 1 = "initial position out of bounds"
+ *   [5] end bit: the bit behind the block's end-of-block code            [6] block length before the inverse BWT
+ *   [7] decoded length                                                    [8] origPtr
+ *   [9] open: 1 = the decode read past the end of the buffer, which does not end the stream
+ *   [10] bytes: kind 0, the stream's first up to 4 bytes; kind 2, up to 4 bytes from the byte boundary behind the stream
+ *        CRC (the next member's header); byte k at bits 8k, their count at bits 32 and up.  0 for a block.
+ * Fields [3]-[9] are 0 for kinds 0 and 2.
+ * finish: `all` = the `count` exported rows of ALL ranks in rank order (all-gathered by the caller).  Walks the chain as
+ * b2_dec_shard_finish does, taking the first header and the bytes behind end-of-stream magics from the rows, expands
+ * and CRC-checks the own blocks into d_out (out_cap: at least the decoded length of the owned blocks that decoded), and
+ * fills res = {offset of the own output in the decoded stream, its length, total decoded length, index of the first
+ * failing event or -1, its code, not settled}.  A bad first header fails with index 0.  When the walk reaches an
+ * on-chain block that its owner decoded as open, the rows cannot settle the stream: res[5] = 1, nothing is delivered,
+ * the call returns 0, and every rank (all see the same rows) decodes from the whole input instead
+ * (b2_dec_shard_*).  Then the result, decoded bytes or error, is exactly that of b2_bzip2_decompress on one GPU.
+ * Compressjs flavor only.  Opening either kind of sharded decode ends the session of the other. */
+#define B2_SHARE_ROW 11
+#define B2_SHARE_HALO_MIN 14
+int b2_dec_share_open(const void* d_buf, size_t hold, uint64_t g0, size_t share_len, size_t total, uint64_t* info);
+int b2_dec_share_export(uint64_t* buf);
+int b2_dec_share_finish(const uint64_t* all, size_t count, int multistream, void* d_out, size_t out_cap, uint64_t* res);
+
 /* ---- instrumentation -------------------------------------------------------------- */
 typedef struct b2_stats {
   /* GPU milliseconds of the last call, from CUDA events on the library's stream */
