@@ -27,6 +27,7 @@ EXPORTS = [
     "b2_bzip2_plan", "b2_bzip2_plan_spec", "b2_bzip2_share_summary", "b2_bzip2_plan_share",
     "b2_bzip2_plan_flavor", "b2_bzip2_share_cut_table", "b2_bzip2_plan_share_flavor", "b2_bzip2_encode_range_dev_flavor",
     "b2_bitshift_dev", "b2_dec_shard_open", "b2_dec_shard_export", "b2_dec_shard_finish", "b2_dec_share_open", "b2_dec_share_export", "b2_dec_share_finish",
+    "b2_dec_shard_open_flavor", "b2_dec_share_open_flavor", "b2_bzip2_decompress_dev_flavor",
     "b2_bzip2_encode_range_dev", "b2_get_stats", "b2_last_trace",
 ]
 
@@ -110,14 +111,18 @@ def lib():
     L.b2_bzip2_bound.argtypes = [C.c_size_t]
     L.b2_bzip2_compress_dev.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t, szp]
     L.b2_bzip2_decompress_dev.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t, szp]
+    L.b2_bzip2_decompress_dev_flavor.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t, szp, C.c_int]
     L.b2_bzip2_plan.argtypes = [C.c_void_p, C.c_size_t, C.c_int, szp]
     L.b2_bzip2_plan_spec.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint64)]
     L.b2_bzip2_share_summary.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64)]
     L.b2_bzip2_plan_share.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_uint64, C.c_uint64, C.c_size_t, C.c_size_t, C.POINTER(C.c_uint64)]
     L.b2_dec_shard_open.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.POINTER(C.c_uint64)]
+    L.b2_dec_shard_open_flavor.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.POINTER(C.c_uint64), C.c_int]
     L.b2_dec_shard_export.argtypes = [C.c_void_p]
     L.b2_dec_shard_finish.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64)]
     L.b2_dec_share_open.argtypes = [C.c_void_p, C.c_size_t, C.c_uint64, C.c_size_t, C.c_size_t, C.POINTER(C.c_uint64)]
+    L.b2_dec_share_open_flavor.argtypes = [C.c_void_p, C.c_size_t, C.c_uint64, C.c_size_t, C.c_size_t, C.POINTER(C.c_uint64),
+                                           C.c_int]
     L.b2_dec_share_export.argtypes = [C.c_void_p]
     L.b2_dec_share_finish.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64)]
     L.b2_bitshift_dev.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_void_p]

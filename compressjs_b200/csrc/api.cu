@@ -749,13 +749,17 @@ int b2_bzip2_plan(const void* d_in, size_t n, int level, size_t* total_blocks) {
 }
 
 int b2_dec_shard_open(const void* d_in, size_t n, int rank, int world, uint64_t* info) {
+  return b2_dec_shard_open_flavor(d_in, n, rank, world, info, B2_BZ2_COMPRESSJS);
+}
+int b2_dec_shard_open_flavor(const void* d_in, size_t n, int rank, int world, uint64_t* info, int flavor) {
   return guarded([&]() {
+    check_flavor(flavor);
     if (world < 1 || rank < 0 || rank >= world) throw B2Error{B2_ERR_BAD_ARG, "bad rank/world"};
     Ctx& c = ctx_locked();
     c.reset_call();
     {
       StageScope tot(c, ST_TOTAL);
-      dec_shard_open(c, (const u8*)d_in, n, rank, world, info);
+      dec_shard_open(c, (const u8*)d_in, n, rank, world, flavor, info);
     }
     c.sync();
     c.collect();
@@ -774,14 +778,18 @@ int b2_dec_shard_finish(const uint64_t* all, int multistream, void* d_out, size_
 }
 
 int b2_dec_share_open(const void* d_buf, size_t hold, uint64_t g0, size_t share_len, size_t total, uint64_t* info) {
+  return b2_dec_share_open_flavor(d_buf, hold, g0, share_len, total, info, B2_BZ2_COMPRESSJS);
+}
+int b2_dec_share_open_flavor(const void* d_buf, size_t hold, uint64_t g0, size_t share_len, size_t total, uint64_t* info, int flavor) {
   return guarded([&]() {
+    check_flavor(flavor);
     if (share_len > hold || g0 > total || hold > total - g0) throw B2Error{B2_ERR_BAD_ARG, "the buffer is not a share of the stream"};
     if (g0 + hold < total && hold - share_len < B2_SHARE_HALO_MIN) throw B2Error{B2_ERR_BAD_ARG, "halo shorter than 14 bytes"};
     Ctx& c = ctx_locked();
     c.reset_call();
     {
       StageScope tot(c, ST_TOTAL);
-      dec_share_open(c, (const u8*)d_buf, hold, g0, share_len, total, info);
+      dec_share_open(c, (const u8*)d_buf, hold, g0, share_len, total, flavor, info);
     }
     c.sync();
     c.collect();
@@ -991,13 +999,17 @@ int b2_bzip2_table(const uint8_t* in, size_t n, int multistream, uint64_t** bitp
 }
 
 int b2_bzip2_decompress_dev(const void* d_in, size_t n, int multistream, void* d_out, size_t out_cap, size_t* out_n) {
+  return b2_bzip2_decompress_dev_flavor(d_in, n, multistream, d_out, out_cap, out_n, B2_BZ2_COMPRESSJS);
+}
+int b2_bzip2_decompress_dev_flavor(const void* d_in, size_t n, int multistream, void* d_out, size_t out_cap, size_t* out_n, int flavor) {
   return guarded([&]() {
+    check_flavor(flavor);
     Ctx& c = ctx_locked();
     c.reset_call();
     {
       StageScope tot(c, ST_TOTAL);
-      if (d_out) bzip2_decompress_dev(c, (const u8*)d_in, n, multistream, (u8*)d_out, out_cap, out_n);
-      else bzip2_decompress_size(c, (const u8*)d_in, n, multistream, out_n);
+      if (d_out) bzip2_decompress_dev(c, (const u8*)d_in, n, multistream, flavor, (u8*)d_out, out_cap, out_n);
+      else bzip2_decompress_size(c, (const u8*)d_in, n, multistream, flavor, out_n);
     }
     c.sync();
     c.collect();

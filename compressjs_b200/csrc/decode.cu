@@ -1460,6 +1460,20 @@ struct Decode {
     for (int k = 0; k < 4; k++) h[k] = (u8)(tails[ci] >> (8 * k));
     return (size_t)(tails[ci] >> 32);
   }
+  // A libbz2 share session's copy of the stream's last bytes, from the rows (kind 3): by the walk the caller's buffer is
+  // gone, and the rank whose block ends the chain may not hold the stream's end.  Unset: the walk reads the input.
+  bool end_rows = false;
+  std::vector<u8> end_bytes;
+  // up to k bytes at bytepos, which lies in the input's last 10 bytes (a magic the input cuts off), into h; returns how
+  // many there are
+  size_t end_head(u64 bytepos, u8* h, size_t k) {
+    if (!end_rows) return in.head(c, bytepos, h, k);
+    const u64 len = in.length(), e0 = len - end_bytes.size();
+    if (bytepos < e0) throw B2Error{B2_ERR_BAD_ARG, "the share rows lack the stream's last bytes"};
+    const size_t avail = (size_t)std::min<u64>(k, len - bytepos);
+    memcpy(h, end_bytes.data() + (bytepos - e0), avail);
+    return avail;
+  }
   // reads no header: every block is held to the largest dbufSize (the recovery decodes blocks wherever they are)
   struct NoHeader {};
   Decode(Ctx& c_, const DecIn& in_, NoHeader) : c(c_), in(in_), DB(dec_batch_blocks(c_)) { ch.cur_dbuf = 900000u; }
@@ -1584,7 +1598,7 @@ static bool cut_magic(Decode& R, u64 pos) {
   const u32 groups = (u32)std::min<u64>(bits / 8, 6);  // whole bytes of the magic (the CRC behind it always agrees)
   if (!groups) return true;
   u8 h[7] = {0};
-  const size_t got = R.in.head(R.c, pos >> 3, h, 7);
+  const size_t got = R.end_head(pos >> 3, h, 7);
   const u32 sh = (u32)(pos & 7);
   bool blk = true, eos = true;
   for (u32 k = 0; k < groups; k++) {
@@ -1796,9 +1810,10 @@ static void chain_decode(Decode& R, int multistream, bool past_error, Deliver de
   CUDA_CHECK(cudaStreamSynchronize(R.c.stream));
 }
 
-void bzip2_decompress_dev(Ctx& c, const u8* d_in, size_t n, int multistream, u8* d_out, size_t out_cap, size_t* out_n) {
+void bzip2_decompress_dev(Ctx& c, const u8* d_in, size_t n, int multistream, int flavor, u8* d_out, size_t out_cap, size_t* out_n) {
   *out_n = 0;
   Decode R(c, DecIn(d_in, n));
+  R.ch.flavor = flavor;
   chain_decode(R, multistream, true, [&](size_t e0, size_t e1) {
     // a walk that settled no block expands nothing
     const auto& ev = R.ch.events;
@@ -1812,9 +1827,10 @@ void bzip2_decompress_dev(Ctx& c, const u8* d_in, size_t n, int multistream, u8*
   R.finish(out_n, 0);
 }
 
-void bzip2_decompress_size(Ctx& c, const u8* d_in, size_t n, int multistream, size_t* out_n) {
+void bzip2_decompress_size(Ctx& c, const u8* d_in, size_t n, int multistream, int flavor, size_t* out_n) {
   *out_n = 0;
   Decode R(c, DecIn(d_in, n));
+  R.ch.flavor = flavor;
   chain_decode(R, multistream, false, [&](size_t e0, size_t e1) { deliver_crc(R, e0, e1, false); });
   R.finish(out_n, 0);
 }
@@ -2081,7 +2097,8 @@ void bzip2_recover(Ctx& c, StreamIn& in, bool repair, StreamOut& out, std::vecto
 //    padded) and decodes the share [lo, hi) of its block candidates; the rows are the block results, in candidate order.
 //  - shares (b2_dec_share_*): a rank holds bytes [g0, g0 + hold) of the stream and owns the magics at bit positions
 //    [8 g0, 8 (g0 + share_len)); it scans and decodes those only (one window over its buffer), and its rows carry the
-//    candidates themselves, the bytes behind its end-of-stream magics and the stream's first bytes (include/b2bz.h).
+//    candidates themselves, the bytes behind its end-of-stream magics and the stream's first bytes (include/b2bz.h); in
+//    the libbz2 flavor, a rank whose buffer ends the stream also exports the stream's last bytes, which R4 reads.
 // finish walks the chain over ALL candidates' results (imported from the other ranks), expands + CRC-checks the blocks
 // of the own share and raises the reference's errors in stream order.  A rank keeps its share's results until the
 // all-gather, so its device memory grows with its share of the file.
@@ -2093,8 +2110,18 @@ struct DecSession {
   u64 own0 = 0, own1 = 0;
   u8 hdr[4] = {0, 0, 0, 0};
   size_t hdr_n = 0;
+  // libbz2 shares: the stream's last bytes, exported by a rank whose buffer ends the stream (ends: it does)
+  bool ends = false;
+  u8 last[10] = {0};
+  size_t last_n = 0;
 
-  DecSession(Ctx& c, const u8* d_in, size_t n, int rank, int world) : R(c, DecIn(d_in, n)) {
+  bool libbz2() const { return R.ch.flavor == B2_BZ2_LIBBZ2; }
+  // the detail word of a block's row: bit 1 carries run4 (R3) in the libbz2 flavor, so that every rank's walk sees it
+  u64 detail(const CandRes& r) const { return r.detail | (libbz2() && r.run4 ? 2u : 0u); }
+  static void set_detail(CandRes& r, u64 w) { r.detail = (u32)(w & ~2ull); r.run4 = (u32)(w >> 1 & 1); }
+
+  DecSession(Ctx& c, const u8* d_in, size_t n, int rank, int world, int flavor) : R(c, DecIn(d_in, n)) {
+    R.ch.flavor = flavor;
     R.load(0, n);
     R.in = DecIn(R.win.p, n);  // later headers are read from the session's copy: the caller's buffer may be gone by then
     R.scan(n * 8);
@@ -2106,9 +2133,13 @@ struct DecSession {
     decode_own(n);
   }
 
-  DecSession(Ctx& c, const u8* d_buf, size_t hold, u64 g0, size_t share_len, size_t total)
+  DecSession(Ctx& c, const u8* d_buf, size_t hold, u64 g0, size_t share_len, size_t total, int flavor)
       : R(c, DecIn(d_buf, hold, g0, total), Decode::NoHeader{}), share(true), own0(8 * g0), own1(8 * (g0 + share_len)) {
+    R.ch.flavor = flavor;
     if (g0 == 0 && share_len) hdr_n = R.in.head(c, 0, hdr);
+    ends = libbz2() && g0 + hold == total;
+    last_n = ends ? std::min<size_t>(hold, sizeof last) : 0;
+    if (last_n) R.in.head(c, total - last_n, last, last_n);
     if (share_len) {
       // One window over the buffer from the word that holds byte g0: k_scan_magic and k_hdec take a window that starts
       // at a multiple of 32 bits, and the bytes in front of g0 read as zeros.  The scan stops at the owned range's end
@@ -2178,8 +2209,8 @@ struct DecSession {
   }
 
   // The rows of b2_dec_share_export, B2_SHARE_ROW words each: the stream's first bytes (on the rank that owns bit 0),
-  // then every owned candidate in position order.
-  size_t share_rows() const { return (size_t)(own0 == 0 && own1 > 0) + R.cands.size(); }
+  // then every owned candidate in position order, then the stream's last bytes (libbz2, on a rank whose buffer ends it).
+  size_t share_rows() const { return (size_t)(own0 == 0 && own1 > 0) + R.cands.size() + ends; }
   void share_export(u64* buf) const {
     u64* o = buf;
     if (own0 == 0 && own1 > 0) {
@@ -2195,8 +2226,13 @@ struct DecSession {
       if (cd.type != 1) continue;
       const CandRes& r = R.hres[j++];
       // an obsolete block's decode stops before its origPtr, which the walk does not read then
-      o[3] = (u64)(long long)r.status; o[4] = r.detail; o[5] = r.endbit; o[6] = r.n; o[7] = r.rawlen;
+      o[3] = (u64)(long long)r.status; o[4] = detail(r); o[5] = r.endbit; o[6] = r.n; o[7] = r.rawlen;
       o[8] = r.status == DEC_OBSOLETE ? 0 : r.orig; o[9] = r.open;
+    }
+    if (ends) {
+      memset(o, 0, 8 * B2_SHARE_ROW);
+      o[0] = R.in.length() - last_n; o[1] = 3; o[2] = last_n;
+      for (size_t k = 0; k < last_n; k++) o[3 + k / 8] |= (u64)last[k] << (8 * (k % 8));
     }
   }
   // Every rank's rows, in rank order, become the candidates and results the walk sees; the own ones keep the results
@@ -2207,8 +2243,17 @@ struct DecSession {
     std::vector<CandRes> hres;
     bool head = false;
     size_t own_c = 0, own_b = 0;
+    const u64 total = R.in.length();
     for (size_t i = 0; i < count; i++) {
       const u64* o = all + i * B2_SHARE_ROW;
+      if (o[1] == 3) {  // the stream's last bytes: the row with the most of them
+        if (o[2] > 10 || o[0] + o[2] != total) throw B2Error{B2_ERR_BAD_ARG, "a share row of the stream's last bytes that does not end it"};
+        if (o[2] > R.end_bytes.size()) {
+          R.end_bytes.resize((size_t)o[2]);
+          for (size_t k = 0; k < o[2]; k++) R.end_bytes[k] = (u8)(o[3 + k / 8] >> (8 * (k % 8)));
+        }
+        continue;
+      }
       if (o[1] > 2 || (o[1] && !cands.empty() && o[0] <= cands.back().pos)) throw B2Error{B2_ERR_BAD_ARG, "share rows out of order or of an unknown kind"};
       if (o[1] == 0) {
         if (!head) for (int k = 0; k < 4; k++) hdr[k] = (u8)(o[10] >> (8 * k));
@@ -2229,7 +2274,7 @@ struct DecSession {
       }
       CandRes r;
       memset(&r, 0, sizeof r);
-      r.status = (int)(long long)o[3]; r.detail = (u32)o[4]; r.endbit = o[5]; r.n = (u32)o[6]; r.rawlen = (u32)o[7]; r.orig = (u32)o[8];
+      r.status = (int)(long long)o[3]; set_detail(r, o[4]); r.endbit = o[5]; r.n = (u32)o[6]; r.rawlen = (u32)o[7]; r.orig = (u32)o[8];
       r.open = (u32)o[9];
       hres.push_back(r);
     }
@@ -2237,6 +2282,7 @@ struct DecSession {
     if (!own_b) lo = 0;
     hi = lo + own_b;
     if (!head) hdr_n = 0;
+    R.end_rows = libbz2();  // cut_magic reads the stream's end from the rows
     R.cands = std::move(cands);
     R.tails = std::move(tails);
     R.hres = std::move(hres);
@@ -2277,9 +2323,9 @@ struct DecSession {
 
 static std::unique_ptr<DecSession> g_shard;
 void dec_shard_release() { g_shard.reset(); }
-void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* info) {
+void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, int flavor, u64* info) {
   g_shard.reset();
-  g_shard = std::make_unique<DecSession>(c, d_in, n, rank, world);
+  g_shard = std::make_unique<DecSession>(c, d_in, n, rank, world, flavor);
   info[0] = g_shard->R.blk.size(); info[1] = g_shard->lo; info[2] = g_shard->hi;
 }
 static DecSession& session(bool share) {
@@ -2291,7 +2337,7 @@ void dec_shard_export(u64* buf) {
   for (size_t i = S.lo; i < S.hi; i++) {
     const CandRes& r = S.R.hres[i];
     u64* o = buf + (i - S.lo) * 6;
-    o[0] = (u64)(long long)r.status; o[1] = r.detail; o[2] = r.endbit; o[3] = r.n; o[4] = r.rawlen; o[5] = r.orig;
+    o[0] = (u64)(long long)r.status; o[1] = S.detail(r); o[2] = r.endbit; o[3] = r.n; o[4] = r.rawlen; o[5] = r.orig;
   }
 }
 void dec_shard_finish(const u64* all, int multistream, u8* d_out, size_t out_cap, u64* res) {
@@ -2301,14 +2347,14 @@ void dec_shard_finish(const u64* all, int multistream, u8* d_out, size_t out_cap
     if (i >= S->lo && i < S->hi) continue;
     const u64* o = all + i * 6;
     CandRes& r = S->R.hres[i];
-    r.status = (int)(long long)o[0]; r.detail = (u32)o[1]; r.endbit = o[2]; r.n = (u32)o[3]; r.rawlen = (u32)o[4]; r.orig = (u32)o[5];
+    r.status = (int)(long long)o[0]; DecSession::set_detail(r, o[1]); r.endbit = o[2]; r.n = (u32)o[3]; r.rawlen = (u32)o[4]; r.orig = (u32)o[5];
   }
   S->finish(multistream, d_out, out_cap, res);
 }
 
-void dec_share_open(Ctx& c, const u8* d_buf, size_t hold, u64 g0, size_t share_len, size_t total, u64* info) {
+void dec_share_open(Ctx& c, const u8* d_buf, size_t hold, u64 g0, size_t share_len, size_t total, int flavor, u64* info) {
   g_shard.reset();
-  g_shard = std::make_unique<DecSession>(c, d_buf, hold, g0, share_len, total);
+  g_shard = std::make_unique<DecSession>(c, d_buf, hold, g0, share_len, total, flavor);
   info[0] = g_shard->share_rows(); info[1] = g_shard->R.cands.size(); info[2] = g_shard->R.blk.size();
 }
 void dec_share_export(u64* buf) { session(true).share_export(buf); }

@@ -166,9 +166,10 @@ void bwtc_decompress(Ctx& c, StreamIn& in, StreamOut& out);
 // Each throws the reference's first error in stream order.  *out_n: the decoded size, or what the call says on an error.
 // b2_bzip2_decompress_dev: d_in[0, n) into d_out, each block at its offset in the decoded stream.  A block that does not
 // fit is only counted and the walk goes on past a data error, so a buffer too small throws with *out_n = the size needed.
-void bzip2_decompress_dev(Ctx& c, const u8* d_in, size_t n, int multistream, u8* d_out, size_t out_cap, size_t* out_n);
+// flavor: as bzip2_decompress_host's.
+void bzip2_decompress_dev(Ctx& c, const u8* d_in, size_t n, int multistream, int flavor, u8* d_out, size_t out_cap, size_t* out_n);
 // b2_bzip2_decompress_dev without an output buffer: the blocks are expanded only for their CRCs.
-void bzip2_decompress_size(Ctx& c, const u8* d_in, size_t n, int multistream, size_t* out_n);
+void bzip2_decompress_size(Ctx& c, const u8* d_in, size_t n, int multistream, int flavor, size_t* out_n);
 // b2_bzip2_decompress_partial and b2_bzip2_decompress_stream: into `out`, which never receives a byte past the prefix the
 // reference writes before an error (*out_n on an error).  flavor B2_BZ2_LIBBZ2 reads as libbz2 reads (b2_bzip2_decompress_flavor).
 void bzip2_decompress_host(Ctx& c, StreamIn& in, int multistream, int flavor, StreamOut& out, size_t* out_n);
@@ -186,10 +187,11 @@ void bzip2_decompress_list(Ctx& c, StreamIn& in, const std::vector<u64>& positio
 void bzip2_recover(Ctx& c, StreamIn& in, bool repair, StreamOut& out, std::vector<b2_recovered_block>& rows);
 // The sharded decodes (b2_dec_shard_open / _export / _finish over the whole input, b2_dec_share_open / _export / _finish
 // over shares): one session of either kind at a time, ended by finish or by the next open, or released by b2_shutdown.
-void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, u64* info);
+// The session reads in the flavor it was opened with.
+void dec_shard_open(Ctx& c, const u8* d_in, size_t n, int rank, int world, int flavor, u64* info);
 void dec_shard_export(u64* buf);
 void dec_shard_finish(const u64* all, int multistream, u8* d_out, size_t out_cap, u64* res);
-void dec_share_open(Ctx& c, const u8* d_buf, size_t hold, u64 g0, size_t share_len, size_t total, u64* info);
+void dec_share_open(Ctx& c, const u8* d_buf, size_t hold, u64 g0, size_t share_len, size_t total, int flavor, u64* info);
 void dec_share_export(u64* buf);
 void dec_share_finish(const u64* all, size_t count, int multistream, u8* d_out, size_t out_cap, u64* res);
 void dec_shard_release();

@@ -29,6 +29,7 @@ with the gloo backend in the unit tests (tests/test_sharded_host.py), where the 
 is injected.
 """
 import ctypes as C
+import functools
 import time
 from collections import namedtuple
 
@@ -684,13 +685,15 @@ def share_bounds(n, rank, world, halo):
 
 
 # ---- sharded decode -------------------------------------------------------------------------------
-def decode_shard_rows(L, d_in, rank, world):
-    """Stage 1 on one rank: returns (info, rows) -- rows = int64 tensor [own candidates, 6] on the CPU."""
+def decode_shard_rows(L, d_in, rank, world, flavor="compressjs"):
+    """Stage 1 on one rank: returns (info, rows) -- rows = int64 tensor [own candidates, 6] on the CPU.  The session
+    reads in `flavor` until its finish."""
     from . import _native
+    fl = _flavor_id(flavor)
     if d_in.is_cuda:
         torch.cuda.current_stream().synchronize()   # the library works on its own stream: the input must have landed
     info = (C.c_uint64 * 3)()
-    rc = L.b2_dec_shard_open(d_in.data_ptr(), d_in.numel(), rank, world, info)
+    rc = L.b2_dec_shard_open_flavor(d_in.data_ptr(), d_in.numel(), rank, world, info, fl)
     if rc:
         raise RuntimeError("b2_dec_shard_open: %s (code %d)" % (_native.last_error(), rc))
     total, lo, hi = int(info[0]), int(info[1]), int(info[2])
@@ -702,9 +705,11 @@ def decode_shard_rows(L, d_in, rank, world):
     return (total, lo, hi), rows
 
 
-def decode_shard_finish(L, all_rows, multistream, device):
-    """Stage 2 on one rank: all_rows = [total candidates, 6] int64 (CPU).  Returns (own output tensor, res)."""
+def decode_shard_finish(L, all_rows, multistream, device, flavor="compressjs"):
+    """Stage 2 on one rank: all_rows = [total candidates, 6] int64 (CPU).  Returns (own output tensor, res).  The
+    session finishes in the flavor it was opened with, which `flavor` names."""
     from . import _native
+    _flavor_id(flavor)
     flat = [int(v) & (2 ** 64 - 1) for v in all_rows.reshape(-1).tolist()]
     arr = (C.c_uint64 * max(len(flat), 1))(*flat)
     res = (C.c_uint64 * 5)()
@@ -721,20 +726,22 @@ def decode_shard_finish(L, all_rows, multistream, device):
                                                       err_code=err_code if rc else 0, msg=msg)
 
 
-def _decode_whole_input(d_in, multistream=False, group=None):
+def _decode_whole_input(d_in, multistream=False, group=None, flavor="compressjs"):
     """The sharded decode of a stream held on every rank, up to the error exchange: (own output tensor or None, res) on
     every rank, as decode_shard_finish returns them."""
     from . import _native
+    fl = _flavor_id(flavor)
     L = _native.lib()
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     device = d_in.device
-    (total, lo, hi), rows = decode_shard_rows(L, d_in, rank, world)
+    (total, lo, hi), rows = decode_shard_rows(L, d_in, rank, world, flavor)
     if world > 1:
         # every rank scanned the same stream: the candidate counts must agree (a cheap guard against mismatched collectives)
-        chk = torch.tensor([total, d_in.numel()], dtype=torch.int64, device=device)
+        chk = torch.tensor([total, d_in.numel(), fl], dtype=torch.int64, device=device)
         allc = [torch.zeros_like(chk) for _ in range(world)]
         dist.all_gather(allc, chk, group=group)
+        _same_flavor([int(v[2]) for v in allc], "decompress_file_sharded")
         if any(int(v[0]) != total or int(v[1]) != d_in.numel() for v in allc):
             raise RuntimeError("decompress_file_sharded: the ranks do not hold the same stream")
         per = max((r + 1) * total // world - r * total // world for r in range(world))
@@ -750,7 +757,14 @@ def _decode_whole_input(d_in, multistream=False, group=None):
         all_rows = torch.cat(parts) if parts else rows
     else:
         all_rows = rows
-    return decode_shard_finish(L, all_rows, multistream, device)
+    return decode_shard_finish(L, all_rows, multistream, device, flavor)
+
+
+def _same_flavor(ids, call):
+    """Every rank's flavor id, from an exchange: ranks that read in different flavors raise together."""
+    if len(set(ids)) > 1:
+        names = {v: k for k, v in FLAVORS.items()}
+        raise ValueError("%s: the ranks ask for different flavors (%s)" % (call, ", ".join(names.get(i, str(i)) for i in ids)))
 
 
 def _settle(res, device, group=None):
@@ -796,10 +810,12 @@ def _place(out, spans, total, device, group=None):
     return full
 
 
-def decompress_file_sharded(d_in, multistream=False, group=None):
-    """Decode a .bz2 stream held on every rank; the decoded bytes are gathered on rank 0 (uint8 tensor)."""
+def decompress_file_sharded(d_in, multistream=False, group=None, flavor="compressjs"):
+    """Decode a .bz2 stream held on every rank; the decoded bytes are gathered on rank 0 (uint8 tensor).  flavor as
+    Bzip2.decompressFile's: "libbz2" reads as bzip2 -d does.  Every rank must ask for the same flavor."""
+    _flavor_id(flavor)
     world = dist.get_world_size(group) if dist.is_initialized() else 1
-    out, res = _decode_whole_input(d_in, multistream, group)
+    out, res = _decode_whole_input(d_in, multistream, group, flavor)
     spans, total = _settle(res, d_in.device, group)
     if world == 1:
         return out
@@ -838,16 +854,18 @@ def share_layout(sizes):
     return g0s, total
 
 
-def _share_open(d_buf, share_len, g0, total):
-    """Stage 1 on one rank (b2_dec_share_open + export): (rows, 0, "") with rows an int64 CPU tensor [k, SHARE_ROW], or
-    (no rows, error code, message) when the open failed, which the caller reports after the exchange."""
+def _share_open(d_buf, share_len, g0, total, flavor="compressjs"):
+    """Stage 1 on one rank (b2_dec_share_open_flavor + export): (rows, 0, "") with rows an int64 CPU tensor [k,
+    SHARE_ROW], or (no rows, error code, message) when the open failed, which the caller reports after the exchange.
+    The session reads in `flavor` until its finish."""
     from . import _native
+    fl = _flavor_id(flavor)
     L = _native.lib()
     if d_buf.is_cuda:
         torch.cuda.current_stream().synchronize()   # the library works on its own stream: the input must have landed
     none = torch.zeros((0, SHARE_ROW), dtype=torch.int64)
     info = (C.c_uint64 * 3)()
-    rc = L.b2_dec_share_open(d_buf.data_ptr(), d_buf.numel(), g0, share_len, total, info)
+    rc = L.b2_dec_share_open_flavor(d_buf.data_ptr(), d_buf.numel(), g0, share_len, total, info, fl)
     if rc:
         return none, rc, "b2_dec_share_open: " + _native.last_error()
     k = int(info[0])
@@ -859,10 +877,12 @@ def _share_open(d_buf, share_len, g0, total):
     return torch.from_numpy(rows.copy()), 0, ""
 
 
-def _share_finish(all_rows, own_rows, multistream, device):
+def _share_finish(all_rows, own_rows, multistream, device, flavor="compressjs"):
     """Stage 2 on one rank (b2_dec_share_finish): all_rows = every rank's rows in rank order, own_rows = this rank's.
-    Returns (own output tensor, or None on an error, res) with res as decode_shard_finish's plus `unsettled`."""
+    Returns (own output tensor, or None on an error, res) with res as decode_shard_finish's plus `unsettled`.  The
+    session finishes in the flavor it was opened with, which `flavor` names."""
     from . import _native
+    _flavor_id(flavor)
     L = _native.lib()
     flat = np.ascontiguousarray(all_rows.numpy(), dtype=np.int64)
     own = own_rows.numpy()
@@ -889,7 +909,7 @@ def _gather_shares(d_buf, share_len, lens, group=None):
     return torch.cat([gl[r][: lens[r]] for r in range(world)])
 
 
-def decompress_shares(d_buf, share_len, multistream=False, group=None, keep_sharded=False):
+def decompress_shares(d_buf, share_len, multistream=False, group=None, keep_sharded=False, flavor="compressjs"):
     """Decode a .bz2 stream that no rank holds whole: the decode counterpart of compress_shares.  d_buf = uint8 tensor
     with the rank's share of the stream (share_len bytes) followed by a halo, the first bytes of the next shares (at least
     DEC_HALO_MIN bytes unless it reaches the end of the stream; DEC_HALO is enough for any intact block).  The shares are
@@ -898,25 +918,32 @@ def decompress_shares(d_buf, share_len, multistream=False, group=None, keep_shar
     that runs past its owner's halo), every rank gathers the shares and decodes the whole input (decompress_file_sharded's
     path) instead.  The decoded bytes, or the error, are exactly those of Bzip2.decompressFile(stream, multistream=...)
     on one GPU; nothing is delivered on an error.  Returns the decoded stream on rank 0 (None elsewhere); with
-    keep_sharded a DecodedShare on every rank (with one rank: the whole stream)."""
-    return _decompress_shares(d_buf, share_len, multistream, group, keep_sharded, _share_open, _share_finish, _decode_whole_input)
+    keep_sharded a DecodedShare on every rank (with one rank: the whole stream).  flavor as Bzip2.decompressFile's
+    ("libbz2": the result is that of decompressFile(..., flavor="libbz2"), bzip2 -d's); every rank must ask for the same
+    one, or all raise ValueError."""
+    _flavor_id(flavor)
+    stages = [functools.partial(f, flavor=flavor) for f in (_share_open, _share_finish, _decode_whole_input)]
+    return _decompress_shares(d_buf, share_len, multistream, group, keep_sharded, *stages, flavor=flavor)
 
 
-def _decompress_shares(d_buf, share_len, multistream, group, keep_sharded, open_stage, finish_stage, whole_stage):
+def _decompress_shares(d_buf, share_len, multistream, group, keep_sharded, open_stage, finish_stage, whole_stage, flavor="compressjs"):
     """decompress_shares with its library stages passed in: open_stage(d_buf, share_len, g0, total) -> (rows, code,
     message); finish_stage(all rows, own rows, multistream, device) -> (own output, res); whole_stage(stream,
-    multistream, group) -> (own output, res) from the whole input on every rank."""
+    multistream, group) -> (own output, res) from the whole input on every rank.  The stages read in `flavor` (bound into
+    them by the caller); it travels with the first exchange, so that ranks that ask for different flavors all raise."""
+    fl = _flavor_id(flavor)
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     dev = d_buf.device
     PHASES.clear()
-    # 1. every rank's (share length, bytes held): where the shares start, the stream's length, every rank's halo
-    mine = torch.tensor([share_len, d_buf.numel()], dtype=torch.int64, device=dev)
+    # 1. every rank's (share length, bytes held, flavor): where the shares start, the stream's length, every rank's halo
+    mine = torch.tensor([share_len, d_buf.numel(), fl], dtype=torch.int64, device=dev)
     if world > 1:
         alls = [torch.zeros_like(mine) for _ in range(world)]
         dist.all_gather(alls, mine, group=group)
     else:
         alls = [mine]
+    _same_flavor([int(v[2]) for v in alls], "decompress_shares")
     sizes = [(int(v[0]), int(v[1])) for v in alls]
     g0s, total = share_layout(sizes)
     # 2. open and export; a failed open travels with the row counts, so that every rank raises after the exchange

@@ -280,8 +280,9 @@ int b2_bzip2_compress_dev_flavor(const void* d_in, size_t n, int level, void* d_
  * The prefix delivered on an error is that of b2_bzip2_decompress_partial: for -3, every block in front (they all passed
  * their CRCs).  Device and host memory bounds are those of the calls without a flavor.  The _flavor calls take the
  * arguments of the call they extend plus the flavor; an unknown flavor returns B2_ERR_BAD_ARG before any callback runs or
- * any work is done.  decompress_block[s], table, b2_bzip2_decompress_dev, the sharded decode and recovery read the
- * compressjs flavor only. */
+ * any work is done.  The device-resident decode (b2_bzip2_decompress_dev_flavor) and both sharded decodes
+ * (b2_dec_shard_open_flavor, b2_dec_share_open_flavor) take the flavor too.  decompress_block[s], table and recovery
+ * read the compressjs flavor only. */
 int b2_bzip2_decompress_flavor(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n, int flavor);
 int b2_bzip2_decompress_partial_flavor(const uint8_t* in, size_t n, int multistream, uint8_t** out, size_t* out_n, int flavor);
 int b2_bzip2_decompress_stream_flavor(b2_read_fn rd, b2_write_fn wr, void* user, int multistream, int flavor);
@@ -295,6 +296,9 @@ int b2_bzip2_compress_dev(const void* d_in, size_t n, int level, void* d_out, si
 /* Decode with device buffers; *out_n receives the decoded size; fails with
  * B2_ERR_BAD_ARG (and the needed size in *out_n) if out_cap is too small. */
 int b2_bzip2_decompress_dev(const void* d_in, size_t n, int multistream, void* d_out, size_t out_cap, size_t* out_n);
+/* The same in a decoder flavor (B2_BZ2_LIBBZ2: the rules R1-R5 above), with the same too-small-buffer rule. */
+int b2_bzip2_decompress_dev_flavor(const void* d_in, size_t n, int multistream, void* d_out, size_t out_cap, size_t* out_n,
+                                   int flavor);
 
 /* ---- block-range encode for multi-GPU sharding (SURVEY.md section 8e) ------------- */
 /* Plan cache: b2_bzip2_plan(_flavor), _plan_spec and _plan_share(_flavor) keep their plan, replacing the one kept
@@ -368,8 +372,14 @@ int b2_bzip2_encode_range_dev_flavor(const void* d_in, size_t n, int level, size
  * export: 6 x uint64 per own candidate (status, detail, end bit, block length, decoded length, 0).
  * finish: `all` = the exported rows of ALL candidates in order (all-gathered by the caller); walks the
  * block chain, expands and CRC-checks the own blocks into d_out; res = {offset of the own output in the
- * decoded stream, its length, total decoded length, index of the first failing event or -1, its code}. */
+ * decoded stream, its length, total decoded length, index of the first failing event or -1, its code}.
+ * _flavor: open in a decoder flavor, which the session keeps until finish; the result, bytes or error, is then that of
+ * b2_bzip2_decompress_flavor.  The calls without a flavor read the compressjs flavor.  The detail word (word [1] of a
+ * row) is 1 for "initial position out of bounds"; in the libbz2 flavor its bit 1 (value 2) is set when the block's
+ * bytes before RLE1 decoding end on an uncounted run of four (R3), so that every rank's walk applies R3 to every block.
+ * The compressjs flavor never sets it. */
 int b2_dec_shard_open(const void* d_in, size_t n, int rank, int world, uint64_t* info);
+int b2_dec_shard_open_flavor(const void* d_in, size_t n, int rank, int world, uint64_t* info, int flavor);
 int b2_dec_shard_export(uint64_t* buf);
 int b2_dec_shard_finish(const uint64_t* all, int multistream, void* d_out, size_t out_cap, uint64_t* res);
 
@@ -392,13 +402,21 @@ int b2_dec_shard_finish(const uint64_t* all, int multistream, void* d_out, size_
  *   [0] bit position of the magic (0 for kind 0)
  *   [1] kind: 0 the stream's first bytes, 1 block, 2 end of stream
  *   [2] the 32 bits behind the magic (block CRC, stream CRC)
- *   [3] block status: 0, or the reference's (negative) error code      [4] detail: 1 = "initial position out of bounds"
+ *   [3] block status: 0, or the reference's (negative) error code      [4] detail: 1 = "initial position out of bounds";
+ *                                                                          bit 1 (value 2): run of four at the end (R3,
+ *                                                                          libbz2 flavor only)
  *   [5] end bit: the bit behind the block's end-of-block code            [6] block length before the inverse BWT
  *   [7] decoded length                                                    [8] origPtr
  *   [9] open: 1 = the decode read past the end of the buffer, which does not end the stream
  *   [10] bytes: kind 0, the stream's first up to 4 bytes; kind 2, up to 4 bytes from the byte boundary behind the stream
  *        CRC (the next member's header); byte k at bits 8k, their count at bits 32 and up.  0 for a block.
  * Fields [3]-[9] are 0 for kinds 0 and 2.
+ * In the libbz2 flavor, a rank whose buffer ends the stream (g0 + hold = total) ends its rows with one of kind 3, the
+ * stream's last min(10, hold) bytes, which R4 reads where a magic is cut off:
+ *   [0] stream offset of the first of these bytes (total - count)     [1] kind: 3     [2] count
+ *   [3], [4] the bytes: byte k at bits 8 (k mod 8) of word 3 + k / 8   every other word 0
+ * finish takes the kind-3 row with the most bytes.  A final share shorter than 10 bytes is covered by the rank in front,
+ * whose halo then reaches the end of the stream.  The compressjs flavor exports no kind-3 row.
  * finish: `all` = the `count` exported rows of ALL ranks in rank order (all-gathered by the caller).  Walks the chain as
  * b2_dec_shard_finish does, taking the first header and the bytes behind end-of-stream magics from the rows, expands
  * and CRC-checks the own blocks into d_out (out_cap: at least the decoded length of the owned blocks that decoded), and
@@ -406,11 +424,15 @@ int b2_dec_shard_finish(const uint64_t* all, int multistream, void* d_out, size_
  * failing event or -1, its code, not settled}.  A bad first header fails with index 0.  When the walk reaches an
  * on-chain block that its owner decoded as open, the rows cannot settle the stream: res[5] = 1, nothing is delivered,
  * the call returns 0, and every rank (all see the same rows) decodes from the whole input instead
- * (b2_dec_shard_*).  Then the result, decoded bytes or error, is exactly that of b2_bzip2_decompress on one GPU.
- * Compressjs flavor only.  Opening either kind of sharded decode ends the session of the other. */
+ * (b2_dec_shard_*, in the same flavor).  Then the result, decoded bytes or error, is exactly that of
+ * b2_bzip2_decompress_flavor on one GPU.  b2_dec_share_open reads the compressjs flavor, b2_dec_share_open_flavor the
+ * flavor it is given, which the session keeps until finish.  Opening either kind of sharded decode ends the session of
+ * the other. */
 #define B2_SHARE_ROW 11
 #define B2_SHARE_HALO_MIN 14
 int b2_dec_share_open(const void* d_buf, size_t hold, uint64_t g0, size_t share_len, size_t total, uint64_t* info);
+int b2_dec_share_open_flavor(const void* d_buf, size_t hold, uint64_t g0, size_t share_len, size_t total, uint64_t* info,
+                             int flavor);
 int b2_dec_share_export(uint64_t* buf);
 int b2_dec_share_finish(const uint64_t* all, size_t count, int multistream, void* d_out, size_t out_cap, uint64_t* res);
 
